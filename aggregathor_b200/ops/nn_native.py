@@ -233,8 +233,14 @@ def mm_tn(x, y, out=None, splits=None, bn=0, groups=1, group_stride=0):
   x = _rows(x)
   y = _rows(y, x.dtype)
   K, M = x.shape
-  K //= groups
   N = y.shape[1]
+  if groups > 1:
+    if K % groups or y.shape[0] != K:
+      raise ValueError("mm_tn: %d and %d rows do not split into %d equal groups" % (K, y.shape[0], groups))
+    # every group needs its own output: with a shared one the groups' products would be summed (split-K) or race
+    if out is None or group_stride < (M - 1) * out.stride(0) + N:
+      raise ValueError("mm_tn: %d groups need an out= and a group_stride of at least one [%d, %d] output, got %s" % (groups, M, N, group_stride))
+  K //= groups
   fresh = out is None
   if fresh:
     out = torch.empty((M, N), dtype=torch.float32, device=x.device)
