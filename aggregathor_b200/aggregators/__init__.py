@@ -24,7 +24,7 @@ __all__ = ["_GAR", "FusedSpec", "register", "instantiate", "itemize", "get"]
 class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
-  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan")
+  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda")
 
   def __init__(self, rule, n, f=0, m=0, beta=0):
     if rule not in self.RULES:

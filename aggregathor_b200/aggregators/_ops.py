@@ -12,6 +12,8 @@ Ordering convention everywhere: finite ascending, then non-finite; ties -> lower
 """
 
 import ctypes
+import itertools
+import math
 
 import torch
 
@@ -44,6 +46,21 @@ def check_bulyan(n, f, m=None):
   theta = n - 2 * f - 2
   if m is not None and not theta <= m <= n:
     raise tools.UserException("Bulyan needs n - 2 f - 2 <= m <= n (got m = %d)" % m)
+
+
+def check_trimmed_mean(n, f):
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("The trimmed mean needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+
+
+MDA_MAX_SETS = 1 << 20
+
+
+def check_mda(n, f):
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("MDA needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+  if math.comb(n, f) > MDA_MAX_SETS:
+    raise tools.UserException("MDA enumerates the C(n, f) subsets of removed workers: C(%d, %d) = %d is above the bound 2^20" % (n, f, math.comb(n, f)))
 
 
 def _rank_key(values):
@@ -114,6 +131,30 @@ def host_bulyan(G, f, m, return_weights=False):
   return (out, weights) if return_weights else out
 
 
+def host_trimmed_mean(G, f):
+  check_trimmed_mean(G.shape[0], f)
+  return _host_call("trimmed_mean", G, f)
+
+
+def host_mda(G, f, return_selected=False):
+  check_mda(G.shape[0], f)
+  selected = torch.empty(G.shape[0] - f, dtype=torch.int64)
+  out = _host_call("mda", G, f, outputs=(selected, None))
+  return (out, selected) if return_selected else out
+
+
+def host_mda_select(dist, f):
+  """Selection stage of MDA on an [n, n] distance matrix -> ascending ids of the n - f kept workers."""
+  dist = dist.detach().to("cpu").contiguous()
+  n = dist.shape[0]
+  check_mda(n, f)
+  selected = torch.empty(n - f, dtype=torch.int64)
+  status = _host("mda_select", dist.dtype)(_ptr(dist), ctypes.c_size_t(n), ctypes.c_size_t(f), _ptr(selected))
+  if status != 0:
+    raise tools.UserException("Host MDA selection rejected its arguments (n = %d, f = %d)" % (n, f))
+  return selected
+
+
 def host_pairwise_distances(G):
   Gc = G.detach().to("cpu").contiguous()
   n, d = Gc.shape
@@ -167,6 +208,38 @@ def torch_averaged_median(G, beta):
   order = torch.argsort(_rank_key(dev), dim=0, stable=True)[:beta]
   keep = torch.zeros_like(G, dtype=torch.bool).scatter_(0, order, True)
   return torch.where(keep, G, torch.zeros_like(G)).sum(dim=0) / beta
+
+
+def torch_trimmed_mean(G, f):
+  """Per coordinate, mean of the values ranked [f, n - f) under the ordering convention."""
+  n = G.shape[0]
+  check_trimmed_mean(n, f)
+  order = torch.argsort(_rank_key(G), dim=0, stable=True)
+  keep = torch.zeros_like(G, dtype=torch.bool).scatter_(0, order[f:n - f], True)
+  return torch.where(keep, G, torch.zeros_like(G)).sum(dim=0) / (n - 2 * f)
+
+
+def mda_select(dist, f, chunk=1 << 22):
+  """[n, n] distances -> ascending ids of the n - f kept workers of minimum diameter; ties -> lexicographically smallest id list.
+  Enumerates the kept sets in lexicographic order (`itertools.combinations`); `argmin` returns the first minimum."""
+  n = dist.shape[0]
+  check_mda(n, f)
+  D = torch.where(torch.isfinite(dist), dist, torch.full_like(dist, float("inf")))
+  size = n - f
+  if size < 2:
+    return torch.arange(size, dtype=torch.int64)
+  sets = torch.tensor(list(itertools.combinations(range(n), size)), dtype=torch.int64, device=dist.device)
+  rows = max(1, chunk // (size * size))
+  diam = torch.cat([D[part[:, :, None], part[:, None, :]].amax(dim=(1, 2)) for part in sets.split(rows)])
+  return sets[int(torch.argmin(diam))].cpu()
+
+
+def torch_mda(G, f, return_selected=False):
+  n = G.shape[0]
+  check_mda(n, f)
+  selected = mda_select(torch_pairwise_distances(G), f)
+  out = G[selected.to(G.device)].sum(dim=0) / (n - f)
+  return (out, selected) if return_selected else out
 
 
 def torch_pairwise_distances(G):

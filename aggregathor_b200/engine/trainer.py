@@ -78,7 +78,7 @@ class Manager:
       # pass is opt-in: AGB_OVERLAP=1 for single-worker ranks of multi-rank jobs, =2 always.
       overlap = os.environ.get("AGB_OVERLAP", "0")
       single_worker_ranks = self.world > 1 and nbworkers == self.world
-      if plain_step and aggregator.fused_spec().rule in ("krum", "bulyan") and (overlap == "2" or (overlap not in ("", "0") and single_worker_ranks)) and "buckets" not in engine_args:
+      if plain_step and aggregator.fused_spec().rule in ("krum", "bulyan", "mda") and (overlap == "2" or (overlap not in ("", "0") and single_worker_ranks)) and "buckets" not in engine_args:
         buckets, self._bucket_layers = self._plan_buckets()
         if len(buckets) > 1:
           engine_args["buckets"] = buckets

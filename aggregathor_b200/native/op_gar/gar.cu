@@ -5,14 +5,15 @@
 // `deprecated_native/native.cpp` median/averaged-median/average-nan, `opt.apply_gradients`,
 // PS->worker variable transfer). Per rank and step:
 //
-//   phase A kernels  (Krum/Bulyan, optional, one per gradient *bucket*, launched on a side stream while the backward pass is still
+//   phase A kernels  (Krum/Bulyan/MDA, optional, one per gradient *bucket*, launched on a side stream while the backward pass is still
 //                    producing the earlier layers' gradients) entry flag of the bucket, then stream this rank's share of the bucket of
 //                    all n gradients straight from the peers' buffers (P2P loads over NVLink), accumulate the partial squared
 //                    distances with direct differences, stage the tile locally
 //   finish kernel    (cooperative) phase A of whatever was not pre-accumulated; partial matrices go to every peer's mailbox together
 //                    with the rank's loss sum; summed in rank order => bit-identical distance matrix (and total loss) on every rank;
-//                    one warp: Krum scores / Bulyan iterative selection (replicated on all ranks); phase D: aggregate the owned
-//                    coordinates (mean of selected / coordinate-wise trimmed mean / median / NaN-aware mean), apply the optimizer,
+//                    one warp: Krum scores / Bulyan iterative selection, or the whole grid: MDA's minimum-diameter search
+//                    (replicated on all ranks); phase D: aggregate the owned coordinates (mean of selected / coordinate-wise
+//                    trimmed mean / median / NaN-aware mean), apply the optimizer,
 //                    store the new parameters into every rank's buffer (P2P stores or one NVLS multimem.st); exit barrier
 //
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
@@ -40,7 +41,8 @@ constexpr int kSlotExit = kMaxSeg + 1;
 constexpr int kFlagSlots = kMaxSeg + 2;
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
-enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5 };
+constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
+enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -80,10 +82,17 @@ struct GarArgs {
 
 struct Shared {
     float dist[kMaxWorkers][kMaxWorkers + 1];
-    float pruned[kMaxWorkers][kMaxWorkers + 1];
+    union {
+        float pruned[kMaxWorkers][kMaxWorkers + 1];      // Bulyan
+        struct {                                          // MDA
+            unsigned short order[kMaxPairs];              // pairs (i | j << 8) by descending distance
+            unsigned binom[kMaxWorkers + 1][kMaxWorkers / 2 + 1];
+            unsigned long long best[16];                  // per-warp minimum keys
+        } mda;
+    };
     float scores[kMaxWorkers];
     float warp_partials[16][kBlockRows * kBlockRows];
-    unsigned selmask[kMaxWorkers];   // Krum: [0]; Bulyan: one per round
+    unsigned selmask[kMaxWorkers];   // Krum, MDA: [0]; Bulyan: one per round
     int selcount[kMaxWorkers];
     int theta;
     float hyper[4];
@@ -235,6 +244,24 @@ template<int N> __device__ __forceinline__ float coord_averaged_median(float con
     return sum / static_cast<float>(beta);
 }
 
+// mean of the values ranked [f, n - f), summed in index order (the f smallest and the f largest or non-finite values are dropped)
+template<int N> __device__ __forceinline__ float coord_trimmed_mean(float const (&v)[N], int n, int f) {
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        if (i < n) {
+            int rank = 0;
+#pragma unroll
+            for (int j = 0; j < N; ++j)
+                if (j < n && j != i)
+                    rank += before(v[j], j, v[i], i) ? 1 : 0;
+            if (rank >= f && rank < n - f)
+                sum += v[i];
+        }
+    }
+    return sum / static_cast<float>(n - 2 * f);
+}
+
 template<int N> __device__ __forceinline__ float coord_average_nan(float const (&v)[N], int n) {
     float sum = 0.f;
     int count = 0;
@@ -371,6 +398,103 @@ __device__ void select_bulyan(GarArgs const& a, Shared& sh) {
     }
     if (lane == 0)
         sh.theta = theta;
+}
+
+// MDA (every thread of the grid): the kept set S, |S| = n - f, of smallest diameter (largest distance between two members); ties -> the
+// lexicographically smallest sorted index list, i.e. the largest __brev(mask). The C(n, f) removal sets are split over all threads: a
+// thread unranks the first set of its range (colexicographic order = ascending masks) and steps with Gosper's hack. A set's diameter
+// is the distance of the first pair, in descending distance order, whose ends are both kept: at most f (n - 1) + 1 steps. Keys
+// (diameter bits, ~__brev(mask)) are exact, so their minimum does not depend on the reduction order: every CTA and every rank (same
+// distance matrix) selects the same set. The per-CTA minima go through `cta_partials`, free again once the distances are exchanged.
+__device__ void select_mda(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
+    constexpr int K = kMaxWorkers / 2 + 1;
+    int const n = a.n, f = a.f, npairs = n * (n - 1) / 2;
+    int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    for (int p = threadIdx.x; p < (kMaxWorkers + 1) * K; p += blockDim.x) {
+        int const m = p / K, k = p % K;
+        unsigned long long c = 1;   // C(m, k) < 2^32 for m <= 32; every partial product is an exact binomial times (m - t)
+        for (int t = 0; t < k && t < m; ++t)
+            c = c * (m - t) / (t + 1);
+        sh.mda.binom[m][k] = k > m ? 0u : static_cast<unsigned>(c);
+    }
+    for (int p = threadIdx.x; p < npairs; p += blockDim.x) {   // rank of pair p by (distance descending, pair index ascending)
+        int i = 0, rest = p;
+        while (rest >= n - 1 - i) {
+            rest -= n - 1 - i;
+            ++i;
+        }
+        int const j = i + 1 + rest;
+        float const dp = sh.dist[i][j];
+        int rank = 0, q = 0;
+        for (int qi = 0; qi < n - 1; ++qi)
+            for (int qj = qi + 1; qj < n; ++qj, ++q) {
+                float const dq = sh.dist[qi][qj];
+                rank += (dq > dp || (dq == dp && q < p)) ? 1 : 0;
+            }
+        sh.mda.order[rank] = static_cast<unsigned short>(i | (j << 8));
+    }
+    __syncthreads();
+    long long const total = sh.mda.binom[n][f];
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const per = (total + nthreads - 1) / nthreads;
+    long long r = tid * per;
+    long long const end = r + per < total ? r + per : total;
+    unsigned const full = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    unsigned long long best = ~0ull;
+    if (r < end) {
+        unsigned removed = 0;   // combinatorial number system: r = sum_k C(c_k, k), c_f > ... > c_1
+        long long rest = r;
+        for (int k = f; k >= 1; --k) {
+            int c = n - 1;
+            while (sh.mda.binom[c][k] > rest)
+                --c;
+            removed |= 1u << c;
+            rest -= sh.mda.binom[c][k];
+        }
+        for (;;) {
+            unsigned const keep = full & ~removed;
+            float diam = 0.f;
+            for (int q = 0; q < npairs; ++q) {
+                unsigned const pr = sh.mda.order[q], i = pr & 0xffu, j = pr >> 8;
+                if ((keep >> i) & (keep >> j) & 1u) {
+                    diam = sh.dist[i][j];
+                    break;
+                }
+            }
+            unsigned long long const key = static_cast<unsigned long long>(__float_as_uint(diam)) << 32 | ~__brev(keep);
+            best = key < best ? key : best;
+            if (++r >= end)
+                break;
+            unsigned const low = removed & (0u - removed), up = removed + low;   // Gosper's hack: next mask with f bits
+            removed = (((up ^ removed) >> 2) >> (__ffs(low) - 1)) | up;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        unsigned long long const other = __shfl_xor_sync(0xffffffffu, best, o);
+        best = other < best ? other : best;
+    }
+    if (lane == 0)
+        sh.mda.best[warp] = best;
+    __syncthreads();
+    unsigned long long* const slots = reinterpret_cast<unsigned long long*>(a.cta_partials);
+    if (threadIdx.x == 0) {
+        for (int w = 0; w < nwarps; ++w)
+            best = sh.mda.best[w] < best ? sh.mda.best[w] : best;
+        slots[static_cast<long long>(blockIdx.x) * (kMaxPairs / 2)] = best;
+    }
+    __threadfence();
+    grid.sync();
+    if (threadIdx.x == 0) {
+        unsigned long long key = ~0ull;
+        for (unsigned b = 0; b < gridDim.x; ++b) {
+            unsigned long long const other = *reinterpret_cast<unsigned long long volatile*>(slots + static_cast<long long>(b) * (kMaxPairs / 2));
+            key = other < key ? other : key;
+        }
+        sh.selmask[0] = __brev(~static_cast<unsigned>(key));
+        sh.selcount[0] = n - f;
+        sh.theta = 1;
+    }
 }
 
 // ---- phase A: partial pairwise squared distances over one owned segment --------------------------------------------- //
@@ -536,7 +660,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
     long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
     bool const multi = a.R > 1;
-    bool const distance_rule = a.rule == kKrum || a.rule == kBulyan;
+    bool const distance_rule = a.rule == kKrum || a.rule == kBulyan || a.rule == kMda;
     if (threadIdx.x == 0) {
         sh.epoch = current_epoch(a);
         for (int i = 0; i < 4; ++i)
@@ -624,7 +748,9 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
             *a.loss_out = total;
         }
         __syncthreads();
-        if (threadIdx.x < 32) {
+        if (a.rule == kMda) {
+            select_mda(a, sh, grid);
+        } else if (threadIdx.x < 32) {
             if (a.rule == kKrum)
                 select_krum(a, sh);
             else
@@ -648,7 +774,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                         V<VEC>::load_stream(a.grad[i] + x, dst);
                 };
                 float out[VEC];
-                if (a.rule == kKrum) {
+                if (a.rule != kBulyan) {   // Krum, MDA: mean of the selected rows
                     unsigned const mask = sh.selmask[0];
                     float sum[VEC];
 #pragma unroll
@@ -678,7 +804,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                             }
                         }
                     }
-                    float const count = static_cast<float>(a.m);
+                    float const count = static_cast<float>(sh.selcount[0]);
 #pragma unroll
                     for (int c = 0; c < VEC; ++c)
                         out[c] = sum[c] / count;
@@ -788,6 +914,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                             r = coord_average_nan<N>(vals, n);
                         else if (a.rule == kMedian)
                             r = coord_median<N>(vals, n);
+                        else if (a.rule == kTrimmedMean)
+                            r = coord_trimmed_mean<N>(vals, n, a.f);
                         else
                             r = coord_averaged_median<N>(vals, n, a.beta);
                         out[c] = r;
@@ -923,8 +1051,17 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kBulyan)
+    if (a.rule < 0 || a.rule > kMda)
         return 102;
+    if ((a.rule == kTrimmedMean || a.rule == kMda) && (a.f < 0 || 2 * a.f >= a.n))
+        return a.rule == kTrimmedMean ? 112 : 113;
+    if (a.rule == kMda) {
+        long long sets = 1;   // C(n, f), exact while it stays below the bound
+        for (int t = 0; t < a.f && sets <= kMdaMaxSets; ++t)
+            sets = sets * (a.n - t) / (t + 1);
+        if (sets > kMdaMaxSets)
+            return 113;
+    }
     if ((a.rule == kKrum || a.rule == kBulyan) && (a.n - a.f - 2 < 1 || a.m < 1 || a.m > a.n))
         return 103;
     if (a.rule == kBulyan && (a.n < 4 * a.f + 3 || a.beta != a.n - 4 * a.f - 2 || a.m < a.n - 2 * a.f - 2))
@@ -960,13 +1097,13 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 107;
     if (a.opt == kAdagrad && !a.slot0)
         return 107;
-    if ((a.rule == kKrum || a.rule == kBulyan) && (!a.cta_partials || !a.mailbox[0]))
+    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && (!a.cta_partials || !a.mailbox[0]))
         return 108;
     if (a.first_seg > 0 && !a.seg_partials)
         return 108;
     if (a.R > 1 && !a.signal[0])
         return 109;
-    if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan) && !a.staging)
+    if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && !a.staging)
         return 110;   // blocked passes over remote rows need the staged copy
     return 0;
 }
@@ -1027,7 +1164,7 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     if (status)
         return status;
     int const ctas = ints[15];
-    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan))
+    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda))
         return 111;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // small CTAs: a 64-thread CTA (8 K registers, 13 KB of static shared memory) fits beside a persistent GEMM CTA of the backward pass

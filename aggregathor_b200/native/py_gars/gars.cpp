@@ -345,6 +345,143 @@ template<class T> int averaged_median(T const* g, size_t n, size_t d, size_t bet
     return 0;
 }
 
+// Coordinate-wise trimmed mean: per coordinate, the values ranked [f, n - f) (the f smallest and the f largest or non-finite ones are
+// dropped), added in index order, divided once by n - 2f. Same order of operations as the device kernel, hence the same bits.
+template<class T> int trimmed_mean(T const* g, size_t n, size_t d, size_t f, T* out) {
+    if (n == 0 || n > kMaxWorkers || 2 * f >= n)
+        return 1;
+    T const count = static_cast<T>(n - 2 * f);
+    if (n <= kRankWorkers) {
+        int const lo = static_cast<int>(f), hi = static_cast<int>(n - f);
+        agb::parallel_for(0, (d + kBlock - 1) / kBlock, kGrainCoord / kBlock, [&](size_t b, size_t e) {
+            Block<T> blk;
+            T res[kBlock];
+            for (size_t blk_i = b; blk_i < e; ++blk_i) {
+                size_t const x0 = blk_i * kBlock, len = std::min(kBlock, d - x0);
+                load_block(g, n, d, x0, len, blk);
+                rank_block<T>(n, blk.key, blk.rank);
+                for (size_t c = 0; c < kBlock; ++c)
+                    res[c] = T(0);
+                for (size_t i = 0; i < n; ++i)
+                    for (size_t c = 0; c < kBlock; ++c)
+                        res[c] += (blk.rank[i][c] >= lo && blk.rank[i][c] < hi) ? blk.val[i][c] : T(0);
+                for (size_t c = 0; c < len; ++c)
+                    out[x0 + c] = res[c] / count;
+            }
+        });
+        return 0;
+    }
+    agb::parallel_for(0, d, kGrainCoord, [&](size_t b, size_t e) {
+        std::vector<size_t> idx(n);
+        std::vector<char> keep(n);
+        for (size_t x = b; x < e; ++x) {
+            for (size_t i = 0; i < n; ++i)
+                idx[i] = i;
+            auto cmp = [&](size_t a, size_t c) { return before(g[a * d + x], a, g[c * d + x], c); };
+            std::nth_element(idx.begin(), idx.begin() + f, idx.end(), cmp);                 // ranks [0, f) first
+            std::nth_element(idx.begin() + f, idx.begin() + (n - f), idx.end(), cmp);       // then [f, n - f)
+            std::fill(keep.begin(), keep.end(), 0);
+            for (size_t k = f; k < n - f; ++k)
+                keep[idx[k]] = 1;
+            T sum = 0;
+            for (size_t i = 0; i < n; ++i)
+                if (keep[i])
+                    sum += g[i * d + x];
+            out[x] = sum / count;
+        }
+    });
+    return 0;
+}
+
+// ------------------------------------------------------------------------ //
+// MDA (minimum-diameter averaging): the kept set S, |S| = n - f, whose diameter (largest pairwise distance inside S, non-finite
+// distances = +inf) is smallest; ties -> the lexicographically smallest sorted index list of S. The removal sets R, |R| = f, are
+// enumerated in lexicographic order: a later R is lexicographically larger, so its S is smaller and wins a tie. A set's diameter is
+// the first pair, in descending distance order, with both ends kept.
+constexpr size_t kMdaMaxSets = size_t(1) << 20;
+
+inline bool mda_params_ok(size_t n, size_t f) {
+    if (n == 0 || n > kMaxWorkers || 2 * f >= n)
+        return false;
+    size_t sets = 1;   // C(n, f), exact while it stays below the bound
+    for (size_t t = 0; t < f && sets <= kMdaMaxSets; ++t)
+        sets = sets * (n - t) / (t + 1);
+    return sets <= kMdaMaxSets;
+}
+
+template<class T> int mda_select(T const* dist, size_t n, size_t f, int64_t* selected) {
+    if (!mda_params_ok(n, f))
+        return 1;
+    T const inf = std::numeric_limits<T>::infinity();
+    std::vector<std::pair<size_t, size_t>> pairs;
+    std::vector<T> value;
+    for (size_t i = 0; i + 1 < n; ++i)
+        for (size_t j = i + 1; j < n; ++j) {
+            T const v = dist[i * n + j];
+            pairs.emplace_back(i, j);
+            value.push_back(std::isfinite(v) ? v : inf);
+        }
+    std::vector<size_t> order(pairs.size());
+    for (size_t p = 0; p < order.size(); ++p)
+        order[p] = p;
+    std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return value[a] > value[b]; });
+    std::vector<size_t> removal(f), best_removal(f);
+    for (size_t k = 0; k < f; ++k)
+        removal[k] = k;
+    std::vector<char> removed(n, 0);
+    T best = inf;
+    bool found = false;
+    for (;;) {
+        for (size_t k = 0; k < f; ++k)
+            removed[removal[k]] = 1;
+        T diam = 0;
+        for (size_t p: order)
+            if (!removed[pairs[p].first] && !removed[pairs[p].second]) {
+                diam = value[p];
+                break;
+            }
+        if (!found || diam <= best) {
+            best = diam;
+            best_removal = removal;
+            found = true;
+        }
+        for (size_t k = 0; k < f; ++k)
+            removed[removal[k]] = 0;
+        size_t k = f;   // next removal set in lexicographic order
+        while (k > 0 && removal[k - 1] == n - f + k - 1)
+            --k;
+        if (k == 0)
+            break;
+        ++removal[k - 1];
+        for (size_t t = k; t < f; ++t)
+            removal[t] = removal[t - 1] + 1;
+    }
+    for (size_t k = 0; k < f; ++k)
+        removed[best_removal[k]] = 1;
+    size_t count = 0;
+    for (size_t i = 0; i < n; ++i)
+        if (!removed[i])
+            selected[count++] = static_cast<int64_t>(i);
+    return 0;
+}
+
+// MDA: mean of the selected rows, added in index order, divided once by n - f; `selected` (optional, [n - f]) receives their ids.
+template<class T> int mda(T const* g, size_t n, size_t d, size_t f, T* out, int64_t* selected, T* dist_out) {
+    if (!mda_params_ok(n, f))
+        return 1;
+    std::vector<T> dist(n * n);
+    std::vector<int64_t> ids(n - f);
+    pairwise_distances(g, n, d, dist.data());
+    if (dist_out)
+        std::copy(dist.begin(), dist.end(), dist_out);
+    if (int status = mda_select(dist.data(), n, f, ids.data()))
+        return status;
+    if (selected)
+        std::copy(ids.begin(), ids.end(), selected);
+    selection_mean(g, d, std::vector<size_t>(ids.begin(), ids.end()), out);
+    return 0;
+}
+
 // Multi-Krum: average of the m smallest-scoring gradients; `selected` (optional, [m]) receives their ids.
 template<class T> int krum(T const* g, size_t n, size_t d, size_t f, size_t m, T* out, int64_t* selected, T* dist_out) {
     if (n == 0 || n > kMaxWorkers || n < f + 3 || m < 1 || m > n)
@@ -530,6 +667,9 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_krum_##S(T const* g, size_t n, size_t d, size_t f, size_t m, T* out, int64_t* selected, T* dist) { return krum<T>(g, n, d, f, m, out, selected, dist); } \
     extern "C" int agb_cpu_bulyan_##S(T const* g, size_t n, size_t d, size_t f, size_t m, T* out, T* weights) { return bulyan<T>(g, n, d, f, m, out, weights); } \
     extern "C" int agb_cpu_bulyan_weights_##S(T const* dist, size_t n, size_t f, size_t m, T* weights) { return bulyan_weights<T>(dist, n, f, m, weights); } \
+    extern "C" int agb_cpu_trimmed_mean_##S(T const* g, size_t n, size_t d, size_t f, T* out) { return trimmed_mean<T>(g, n, d, f, out); } \
+    extern "C" int agb_cpu_mda_##S(T const* g, size_t n, size_t d, size_t f, T* out, int64_t* selected, T* dist) { return mda<T>(g, n, d, f, out, selected, dist); } \
+    extern "C" int agb_cpu_mda_select_##S(T const* dist, size_t n, size_t f, int64_t* selected) { return mda_select<T>(dist, n, f, selected); } \
     extern "C" int agb_cpu_pairwise_distances_##S(T const* g, size_t n, size_t d, T* dist) { if (n < 1) return 1; pairwise_distances<T>(g, n, d, dist); return 0; } \
     extern "C" int agb_cpu_weighted_sum_##S(T const* g, size_t n, size_t d, T const* w, T* out) { weighted_sum<T>(g, n, d, w, out); return 0; } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }

@@ -28,7 +28,8 @@ _ERRORS = {
   100: "unsupported number of workers/ranks (n <= 32, R <= 16)", 101: "segment bounds must be multiples of 4 elements (at most 8 segments)",
   102: "unknown rule", 103: "invalid Krum parameters", 104: "invalid Bulyan parameters", 105: "invalid beta",
   106: "optimizer requested without parameter buffers", 107: "optimizer slots missing", 108: "scratch buffers missing",
-  109: "signal pads missing", 110: "more than 8 workers over several ranks need the staging buffer", 111: "invalid phase A launch"}
+  109: "signal pads missing", 110: "more than 8 workers over several ranks need the staging buffer", 111: "invalid phase A launch",
+  112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)"}
 
 
 def _lib():
@@ -135,7 +136,8 @@ def _torch_rules(spec):
   from ..aggregators import _ops
   return {"average": _ops.torch_average, "average-nan": _ops.torch_average_nan, "median": _ops.torch_median,
           "averaged-median": lambda M: _ops.torch_averaged_median(M, spec.beta), "krum": lambda M: _ops.torch_krum(M, spec.f, spec.m),
-          "bulyan": lambda M: _ops.torch_bulyan(M, spec.f, spec.m)}[spec.rule]
+          "bulyan": lambda M: _ops.torch_bulyan(M, spec.f, spec.m), "trimmed-mean": lambda M: _ops.torch_trimmed_mean(M, spec.f),
+          "mda": lambda M: _ops.torch_mda(M, spec.f)}[spec.rule]
 
 
 def aggregate(spec, G, return_details=False):

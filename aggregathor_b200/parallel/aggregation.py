@@ -164,7 +164,7 @@ class FusedAggregation(_AggregationBase):
     if self.spec.n != nbworkers:
       raise tools.UserException("GAR built for %d workers used with %d" % (self.spec.n, nbworkers))
     d, w, R = self.d, self.w, self.world
-    self.distance_rule = self.spec.rule in ("krum", "bulyan")
+    self.distance_rule = self.spec.rule in ("krum", "bulyan", "mda")
     self.buckets = self._check_buckets(buckets, d)
     self.segments_of = [[self._share(lo, hi, q, R) for lo, hi in self.buckets] for q in range(R)]
     self.segments = self.segments_of[self.rank]
@@ -230,7 +230,7 @@ class FusedAggregation(_AggregationBase):
 
   @property
   def overlappable(self):
-    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan is additive over coordinates)."""
+    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates)."""
     return self.distance_rule and len(self.buckets) > 1
 
   def visible_rows(self):

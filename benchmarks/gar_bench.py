@@ -33,6 +33,7 @@ def main():
   parser.add_argument("--gar-iters", dest="iters", type=int, default=10)
   parser.add_argument("--gar-rules", dest="rules", type=str, default="average,average-nan,median,averaged-median,krum,bulyan")
   parser.add_argument("--gar-out", dest="out", type=str, default=".")
+  parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -83,7 +84,7 @@ def main():
   w = n // world
   results = {}
   for rule in args.rules.split(","):
-    f = 1 if rule == "bulyan" and n < 11 else 2
+    f = args.byz if args.byz is not None else 1 if rule == "bulyan" and n < 11 else 2
     name = {"krum": "krum", "bulyan": "bulyan"}.get(rule, rule)
     gar = aggregators.instantiate(name, n, f, [])
     sgd = build(optimizers, "optimizer", "sgd", [])
@@ -140,7 +141,7 @@ def main():
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
-    if rule in ("krum", "bulyan"):
+    if rule in ("krum", "bulyan", "mda"):
       c1, c2, c3 = (d // 2) // 8 * 8, (d // 5) // 8 * 8, (d // 16) // 8 * 8
       over = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True,
                               buckets=[(c1, d), (c2, c1), (c3, c2), (0, c3)], device_state=True)
