@@ -315,6 +315,58 @@ def torch_bulyan(G, f, m, return_weights=False):
 
 
 # ---------------------------------------------------------------------------- #
+# Omniscient Byzantine rows (`attacks/omniscient.py`): the literal definition, the CPU back-end and the oracle of the sm_90a kernel
+
+def check_byzantine_slots(n, byz_slots, mode):
+  """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("alie" needs 2 honest rows, "ipm" one)."""
+  if mode not in ("alie", "ipm"):
+    raise tools.UserException("Unknown omniscient attack mode " + repr(mode))
+  slots = sorted({int(i) for i in byz_slots})
+  if not slots or slots[0] < 0 or slots[-1] >= n:
+    raise tools.UserException("Byzantine slots must be a non-empty subset of [0, %d) (got %r)" % (n, list(byz_slots)))
+  need = 2 if mode == "alie" else 1
+  if n - len(slots) < need:
+    raise tools.UserException("%s needs at least %d honest row(s) (n = %d, %d Byzantine)" % (mode.upper(), need, n, len(slots)))
+  return slots
+
+
+def torch_byzantine_row(G, byz_slots, mode, coef):
+  """The row every Byzantine slot receives: per coordinate, from the honest rows h (ascending slots, H of them),
+  mu = ((h0 + h1) + ...) / H; ALIE: mu + z * sqrt(sum_i (h_i - mu)^2 / (H - 1)); IPM: (-epsilon) * mu. fp32, one rounded operation at a
+  time (separate torch calls, nothing that may fuse into an FMA)."""
+  byz = set(check_byzantine_slots(G.shape[0], byz_slots, mode))
+  honest = [G[i] for i in range(G.shape[0]) if i not in byz]
+  # divisors are device tensors: a Python-number divisor may be turned into a multiplication by its reciprocal on the GPU
+  scalar = lambda value: torch.tensor(value, dtype=torch.float32, device=G.device)
+  coef = scalar(coef)
+  mu = honest[0]
+  for h in honest[1:]:
+    mu = mu + h
+  mu = mu / scalar(len(honest))
+  if mode == "ipm":
+    return torch.neg(coef) * mu
+  var = None
+  for h in honest:
+    dev = h - mu
+    square = dev * dev
+    var = square if var is None else var + square
+  # torch's vectorised fp32 sqrt on the CPU is not always correctly rounded: the square root of an fp32 value taken in fp64 and
+  # rounded once to fp32 is (fp64 carries more than 2 * 24 + 2 bits)
+  sigma = torch.sqrt((var / scalar(len(honest) - 1)).double()).float()
+  return mu + coef * sigma
+
+
+def torch_craft_byzantine_(G, byz_slots, mode, coef):
+  """In place on the [n, d] fp32 matrix G: every Byzantine row <- `torch_byzantine_row`; honest rows are not written."""
+  if G.dtype != torch.float32:
+    raise tools.UserException("Omniscient attacks craft fp32 rows (got %s)" % G.dtype)
+  row = torch_byzantine_row(G, byz_slots, mode, coef)
+  for i in check_byzantine_slots(G.shape[0], byz_slots, mode):
+    G[i].copy_(row)
+  return G
+
+
+# ---------------------------------------------------------------------------- #
 # Stand-alone CUDA back-end (native/op_gar)
 
 def cuda_aggregate(spec, G):

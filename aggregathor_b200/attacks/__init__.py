@@ -7,6 +7,9 @@ overwrites their row of the gradient matrix, on the device, before the aggregati
 
 Contract: `cls(nbworkers, nbbyzwrks, args)`; `apply(row, worker, step, state)` mutates the flat fp32 gradient `row`
 in place (`state` is a per-worker dict that persists across steps). Dropping a `.py` file here auto-registers it.
+Omniscient attacks (`omniscient = True`, `omniscient.py`) see every honest row instead: they implement no `apply`, and expose `mode`
+("alie" or "ipm") and the fp32 coefficient `coef`; the aggregation engine crafts the Byzantine rows (`craft_byzantine`) on every rank.
+Construction raises `UserException` for arguments outside an attack's bounds.
 """
 
 import pathlib
@@ -18,6 +21,7 @@ __all__ = ["_Attack", "register", "instantiate", "itemize"]
 
 class _Attack:
   forges = False  # True: the attack tampers with the row *after* it was signed (only meaningful with `--authenticate`)
+  omniscient = False  # True: the rows are crafted from the honest rows by the aggregation engine (no `apply`)
 
   def __init__(self, nbworkers, nbbyzwrks, args):
     raise NotImplementedError

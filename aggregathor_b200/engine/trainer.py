@@ -10,7 +10,8 @@ One synchronous step on a rank:
   1. for each local worker: next batch (already prefetched to the device), forward, loss, backward — gradients are
      written by the layer kernels directly into that worker's row of the peer-mapped `[w, d]` gradient matrix;
   2. optional l1 / l2 regularisation gradient (same formulas as `graph.py:125-139`);
-  3. real Byzantine workers overwrite their row with the selected attack;
+  3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
+     Byzantine rows from the honest ones, a collective call on every rank);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast);
   5. the bf16 compute copy of the parameters is refreshed (unless the fused kernel already wrote it).
 """
@@ -42,6 +43,8 @@ class Manager:
   def __init__(self, experiment, aggregator, nbworkers, optimizer="sgd", optimizer_args=None, learning_rate="fixed", learning_rate_args=None,
                regularizations=(-1., -1.), trace=False, *, attack=None, nb_real_byz=0, device=None, group=None, engine="auto", backend="auto",
                dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False):
+    if authenticate and getattr(attack, "omniscient", False):
+      raise tools.UserException("Omniscient attacks craft the Byzantine rows on every rank: they cannot be combined with '--authenticate'")
     self.device = torch.device(device) if device is not None else _default_device()
     if self.device.type == "cuda" and self.device.index is None:
       self.device = torch.device("cuda", torch.cuda.current_device())
@@ -157,6 +160,8 @@ class Manager:
     self.attack = attack
     self.byzantine = set(range(nbworkers - nb_real_byz, nbworkers)) if (attack is not None and nb_real_byz > 0) else set()
     self._attack_state = {i: {} for i in self.byzantine}
+    # rows in the gathered matrix (slots) of the Byzantine workers, as the aggregation engines address them
+    self.byzantine_slots = sorted(placement[i][0] * self.w + placement[i][1] for i in self.byzantine)
     # -- gradient authentication (opt-in; reference: signed worker -> PS messages of the hardened transport) -- #
     self.authenticator = None
     if authenticate:
@@ -348,6 +353,10 @@ class Manager:
       for j in range(len(self.local_workers)):
         self.grads[self.placement[self.local_workers[j]][1]].add_(reg_grad)
         losses[j] = losses[j] + reg_loss
+    if getattr(self.attack, "omniscient", False):
+      if self.byzantine_slots:   # collective: every rank crafts its share, whether or not it hosts a Byzantine worker
+        self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef)
+      return losses
     forging = self.authenticator is not None and getattr(self.attack, "forges", False)
     for j, i in enumerate(self.local_workers):
       if i in self.byzantine and not forging:

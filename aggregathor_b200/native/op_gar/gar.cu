@@ -16,6 +16,8 @@
 //                    trimmed mean / median / NaN-aware mean), apply the optimizer,
 //                    store the new parameters into every rank's buffer (P2P stores or one NVLS multimem.st); exit barrier
 //
+// Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
+// every Byzantine row from the honest values.
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
 // registers at a time; more rows are processed in 8-row blocks (diagonal + cross passes over the staged copy).
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
@@ -38,7 +40,8 @@ constexpr int kMaxPairs = kMaxWorkers * (kMaxWorkers - 1) / 2;   // 496
 constexpr int kMaxSeg = 8;                // owned coordinate segments (one per gradient bucket)
 constexpr int kSlotExchange = kMaxSeg;    // flag slots: [0, kMaxSeg) bucket entry, then exchange, then exit
 constexpr int kSlotExit = kMaxSeg + 1;
-constexpr int kFlagSlots = kMaxSeg + 2;
+constexpr int kSlotCraft = kMaxSeg + 2;   // entry barrier of the Byzantine crafting kernel
+constexpr int kFlagSlots = kMaxSeg + 3;
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
@@ -275,15 +278,16 @@ template<int N> __device__ __forceinline__ float coord_average_nan(float const (
 }
 
 // ---- cross-rank flag barrier ---------------------------------------------------- //
-__device__ __forceinline__ void signal_all(GarArgs const& a, int slot, uint32_t epoch) {
+// `Args`: any kernel argument block with R, rank, signal[], epoch and epoch_ptr (GarArgs, ByzArgs)
+template<class Args> __device__ __forceinline__ void signal_all(Args const& a, int slot, uint32_t epoch) {
     if (threadIdx.x < a.R)
         st_release_sys(a.signal[threadIdx.x] + slot * a.R + a.rank, epoch);
 }
-__device__ __forceinline__ void wait_all(GarArgs const& a, int slot, uint32_t epoch) {
+template<class Args> __device__ __forceinline__ void wait_all(Args const& a, int slot, uint32_t epoch) {
     if (threadIdx.x < a.R)
         wait_flag_sys(a.signal[a.rank] + slot * a.R + threadIdx.x, epoch);
 }
-__device__ __forceinline__ uint32_t current_epoch(GarArgs const& a) {
+template<class Args> __device__ __forceinline__ uint32_t current_epoch(Args const& a) {
     return a.epoch_ptr ? ld_acquire_sys(a.epoch_ptr) + 1u : a.epoch;
 }
 
@@ -953,6 +957,123 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
         *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
 }
 
+// ---- omniscient Byzantine rows (ALIE / IPM) ------------------------------------------ //
+// Every Byzantine row receives, at each owned coordinate, a value computed from the honest values of that coordinate only:
+//   mu = ((h[Hs0] + h[Hs1]) + ...) / H           honest slots ascending, one division
+//   v  = (sum_i (h_i - mu) * (h_i - mu)) / (H - 1)  ALIE only, same order
+//   ALIE: b = mu + z * sqrt(v)          IPM: b = (-eps) * mu
+// one IEEE-rounded operation at a time (explicit _rn intrinsics: no FMA contraction), so that every back-end gets the same bits.
+//
+// With R > 1 each rank crafts its owned segments of every Byzantine row, wherever that row lives (P2P stores into peers' gradient
+// buffers). Entry barrier (slot kSlotCraft, the step's epoch): every rank's backward has written its rows before any honest value is
+// read or any Byzantine row is overwritten. The kernel is not cooperative, so every CTA signals (idempotent) before it waits: no CTA
+// waits on a CTA that may never be scheduled. No exit barrier: rank q writes only its own segments of each Byzantine row, and only
+// rank q's finish kernel (next in the same stream) reads them; the closing system-scope fence orders these stores before that
+// kernel's loads, including its NVLS multimem.ld_reduce of `average`. The rows are overwritten again only by the next step's
+// backward, which every rank starts after the finish kernels' exit barrier.
+//
+// Up to N = 8 honest values are held in registers across both passes; with more, the variance pass re-reads them from memory.
+struct ByzArgs {
+    float* rows[kMaxWorkers];          // row base pointers (local or peer-mapped)
+    int honest[kMaxWorkers];           // honest slots, ascending
+    int byz[kMaxWorkers];              // Byzantine slots
+    int H, K;
+    int mode;                          // 0: ALIE, 1: IPM
+    float coef;                        // ALIE: z; IPM: epsilon
+    int nseg;
+    long long seg_lo[kMaxSeg], seg_hi[kMaxSeg];
+    int R, rank;
+    uint32_t* signal[kMaxRanks];
+    uint32_t epoch;
+    uint32_t* epoch_ptr;
+};
+enum ByzMode { kAlie = 0, kIpm = 1 };
+
+template<int N>
+__global__ void __launch_bounds__(256) gar_byzantine_kernel(ByzArgs const a) {
+    if (a.R > 1) {
+        uint32_t const epoch = current_epoch(a);
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const H = a.H;
+    float const count = static_cast<float>(H);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            float mu[4], out[4];
+            if constexpr (N > 0) {   // registers: the H honest values are loaded once
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    mu[c] = g[0][c];
+#pragma unroll
+                for (int i = 1; i < N; ++i)
+                    if (i < H) {
+#pragma unroll
+                        for (int c = 0; c < 4; ++c)
+                            mu[c] = __fadd_rn(mu[c], g[i][c]);
+                    }
+            } else {
+                V<4>::load(a.rows[a.honest[0]] + x, mu);
+                for (int i = 1; i < H; ++i) {
+                    float h[4];
+                    V<4>::load(a.rows[a.honest[i]] + x, h);
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        mu[c] = __fadd_rn(mu[c], h[c]);
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                mu[c] = __fdiv_rn(mu[c], count);
+            if (a.mode == kIpm) {
+                float const neg = -a.coef;
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    out[c] = __fmul_rn(neg, mu[c]);
+            } else {
+                float var[4];
+                auto add_square = [&](int i, float const (&h)[4]) {
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        float const dev = __fsub_rn(h[c], mu[c]);
+                        float const sq = __fmul_rn(dev, dev);
+                        var[c] = i == 0 ? sq : __fadd_rn(var[c], sq);
+                    }
+                };
+                if constexpr (N > 0) {
+#pragma unroll
+                    for (int i = 0; i < N; ++i)
+                        if (i < H)
+                            add_square(i, g[i]);
+                } else {
+                    for (int i = 0; i < H; ++i) {
+                        float h[4];
+                        V<4>::load(a.rows[a.honest[i]] + x, h);
+                        add_square(i, h);
+                    }
+                }
+                float const dof = static_cast<float>(H - 1);
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    out[c] = __fadd_rn(mu[c], __fmul_rn(a.coef, __fsqrt_rn(__fdiv_rn(var[c], dof))));
+            }
+            for (int k = 0; k < a.K; ++k)
+                V<4>::store_stream(a.rows[a.byz[k]] + x, out);
+        }
+    }
+    fence_sys();
+}
+
 // ---- small stand-alone kernels (baseline path, attacks, diagnostics) ------------- //
 __global__ void sgd_kernel(float* __restrict__ p, float const* __restrict__ g, float lr, long long d) {
     long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
@@ -1113,7 +1234,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
 extern "C" {
 
 char const* agb_op_list() {
-    return "gar_fused,gar_phase_a,gar_max_ctas,sgd,drop_chunks,checksum,cast_bf16";
+    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,sgd,drop_chunks,checksum,cast_bf16";
 }
 
 // Wall-clock bound (seconds, 0 = none) of the cross-GPU flag waits of this library's kernels.
@@ -1174,6 +1295,65 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
         gar_phase_a_kernel<false><<<ctas, threads, 0, s>>>(a, seg);
     else
         gar_phase_a_kernel<true><<<ctas, threads < 64 ? 64 : threads, 0, s>>>(a, seg);
+    AGB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// Omniscient Byzantine rows (ALIE: mode 0, coef = z; IPM: mode 1, coef = epsilon) over this rank's owned segments; see
+// `gar_byzantine_kernel`. `rows`: n row addresses; `honest` / `byzantine`: disjoint slot masks; `signals`: R signal pads (R > 1);
+// flags use *epoch_ptr + 1 when `epoch_ptr` is set, `epoch` otherwise. Collective when R > 1: every rank calls it.
+int agb_gar_byzantine(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                      unsigned byzantine, int mode, float coef, int R, int rank, unsigned long long const* signals, unsigned epoch,
+                      unsigned long long epoch_ptr, void* stream) {
+    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
+        return 100;
+    if (nseg < 1 || nseg > kMaxSeg)
+        return 101;
+    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
+    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < (mode == kAlie ? 2 : 1) || (mode != kAlie && mode != kIpm))
+        return 114;
+    ByzArgs a{};
+    a.H = H;
+    a.K = K;
+    for (int i = 0, h = 0, b = 0; i < n; ++i) {
+        a.rows[i] = reinterpret_cast<float*>(rows[i]);
+        if ((honest >> i) & 1u)
+            a.honest[h++] = i;
+        if ((byzantine >> i) & 1u)
+            a.byz[b++] = i;
+    }
+    a.mode = mode;
+    a.coef = coef;
+    a.nseg = nseg;
+    long long work = 0;
+    for (int s = 0; s < nseg; ++s) {
+        a.seg_lo[s] = seg_lo[s];
+        a.seg_hi[s] = seg_hi[s];
+        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
+            return 101;
+        work += (seg_hi[s] - seg_lo[s]) / 4;
+    }
+    a.R = R;
+    a.rank = rank;
+    for (int q = 0; q < R; ++q) {
+        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
+        if (R > 1 && !a.signal[q])
+            return 109;
+    }
+    a.epoch = epoch;
+    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
+    if (work == 0 && R == 1)
+        return 0;
+    int const threads = 256;
+    long long grid = (work + threads - 1) / threads;
+    long long const cap = static_cast<long long>(agb::sm_count()) * 8;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (H <= kBlockRows)
+        gar_byzantine_kernel<kBlockRows><<<static_cast<int>(grid), threads, 0, s>>>(a);
+    else
+        gar_byzantine_kernel<0><<<static_cast<int>(grid), threads, 0, s>>>(a);
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }

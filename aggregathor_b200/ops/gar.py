@@ -19,7 +19,7 @@ MAX_WORKERS = 32
 MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
-FLAG_SLOTS = MAX_SEGMENTS + 2
+FLAG_SLOTS = MAX_SEGMENTS + 3   # per segment: bucket entry; then exchange, exit, Byzantine crafting entry
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 MAILBOX_BYTES = MAX_RANKS * (MAX_PAIRS + 1) * 4
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
@@ -29,7 +29,9 @@ _ERRORS = {
   102: "unknown rule", 103: "invalid Krum parameters", 104: "invalid Bulyan parameters", 105: "invalid beta",
   106: "optimizer requested without parameter buffers", 107: "optimizer slots missing", 108: "scratch buffers missing",
   109: "signal pads missing", 110: "more than 8 workers over several ranks need the staging buffer", 111: "invalid phase A launch",
-  112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)"}
+  112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)",
+  114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)"}
+BYZANTINE_MODES = {"alie": 0, "ipm": 1}
 
 
 def _lib():
@@ -174,6 +176,53 @@ def aggregate(spec, G, return_details=False):
   if return_details:
     return out, launcher.dist_out.view(n, n).clone(), launcher.info.clone()
   return out
+
+
+def craft(rows, segments, honest, byzantine, mode, coef, *, R=1, rank=0, signals=None, epoch=1, epoch_ptr=None, stream=None):
+  """Craft the omniscient Byzantine rows (`attacks/omniscient.py`) over the owned `segments` of the n rows at device addresses `rows`
+  (raw ints, local or peer-mapped): every slot of `byzantine` receives the ALIE / IPM value of the `honest` slots. Collective when R > 1
+  (entry barrier through the signal pads, at flag value `epoch`, or `*epoch_ptr + 1` when given)."""
+  n = len(rows)
+  if n > MAX_WORKERS:
+    raise tools.UserException("The sm_90a crafting kernel supports n <= %d workers (got %d)" % (MAX_WORKERS, n))
+  if not 1 <= len(segments) <= MAX_SEGMENTS:
+    raise tools.UserException("Between 1 and %d coordinate segments per rank (got %d)" % (MAX_SEGMENTS, len(segments)))
+  mask = lambda slots: sum(1 << int(i) for i in set(slots))
+  addr = lambda t: 0 if t is None else (t if isinstance(t, int) else t.data_ptr())
+  c_rows = (ctypes.c_ulonglong * n)(*[int(r) for r in rows])
+  lo = (ctypes.c_longlong * len(segments))(*[int(a) for a, _ in segments])
+  hi = (ctypes.c_longlong * len(segments))(*[int(b) for _, b in segments])
+  c_signals = (ctypes.c_ulonglong * R)(*[addr(signals[q]) for q in range(R)]) if signals is not None else None
+  func = _lib().agb_gar_byzantine
+  func.restype = ctypes.c_int
+  _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
+              ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_float(coef), ctypes.c_int(R), ctypes.c_int(rank), c_signals,
+              ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine")
+
+
+def craft_byzantine_(G, byz_slots, mode, coef):
+  """Stand-alone omniscient attack on the [n, d] fp32 matrix `G`, in place: rows `byz_slots` <- the ALIE (`coef` = z) or IPM
+  (`coef` = epsilon) row of the other rows. CUDA tensors with n <= 32 run the sm_90a kernel; others the torch reference."""
+  from ..aggregators import _ops
+  n, d = G.shape
+  byz_slots = _ops.check_byzantine_slots(n, byz_slots, mode)
+  if not G.is_cuda or n > MAX_WORKERS:
+    return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef)
+  if G.dtype != torch.float32:
+    raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
+  pad = (-d) % 4
+  work = G
+  if pad or not G.is_contiguous() or G.data_ptr() % 16:
+    work = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
+    work[:, :d] = G
+  dp = d + pad
+  rows = [work.data_ptr() + i * dp * 4 for i in range(n)]
+  with torch.cuda.device(G.device):
+    craft(rows, [(0, dp)], [i for i in range(n) if i not in byz_slots], byz_slots, mode, coef)
+  if work is not G:
+    index = torch.tensor(byz_slots, dtype=torch.int64, device=G.device)
+    G[index] = work[index, :d]
+  return G
 
 
 def sgd_(param, grad, lr):

@@ -14,6 +14,8 @@ Three interchangeable engines share one interface (`params`, `grads`, `step()`):
   (`mnist` + `average`, 2 workers) and the fallback for user plug-in GARs without a fused spec.
 
 Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always sees n rows.
+Every engine also has `craft_byzantine(byz_slots, mode, coef)`, the omniscient attacks (`attacks/omniscient.py`): the rows at the
+given slots of the gathered matrix are overwritten with the ALIE / IPM row of the others, on every rank (a collective call).
 """
 
 import os
@@ -99,6 +101,12 @@ class HostAggregation(_AggregationBase):
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
+  def craft_byzantine(self, byz_slots, mode, coef):
+    """Gather, then the torch reference on the gathered matrix (every rank computes the same bits)."""
+    from ..aggregators import _ops
+    self.visible_rows()
+    _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef)
+
   def step(self, rate):
     self._gather()
     aggregated = self.gar.aggregate(self._gathered)
@@ -127,6 +135,11 @@ class BaselineAggregation(_AggregationBase):
     self._gather()
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
+
+  def craft_byzantine(self, byz_slots, mode, coef):
+    """Gather, then the stand-alone crafting kernel on the gathered matrix (every rank computes the same bits)."""
+    self.visible_rows()
+    gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef)
 
   def step(self, rate):
     self._gather()
@@ -194,6 +207,7 @@ class FusedAggregation(_AggregationBase):
     self._hyper_host = torch.zeros(4, dtype=torch.float32).pin_memory() if device_state else None
     self.loss_out = torch.zeros(1, dtype=torch.float32, device=self.device)
     self._pre_accumulated = 0
+    self._prepared = False   # `prepare` ran for the step that has not been aggregated yet
     self._row_views = None
     heap = self.heap
     self._rows = [heap.peer(i // w, "grads") + (i % w) * d * 4 for i in range(self.n)]
@@ -260,11 +274,21 @@ class FusedAggregation(_AggregationBase):
     Stream-ordered before the kernels of the step; never part of a captured graph."""
     self.updates += 1
     self.epoch += 1
+    self._prepared = True
     self._rate_args = self.optimizer.kernel_args(rate, self.updates)
     if self.device_state:
       lr, hyper = self._rate_args
       self._hyper_host[0], self._hyper_host[1], self._hyper_host[2], self._hyper_host[3] = lr, hyper[0], hyper[1], hyper[2]
       self.hyper_dev.copy_(self._hyper_host, non_blocking=True)
+
+  def craft_byzantine(self, byz_slots, mode, coef, stream=None):
+    """Collective: this rank crafts its owned segments of every Byzantine row, local or on a peer (`ops.gar.craft`), behind an entry
+    barrier at the epoch of the step about to be aggregated. Every rank calls it, including ranks that host no Byzantine worker."""
+    from ..aggregators import _ops
+    byz_slots = _ops.check_byzantine_slots(self.n, byz_slots, mode)
+    epoch = self.epoch if self._prepared else self.epoch + 1
+    gar_ops.craft(self._rows, self.segments, [i for i in range(self.n) if i not in byz_slots], byz_slots, mode, coef, R=self.world, rank=self.rank,
+                  signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream)
 
   def phase_a(self, seg, stream=None):
     """Distance pass + staging of bucket `seg` (buckets must be pre-accumulated in order 0, 1, ...). Call between `prepare` and `step`."""
@@ -277,6 +301,7 @@ class FusedAggregation(_AggregationBase):
     """The finish kernel. `rate` is ignored when `prepare(rate)` was already called for this step (`prepared=True`)."""
     if not prepared:
       self.prepare(rate)
+    self._prepared = False
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
                          loss_in=loss_in, loss_out=self.loss_out, **self._common(self._rate_args))

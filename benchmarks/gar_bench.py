@@ -6,6 +6,11 @@ identical parameters/gradients, check that (a) both produce the same parameters 
 with bit-identical parameters (checksum), then time each engine's step with CUDA events (max over ranks).
 Reports, per rule: ms per step for both engines, the bytes that must cross NVLink into each GPU, GB/s and the
 fraction of the peer-copy rate measured at start-up; writes JSON to <--gar-out>/gar_bench_<N>.json.
+
+`--gar-attack alie|ipm`: the last f workers are omniscient Byzantine workers. Every step of both engines first crafts their rows
+(`craft_byzantine`: the sm_90a kernel, sharded over the ranks on the fused engine, after the NCCL all-gather on the baseline one);
+the crafting kernel is also timed alone, next to the torch reference on the same device, with the (H + k) * d * 4 bytes it must move.
+`--gar-dump-rows` then saves, from the last rank, every row the fused engine aggregated (honest and crafted, all d coordinates).
 """
 
 import argparse
@@ -18,7 +23,8 @@ import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from aggregathor_b200 import aggregators, tools  # noqa: E402
+from aggregathor_b200 import aggregators, attacks, tools  # noqa: E402
+from aggregathor_b200.aggregators import _ops  # noqa: E402
 from aggregathor_b200.engine.flat import FlatLayout  # noqa: E402
 from aggregathor_b200.engine.optimizers import optimizers  # noqa: E402
 from aggregathor_b200.engine.schedules import build  # noqa: E402
@@ -34,6 +40,8 @@ def main():
   parser.add_argument("--gar-rules", dest="rules", type=str, default="average,average-nan,median,averaged-median,krum,bulyan")
   parser.add_argument("--gar-out", dest="out", type=str, default=".")
   parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
+  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm"), default=None, help="omniscient attack by the last f workers, crafted every step")
+  parser.add_argument("--gar-dump-rows", dest="dump_rows", action="store_true", help="with --gar-attack: save the last rank's view of every row to <--gar-out>")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -102,12 +110,26 @@ def main():
         grads[j].mul_(20.0).add_(3.0)  # the last f workers are outliers
     fused.grads.copy_(grads)
     base.grads.copy_(grads)
+    attack = attacks.instantiate(args.attack, n, f, []) if args.attack else None
+    byz_slots = list(range(n - f, n))
+
+    def craft(engine):
+      if attack is not None:
+        engine.craft_byzantine(byz_slots, attack.mode, attack.coef)
+
     torch.cuda.synchronize()
     if world > 1:
       dist.barrier()
+    craft(fused)
     fused.step(0.1)
+    craft(base)
     base.step(0.1)
     torch.cuda.synchronize()
+    if attack is not None and args.dump_rows and rank == world - 1:
+      rows = fused.visible_rows()
+      os.makedirs(args.out, exist_ok=True)
+      torch.save({"rows": torch.stack([rows[i].cpu() for i in range(n)]), "byzantine": byz_slots, "mode": attack.mode, "coef": attack.coef},
+                 os.path.join(args.out, "gar_rows_%s_%d.pt" % (rule, world)))
     diff = float((fused.params - base.params).abs().max())
     digest = gar_ops.checksum(fused.params)
     digests = [torch.zeros_like(digest) for _ in range(world)]
@@ -125,6 +147,7 @@ def main():
       begin, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
       begin.record()
       for _ in range(args.iters):
+        craft(engine)
         engine.step(0.1)
       end.record()
       torch.cuda.synchronize()
@@ -135,9 +158,36 @@ def main():
 
     for engine in (fused, base):
       for _ in range(3):
+        craft(engine)
         engine.step(0.1)
     fused_ms = time_engine(fused)
     base_ms = time_engine(base)
+    attack_entry = {}
+    if attack is not None:
+      def time_craft(fn):
+        for _ in range(3):
+          fn()
+        torch.cuda.synchronize()
+        if world > 1:
+          dist.barrier()
+        torch.cuda.synchronize()
+        begin, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        begin.record()
+        for _ in range(args.iters):
+          fn()
+        end.record()
+        torch.cuda.synchronize()
+        ms = torch.tensor([begin.elapsed_time(end) / args.iters], device=device, dtype=torch.float64)
+        if world > 1:
+          dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+        return float(ms.item())
+      craft_ms = time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef))
+      # the torch reference on this device, over the full [n, d] matrix (what a torch attack would run after an all-gather)
+      reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef))
+      craft_bytes = n * d * 4   # (H + k) * d * 4: every honest value read once, every Byzantine value written once (over all ranks)
+      attack_entry = {"attack": attack.mode, "coef": attack.coef, "k": f, "craft_ms": craft_ms, "torch_reference_ms": reference_ms,
+                      "craft_bytes": craft_bytes, "craft_gbs": craft_bytes / craft_ms / 1e6,
+                      "torch_reference_gbs": craft_bytes / reference_ms / 1e6}
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
@@ -191,6 +241,7 @@ def main():
                      "measured_peer_gbs": peer_gbs, "frac_of_measured_peer": (nvlink_in / fused_ms / 1e6) / peer_gbs if peer_gbs else None,
                      "bucketed_total_ms": bucketed_ms, "finish_kernel_exposed_ms": exposed_ms,
                      "local_hbm_bytes": hbm, "hbm_gbs": hbm / fused_ms / 1e6 if world == 1 else None}
+    results[rule].update(attack_entry)
     if rank == 0:
       print(rule, json.dumps(results[rule]))
     del fused, base
