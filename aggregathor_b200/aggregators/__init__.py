@@ -24,19 +24,22 @@ __all__ = ["_GAR", "FusedSpec", "register", "instantiate", "itemize", "get"]
 class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
-  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda")
+  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median")
 
-  def __init__(self, rule, n, f=0, m=0, beta=0):
+  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6):
+    """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing; the other rules ignore them."""
     if rule not in self.RULES:
       raise tools.UserException("Unknown fused rule " + repr(rule))
     self.rule, self.n, self.f, self.m, self.beta = rule, int(n), int(f), int(m), int(beta)
+    self.iterations, self.nu = int(iterations), float(nu)
 
   @property
   def rule_id(self):
     return self.RULES.index(self.rule)
 
   def __repr__(self):
-    return "FusedSpec(rule=%r, n=%d, f=%d, m=%d, beta=%d)" % (self.rule, self.n, self.f, self.m, self.beta)
+    extra = ", iterations=%d, nu=%r" % (self.iterations, self.nu) if self.rule == "geometric-median" else ""
+    return "FusedSpec(rule=%r, n=%d, f=%d, m=%d, beta=%d%s)" % (self.rule, self.n, self.f, self.m, self.beta, extra)
 
 
 class _GAR:

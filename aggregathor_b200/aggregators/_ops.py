@@ -63,6 +63,22 @@ def check_mda(n, f):
     raise tools.UserException("MDA enumerates the C(n, f) subsets of removed workers: C(%d, %d) = %d is above the bound 2^20" % (n, f, math.comb(n, f)))
 
 
+GEOMETRIC_MEDIAN_MAX_ITERATIONS = 16
+
+
+def check_geometric_median(n, f, iterations, nu):
+  """Validate the geometric median's parameters -> (iterations, nu rounded once to fp32). `f` is not used by the algorithm; its
+  breakdown point 1/2 still requires 0 <= 2 f < n."""
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("The geometric median needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+  if isinstance(iterations, bool) or int(iterations) != iterations or not 1 <= iterations <= GEOMETRIC_MEDIAN_MAX_ITERATIONS:
+    raise tools.UserException("The geometric median needs 1 <= iterations <= %d (got %r)" % (GEOMETRIC_MEDIAN_MAX_ITERATIONS, iterations))
+  nu32 = float(torch.tensor(float(nu), dtype=torch.float32)) if math.isfinite(float(nu)) else float(nu)
+  if not (math.isfinite(nu32) and nu32 > 0):
+    raise tools.UserException("The geometric median needs a finite smoothing nu > 0 in fp32 (got %r)" % (nu,))
+  return int(iterations), nu32
+
+
 def _rank_key(values):
   """Sort key implementing (finite ascending, non-finite last); argsort(stable) then breaks ties by index."""
   return torch.where(torch.isfinite(values), values, torch.full_like(values, float("inf")))
@@ -155,6 +171,21 @@ def host_mda_select(dist, f):
   return selected
 
 
+def host_geometric_median(G, iterations, nu, return_distances=False):
+  """Host library's geometric median; `return_distances` also gives the [iterations, n] squared distances D of every iteration."""
+  iterations, nu = check_geometric_median(G.shape[0], 0, iterations, nu)
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  out = torch.empty(d, dtype=Gc.dtype)
+  dist = torch.empty((iterations, n), dtype=Gc.dtype)
+  status = _host("geometric_median", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), ctypes.c_size_t(iterations), ctypes.c_double(nu),
+                                               _ptr(out), _ptr(dist))
+  if status != 0:
+    raise tools.UserException("Host geometric median rejected its arguments (n = %d, d = %d, iterations = %d, nu = %r)" % (n, d, iterations, nu))
+  out = out.to(G.device)
+  return (out, dist) if return_distances else out
+
+
 def host_pairwise_distances(G):
   Gc = G.detach().to("cpu").contiguous()
   n, d = Gc.shape
@@ -240,6 +271,35 @@ def torch_mda(G, f, return_selected=False):
   selected = mda_select(torch_pairwise_distances(G), f)
   out = G[selected.to(G.device)].sum(dim=0) / (n - f)
   return (out, selected) if return_selected else out
+
+
+def torch_geometric_median(G, iterations, nu, return_distances=False):
+  """Smoothed Weiszfeld iterations from the coordinate-wise median, in G's dtype (double inputs, more than 32 workers on a device):
+  rows with a non-finite squared distance are skipped, beta_i = 1 / max(nu, sqrt(D_i)), z = (sum beta_i x_i) / (sum beta_i) with
+  both sums over the kept rows in ascending order; no kept row keeps z."""
+  iterations, nu = check_geometric_median(G.shape[0], 0, iterations, nu)
+  n = G.shape[0]
+  scalar = lambda value: torch.tensor(value, dtype=G.dtype, device=G.device)
+  one, smooth = scalar(1.0), scalar(nu)
+  z = torch_median(G)
+  dists = []
+  for _ in range(iterations):
+    delta = G - z.unsqueeze(0)
+    D = (delta * delta).sum(dim=1)
+    dists.append(D)
+    kept = [i for i in range(n) if math.isfinite(float(D[i]))]
+    if not kept:
+      continue
+    # the square root of an fp32 value taken in fp64 and rounded once is correctly rounded (torch's CPU fp32 sqrt is not always)
+    root = torch.sqrt(D.double()).to(G.dtype)
+    beta = one / torch.maximum(root, smooth)
+    total = torch.zeros((), dtype=G.dtype, device=G.device)
+    num = torch.zeros_like(z)
+    for i in kept:
+      total = total + beta[i]
+      num = num + beta[i] * G[i]
+    z = num / total
+  return (z, torch.stack(dists)) if return_distances else z
 
 
 def torch_pairwise_distances(G):

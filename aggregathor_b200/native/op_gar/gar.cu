@@ -15,6 +15,8 @@
 //                    (replicated on all ranks); phase D: aggregate the owned coordinates (mean of selected / coordinate-wise
 //                    trimmed mean / median / NaN-aware mean), apply the optimizer,
 //                    store the new parameters into every rank's buffer (P2P stores or one NVLS multimem.st); exit barrier
+//                    geometric median instead: T + 1 passes over the owned coordinates (median, then Weiszfeld steps), with one
+//                    exchange of the n row distances per iteration (see `geometric_median`)
 //
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values.
@@ -23,6 +25,8 @@
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
 // launches can be captured once in a CUDA graph.
 // Ordering convention: finite ascending, non-finite last, ties -> lower worker index.
+
+#include <cmath>
 
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
@@ -41,11 +45,13 @@ constexpr int kMaxSeg = 8;                // owned coordinate segments (one per 
 constexpr int kSlotExchange = kMaxSeg;    // flag slots: [0, kMaxSeg) bucket entry, then exchange, then exit
 constexpr int kSlotExit = kMaxSeg + 1;
 constexpr int kSlotCraft = kMaxSeg + 2;   // entry barrier of the Byzantine crafting kernel
-constexpr int kFlagSlots = kMaxSeg + 3;
+constexpr int kMaxIterations = 16;        // geometric median: Weiszfeld iterations
+constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median: one exchange slot per iteration
+constexpr int kFlagSlots = kSlotGeoMedian + kMaxIterations;
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
-enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7 };
+enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -76,11 +82,13 @@ struct GarArgs {
     float* cta_partials;               // [grid][kMaxPairs]
     float* seg_partials;               // [kMaxSeg][seg_max_ctas][kMaxPairs]
     float* staging;                    // [n][owned length] or null
-    float* dist_out;                   // optional [n * n]
+    float* dist_out;                   // optional [n * n] (geometric median: [iterations][n])
     int* info;                         // optional [64]: selection masks for tests/diagnostics
     float const* loss_in;              // optional [nloss] local per-worker losses
     int nloss;
     float* loss_out;                   // [1]: total loss over all ranks (summed in rank order)
+    int iterations;                    // geometric median: Weiszfeld iterations T in [1, kMaxIterations]
+    float nu;                          // geometric median: smoothing, finite and > 0
 };
 
 struct Shared {
@@ -92,6 +100,11 @@ struct Shared {
             unsigned binom[kMaxWorkers + 1][kMaxWorkers / 2 + 1];
             unsigned long long best[16];                  // per-warp minimum keys
         } mda;
+        struct {                                          // geometric median: weights of the current iterate
+            float beta[kMaxWorkers];                      // 1 / max(nu, sqrt(D_i)) of the kept rows
+            float sum;                                    // their sum, in ascending worker order
+            unsigned mask;                                // kept rows; 0: no weights yet, the iterate is the median
+        } geo;
     };
     float scores[kMaxWorkers];
     float warp_partials[16][kBlockRows * kBlockRows];
@@ -654,6 +667,162 @@ __global__ void __launch_bounds__(256, 1) gar_phase_a_kernel(GarArgs const a, in
     phase_a_segment<CROSS>(a, sh, pair_of, seg, out, tid, nthreads);
 }
 
+// ---- geometric median: smoothed Weiszfeld iterations (RFA) ------------------------------ //
+// z_0 = coordinate-wise median; for t < T: D_i = ||z_t - x_i||^2, rows with a non-finite D_i are skipped, beta_i = 1 / max(nu, sqrt(D_i)),
+// S = sum beta_i and z_{t+1} = (sum beta_i x_i) / S, both sums over the kept rows in ascending worker order from +0, every operation
+// rounded once (explicit _rn intrinsics: no FMA contraction); no kept row: z_{t+1} = z_t. Output z_T.
+// T + 1 passes over the owned coordinates. Pass 0 loads the n values of each coordinate (P2P from the peers) and stages them when
+// R > 1; later passes read the staged tile, or the local rows when R = 1. Pass t recomputes z_t from the rows and the weights every
+// CTA keeps in shared memory (z_t is never stored) and accumulates the partial D_i in registers; the last pass goes through the
+// optimizer and the broadcast instead.
+// Exchange of iteration t: lanes -> warps -> CTA -> `cta_partials` -> grid barrier; block 0 folds the CTAs in order and stores the
+// rank's partials into every rank's mailbox (floats [(t & 1) * 32, + n) of its [kMaxPairs + 1] region), then signals slot
+// kSlotGeoMedian + t; every rank sums the R partials in rank order, so all ranks (and all CTAs) get the same D and the same weights.
+// Double buffering makes the mailbox safe to reuse: the half written at iteration t + 1 was last read at iteration t - 1; a rank
+// reads it before its block 0 reaches the grid barrier of iteration t, hence before it signals iteration t, and a writer stores
+// iteration t + 1 only after it has passed the barrier of iteration t, i.e. after every rank's iteration-t signal. With R = 1 a
+// second grid barrier takes the place of the flags. The loss travels through the exit barrier, as for the coordinate-wise rules.
+template<int N, int VEC>
+__device__ __forceinline__ void geometric_median(GarArgs const& a, Shared& sh, cg::grid_group& grid, float const (&hyper)[4], uint32_t epoch,
+                                                 long long tid, long long nthreads) {
+    int const n = a.n, T = a.iterations, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    bool const multi = a.R > 1;
+    long long const owned = owned_length(a);
+    if (threadIdx.x == 0)
+        sh.geo.mask = 0u;
+    __syncthreads();
+    for (int t = 0; t <= T; ++t) {
+        unsigned const mask = sh.geo.mask;
+        float const S = sh.geo.sum;
+        float acc[N];
+#pragma unroll
+        for (int i = 0; i < N; ++i)
+            acc[i] = 0.f;
+        for (int seg = 0; seg < a.nseg; ++seg) {
+            long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+            for (long long v = tid; v < lenv; v += nthreads) {
+                long long const x = lo + v * VEC;
+                float g[N][VEC];
+#pragma unroll
+                for (int i = 0; i < N; ++i) {
+                    if (i < n) {
+                        float* const staged = a.staging ? a.staging + i * owned + soff + v * VEC : nullptr;
+                        if (t == 0 || !staged) {
+                            V<VEC>::load_stream(a.grad[i] + x, g[i]);
+                            if (staged)
+                                V<VEC>::store(staged, g[i]);
+                        } else {
+                            V<VEC>::load(staged, g[i]);
+                        }
+                    } else {
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            g[i][c] = 0.f;
+                    }
+                }
+                float z[VEC];
+#pragma unroll
+                for (int c = 0; c < VEC; ++c) {
+                    if (mask == 0u) {
+                        float vals[N];
+#pragma unroll
+                        for (int i = 0; i < N; ++i)
+                            vals[i] = g[i][c];
+                        z[c] = coord_median<N>(vals, n);
+                    } else {
+                        float num = 0.f;
+#pragma unroll
+                        for (int i = 0; i < N; ++i)
+                            if ((mask >> i) & 1u)
+                                num = __fadd_rn(num, __fmul_rn(sh.geo.beta[i], g[i][c]));
+                        z[c] = __fdiv_rn(num, S);
+                    }
+                }
+                if (t == T) {
+                    apply_update<VEC>(a, hyper, x, z);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < N; ++i)
+                        if (i < n) {
+#pragma unroll
+                            for (int c = 0; c < VEC; ++c) {
+                                float const e = __fsub_rn(z[c], g[i][c]);
+                                acc[i] = __fmaf_rn(e, e, acc[i]);
+                            }
+                        }
+                }
+            }
+        }
+        if (t == T)
+            break;
+        // -------- exchange of the n squared distances of iteration t -------- //
+#pragma unroll
+        for (int i = 0; i < N; ++i) {
+            if (i < n) {
+                float const s = warp_sum(acc[i]);
+                if (lane == 0)
+                    sh.warp_partials[warp][i] = s;
+            }
+        }
+        __syncthreads();
+        if (threadIdx.x < n) {
+            float s = 0.f;
+            for (int w = 0; w < nwarps; ++w)
+                s += sh.warp_partials[w][threadIdx.x];
+            a.cta_partials[static_cast<long long>(blockIdx.x) * kMaxPairs + threadIdx.x] = s;
+        }
+        __threadfence();
+        grid.sync();
+        int const half = (t & 1) * kMaxWorkers;
+        if (blockIdx.x == 0) {
+            if (threadIdx.x < n) {
+                float s = 0.f;
+                for (unsigned b = 0; b < gridDim.x; ++b)
+                    s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kMaxPairs + threadIdx.x);
+                for (int q = 0; q < a.R; ++q)
+                    a.mailbox[q][a.rank * (kMaxPairs + 1) + half + threadIdx.x] = s;
+            }
+            fence_sys();
+            __syncthreads();
+            if (multi)
+                signal_all(a, kSlotGeoMedian + t, epoch);
+        }
+        if (multi) {
+            wait_all(a, kSlotGeoMedian + t, epoch);
+            __syncthreads();
+        } else {
+            grid.sync();
+        }
+        // -------- weights of z_{t+1} (warp 0 of every CTA, identical everywhere) -------- //
+        if (warp == 0) {
+            float D = 0.f;
+            if (lane < n) {
+                for (int q = 0; q < a.R; ++q)
+                    D += ld_volatile_f(a.mailbox[a.rank] + q * (kMaxPairs + 1) + half + lane);
+                if (a.dist_out && blockIdx.x == 0)
+                    a.dist_out[t * n + lane] = D;
+            }
+            bool const keep = lane < n && is_finite(D);
+            float const beta = keep ? __fdiv_rn(1.f, fmaxf(a.nu, __fsqrt_rn(D))) : 0.f;
+            unsigned const kept = __ballot_sync(0xffffffffu, keep);
+            if (kept != 0u) {   // no kept row: z_{t+1} = z_t, the weights stay
+                float sum = 0.f;
+                for (int j = 0; j < n; ++j) {
+                    float const bj = __shfl_sync(0xffffffffu, beta, j);
+                    if ((kept >> j) & 1u)
+                        sum = __fadd_rn(sum, bj);
+                }
+                sh.geo.beta[lane] = beta;
+                if (lane == 0) {
+                    sh.geo.mask = kept;
+                    sh.geo.sum = sum;
+                }
+            }
+        }
+        __syncthreads();
+    }
+}
+
 // ---- the finish kernel -------------------------------------------------------------- //
 template<int N, int VEC>
 __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArgs const a) {
@@ -849,6 +1018,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                 apply_update<VEC>(a, hyper, x, out);
             }
         }
+    } else if (a.rule == kGeoMedian) {
+        geometric_median<N, VEC>(a, sh, grid, hyper, epoch, tid, nthreads);
     } else {
         // -------- coordinate-wise rules: one streaming pass -------- //
         bool const in_switch = a.rule == kAverage && a.grad_mc != nullptr;
@@ -1153,14 +1324,16 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t strea
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2
+//       [25] iterations
+// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2 nu
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
     a.R = ints[5]; a.rank = ints[6]; a.opt = ints[7]; a.epoch = static_cast<uint32_t>(ints[8]);
     a.workers_per_rank = ints[10];
     a.nseg = ints[11]; a.first_seg = ints[12]; a.nloss = ints[13]; a.seg_max_ctas = ints[14];
+    a.iterations = ints[25];
     a.row_stride = longs[0];
-    a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3];
+    a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4];
     if (a.n < 1 || a.n > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
@@ -1172,8 +1345,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kMda)
+    if (a.rule < 0 || a.rule > kGeoMedian)
         return 102;
+    if (a.rule == kGeoMedian && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.nu > 0.f) || !std::isfinite(a.nu)))
+        return 115;
     if ((a.rule == kTrimmedMean || a.rule == kMda) && (a.f < 0 || 2 * a.f >= a.n))
         return a.rule == kTrimmedMean ? 112 : 113;
     if (a.rule == kMda) {
@@ -1218,8 +1393,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 107;
     if (a.opt == kAdagrad && !a.slot0)
         return 107;
-    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && (!a.cta_partials || !a.mailbox[0]))
+    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kGeoMedian) && (!a.cta_partials || !a.mailbox[0]))
         return 108;
+    if (a.rule == kGeoMedian && a.R > 1 && !a.staging)
+        return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)
         return 108;
     if (a.R > 1 && !a.signal[0])

@@ -482,6 +482,59 @@ template<class T> int mda(T const* g, size_t n, size_t d, size_t f, T* out, int6
     return 0;
 }
 
+// ------------------------------------------------------------------------ //
+// Geometric median, smoothed Weiszfeld iterations (RFA, Pillutla et al.): z_0 = the coordinate-wise median; for t < T,
+// D_i = ||z_t - x_i||^2 (chunked, folded in chunk order), rows with a non-finite D_i are skipped, beta_i = 1 / max(nu, sqrt(D_i)),
+// z_{t+1} = (sum beta_i x_i) / (sum beta_i), both sums over the kept rows in index order from +0, one rounding per operation (the
+// device kernel's definition: given the distances, the same bits). No kept row: z_{t+1} = z_t. `dist` (optional, [T, n]) receives D.
+constexpr size_t kGeoMaxIterations = 16;
+
+template<class T> int geometric_median(T const* g, size_t n, size_t d, size_t iterations, double nu_arg, T* out, T* dist_out) {
+    T const nu = static_cast<T>(nu_arg);
+    if (n == 0 || n > kMaxWorkers || iterations < 1 || iterations > kGeoMaxIterations || !(nu > T(0)) || !std::isfinite(nu))
+        return 1;
+    if (int status = median<T>(g, n, d, out))
+        return status;
+    size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
+    std::vector<T> next(d), partial(chunks * n), beta(n);
+    T* z = out;
+    T* z_next = next.data();
+    for (size_t t = 0; t < iterations; ++t) {
+        global_pool().run(0, d, kGrainCoord, [&](size_t chunk, size_t b, size_t e) {
+            for (size_t i = 0; i < n; ++i)
+                partial[chunk * n + i] = squared_difference(z, g + i * d, b, e);
+        });
+        std::vector<size_t> kept;
+        T sum = 0;
+        for (size_t i = 0; i < n; ++i) {
+            T D = 0;
+            for (size_t c = 0; c < chunks; ++c)
+                D += partial[c * n + i];
+            if (dist_out)
+                dist_out[t * n + i] = D;
+            if (std::isfinite(D)) {   // skipped, not weighted by 0: 0 * NaN is NaN
+                beta[i] = T(1) / std::max(nu, std::sqrt(D));
+                sum += beta[i];
+                kept.push_back(i);
+            }
+        }
+        if (kept.empty())
+            continue;   // z_{t+1} = z_t: the next iteration sees the same distances
+        agb::parallel_for(0, d, kGrainCoord, [&](size_t b, size_t e) {
+            for (size_t x = b; x < e; ++x) {
+                T num = 0;
+                for (size_t i: kept)
+                    num += beta[i] * g[i * d + x];
+                z_next[x] = num / sum;
+            }
+        });
+        std::swap(z, z_next);
+    }
+    if (z != out)
+        std::copy(z, z + d, out);
+    return 0;
+}
+
 // Multi-Krum: average of the m smallest-scoring gradients; `selected` (optional, [m]) receives their ids.
 template<class T> int krum(T const* g, size_t n, size_t d, size_t f, size_t m, T* out, int64_t* selected, T* dist_out) {
     if (n == 0 || n > kMaxWorkers || n < f + 3 || m < 1 || m > n)
@@ -670,6 +723,7 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_trimmed_mean_##S(T const* g, size_t n, size_t d, size_t f, T* out) { return trimmed_mean<T>(g, n, d, f, out); } \
     extern "C" int agb_cpu_mda_##S(T const* g, size_t n, size_t d, size_t f, T* out, int64_t* selected, T* dist) { return mda<T>(g, n, d, f, out, selected, dist); } \
     extern "C" int agb_cpu_mda_select_##S(T const* dist, size_t n, size_t f, int64_t* selected) { return mda_select<T>(dist, n, f, selected); } \
+    extern "C" int agb_cpu_geometric_median_##S(T const* g, size_t n, size_t d, size_t iterations, double nu, T* out, T* dist) { return geometric_median<T>(g, n, d, iterations, nu, out, dist); } \
     extern "C" int agb_cpu_pairwise_distances_##S(T const* g, size_t n, size_t d, T* dist) { if (n < 1) return 1; pairwise_distances<T>(g, n, d, dist); return 0; } \
     extern "C" int agb_cpu_weighted_sum_##S(T const* g, size_t n, size_t d, T const* w, T* out) { weighted_sum<T>(g, n, d, w, out); return 0; } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }

@@ -19,7 +19,8 @@ MAX_WORKERS = 32
 MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
-FLAG_SLOTS = MAX_SEGMENTS + 3   # per segment: bucket entry; then exchange, exit, Byzantine crafting entry
+MAX_ITERATIONS = 16   # geometric median: Weiszfeld iterations
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS   # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 MAILBOX_BYTES = MAX_RANKS * (MAX_PAIRS + 1) * 4
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
@@ -30,7 +31,8 @@ _ERRORS = {
   106: "optimizer requested without parameter buffers", 107: "optimizer slots missing", 108: "scratch buffers missing",
   109: "signal pads missing", 110: "more than 8 workers over several ranks need the staging buffer", 111: "invalid phase A launch",
   112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)",
-  114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)"}
+  114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)",
+  115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)"}
 BYZANTINE_MODES = {"alie": 0, "ipm": 1}
 
 
@@ -70,11 +72,12 @@ class FusedLauncher:
     self.seg_partials = torch.zeros(MAX_SEGMENTS * self.phase_a_ctas * MAX_PAIRS, dtype=torch.float32, device=self.device)
     self.local_mailbox = torch.zeros(MAILBOX_BYTES // 4, dtype=torch.float32, device=self.device)
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
+    self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # geometric median: D of every iteration, [T, n]
     self.info = torch.zeros(64, dtype=torch.int32, device=self.device)
     self._ptrs = (ctypes.c_ulonglong * 112)()
     self._ints = (ctypes.c_int * 32)()
     self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS))()
-    self._floats = (ctypes.c_float * 4)()
+    self._floats = (ctypes.c_float * 5)()
     self._func = _lib().agb_gar_fused
     self._func.restype = ctypes.c_int
     self._phase_a = _lib().agb_gar_phase_a
@@ -98,7 +101,8 @@ class FusedLauncher:
       ptrs[i] = row
     addr = lambda t: 0 if t is None else (t if isinstance(t, int) else t.data_ptr())
     ptrs[32], ptrs[33], ptrs[34], ptrs[35], ptrs[36] = addr(agg_out), addr(param), addr(slot0), addr(slot1), int(param_mc or 0)
-    ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), self.dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
+    dist_out = self.geo_dist_out if spec.rule == "geometric-median" else self.dist_out
+    ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
     ptrs[42], ptrs[43], ptrs[44], ptrs[45], ptrs[46] = addr(epoch_ptr), addr(hyper_ptr), self.seg_partials.data_ptr(), addr(loss_in), addr(loss_out)
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
@@ -109,13 +113,13 @@ class FusedLauncher:
     ints[0], ints[1], ints[2], ints[3], ints[4] = spec.n, spec.f, spec.m, spec.beta, spec.rule_id
     ints[5], ints[6], ints[7], ints[8], ints[9] = R, rank, OPTIMIZERS[opt], epoch & 0x7fffffff, max_ctas_limit
     ints[10], ints[11], ints[12], ints[13] = workers_per_rank, len(segments), first_seg, (loss_in.numel() if loss_in is not None else 0)
-    ints[14], ints[15], ints[24] = self.phase_a_ctas, self.phase_a_ctas, self.phase_a_threads
+    ints[14], ints[15], ints[24], ints[25] = self.phase_a_ctas, self.phase_a_ctas, self.phase_a_threads, spec.iterations
     self._longs[0] = row_stride
     for s in range(MAX_SEGMENTS):
       lo, hi = segments[s] if s < len(segments) else (0, 0)
       self._longs[1 + s], self._longs[1 + MAX_SEGMENTS + s] = lo, hi
       ints[16 + s] = self.phase_a_ctas if s < first_seg else 0
-    self._floats[0], self._floats[1], self._floats[2], self._floats[3] = lr, hyper[0], hyper[1], hyper[2]
+    self._floats[0], self._floats[1], self._floats[2], self._floats[3], self._floats[4] = lr, hyper[0], hyper[1], hyper[2], spec.nu
 
   def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
@@ -139,16 +143,18 @@ def _torch_rules(spec):
   return {"average": _ops.torch_average, "average-nan": _ops.torch_average_nan, "median": _ops.torch_median,
           "averaged-median": lambda M: _ops.torch_averaged_median(M, spec.beta), "krum": lambda M: _ops.torch_krum(M, spec.f, spec.m),
           "bulyan": lambda M: _ops.torch_bulyan(M, spec.f, spec.m), "trimmed-mean": lambda M: _ops.torch_trimmed_mean(M, spec.f),
-          "mda": lambda M: _ops.torch_mda(M, spec.f)}[spec.rule]
+          "mda": lambda M: _ops.torch_mda(M, spec.f), "geometric-median": lambda M: _ops.torch_geometric_median(M, spec.iterations, spec.nu)}[spec.rule]
 
 
 def aggregate(spec, G, return_details=False):
-  """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor."""
+  """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
+  distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median: the [iterations, n] row distances of every iteration) and the
+  selection masks."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   n, d = G.shape
   if n != spec.n:
-    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta)
+    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
@@ -174,7 +180,8 @@ def aggregate(spec, G, return_details=False):
   launcher.launch(spec, rows, 0, dp, agg_out=out)
   out = out[:d]
   if return_details:
-    return out, launcher.dist_out.view(n, n).clone(), launcher.info.clone()
+    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule == "geometric-median" else launcher.dist_out.view(n, n)
+    return out, dist.clone(), launcher.info.clone()
   return out
 
 

@@ -196,7 +196,8 @@ class FusedAggregation(_AggregationBase):
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
-    need_staging = self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)
+    # the geometric median's passes after the first re-read the staged copy rather than the peers' rows
+    need_staging = (self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule == "geometric-median" and R > 1)
     self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     self.max_ctas = max_ctas

@@ -11,6 +11,8 @@ fraction of the peer-copy rate measured at start-up; writes JSON to <--gar-out>/
 (`craft_byzantine`: the sm_90a kernel, sharded over the ranks on the fused engine, after the NCCL all-gather on the baseline one);
 the crafting kernel is also timed alone, next to the torch reference on the same device, with the (H + k) * d * 4 bytes it must move.
 `--gar-dump-rows` then saves, from the last rank, every row the fused engine aggregated (honest and crafted, all d coordinates).
+`--gar-rule-args key:value ...` passes the same `--aggregator-args` to every rule (rules ignore keys they do not use). The
+`geometric-median` entry also reports its T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
 """
 
 import argparse
@@ -42,6 +44,8 @@ def main():
   parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
   parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm"), default=None, help="omniscient attack by the last f workers, crafted every step")
   parser.add_argument("--gar-dump-rows", dest="dump_rows", action="store_true", help="with --gar-attack: save the last rank's view of every row to <--gar-out>")
+  parser.add_argument("--gar-rule-args", dest="rule_args", nargs="*", default=None, metavar="KEY:VALUE",
+                      help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -94,7 +98,7 @@ def main():
   for rule in args.rules.split(","):
     f = args.byz if args.byz is not None else 1 if rule == "bulyan" and n < 11 else 2
     name = {"krum": "krum", "bulyan": "bulyan"}.get(rule, rule)
-    gar = aggregators.instantiate(name, n, f, [])
+    gar = aggregators.instantiate(name, n, f, args.rule_args or [])
     sgd = build(optimizers, "optimizer", "sgd", [])
     fused = FusedAggregation(gar, layout, n, sgd, device=device, keep_aggregate=True)
     base = BaselineAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device)
@@ -242,6 +246,13 @@ def main():
                      "bucketed_total_ms": bucketed_ms, "finish_kernel_exposed_ms": exposed_ms,
                      "local_hbm_bytes": hbm, "hbm_gbs": hbm / fused_ms / 1e6 if world == 1 else None}
     results[rule].update(attack_entry)
+    if args.rule_args is not None:
+      results[rule]["rule_args"] = args.rule_args
+    if rule == "geometric-median":
+      # T + 1 passes, each reading the n rows of the owned coordinates once (the first from the peers, the others from the staged copy)
+      spec = gar.fused_spec()
+      passes_bytes = (spec.iterations + 1) * n * slice_bytes
+      results[rule].update({"iterations": spec.iterations, "nu": spec.nu, "pass_bytes": passes_bytes, "pass_gbs": passes_bytes / fused_ms / 1e6})
     if rank == 0:
       print(rule, json.dumps(results[rule]))
     del fused, base
