@@ -24,21 +24,24 @@ __all__ = ["_GAR", "FusedSpec", "register", "instantiate", "itemize", "get"]
 class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
-  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median")
+  RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
+           "centered-clipping")
 
-  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6):
-    """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing; the other rules ignore them."""
+  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0):
+    """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing, `iterations` and `tau` centered
+    clipping's iterations and clipping radius; the other rules ignore them."""
     if rule not in self.RULES:
       raise tools.UserException("Unknown fused rule " + repr(rule))
     self.rule, self.n, self.f, self.m, self.beta = rule, int(n), int(f), int(m), int(beta)
-    self.iterations, self.nu = int(iterations), float(nu)
+    self.iterations, self.nu, self.tau = int(iterations), float(nu), float(tau)
 
   @property
   def rule_id(self):
     return self.RULES.index(self.rule)
 
   def __repr__(self):
-    extra = ", iterations=%d, nu=%r" % (self.iterations, self.nu) if self.rule == "geometric-median" else ""
+    extra = {"geometric-median": ", iterations=%d, nu=%r" % (self.iterations, self.nu),
+             "centered-clipping": ", iterations=%d, tau=%r" % (self.iterations, self.tau)}.get(self.rule, "")
     return "FusedSpec(rule=%r, n=%d, f=%d, m=%d, beta=%d%s)" % (self.rule, self.n, self.f, self.m, self.beta, extra)
 
 

@@ -79,6 +79,41 @@ def check_geometric_median(n, f, iterations, nu):
   return int(iterations), nu32
 
 
+def fp32(value):
+  """`value` rounded once to fp32 (non-finite values pass through)."""
+  value = float(value)
+  return float(torch.tensor(value, dtype=torch.float32)) if math.isfinite(value) else value
+
+
+def check_centered_clipping(n, f, iterations, tau):
+  """Validate centered clipping's parameters -> (iterations, tau rounded once to fp32). `f` is not used by the algorithm; as for the
+  geometric median, 0 <= 2 f < n is still required."""
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("Centered clipping needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+  if isinstance(iterations, bool) or int(iterations) != iterations or not 1 <= iterations <= GEOMETRIC_MEDIAN_MAX_ITERATIONS:
+    raise tools.UserException("Centered clipping needs 1 <= iterations <= %d (got %r)" % (GEOMETRIC_MEDIAN_MAX_ITERATIONS, iterations))
+  tau32 = fp32(tau)
+  if not (math.isfinite(tau32) and tau32 > 0):
+    raise tools.UserException("Centered clipping needs a finite clipping radius tau > 0 in fp32 (got %r)" % (tau,))
+  return int(iterations), tau32
+
+
+def check_worker_momentum(beta, dampening):
+  """Validate worker momentum's coefficients -> (beta, c = 1 - dampening), both in fp32: beta and dampening are rounded once to fp32,
+  then c is computed in float64 from the rounded dampening and rounded once."""
+  values = []
+  for name, value in (("--worker-momentum", beta), ("--worker-momentum-dampening", dampening)):
+    try:
+      value = fp32(value)
+    except (TypeError, ValueError):
+      raise tools.UserException("%s expects a number (got %r)" % (name, value))
+    if not (math.isfinite(value) and 0.0 <= value < 1.0):
+      raise tools.UserException("%s must be finite, >= 0 and < 1 in fp32 (got %r)" % (name, value))
+    values.append(value)
+  beta32, dampening32 = values
+  return beta32, fp32(1.0 - dampening32)
+
+
 def _rank_key(values):
   """Sort key implementing (finite ascending, non-finite last); argsort(stable) then breaks ties by index."""
   return torch.where(torch.isfinite(values), values, torch.full_like(values, float("inf")))
@@ -183,6 +218,25 @@ def host_geometric_median(G, iterations, nu, return_distances=False):
   if status != 0:
     raise tools.UserException("Host geometric median rejected its arguments (n = %d, d = %d, iterations = %d, nu = %r)" % (n, d, iterations, nu))
   out = out.to(G.device)
+  return (out, dist) if return_distances else out
+
+
+def host_centered_clipping(G, iterations, tau, center, return_distances=False):
+  """Host library's centered clipping from the [d] `center`, which is updated in place (v <- z_T); returns z_T, and with
+  `return_distances` also the [iterations, n] squared distances D of every iteration."""
+  iterations, tau = check_centered_clipping(G.shape[0], 0, iterations, tau)
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  if center.shape != (d,) or center.dtype != Gc.dtype:
+    raise tools.UserException("Centered clipping needs a [%d] center of type %s (got %s, %s)" % (d, Gc.dtype, tuple(center.shape), center.dtype))
+  work = center.detach().to("cpu", copy=True).contiguous()
+  dist = torch.empty((iterations, n), dtype=Gc.dtype)
+  status = _host("centered_clipping", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), ctypes.c_size_t(iterations), ctypes.c_double(tau),
+                                                _ptr(work), _ptr(dist))
+  if status != 0:
+    raise tools.UserException("Host centered clipping rejected its arguments (n = %d, d = %d, iterations = %d, tau = %r)" % (n, d, iterations, tau))
+  center.copy_(work)
+  out = work.to(G.device)
   return (out, dist) if return_distances else out
 
 
@@ -299,6 +353,34 @@ def torch_geometric_median(G, iterations, nu, return_distances=False):
       total = total + beta[i]
       num = num + beta[i] * G[i]
     z = num / total
+  return (z, torch.stack(dists)) if return_distances else z
+
+
+def torch_centered_clipping(G, iterations, tau, center, return_distances=False):
+  """Centered clipping in G's dtype (double inputs, more than 32 workers on a device), from the [d] `center`, updated in place:
+  rows with a non-finite squared distance are skipped, c_i = 1 if sqrt(D_i) <= tau else tau / sqrt(D_i),
+  z = z + (sum c_i (x_i - z)) / n with the sum over the kept rows in ascending order and n all the rows; no kept row keeps z."""
+  iterations, tau = check_centered_clipping(G.shape[0], 0, iterations, tau)
+  n = G.shape[0]
+  scalar = lambda value: torch.tensor(value, dtype=G.dtype, device=G.device)
+  one, radius, count = scalar(1.0), scalar(tau), scalar(float(n))
+  z = center.to(device=G.device, dtype=G.dtype, copy=True)
+  dists = []
+  for _ in range(iterations):
+    delta = G - z.unsqueeze(0)
+    D = (delta * delta).sum(dim=1)
+    dists.append(D)
+    kept = [i for i in range(n) if math.isfinite(float(D[i]))]
+    if not kept:
+      continue
+    # the square root of an fp32 value taken in fp64 and rounded once is correctly rounded (torch's CPU fp32 sqrt is not always)
+    root = torch.sqrt(D.double()).to(G.dtype)
+    clip = torch.where(root <= radius, one, radius / root)
+    u = torch.zeros_like(z)
+    for i in kept:
+      u = u + clip[i] * (G[i] - z)
+    z = z + u / count
+  center.copy_(z)
   return (z, torch.stack(dists)) if return_distances else z
 
 
@@ -423,6 +505,21 @@ def torch_craft_byzantine_(G, byz_slots, mode, coef):
   row = torch_byzantine_row(G, byz_slots, mode, coef)
   for i in check_byzantine_slots(G.shape[0], byz_slots, mode):
     G[i].copy_(row)
+  return G
+
+
+# ---------------------------------------------------------------------------- #
+# Worker momentum (El Mhamdi et al., "Distributed Momentum for Byzantine-resilient SGD"): the CPU back-end and the oracle of the kernel
+
+def torch_worker_momentum_(G, M, beta, c):
+  """In place on the [w, d] rows G and momenta M: M <- beta * M + c * G, then G <- M, in G's dtype with one rounding per operation:
+  separate `torch.mul` / `torch.add` calls on 0-d tensors of the coefficients (CPU `add_(alpha=)` and `addcmul` may contract to FMA)."""
+  if G.shape != M.shape or G.dtype != M.dtype:
+    raise tools.UserException("Worker momentum needs rows and momenta of the same shape and type (got %s %s, %s %s)" % (
+      tuple(G.shape), G.dtype, tuple(M.shape), M.dtype))
+  scalar = lambda value: torch.tensor(value, dtype=G.dtype, device=G.device)
+  M.copy_(torch.add(torch.mul(M, scalar(beta)), torch.mul(G, scalar(c))))
+  G.copy_(M)
   return G
 
 

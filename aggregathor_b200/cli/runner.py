@@ -78,6 +78,8 @@ def make_parser():
   add("--dtype", type=str, default="auto", choices=("auto", "bf16", "tf32", "fp32"), help="Compute precision on the GPU: bf16 tensor-core products (default), or fp32 storage with TF32 products (the precision class of the fp32 reference); fp32 on CPU")
   add("--debug-checksum", action="store_true", default=False, help="Check after every step that all ranks hold bit-identical parameters")
   add("--authenticate", action="store_true", default=False, help="Sign every published gradient (ed25519) and verify before aggregating; slices failing the check become NaN")
+  add("--worker-momentum", type=float, default=0.0, help="Worker momentum beta in [0, 1): every worker submits its momentum m <- beta m + (1 - dampening) g instead of its gradient (0 with a zero dampening: off)")
+  add("--worker-momentum-dampening", type=float, default=0.0, help="Dampening of the worker momentum in [0, 1)")
   return parser
 
 
@@ -249,6 +251,7 @@ def main(argv=None):
     graph_mgr = Manager(experiment, aggregator, nb_instantiated, args.optimizer, args.optimizer_args, args.learning_rate, args.learning_rate_args,
                         (args.l1_regularize, args.l2_regularize), trace=args.trace, attack=attack, nb_real_byz=args.nb_real_byz_workers if attacked else 0,
                         device=device, engine=engine, backend=args.nn_backend, seed=args.seed, placement=placement, debug_checksum=args.debug_checksum, authenticate=args.authenticate,
+                        worker_momentum=args.worker_momentum, worker_momentum_dampening=args.worker_momentum_dampening,
                         dtype={"bf16": torch.bfloat16, "tf32": torch.float32, "fp32": torch.float32}.get(args.dtype))
   if exit_pending:
     return 0

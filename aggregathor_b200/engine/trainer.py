@@ -10,6 +10,9 @@ One synchronous step on a rank:
   1. for each local worker: next batch (already prefetched to the device), forward, loss, backward — gradients are
      written by the layer kernels directly into that worker's row of the peer-mapped `[w, d]` gradient matrix;
   2. optional l1 / l2 regularisation gradient (same formulas as `graph.py:125-139`);
+  2b. optional worker momentum (`worker_momentum` beta, `worker_momentum_dampening` delta; El Mhamdi et al., "Distributed Momentum for
+     Byzantine-resilient SGD"): every local row becomes its worker's momentum M <- beta M + (1 - delta) G, before anything else
+     reads it — a real Byzantine worker keeps its honest momentum, the attack then transforms or replaces what is submitted;
   3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
      Byzantine rows from the honest ones, a collective call on every rank);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast);
@@ -42,7 +45,12 @@ class Manager:
 
   def __init__(self, experiment, aggregator, nbworkers, optimizer="sgd", optimizer_args=None, learning_rate="fixed", learning_rate_args=None,
                regularizations=(-1., -1.), trace=False, *, attack=None, nb_real_byz=0, device=None, group=None, engine="auto", backend="auto",
-               dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False):
+               dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False,
+               worker_momentum=0.0, worker_momentum_dampening=0.0):
+    from ..aggregators import _ops
+    # (beta, c = 1 - dampening) in fp32; beta = dampening = 0 is off: no buffer, no kernel, the step is unchanged
+    self.momentum = _ops.check_worker_momentum(worker_momentum, worker_momentum_dampening)
+    self.momentum_on = self.momentum[0] != 0.0 or _ops.fp32(worker_momentum_dampening) != 0.0
     if authenticate and getattr(attack, "omniscient", False):
       raise tools.UserException("Omniscient attacks craft the Byzantine rows on every rank: they cannot be combined with '--authenticate'")
     self.device = torch.device(device) if device is not None else _default_device()
@@ -72,7 +80,8 @@ class Manager:
     # -- aggregation engine (owns params + gradient rows) -------------------------- #
     engine_args = dict(engine_args or {})
     self._bucket_layers = {}
-    plain_step = attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.)
+    # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum)
+    plain_step = attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
     if cuda and engine in ("auto", "fused") and aggregator.fused_spec() is not None:
       engine_args.setdefault("device_state", True)
       # The bucketed distance pass moves the gather + distance work of Krum / Bulyan under the backward pass (`gar_phase_a_kernel` on a side
@@ -98,6 +107,8 @@ class Manager:
     self.w = self.aggregation.w
     self.params = self.aggregation.params
     self.grads = self.aggregation.grads
+    # worker momentum: one fp32 row per local row of `grads` (same local index), +0 at the start
+    self.worker_momentum = torch.zeros((self.w, self.layout.padded_size), dtype=torch.float32, device=self.device) if self.momentum_on else None
     self.states = {name: torch.zeros(shape, dtype=torch.float32, device=self.device) for name, shape in state_shapes.items()}
     # identical initial parameters on every rank: same seed, CPU generator, then copy
     generator = torch.Generator().manual_seed(seed)
@@ -231,6 +242,7 @@ class Manager:
       with torch.cuda.graph(graph):
         self._static_losses = self._run_workers(self._static_batches, None)
         if whole:
+          self._apply_momentum()
           self.aggregation.step(stream=None, loss_in=self._static_losses, prepared=True)
           self._refresh_weights()
     except Exception as err:
@@ -336,6 +348,11 @@ class Manager:
     counters.bump(self._graph_launches)
     return list(self._static_losses.unbind(0))
 
+  def _apply_momentum(self):
+    """Worker momentum on every local row (one kernel launch for the rank): M <- beta M + c G, then G <- M."""
+    if self.momentum_on:
+      gar_ops.worker_momentum_(self.grads, self.worker_momentum, *self.momentum)
+
   def compute_gradients(self):
     """Phase 1-3 of a step: local workers' losses and gradients (+ regularisation, + attacks). Returns the list of losses."""
     group = self._stream_group
@@ -353,6 +370,8 @@ class Manager:
       for j in range(len(self.local_workers)):
         self.grads[self.placement[self.local_workers[j]][1]].add_(reg_grad)
         losses[j] = losses[j] + reg_loss
+    if not (self._last_step_replayed and self._graph_whole):   # the whole-step graph holds the momentum step
+      self._apply_momentum()
     if getattr(self.attack, "omniscient", False):
       if self.byzantine_slots:   # collective: every rank crafts its share, whether or not it hosts a Byzantine worker
         self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef)
@@ -438,10 +457,24 @@ class Manager:
 
   # ---------------------------------------------------------------------------- #
   def state_dict(self):
+    """Collective when R > 1. With worker momentum, "worker_momentum" is the [n, d] fp32 matrix of every worker's momentum, indexed by
+    logical worker id (n * d * 4 bytes more)."""
     agg = self.aggregation.state_dict()
-    return {"global_step": self.step, "params": self.params.detach().to("cpu", copy=True), "optimizer": self.optimizer.name,
-            "aggregation": agg, "states": {k: v.detach().to("cpu", copy=True) for k, v in self.states.items()},
-            "layout": self.layout.describe(), "time": time.time()}
+    state = {"global_step": self.step, "params": self.params.detach().to("cpu", copy=True), "optimizer": self.optimizer.name,
+             "aggregation": agg, "states": {k: v.detach().to("cpu", copy=True) for k, v in self.states.items()},
+             "layout": self.layout.describe(), "time": time.time()}
+    if self.momentum_on:
+      state["worker_momentum"] = self._gather_momentum()
+    return state
+
+  def _gather_momentum(self):
+    """Every rank's momentum rows -> [n, d] CPU tensor by logical worker id (collective when R > 1)."""
+    if self.world > 1:
+      parts = [torch.empty_like(self.worker_momentum) for _ in range(self.world)]
+      dist.all_gather(parts, self.worker_momentum.contiguous(), group=self.group)
+    else:
+      parts = [self.worker_momentum]
+    return torch.stack([parts[rank][row].detach().to("cpu", copy=True) for rank, row in self.placement])
 
   def load_state_dict(self, state):
     if "tf_variables" in state:  # a checkpoint of the reference: variables by name in TensorFlow's layouts, optimizer slots not carried over
@@ -459,6 +492,18 @@ class Manager:
       self.aggregation.load_state_dict(state["aggregation"])
     elif state.get("optimizer") is not None:
       tools.warning("Checkpoint was written with optimizer %r, now using %r: slots are reset" % (state.get("optimizer"), self.optimizer.name))
+    saved = state.get("worker_momentum")
+    if self.momentum_on:
+      self.worker_momentum.zero_()
+      if saved is None:
+        tools.warning("The checkpoint holds no worker momentum: the momenta start from zero", context="restore")
+      elif tuple(saved.shape) != (self.n, self.worker_momentum.shape[1]):
+        raise tools.UserException("Checkpoint holds worker momenta of shape %s, expected %s" % (tuple(saved.shape), (self.n, self.worker_momentum.shape[1])))
+      else:
+        for i in self.local_workers:
+          self.worker_momentum[self.placement[i][1]].copy_(saved[i].to(self.device))
+    elif saved is not None:
+      tools.warning("The checkpoint holds worker momenta but worker momentum is off: they are ignored", context="restore")
     self.step = int(state["global_step"])
     self._refresh_weights(force=True)
     if self.device.type == "cuda":

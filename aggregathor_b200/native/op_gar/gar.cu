@@ -15,8 +15,8 @@
 //                    (replicated on all ranks); phase D: aggregate the owned coordinates (mean of selected / coordinate-wise
 //                    trimmed mean / median / NaN-aware mean), apply the optimizer,
 //                    store the new parameters into every rank's buffer (P2P stores or one NVLS multimem.st); exit barrier
-//                    geometric median instead: T + 1 passes over the owned coordinates (median, then Weiszfeld steps), with one
-//                    exchange of the n row distances per iteration (see `geometric_median`)
+//                    geometric median / centered clipping instead: T + 1 passes over the owned coordinates, with one exchange of
+//                    the n row distances per iteration (see `iterative_rule`)
 //
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values.
@@ -45,13 +45,14 @@ constexpr int kMaxSeg = 8;                // owned coordinate segments (one per 
 constexpr int kSlotExchange = kMaxSeg;    // flag slots: [0, kMaxSeg) bucket entry, then exchange, then exit
 constexpr int kSlotExit = kMaxSeg + 1;
 constexpr int kSlotCraft = kMaxSeg + 2;   // entry barrier of the Byzantine crafting kernel
-constexpr int kMaxIterations = 16;        // geometric median: Weiszfeld iterations
-constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median: one exchange slot per iteration
+constexpr int kMaxIterations = 16;        // geometric median, centered clipping: iterations
+constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median, centered clipping: one exchange slot per iteration
 constexpr int kFlagSlots = kSlotGeoMedian + kMaxIterations;
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
-enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8 };
+enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8,
+           kCenteredClipping = 9 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -82,13 +83,15 @@ struct GarArgs {
     float* cta_partials;               // [grid][kMaxPairs]
     float* seg_partials;               // [kMaxSeg][seg_max_ctas][kMaxPairs]
     float* staging;                    // [n][owned length] or null
-    float* dist_out;                   // optional [n * n] (geometric median: [iterations][n])
+    float* dist_out;                   // optional [n * n] (geometric median, centered clipping: [iterations][n])
     int* info;                         // optional [64]: selection masks for tests/diagnostics
     float const* loss_in;              // optional [nloss] local per-worker losses
     int nloss;
     float* loss_out;                   // [1]: total loss over all ranks (summed in rank order)
-    int iterations;                    // geometric median: Weiszfeld iterations T in [1, kMaxIterations]
+    int iterations;                    // geometric median, centered clipping: iterations T in [1, kMaxIterations]
     float nu;                          // geometric median: smoothing, finite and > 0
+    float tau;                         // centered clipping: clipping radius, finite and > 0
+    float* center;                     // centered clipping: [d] (local) center v, read and updated on the owned coordinates
 };
 
 struct Shared {
@@ -100,10 +103,10 @@ struct Shared {
             unsigned binom[kMaxWorkers + 1][kMaxWorkers / 2 + 1];
             unsigned long long best[16];                  // per-warp minimum keys
         } mda;
-        struct {                                          // geometric median: weights of the current iterate
-            float beta[kMaxWorkers];                      // 1 / max(nu, sqrt(D_i)) of the kept rows
-            float sum;                                    // their sum, in ascending worker order
-            unsigned mask;                                // kept rows; 0: no weights yet, the iterate is the median
+        struct {                                          // geometric median, centered clipping: weights of the current iterate
+            float beta[kMaxWorkers];                      // 1 / max(nu, sqrt(D_i)) (CC: the clipping factors c_i) of the kept rows
+            float sum;                                    // geometric median: their sum, in ascending worker order
+            unsigned mask;                                // kept rows; 0: no weights, the iterate is the median (CC: z_t is unchanged)
         } geo;
     };
     float scores[kMaxWorkers];
@@ -667,14 +670,20 @@ __global__ void __launch_bounds__(256, 1) gar_phase_a_kernel(GarArgs const a, in
     phase_a_segment<CROSS>(a, sh, pair_of, seg, out, tid, nthreads);
 }
 
-// ---- geometric median: smoothed Weiszfeld iterations (RFA) ------------------------------ //
-// z_0 = coordinate-wise median; for t < T: D_i = ||z_t - x_i||^2, rows with a non-finite D_i are skipped, beta_i = 1 / max(nu, sqrt(D_i)),
-// S = sum beta_i and z_{t+1} = (sum beta_i x_i) / S, both sums over the kept rows in ascending worker order from +0, every operation
-// rounded once (explicit _rn intrinsics: no FMA contraction); no kept row: z_{t+1} = z_t. Output z_T.
+// ---- iterative rules: geometric median (smoothed Weiszfeld, RFA) and centered clipping ---------- //
+// Geometric median: z_0 = coordinate-wise median; for t < T: D_i = ||z_t - x_i||^2, rows with a non-finite D_i are skipped,
+// beta_i = 1 / max(nu, sqrt(D_i)), S = sum beta_i and z_{t+1} = (sum beta_i x_i) / S, both sums over the kept rows in ascending worker
+// order from +0; no kept row: z_{t+1} = z_t.
+// Centered clipping (Karimireddy et al.): z_0 = the center v; for t < T: the same D_i and skipped rows, s_i = sqrt(D_i),
+// c_i = 1 if s_i <= tau else tau / s_i, u = sum c_i (x_i - z_t) over the kept rows in ascending worker order from +0,
+// z_{t+1} = z_t + u / n (all n rows); no kept row: z_{t+1} = z_t. v <- z_T.
+// Every operation rounded once (explicit _rn intrinsics: no FMA contraction). Output z_T.
 // T + 1 passes over the owned coordinates. Pass 0 loads the n values of each coordinate (P2P from the peers) and stages them when
-// R > 1; later passes read the staged tile, or the local rows when R = 1. Pass t recomputes z_t from the rows and the weights every
-// CTA keeps in shared memory (z_t is never stored) and accumulates the partial D_i in registers; the last pass goes through the
-// optimizer and the broadcast instead.
+// R > 1; later passes read the staged tile, or the local rows when R = 1. The geometric median's pass t recomputes z_t from the rows
+// and the weights every CTA keeps in shared memory (z_t is never stored). Centered clipping keeps z_t in the center buffer: pass 0
+// reads z_0, pass t >= 1 reads z_{t-1}, applies the weights of iteration t - 1 and stores z_t; every element is read and written by
+// the same thread, between grid barriers. Each pass but the last accumulates the partial D_i in registers; the last pass goes
+// through the optimizer and the broadcast instead.
 // Exchange of iteration t: lanes -> warps -> CTA -> `cta_partials` -> grid barrier; block 0 folds the CTAs in order and stores the
 // rank's partials into every rank's mailbox (floats [(t & 1) * 32, + n) of its [kMaxPairs + 1] region), then signals slot
 // kSlotGeoMedian + t; every rank sums the R partials in rank order, so all ranks (and all CTAs) get the same D and the same weights.
@@ -683,8 +692,8 @@ __global__ void __launch_bounds__(256, 1) gar_phase_a_kernel(GarArgs const a, in
 // iteration t + 1 only after it has passed the barrier of iteration t, i.e. after every rank's iteration-t signal. With R = 1 a
 // second grid barrier takes the place of the flags. The loss travels through the exit barrier, as for the coordinate-wise rules.
 template<int N, int VEC>
-__device__ __forceinline__ void geometric_median(GarArgs const& a, Shared& sh, cg::grid_group& grid, float const (&hyper)[4], uint32_t epoch,
-                                                 long long tid, long long nthreads) {
+__device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg::grid_group& grid, float const (&hyper)[4], uint32_t epoch,
+                                               long long tid, long long nthreads) {
     int const n = a.n, T = a.iterations, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     bool const multi = a.R > 1;
     long long const owned = owned_length(a);
@@ -720,10 +729,23 @@ __device__ __forceinline__ void geometric_median(GarArgs const& a, Shared& sh, c
                             g[i][c] = 0.f;
                     }
                 }
+                // z_t coordinate by coordinate, each followed by its share of the partial D_i: a coordinate's n values are dead
+                // once it is done, which keeps the pass within the register budget of the 8-worker instance
                 float z[VEC];
+                if (a.rule == kCenteredClipping)
+                    V<VEC>::load(a.center + x, z);   // z_0, or z_{t-1}
 #pragma unroll
                 for (int c = 0; c < VEC; ++c) {
-                    if (mask == 0u) {
+                    if (a.rule == kCenteredClipping) {
+                        if (mask != 0u) {
+                            float u = 0.f;
+#pragma unroll
+                            for (int i = 0; i < N; ++i)
+                                if ((mask >> i) & 1u)
+                                    u = __fadd_rn(u, __fmul_rn(sh.geo.beta[i], __fsub_rn(g[i][c], z[c])));
+                            z[c] = __fadd_rn(z[c], __fdiv_rn(u, static_cast<float>(n)));
+                        }
+                    } else if (mask == 0u) {
                         float vals[N];
 #pragma unroll
                         for (int i = 0; i < N; ++i)
@@ -737,20 +759,19 @@ __device__ __forceinline__ void geometric_median(GarArgs const& a, Shared& sh, c
                                 num = __fadd_rn(num, __fmul_rn(sh.geo.beta[i], g[i][c]));
                         z[c] = __fdiv_rn(num, S);
                     }
-                }
-                if (t == T) {
-                    apply_update<VEC>(a, hyper, x, z);
-                } else {
+                    if (t < T) {
 #pragma unroll
-                    for (int i = 0; i < N; ++i)
-                        if (i < n) {
-#pragma unroll
-                            for (int c = 0; c < VEC; ++c) {
+                        for (int i = 0; i < N; ++i)
+                            if (i < n) {
                                 float const e = __fsub_rn(z[c], g[i][c]);
                                 acc[i] = __fmaf_rn(e, e, acc[i]);
                             }
-                        }
+                    }
                 }
+                if (a.rule == kCenteredClipping && mask != 0u)
+                    V<VEC>::store(a.center + x, z);   // z_t
+                if (t == T)
+                    apply_update<VEC>(a, hyper, x, z);
             }
         }
         if (t == T)
@@ -803,9 +824,14 @@ __device__ __forceinline__ void geometric_median(GarArgs const& a, Shared& sh, c
                     a.dist_out[t * n + lane] = D;
             }
             bool const keep = lane < n && is_finite(D);
-            float const beta = keep ? __fdiv_rn(1.f, fmaxf(a.nu, __fsqrt_rn(D))) : 0.f;
             unsigned const kept = __ballot_sync(0xffffffffu, keep);
-            if (kept != 0u) {   // no kept row: z_{t+1} = z_t, the weights stay
+            if (a.rule == kCenteredClipping) {   // no kept row: mask 0, the next pass keeps z_t
+                float const s = __fsqrt_rn(D);
+                sh.geo.beta[lane] = keep ? (s <= a.tau ? 1.f : __fdiv_rn(a.tau, s)) : 0.f;
+                if (lane == 0)
+                    sh.geo.mask = kept;
+            } else if (kept != 0u) {   // no kept row: z_{t+1} = z_t, the weights stay
+                float const beta = keep ? __fdiv_rn(1.f, fmaxf(a.nu, __fsqrt_rn(D))) : 0.f;
                 float sum = 0.f;
                 for (int j = 0; j < n; ++j) {
                     float const bj = __shfl_sync(0xffffffffu, beta, j);
@@ -1018,8 +1044,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                 apply_update<VEC>(a, hyper, x, out);
             }
         }
-    } else if (a.rule == kGeoMedian) {
-        geometric_median<N, VEC>(a, sh, grid, hyper, epoch, tid, nthreads);
+    } else if (a.rule == kGeoMedian || a.rule == kCenteredClipping) {
+        iterative_rule<N, VEC>(a, sh, grid, hyper, epoch, tid, nthreads);
     } else {
         // -------- coordinate-wise rules: one streaming pass -------- //
         bool const in_switch = a.rule == kAverage && a.grad_mc != nullptr;
@@ -1256,6 +1282,28 @@ __global__ void sgd_kernel(float* __restrict__ p, float const* __restrict__ g, f
     }
 }
 
+// Worker momentum (El Mhamdi et al., "Distributed Momentum for Byzantine-resilient SGD"): every element of the w rows of a rank,
+// M <- beta * M + c * G, then G <- M, each operation rounded once (explicit _rn intrinsics: no FMA contraction); c = 1 - dampening.
+// One launch for the w rows (blockIdx.y = row), grid-stride along a row; streaming: G and M are read and written once, 16 bytes per
+// coordinate. M is only read again at the next step, G right away by the aggregation.
+template<int VEC>
+__global__ void worker_momentum_kernel(float* __restrict__ g, long long g_stride, float* __restrict__ m, long long m_stride, long long d,
+                                       float beta, float c) {
+    float* const grow = g + static_cast<long long>(blockIdx.y) * g_stride;
+    float* const mrow = m + static_cast<long long>(blockIdx.y) * m_stride;
+    long long const stride = static_cast<long long>(gridDim.x) * blockDim.x * VEC;
+    for (long long x = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * VEC; x < d; x += stride) {
+        float gv[VEC], mv[VEC];
+        V<VEC>::load(grow + x, gv);
+        V<VEC>::load_stream(mrow + x, mv);
+#pragma unroll
+        for (int k = 0; k < VEC; ++k)
+            mv[k] = __fadd_rn(__fmul_rn(beta, mv[k]), __fmul_rn(c, gv[k]));
+        V<VEC>::store_stream(mrow + x, mv);
+        V<VEC>::store(grow + x, mv);
+    }
+}
+
 // Lossy-transport emulation (reference: tf_patches mpi_rendezvous_mgr.patch:814-843): every `chunk`-byte
 // datagram of the serialized gradient is lost with probability `rate`; lost chunks become NaN (mode 0),
 // zeros (mode 1) or the previous gradient's bytes (mode 2, "CLEVER").
@@ -1324,8 +1372,9 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t strea
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
+//   [47] center (centered clipping)
 //       [25] iterations
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2 nu
+// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
     a.R = ints[5]; a.rank = ints[6]; a.opt = ints[7]; a.epoch = static_cast<uint32_t>(ints[8]);
@@ -1333,7 +1382,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.nseg = ints[11]; a.first_seg = ints[12]; a.nloss = ints[13]; a.seg_max_ctas = ints[14];
     a.iterations = ints[25];
     a.row_stride = longs[0];
-    a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4];
+    a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4]; a.tau = floats[5];
+    a.center = reinterpret_cast<float*>(ptrs[47]);
     if (a.n < 1 || a.n > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
@@ -1345,8 +1395,11 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kGeoMedian)
+    if (a.rule < 0 || a.rule > kCenteredClipping)
         return 102;
+    if (a.rule == kCenteredClipping && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.tau > 0.f) ||
+                                        !std::isfinite(a.tau) || !a.center))
+        return 116;
     if (a.rule == kGeoMedian && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.nu > 0.f) || !std::isfinite(a.nu)))
         return 115;
     if ((a.rule == kTrimmedMean || a.rule == kMda) && (a.f < 0 || 2 * a.f >= a.n))
@@ -1393,9 +1446,9 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 107;
     if (a.opt == kAdagrad && !a.slot0)
         return 107;
-    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kGeoMedian) && (!a.cta_partials || !a.mailbox[0]))
+    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kGeoMedian || a.rule == kCenteredClipping) && (!a.cta_partials || !a.mailbox[0]))
         return 108;
-    if (a.rule == kGeoMedian && a.R > 1 && !a.staging)
+    if ((a.rule == kGeoMedian || a.rule == kCenteredClipping) && a.R > 1 && !a.staging)
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)
         return 108;
@@ -1411,7 +1464,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
 extern "C" {
 
 char const* agb_op_list() {
-    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,sgd,drop_chunks,checksum,cast_bf16";
+    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,sgd,worker_momentum,drop_chunks,checksum,cast_bf16";
 }
 
 // Wall-clock bound (seconds, 0 = none) of the cross-GPU flag waits of this library's kernels.
@@ -1543,6 +1596,30 @@ int agb_sgd(void* p, void const* g, float lr, long long d, void* stream) {
         blocks = agb::sm_count() * 8;
     if (blocks > 0)
         sgd_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<float*>(p), static_cast<float const*>(g), lr, d);
+    AGB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// Worker momentum over `w` rows of `d` fp32 elements: G rows `g_stride` elements apart, M rows `m_stride` apart (see
+// `worker_momentum_kernel`). float4 accesses when d, both strides and both base addresses allow them, scalar ones otherwise.
+int agb_worker_momentum(void* g, long long g_stride, void* m, long long m_stride, long long w, long long d, float beta, float c, void* stream) {
+    if (w < 0 || w > 65535 || d < 0 || g_stride < d || m_stride < d || ((!g || !m) && w > 0 && d > 0))
+        return 101;
+    if (w == 0 || d == 0)
+        return 0;
+    bool const vec = (d % 4 == 0) && (g_stride % 4 == 0) && (m_stride % 4 == 0) && (reinterpret_cast<uintptr_t>(g) % 16 == 0) &&
+                     (reinterpret_cast<uintptr_t>(m) % 16 == 0);
+    long long const items = vec ? d / 4 : d;
+    long long blocks = (items + 255) / 256;
+    long long const cap = (static_cast<long long>(agb::sm_count()) * 8 + w - 1) / w;   // about 8 CTAs per SM over all the rows
+    if (blocks > cap)
+        blocks = cap;
+    dim3 const grid(static_cast<unsigned>(blocks), static_cast<unsigned>(w));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (vec)
+        worker_momentum_kernel<4><<<grid, 256, 0, s>>>(static_cast<float*>(g), g_stride, static_cast<float*>(m), m_stride, d, beta, c);
+    else
+        worker_momentum_kernel<1><<<grid, 256, 0, s>>>(static_cast<float*>(g), g_stride, static_cast<float*>(m), m_stride, d, beta, c);
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -535,6 +535,53 @@ template<class T> int geometric_median(T const* g, size_t n, size_t d, size_t it
     return 0;
 }
 
+// ------------------------------------------------------------------------ //
+// Centered clipping (Karimireddy, He and Jaggi, "Learning from History for Byzantine Robust Optimization"): z_0 = the center v; for
+// t < T, D_i = ||x_i - z_t||^2 (chunked, folded in chunk order), rows with a non-finite D_i are skipped, s_i = sqrt(D_i),
+// c_i = 1 if s_i <= tau else tau / s_i, z_{t+1} = z_t + (sum c_i (x_i - z_t)) / n, the sum over the kept rows in index order from +0
+// and divided by all n rows, one rounding per operation (the device kernel's definition: given the distances, the same bits). No
+// kept row: z_{t+1} = z_t. `center` is v on entry and z_T on return; `dist` (optional, [T, n]) receives D.
+template<class T> int centered_clipping(T const* g, size_t n, size_t d, size_t iterations, double tau_arg, T* center, T* dist_out) {
+    T const tau = static_cast<T>(tau_arg);
+    if (n == 0 || n > kMaxWorkers || iterations < 1 || iterations > kGeoMaxIterations || !(tau > T(0)) || !std::isfinite(tau) || !center)
+        return 1;
+    size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
+    std::vector<T> partial(chunks * n), clip(n);
+    T const count = static_cast<T>(n);
+    for (size_t t = 0; t < iterations; ++t) {
+        global_pool().run(0, d, kGrainCoord, [&](size_t chunk, size_t b, size_t e) {
+            for (size_t i = 0; i < n; ++i)
+                partial[chunk * n + i] = squared_difference(center, g + i * d, b, e);
+        });
+        std::vector<size_t> kept;
+        for (size_t i = 0; i < n; ++i) {
+            T D = 0;
+            for (size_t c = 0; c < chunks; ++c)
+                D += partial[c * n + i];
+            if (dist_out)
+                dist_out[t * n + i] = D;
+            if (std::isfinite(D)) {   // skipped, not weighted by 0: 0 * NaN is NaN
+                T const s = std::sqrt(D);
+                clip[i] = s <= tau ? T(1) : tau / s;
+                kept.push_back(i);
+            }
+        }
+        if (kept.empty())
+            continue;   // z_{t+1} = z_t
+        agb::parallel_for(0, d, kGrainCoord, [&](size_t b, size_t e) {
+            for (size_t x = b; x < e; ++x) {
+                T u = 0;
+                for (size_t i: kept) {
+                    T const diff = g[i * d + x] - center[x];
+                    u += clip[i] * diff;
+                }
+                center[x] = center[x] + u / count;
+            }
+        });
+    }
+    return 0;
+}
+
 // Multi-Krum: average of the m smallest-scoring gradients; `selected` (optional, [m]) receives their ids.
 template<class T> int krum(T const* g, size_t n, size_t d, size_t f, size_t m, T* out, int64_t* selected, T* dist_out) {
     if (n == 0 || n > kMaxWorkers || n < f + 3 || m < 1 || m > n)
@@ -724,6 +771,7 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_mda_##S(T const* g, size_t n, size_t d, size_t f, T* out, int64_t* selected, T* dist) { return mda<T>(g, n, d, f, out, selected, dist); } \
     extern "C" int agb_cpu_mda_select_##S(T const* dist, size_t n, size_t f, int64_t* selected) { return mda_select<T>(dist, n, f, selected); } \
     extern "C" int agb_cpu_geometric_median_##S(T const* g, size_t n, size_t d, size_t iterations, double nu, T* out, T* dist) { return geometric_median<T>(g, n, d, iterations, nu, out, dist); } \
+    extern "C" int agb_cpu_centered_clipping_##S(T const* g, size_t n, size_t d, size_t iterations, double tau, T* center, T* dist) { return centered_clipping<T>(g, n, d, iterations, tau, center, dist); } \
     extern "C" int agb_cpu_pairwise_distances_##S(T const* g, size_t n, size_t d, T* dist) { if (n < 1) return 1; pairwise_distances<T>(g, n, d, dist); return 0; } \
     extern "C" int agb_cpu_weighted_sum_##S(T const* g, size_t n, size_t d, T const* w, T* out) { weighted_sum<T>(g, n, d, w, out); return 0; } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }

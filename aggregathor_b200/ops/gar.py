@@ -19,7 +19,7 @@ MAX_WORKERS = 32
 MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
-MAX_ITERATIONS = 16   # geometric median: Weiszfeld iterations
+MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
 FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS   # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 MAILBOX_BYTES = MAX_RANKS * (MAX_PAIRS + 1) * 4
@@ -32,7 +32,9 @@ _ERRORS = {
   109: "signal pads missing", 110: "more than 8 workers over several ranks need the staging buffer", 111: "invalid phase A launch",
   112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)",
   114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)",
-  115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)"}
+  115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)",
+  116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)"}
+ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1}
 
 
@@ -72,12 +74,12 @@ class FusedLauncher:
     self.seg_partials = torch.zeros(MAX_SEGMENTS * self.phase_a_ctas * MAX_PAIRS, dtype=torch.float32, device=self.device)
     self.local_mailbox = torch.zeros(MAILBOX_BYTES // 4, dtype=torch.float32, device=self.device)
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
-    self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # geometric median: D of every iteration, [T, n]
+    self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
     self.info = torch.zeros(64, dtype=torch.int32, device=self.device)
     self._ptrs = (ctypes.c_ulonglong * 112)()
     self._ints = (ctypes.c_int * 32)()
     self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS))()
-    self._floats = (ctypes.c_float * 5)()
+    self._floats = (ctypes.c_float * 6)()
     self._func = _lib().agb_gar_fused
     self._func.restype = ctypes.c_int
     self._phase_a = _lib().agb_gar_phase_a
@@ -89,7 +91,7 @@ class FusedLauncher:
 
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
-            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None):
+            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None):
     ptrs = self._ptrs
     for i in range(112):
       ptrs[i] = 0
@@ -101,9 +103,10 @@ class FusedLauncher:
       ptrs[i] = row
     addr = lambda t: 0 if t is None else (t if isinstance(t, int) else t.data_ptr())
     ptrs[32], ptrs[33], ptrs[34], ptrs[35], ptrs[36] = addr(agg_out), addr(param), addr(slot0), addr(slot1), int(param_mc or 0)
-    dist_out = self.geo_dist_out if spec.rule == "geometric-median" else self.dist_out
+    dist_out = self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dist_out
     ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
     ptrs[42], ptrs[43], ptrs[44], ptrs[45], ptrs[46] = addr(epoch_ptr), addr(hyper_ptr), self.seg_partials.data_ptr(), addr(loss_in), addr(loss_out)
+    ptrs[47] = addr(center)
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -120,6 +123,7 @@ class FusedLauncher:
       self._longs[1 + s], self._longs[1 + MAX_SEGMENTS + s] = lo, hi
       ints[16 + s] = self.phase_a_ctas if s < first_seg else 0
     self._floats[0], self._floats[1], self._floats[2], self._floats[3], self._floats[4] = lr, hyper[0], hyper[1], hyper[2], spec.nu
+    self._floats[5] = spec.tau
 
   def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
@@ -146,15 +150,17 @@ def _torch_rules(spec):
           "mda": lambda M: _ops.torch_mda(M, spec.f), "geometric-median": lambda M: _ops.torch_geometric_median(M, spec.iterations, spec.nu)}[spec.rule]
 
 
-def aggregate(spec, G, return_details=False):
+def aggregate(spec, G, return_details=False, center=None):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
-  distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median: the [iterations, n] row distances of every iteration) and the
-  selection masks."""
+  distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
+  iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   n, d = G.shape
   if n != spec.n:
-    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu)
+    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau)
+  if spec.rule == "centered-clipping":
+    return _aggregate_centered_clipping(spec, G, return_details, center)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
@@ -171,18 +177,82 @@ def aggregate(spec, G, return_details=False):
     Gp[:, :d] = G
     G = Gp
   dp = d + pad
-  key = (G.device.index, n)
-  launcher = _launchers.get(key)
-  if launcher is None:
-    launcher = _launchers[key] = FusedLauncher(G.device, n)
+  launcher = _launcher(G.device, n)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
   launcher.launch(spec, rows, 0, dp, agg_out=out)
   out = out[:d]
   if return_details:
-    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule == "geometric-median" else launcher.dist_out.view(n, n)
+    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule in ITERATIVE_RULES else launcher.dist_out.view(n, n)
     return out, dist.clone(), launcher.info.clone()
   return out
+
+
+def _launcher(device, n):
+  key = (device.index, n)
+  launcher = _launchers.get(key)
+  if launcher is None:
+    launcher = _launchers[key] = FusedLauncher(device, n)
+  return launcher
+
+
+def _aggregate_centered_clipping(spec, G, return_details, center):
+  """`aggregate` for centered clipping: the sm_90a kernel for fp32 and n <= 32, the torch reference on the device otherwise."""
+  from ..aggregators import _ops
+  n, d = G.shape
+  if center is None or center.shape != (d,) or center.device != G.device:
+    raise tools.UserException("Centered clipping needs a [%d] center on %s" % (d, G.device))
+  if G.dtype == torch.float64 or n > MAX_WORKERS:
+    if center.dtype != G.dtype:
+      raise tools.UserException("Centered clipping needs a center of type %s (got %s)" % (G.dtype, center.dtype))
+    if return_details:
+      raise tools.UserException("Centered clipping returns its details from the sm_90a kernel only (fp32, n <= %d)" % MAX_WORKERS)
+    return _ops.torch_centered_clipping(G, spec.iterations, spec.tau, center)
+  if G.dtype != torch.float32 or center.dtype != torch.float32:
+    raise tools.UserException("Centered clipping on the device needs fp32 rows and center (got %s, %s)" % (G.dtype, center.dtype))
+  G = G.contiguous()
+  pad = (-d) % 4
+  if pad or G.data_ptr() % 16:
+    Gp = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
+    Gp[:, :d] = G
+    G = Gp
+  dp = d + pad
+  work = center
+  if pad or not center.is_contiguous() or center.data_ptr() % 16:
+    work = torch.zeros(dp, dtype=torch.float32, device=G.device)
+    work[:d] = center
+  launcher = _launcher(G.device, n)
+  out = torch.empty(dp, dtype=torch.float32, device=G.device)
+  rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
+  launcher.launch(spec, rows, 0, dp, agg_out=out, center=work)
+  if work is not center:
+    center.copy_(work[:d])
+  out = out[:d]
+  if return_details:
+    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n)
+    return out, dist.clone(), launcher.info.clone()
+  return out
+
+
+def worker_momentum_(G, M, beta, c):
+  """Worker momentum on the [w, d] rows `G` and momenta `M`, in place: M <- beta * M + c * G, then G <- M, one rounding per operation.
+  CUDA fp32 tensors run the sm_90a kernel (one launch for the w rows; G's rows may be strided); others the torch reference."""
+  from ..aggregators import _ops
+  if G.dim() != 2 or G.shape != M.shape:
+    raise tools.UserException("Worker momentum needs [w, d] rows and momenta of the same shape (got %s, %s)" % (tuple(G.shape), tuple(M.shape)))
+  if not G.is_cuda or G.dtype != torch.float32:
+    return _ops.torch_worker_momentum_(G, M, beta, c)
+  if M.dtype != torch.float32 or M.device != G.device:
+    raise tools.UserException("Worker momentum needs fp32 momenta on the rows' device (got %s on %s)" % (M.dtype, M.device))
+  w, d = G.shape
+  if d > 1 and (G.stride(1) != 1 or M.stride(1) != 1):
+    raise tools.UserException("Worker momentum needs rows with contiguous elements")
+  func = _lib().agb_worker_momentum
+  with torch.cuda.device(G.device):
+    _check(func(ctypes.c_void_p(G.data_ptr()), ctypes.c_longlong(G.stride(0) if w > 1 else d), ctypes.c_void_p(M.data_ptr()),
+                ctypes.c_longlong(M.stride(0) if w > 1 else d), ctypes.c_longlong(w), ctypes.c_longlong(d), ctypes.c_float(beta), ctypes.c_float(c),
+                _stream_ptr()), "worker_momentum")
+  return G
 
 
 def craft(rows, segments, honest, byzantine, mode, coef, *, R=1, rank=0, signals=None, epoch=1, epoch_ptr=None, stream=None):

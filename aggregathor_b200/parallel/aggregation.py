@@ -16,6 +16,7 @@ Three interchangeable engines share one interface (`params`, `grads`, `step()`):
 Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always sees n rows.
 Every engine also has `craft_byzantine(byz_slots, mode, coef)`, the omniscient attacks (`attacks/omniscient.py`): the rows at the
 given slots of the gathered matrix are overwritten with the ALIE / IPM row of the others, on every rank (a collective call).
+Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
 """
 
 import os
@@ -50,21 +51,40 @@ class _AggregationBase:
     self.d = layout.padded_size
     self.updates = 0  # number of optimizer updates applied so far
     self.slots = []
+    self.center = None   # centered clipping: the rule's center v, [d] fp32
+
+  def _make_center(self):
+    """Allocate the center (+0) when the rule is centered clipping; it lives as long as the engine and travels in checkpoints."""
+    spec = self.gar.fused_spec()
+    if spec is not None and spec.rule == "centered-clipping":
+      self.center = torch.zeros(self.d, dtype=torch.float32, device=self.device)
 
   @property
   def first_worker(self):
     return self.rank * self.w
 
   def state_dict(self):
-    return {"updates": self.updates, "slots": [s.detach().to("cpu", copy=True) for s in self.full_slots()]}
+    state = {"updates": self.updates, "slots": [s.detach().to("cpu", copy=True) for s in self.full_slots()]}
+    if self.center is not None:
+      state["rule_state"] = self.full_center().detach().to("cpu", copy=True)
+    return state
 
   def load_state_dict(self, state):
     self.updates = int(state["updates"])
     for mine, saved in zip(self.slots, state["slots"]):
       mine.copy_(saved.to(mine.device))
+    if self.center is not None:
+      if state.get("rule_state") is not None:
+        self.center.copy_(state["rule_state"].to(self.center.device))
+      else:
+        tools.warning("The checkpoint holds no center for centered clipping: it starts from zero", context="restore")
+        self.center.zero_()
 
   def full_slots(self):
     return self.slots
+
+  def full_center(self):
+    return self.center
 
   # -- authentication hooks (`parallel/signing.py`) --------------------------------- #
   def visible_rows(self):
@@ -92,6 +112,7 @@ class HostAggregation(_AggregationBase):
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
     self.slots = optimizer.make_slots(self.params)
+    self._make_center()
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -109,7 +130,7 @@ class HostAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
-    aggregated = self.gar.aggregate(self._gathered)
+    aggregated = self.gar.aggregate(self._gathered) if self.center is None else self.gar.aggregate(self._gathered, center=self.center)
     self.updates += 1
     self.optimizer.apply_torch(self.params, aggregated, self.slots, rate, self.updates)
     self.last_aggregate = aggregated
@@ -127,6 +148,7 @@ class BaselineAggregation(_AggregationBase):
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
     self.slots = optimizer.make_slots(self.params)
+    self._make_center()
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -143,10 +165,11 @@ class BaselineAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
+    state = {} if self.center is None else {"center": self.center}
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
-      aggregated = gar_ops.aggregate(self.spec, self._gathered)
+      aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)
     else:
-      aggregated = self.gar.aggregate(self._gathered)
+      aggregated = self.gar.aggregate(self._gathered, **state)
     self.updates += 1
     if self.optimizer.name == "sgd":
       gar_ops.sgd_(self.params, aggregated, rate)
@@ -193,11 +216,12 @@ class FusedAggregation(_AggregationBase):
     self.params = self.heap.local("params", torch.float32)
     self.params_bf16 = self.heap.local("params_bf16", torch.bfloat16) if bf16_copy else None
     self.slots = optimizer.make_slots(self.params)
+    self._make_center()   # centered clipping: maintained on the owned segments only, like the optimizer slots
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
-    # the geometric median's passes after the first re-read the staged copy rather than the peers' rows
-    need_staging = (self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule == "geometric-median" and R > 1)
+    # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows
+    need_staging = (self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
     self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     self.max_ctas = max_ctas
@@ -305,24 +329,31 @@ class FusedAggregation(_AggregationBase):
     self._prepared = False
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
-                         loss_in=loss_in, loss_out=self.loss_out, **self._common(self._rate_args))
+                         loss_in=loss_in, loss_out=self.loss_out, center=self.center, **self._common(self._rate_args))
+
+  def _assemble(self, vector):
+    """Full copy of a [d] vector maintained on the owned segments only (collective when R > 1)."""
+    if self.world == 1:
+      return vector
+    merged = vector.clone()
+    for q in range(self.world):
+      for lo, hi in self.segments_of[q]:
+        if hi == lo:
+          continue
+        piece = merged[lo:hi].contiguous() if q == self.rank else torch.empty(hi - lo, dtype=vector.dtype, device=vector.device)
+        dist.broadcast(piece, src=dist.get_global_rank(self.group, q) if self.group is not None else q, group=self.group)
+        merged[lo:hi] = piece
+    return merged
 
   def full_slots(self):
     """Optimizer slots are only maintained on the owned segments: assemble the full vectors (checkpoints)."""
     if self.world == 1 or not self.slots:
       return self.slots
-    full = []
-    for slot in self.slots:
-      merged = slot.clone()
-      for q in range(self.world):
-        for lo, hi in self.segments_of[q]:
-          if hi == lo:
-            continue
-          piece = merged[lo:hi].contiguous() if q == self.rank else torch.empty(hi - lo, dtype=slot.dtype, device=slot.device)
-          dist.broadcast(piece, src=dist.get_global_rank(self.group, q) if self.group is not None else q, group=self.group)
-          merged[lo:hi] = piece
-      full.append(merged)
-    return full
+    return [self._assemble(slot) for slot in self.slots]
+
+  def full_center(self):
+    """The center of centered clipping, assembled from the owned segments of every rank (checkpoints)."""
+    return None if self.center is None else self._assemble(self.center)
 
 
 def _single_host(group=None):

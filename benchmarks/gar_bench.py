@@ -12,7 +12,9 @@ fraction of the peer-copy rate measured at start-up; writes JSON to <--gar-out>/
 the crafting kernel is also timed alone, next to the torch reference on the same device, with the (H + k) * d * 4 bytes it must move.
 `--gar-dump-rows` then saves, from the last rank, every row the fused engine aggregated (honest and crafted, all d coordinates).
 `--gar-rule-args key:value ...` passes the same `--aggregator-args` to every rule (rules ignore keys they do not use). The
-`geometric-median` entry also reports its T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
+`geometric-median` and `centered-clipping` entries also report their T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
+`--gar-worker-momentum beta` also times the worker-momentum kernel alone on the [w, d] rows of a rank (`ops.gar.worker_momentum_`,
+dampening 0), with the 16 * w * d bytes it must move (G and M read and written once).
 """
 
 import argparse
@@ -46,6 +48,8 @@ def main():
   parser.add_argument("--gar-dump-rows", dest="dump_rows", action="store_true", help="with --gar-attack: save the last rank's view of every row to <--gar-out>")
   parser.add_argument("--gar-rule-args", dest="rule_args", nargs="*", default=None, metavar="KEY:VALUE",
                       help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
+  parser.add_argument("--gar-worker-momentum", dest="worker_momentum", type=float, default=None, metavar="BETA",
+                      help="also time the worker-momentum kernel with this beta on the [w, d] rows of a rank")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -248,19 +252,45 @@ def main():
     results[rule].update(attack_entry)
     if args.rule_args is not None:
       results[rule]["rule_args"] = args.rule_args
-    if rule == "geometric-median":
+    if rule in ("geometric-median", "centered-clipping"):
       # T + 1 passes, each reading the n rows of the owned coordinates once (the first from the peers, the others from the staged copy)
       spec = gar.fused_spec()
       passes_bytes = (spec.iterations + 1) * n * slice_bytes
-      results[rule].update({"iterations": spec.iterations, "nu": spec.nu, "pass_bytes": passes_bytes, "pass_gbs": passes_bytes / fused_ms / 1e6})
+      radius = {"nu": spec.nu} if rule == "geometric-median" else {"tau": spec.tau}
+      results[rule].update({"iterations": spec.iterations, **radius, "pass_bytes": passes_bytes, "pass_gbs": passes_bytes / fused_ms / 1e6})
     if rank == 0:
       print(rule, json.dumps(results[rule]))
     del fused, base
     torch.cuda.empty_cache()
+  report = {"world": world, "n": n, "d": args.d, "results": results}
+  if args.worker_momentum is not None:
+    beta, c = _ops.check_worker_momentum(args.worker_momentum, 0.0)
+    rows = torch.randn((w, d), device=device)
+    momenta = torch.zeros((w, d), device=device)
+    for _ in range(3):
+      gar_ops.worker_momentum_(rows, momenta, beta, c)
+    torch.cuda.synchronize()
+    if world > 1:
+      dist.barrier()
+    begin, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    begin.record()
+    for _ in range(args.iters):
+      gar_ops.worker_momentum_(rows, momenta, beta, c)
+    end.record()
+    torch.cuda.synchronize()
+    ms = torch.tensor([begin.elapsed_time(end) / args.iters], device=device, dtype=torch.float64)
+    if world > 1:
+      dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+    momentum_bytes = 16 * w * d   # G and M of every element read and written once
+    report["worker_momentum"] = {"beta": beta, "w": w, "d": d, "ms": float(ms.item()), "bytes": momentum_bytes,
+                                 "gbs": momentum_bytes / float(ms.item()) / 1e6}
+    if rank == 0:
+      print("worker-momentum", json.dumps(report["worker_momentum"]))
+    del rows, momenta
   if rank == 0:
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "gar_bench_%d.json" % world), "w") as fd:
-      json.dump({"world": world, "n": n, "d": args.d, "results": results}, fd, indent=1)
+      json.dump(report, fd, indent=1)
   if world > 1:
     dist.barrier()
     dist.destroy_process_group()
