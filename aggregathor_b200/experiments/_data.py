@@ -208,6 +208,15 @@ def _guarded(producer):
   return run
 
 
+def _stop_producer(self):
+  """Stops the producer thread and waits for it (it checks `_stop` at least every 0.1 s): a daemon thread still inside torch when
+  the interpreter exits is torn down mid-call, which aborts the process."""
+  self._stop = True
+  thread = self._thread
+  if thread is not None and thread is not threading.current_thread():
+    thread.join(timeout=30)
+
+
 def _take(self):
   item = self._queue.get()
   if item is None:
@@ -305,7 +314,7 @@ class BatchStream:
     return (x, y) if self.transform is None else self.transform(x, y)
 
   def close(self):
-    self._stop = True
+    _stop_producer(self)
 
 
 class GroupedBatches(list):
@@ -390,7 +399,7 @@ class StreamGroup:
     return batches
 
   def close(self):
-    self._stop = True
+    _stop_producer(self)
 
 
 class ShardStream(BatchStream):

@@ -78,6 +78,32 @@ __device__ __forceinline__ void tma_load_4d(void* dst, CUtensorMap const* map, u
                  :: "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
+// Shared -> global tensor stores and fp32 add-reductions (bulk async-group completion, tracked per issuing thread). The box lands
+// where the map says; coordinates outside the map's extents are clipped, so partial tiles need no bounds tests.
+template<bool kReduce> __device__ __forceinline__ void tma_store_4d(CUtensorMap const* map, void const* src, int c0, int c1, int c2, int c3) {
+    if constexpr (kReduce)
+        asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                     :: "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+    else
+        asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                     :: "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() {
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+// All but the `kPending` most recent bulk groups of this thread have finished READING shared memory (their buffers may be rewritten).
+template<int kPending> __device__ __forceinline__ void bulk_wait_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(kPending) : "memory");
+}
+// Every bulk group of this thread is complete, its global writes included.
+__device__ __forceinline__ void bulk_wait_all() {
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+// Generic-proxy writes to shared memory become visible to the async proxy (TMA) of this CTA.
+__device__ __forceinline__ void fence_proxy_async_smem() {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
 // ---- wgmma (warpgroup MMA: 4 consecutive warps, the first one's index a multiple of 4) ---------------- //
 // Operands from shared-memory descriptors, fp32 accumulators in registers. Fragment of an m64nN accumulator held by thread
 // t of the warpgroup: d[4 j + 2 i + c] = D[16 (t / 32) + (t % 32) / 4 + 8 i][8 j + 2 (t % 4) + c]  (j < N / 8, i, c in {0, 1}).

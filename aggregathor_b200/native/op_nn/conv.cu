@@ -33,7 +33,31 @@ struct ConvParams {
     int bw, bh, bn;         // pixel box of one M tile (fwd/dgrad: product <= 128) or one K block (wgrad: product <= 64)
     int tiles_w, tiles_h, tiles_n;
     int groups, images_per_group;   // wgrad of several logical workers: K ranges = image ranges, one output per group
+    int sbw, sbh, sbn;      // staged epilogue of fwd / dgrad: one warp's 16 rows as a sub-box of the pixel box
 };
+
+// The 16 consecutive rows (w fastest, then h, then n) of a warp's slab form a sub-box sbw x sbh x sbn of every bw x bh x bn pixel
+// box when the widths nest: 8x8x2 -> 8x2x1, 4x4x8 -> 4x4x1, 2x2x32 -> 2x2x4. The 7x1x16 box of the 7x7 maps does not nest.
+bool slab_box(int bw, int bh, int bn, int& sbw, int& sbh, int& sbn) {
+    if ((bw * bh * bn) % 16)
+        return false;
+    if (bw >= 16) {
+        sbw = 16; sbh = 1; sbn = 1;
+        return bw % 16 == 0;
+    }
+    if (16 % bw)
+        return false;
+    sbw = bw;
+    int const lines = 16 / bw;
+    if (bh >= lines) {
+        sbh = lines; sbn = 1;
+        return bh % lines == 0;
+    }
+    if (lines % bh)
+        return false;
+    sbh = bh; sbn = lines / bh;
+    return bn % sbn == 0;
+}
 
 enum ConvMode { kFwd = 0, kDgrad = 1, kWgrad = 2 };
 
@@ -53,12 +77,12 @@ inline int make_tmap_4d(CUtensorMap* map, void const* base, int C, int W, int H,
 // the 4-D map of x (wgrad).
 template<int BN, int MODE, typename E = ElemBF16>
 __global__ void __launch_bounds__(kThreads, 1) conv_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                                                                    GemmParams const p, ConvParams const cp, int items_mn, int splits) {
+                                                                    const __grid_constant__ CUtensorMap tmap_c, GemmParams const p, ConvParams const cp, int items_mn, int splits) {
     constexpr bool A_MN = MODE == kWgrad, B_MN = MODE != kFwd;
     using Cfg = Config<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kRingBytes + kStagingBytes);
     uint64_t* empty = full + Cfg::kStages;
 
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -89,6 +113,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_sm90_kernel(const __grid_con
         }
         mbar_fence_init();
     }
+    if (p.staged && warp == 0 && lane == 0)
+        tma_prefetch_desc(&tmap_c);
     __syncthreads();
     pdl_trigger();   // set-up done: the next kernel may start its own; ...
     pdl_wait();      // ... our inputs are complete only once the previous kernel has finished
@@ -198,11 +224,26 @@ __global__ void __launch_bounds__(kThreads, 1) conv_sm90_kernel(const __grid_con
         return;
     }
     consumer_registers();
-    uint32_t ring = 0;
+    uint32_t ring = 0, issued = 0;
+    uint8_t* staging = smem + Cfg::kRingBytes + warp * 2 * kPieceBytes;
     float acc[BN / 2];
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
         Item const it = decode(item);
         mainloop<BN, A_MN, B_MN, E>(smem, full, empty, ring, it.nkb, warp, acc);
+        if (p.staged) {
+            if (MODE == kWgrad) {   // output map (Cin, taps, Cout, groups)
+                epilogue_staged<BN>(p, &tmap_c, acc, staging, issued, it.n0, [&](int col, int (&c)[4]) {
+                    c[0] = col; c[1] = it.tap; c[2] = it.m0 + 16 * warp; c[3] = it.group;
+                });
+            } else if (16 * warp < box_rows) {   // output map (C, W, H, N) of y / dx; the slab is a sbw x sbh x sbn sub-box
+                int const r = 16 * warp;
+                int const bi_w = r % cp.bw, bi_h = (r / cp.bw) % cp.bh, bi_n = r / (cp.bw * cp.bh);
+                epilogue_staged<BN>(p, &tmap_c, acc, staging, issued, it.n0, [&](int col, int (&c)[4]) {
+                    c[0] = col; c[1] = it.pw + bi_w; c[2] = it.ph + bi_h; c[3] = it.pn + bi_n;
+                });
+            }
+            continue;
+        }
         epilogue_slab<BN>(p, acc, 16 * warp, it.n0, [&](int r, bool& valid, long long& offset) {
             if (MODE == kWgrad) {   // row = output channel; columns = (tap, ci) inside dW[Cout][k*k*Cin]
                 int const co = it.m0 + r;
@@ -219,11 +260,41 @@ __global__ void __launch_bounds__(kThreads, 1) conv_sm90_kernel(const __grid_con
             }
         });
     }
+    if (p.staged && lane == 0)
+        bulk_wait_all();   // outputs complete (and staging read) before the CTA retires: PDL dependents and graph replays see them
+}
+
+// Output map of the staged epilogue; false leaves the register epilogue in charge: the strided data gradient (its rows scatter to
+// one pixel parity of dx), pixel boxes whose 16-row slabs are not sub-boxes (7x1x16), outputs TMA cannot address.
+template<int MODE>
+bool conv_out_map(CUtensorMap* map, GemmParams const& p, ConvParams& cp) {
+    if (MODE == kWgrad) {   // dW[group][Cout][taps][Cin]
+        uint64_t const taps = static_cast<uint64_t>(cp.k) * cp.k, groups = cp.groups > 1 ? cp.groups : 1;
+        uint64_t const gstride = groups > 1 ? static_cast<uint64_t>(p.c_group_stride) : static_cast<uint64_t>(p.ldc) * cp.Cout;
+        uint64_t const dims[4] = {static_cast<uint64_t>(cp.Cin), taps, static_cast<uint64_t>(cp.Cout), groups};
+        uint64_t const strides[3] = {static_cast<uint64_t>(cp.Cin), static_cast<uint64_t>(p.ldc), gstride};
+        uint32_t const box[3] = {1, 16, 1};
+        return make_tmap_out(map, p.C, p.out_fp32, dims, strides, box);
+    }
+    if (MODE == kDgrad && cp.stride > 1)
+        return false;
+    if (!slab_box(cp.bw, cp.bh, cp.bn, cp.sbw, cp.sbh, cp.sbn))
+        return false;
+    int const C = MODE == kFwd ? cp.Cout : cp.Cin, W = MODE == kFwd ? cp.OW : cp.W, H = MODE == kFwd ? cp.OH : cp.H;   // y or dx, NHWC
+    uint64_t const dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(W), static_cast<uint64_t>(H), static_cast<uint64_t>(cp.N)};
+    uint64_t const strides[3] = {static_cast<uint64_t>(C), static_cast<uint64_t>(W) * C, static_cast<uint64_t>(H) * W * C};
+    uint32_t const box[3] = {static_cast<uint32_t>(cp.sbw), static_cast<uint32_t>(cp.sbh), static_cast<uint32_t>(cp.sbn)};
+    return make_tmap_out(map, p.C, p.out_fp32, dims, strides, box);
 }
 
 template<int BN, int MODE, typename E = ElemBF16>
-int launch_conv(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& p, ConvParams const& cp, int items_mn, int splits, cudaStream_t stream) {
+int launch_conv(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& params, ConvParams const& conv, int items_mn, int splits, cudaStream_t stream) {
     using Cfg = Config<BN>;
+    GemmParams p = params;
+    ConvParams cp = conv;
+    CUtensorMap tc;
+    std::memset(&tc, 0, sizeof(tc));
+    p.staged = agb_gemm_epilogue_staged() && conv_out_map<MODE>(&tc, p, cp);
     auto kernel = conv_sm90_kernel<BN, MODE, E>;
     static bool configured = false;
     if (!configured) {
@@ -233,7 +304,7 @@ int launch_conv(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& 
     int const sms = sm_count();
     long long const items = static_cast<long long>(items_mn) * splits * ((MODE == kWgrad && cp.groups > 1) ? cp.groups : 1);
     int const grid = static_cast<int>(items < sms ? items : sms);
-    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, p, cp, items_mn, splits));
+    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, tc, p, cp, items_mn, splits));
     return 0;
 }
 

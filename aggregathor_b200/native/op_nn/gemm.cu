@@ -22,6 +22,25 @@ int agb_gemm_set_persistent(int enabled) {
     return 0;
 }
 
+// Epilogue of the GEMM and implicit-convolution kernels. 1 = staged (default): each warp converts its slab into shared memory and
+// TMA stores (or, for split-K, add-reduces) it, wherever a tensor map can address the output; 0 = stores straight from registers.
+// AGB_GEMM_EPILOGUE=staged|regs sets the initial value. Both give bit-identical outputs (split-K sums aside, whose order varies anyway).
+static int g_epilogue = -1;
+int agb_gemm_set_epilogue(int staged) {
+    g_epilogue = staged ? 1 : 0;
+    return 0;
+}
+int agb_gemm_epilogue_staged() {
+    if (g_epilogue < 0) {
+        char const* env = std::getenv("AGB_GEMM_EPILOGUE");
+        bool const regs = env && std::strcmp(env, "regs") == 0;
+        if (env && *env && !regs && std::strcmp(env, "staged") != 0)
+            std::fprintf(stderr, "[agb] AGB_GEMM_EPILOGUE=%s: expected 'staged' or 'regs', using 'staged'\n", env);
+        g_epilogue = regs ? 0 : 1;
+    }
+    return g_epilogue;
+}
+
 // C[M,N] = op(A) op(B)  (+bias, ReLU). bf16 operands:
 //   a_mn == 0: A is [M rows][K] with row stride lda      a_mn == 1: A is [K rows][M] with row stride lda
 //   b_mn == 0: B is [N rows][K] with row stride ldb      b_mn == 1: B is [K rows][N] with row stride ldb

@@ -11,7 +11,8 @@
 //   warps 0-7   two consumer warpgroups, each owning 64 rows of the tile and all BN columns. bf16: wgmma m64 x BN x k16 straight
 //               from the swizzled ring (shared-memory descriptors; MN-major operands through the transpose bits). TF32: wgmma reads
 //               32-bit operands K-major only, so every warp issues m16n8k8 mma.sync on fragments it loads from the ring (same
-//               accumulator layout). The epilogue (+ bias, ReLU, convert, store, or fp32 red.add for split-K) stores from registers.
+//               accumulator layout). The epilogue (+ bias, ReLU, convert) goes through per-warp shared buffers and TMA stores, or
+//               fp32 TMA add-reductions for split-K (epilogue_staged); what no tensor map can address is stored from registers.
 //   warps 8-11  producer warpgroup: one lane issues the cp.async.bulk.tensor tiles (128B swizzle) into a kStages-deep smem ring,
 //               completion signalled on `full` mbarriers (complete_tx::bytes); every consumer warp arrives on `empty` once its MMAs
 //               have read a slot. The producer hands its registers to the consumers (setmaxnreg): a 64 x 256 fp32 accumulator is
@@ -29,6 +30,10 @@
 
 using namespace agb;
 using namespace agb::sm90;
+
+// AGB_GEMM_EPILOGUE / agb_gemm_set_epilogue (gemm.cu): 1 = staged epilogue where TMA can address the output (default), 0 = register
+// stores everywhere.
+extern "C" int agb_gemm_epilogue_staged();
 
 namespace {
 
@@ -53,12 +58,17 @@ struct ElemTF32 {
     static constexpr bool kTf32 = true;
 };
 
+// Staged epilogue: every consumer warp owns two 16-row x 128-byte pieces of shared memory (64 bf16 or 32 fp32 columns of its slab).
+constexpr uint32_t kPieceBytes = 16 * 128;
+constexpr uint32_t kStagingBytes = kConsumerWarps * 2 * kPieceBytes;   // 32 KB
+
 template<int BN> struct Config {
     static constexpr uint32_t kABytes = kBM * 128;   // 128 rows x 128 bytes of K (either element type)
     static constexpr uint32_t kBBytes = BN * 128;
     static constexpr uint32_t kStageBytes = kABytes + kBBytes;
     static constexpr int kStages = (192 * 1024) / kStageBytes;   // 8 / 6 / 4 stages for BN = 64 / 128 / 256: 192 KB of the 227 KB
-    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 256 /* barriers */;
+    static constexpr uint32_t kRingBytes = kStages * kStageBytes;   // staging buffers follow the ring (1024-byte aligned), then the barriers
+    static constexpr uint32_t kSmemBytes = kRingBytes + kStagingBytes + 1024 /* alignment slack */ + 256 /* barriers */;
 };
 
 // Register split between the producer warpgroup and the two consumer warpgroups (3 x 128 threads, 64 K registers).
@@ -80,7 +90,99 @@ struct GemmParams {
     int kblocks_per_split;
     int groups;              // grouped weight gradients: independent K ranges (one per logical worker) ...
     long long c_group_stride; // ... each accumulating into C + group * c_group_stride
+    int staged;              // 1: epilogue through shared memory and TMA stores / reductions (the output tensor map), 0: from registers
 };
+
+// 4-D tensor map over the epilogue output, 128-byte swizzle, box = one warp's piece: 128 bytes of columns x `box` (16 rows in all)
+// along dims 1..3. Returns 0 (and leaves the register epilogue in charge) when TMA cannot address C: base or a stride not a
+// multiple of 16 bytes.
+inline bool make_tmap_out(CUtensorMap* map, void const* base, bool fp32, uint64_t const (&dims)[4], uint64_t const (&strides)[3], uint32_t const (&box)[3]) {
+    uint64_t const e = fp32 ? 4 : 2;
+    if (reinterpret_cast<uintptr_t>(base) & 15)
+        return false;
+    cuuint64_t d[4], s[3];
+    for (int i = 0; i < 4; ++i)
+        d[i] = dims[i];
+    for (int i = 0; i < 3; ++i) {
+        s[i] = strides[i] * e;
+        if ((s[i] & 15) || s[i] == 0 || s[i] >= (1ull << 40))
+            return false;
+    }
+    cuuint32_t b[4] = {static_cast<cuuint32_t>(128 / e), box[0], box[1], box[2]};
+    cuuint32_t elem[4] = {1, 1, 1, 1};
+    return encode_cached(map, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, d, s, b, elem) == 0;
+}
+
+// Staged epilogue of one warp's 16 x BN slab: for every 128-byte column piece, the same bias / ReLU / rounding as epilogue_slab into
+// a 128B-swizzled shared buffer (conflict-free for bf16), then one lane issues a TMA store (or fp32 add-reduction for split-K) of the
+// 16-row box whose coordinates `coords(col, c)` gives. The two buffers of a warp alternate; a buffer is rewritten only once the bulk
+// group that read it has finished reading (`issued` counts this warp's pieces across work items). Rows past M and columns past N
+// are clipped by the map.
+template<int BN, bool kFp32, bool kReduce, typename CoordFn>
+__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords) {
+    constexpr int kCols = kFp32 ? 32 : 64;
+    int const lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int q = 0; q < BN / kCols; ++q) {
+        int const col0 = n0 + q * kCols;
+        if (col0 >= p.N)
+            break;
+        uint8_t* buf = staging + (issued & 1) * kPieceBytes;
+        if (lane == 0)
+            bulk_wait_read<1>();
+        __syncwarp();
+#pragma unroll
+        for (int jj = 0; jj < kCols / 8; ++jj) {
+            int const j = q * (kCols / 8) + jj;
+            int const col = col0 + 8 * jj + 2 * t;
+            float b0 = 0.f, b1 = 0.f;
+            if (p.bias) {
+                if (col < p.N)
+                    b0 = __ldg(p.bias + col);
+                if (col + 1 < p.N)
+                    b1 = __ldg(p.bias + col + 1);
+            }
+            uint32_t const byte = (8 * jj + 2 * t) * (kFp32 ? 4 : 2);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                int const row = g + 8 * i;
+                float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+                if (p.bias) {
+                    v0 += b0;
+                    v1 += b1;
+                }
+                if (p.relu) {
+                    v0 = fmaxf(v0, 0.f);
+                    v1 = fmaxf(v1, 0.f);
+                }
+                uint8_t* dst = buf + row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15);
+                if constexpr (kFp32)
+                    *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+                else
+                    *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+            }
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+            int c[4];
+            coords(col0, c);
+            tma_store_4d<kReduce>(tmap_c, buf, c[0], c[1], c[2], c[3]);
+            bulk_commit();
+        }
+        ++issued;
+    }
+}
+
+template<int BN, typename CoordFn>
+__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords) {
+    if (!p.out_fp32)
+        epilogue_staged<BN, false, false>(p, tmap_c, acc, staging, issued, n0, coords);
+    else if (p.atomic)
+        epilogue_staged<BN, true, true>(p, tmap_c, acc, staging, issued, n0, coords);
+    else
+        epilogue_staged<BN, true, false>(p, tmap_c, acc, staging, issued, n0, coords);
+}
 
 // Epilogue of one warp's 16 x BN slab of the accumulator (fragment layout: agb_sm90.cuh). `row_at(r, valid, offset)` tells whether
 // tile row r is a real output row and the element offset of that row in C (lets implicit-GEMM convolutions scatter pixel-box rows to
@@ -247,11 +349,12 @@ __device__ __forceinline__ void produce_stage(CUtensorMap const* tmap_a, CUtenso
 }
 
 template<int BN, bool A_MN, bool B_MN, typename E = ElemBF16>
-__global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, GemmParams const p, int m_tiles, int n_tiles, int splits) {
+__global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                                                 const __grid_constant__ CUtensorMap tmap_c, GemmParams const p, int m_tiles, int n_tiles, int splits) {
     using Cfg = Config<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kRingBytes + kStagingBytes);
     uint64_t* empty = full + Cfg::kStages;
 
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -267,6 +370,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         }
         mbar_fence_init();
     }
+    if (p.staged && warp == 0 && lane == 0)
+        tma_prefetch_desc(&tmap_c);
     __syncthreads();
     pdl_trigger();   // set-up done: the next kernel may start its own; ...
     pdl_wait();      // ... our inputs are complete only once the previous kernel has finished
@@ -308,29 +413,52 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         return;
     }
     consumer_registers();
-    uint32_t ring = 0;
+    uint32_t ring = 0, issued = 0;
+    uint8_t* staging = smem + Cfg::kRingBytes + warp * 2 * kPieceBytes;
     float acc[BN / 2];
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
         int m0, n0, kb_begin, nkb, group;
         decode(item, m0, n0, kb_begin, nkb, group);
         mainloop<BN, A_MN, B_MN, E>(smem, full, empty, ring, nkb, warp, acc);
+        if (p.staged) {   // output map (N, M, groups, 1)
+            epilogue_staged<BN>(p, &tmap_c, acc, staging, issued, n0, [&](int col, int (&c)[4]) {
+                c[0] = col; c[1] = m0 + 16 * warp; c[2] = group; c[3] = 0;
+            });
+            continue;
+        }
         epilogue_slab<BN>(p, acc, 16 * warp, n0, [&](int r, bool& valid, long long& offset) {
             int const row = m0 + r;
             valid = row < p.M;
             offset = static_cast<long long>(row) * p.ldc + group * p.c_group_stride;
         });
     }
+    if (p.staged && lane == 0)
+        bulk_wait_all();   // outputs complete (and staging read) before the CTA retires: PDL dependents and graph replays see them
+}
+
+// Output map of a plain / grouped product: C viewed as (N, M, groups, 1), box 128 bytes x 16 rows. False: TMA cannot address it.
+inline bool gemm_out_map(CUtensorMap* map, GemmParams const& p) {
+    uint64_t const groups = p.groups > 1 ? p.groups : 1;
+    uint64_t const gstride = groups > 1 ? static_cast<uint64_t>(p.c_group_stride) : static_cast<uint64_t>(p.ldc) * p.M;
+    uint64_t const dims[4] = {static_cast<uint64_t>(p.N), static_cast<uint64_t>(p.M), groups, 1};
+    uint64_t const strides[3] = {static_cast<uint64_t>(p.ldc), gstride, gstride * groups};
+    uint32_t const box[3] = {16, 1, 1};
+    return p.ldc >= p.N && make_tmap_out(map, p.C, p.out_fp32, dims, strides, box);
 }
 
 static int g_persistent = -1;   // -1: read AGB_GEMM_PERSISTENT at first use
 
 template<int BN, bool A_MN, bool B_MN, typename E = ElemBF16>
-int launch_gemm(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& p, int splits, cudaStream_t stream) {
+int launch_gemm(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& params, int splits, cudaStream_t stream) {
     using Cfg = Config<BN>;
     if (g_persistent < 0) {
         char const* env = std::getenv("AGB_GEMM_PERSISTENT");
         g_persistent = env ? std::atoi(env) : 1;
     }
+    GemmParams p = params;
+    CUtensorMap tc;
+    std::memset(&tc, 0, sizeof(tc));
+    p.staged = agb_gemm_epilogue_staged() && gemm_out_map(&tc, p);
     int const m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + BN - 1) / BN;
     auto kernel = gemm_sm90_kernel<BN, A_MN, B_MN, E>;
     static bool configured = false;
@@ -342,7 +470,7 @@ int launch_gemm(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& 
     long long const items = static_cast<long long>(m_tiles) * n_tiles * splits * (p.groups > 1 ? p.groups : 1);
     long long const cap = g_persistent ? sm_count() : 0x7fffffffll;
     int const grid = static_cast<int>(items < cap ? items : cap);
-    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, p, m_tiles, n_tiles, splits));
+    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, tc, p, m_tiles, n_tiles, splits));
     return 0;
 }
 

@@ -148,6 +148,14 @@ def set_gemm_persistent(enabled):
   _lib().agb_gemm_set_persistent(ctypes.c_int(1 if enabled else 0))
 
 
+def set_gemm_epilogue(mode):
+  """GEMM / implicit-convolution epilogue: "staged" (shared memory + TMA stores where TMA can address the output; the default,
+  also `AGB_GEMM_EPILOGUE`) or "regs" (stores straight from the accumulator registers). Outputs are bit-identical."""
+  if mode not in ("staged", "regs"):
+    raise ValueError("GEMM epilogue must be 'staged' or 'regs', got %r" % (mode,))
+  _lib().agb_gemm_set_epilogue(ctypes.c_int(1 if mode == "staged" else 0))
+
+
 def alloc_out(m, n, dtype, device):
   """[m, n] view of a buffer whose row stride is a multiple of 8 elements (so it can feed the next GEMM through TMA)."""
   ld = (n + 7) // 8 * 8
