@@ -27,21 +27,39 @@ class FusedSpec:
   RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
            "centered-clipping")
 
-  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0):
+  RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping")   # the others ignore f
+  MIXES = (None, "nnm")
+
+  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None):
     """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing, `iterations` and `tau` centered
-    clipping's iterations and clipping radius; the other rules ignore them."""
+    clipping's iterations and clipping radius; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
+    rule: None, or "nnm" (nearest-neighbour mixing with the same f)."""
     if rule not in self.RULES:
       raise tools.UserException("Unknown fused rule " + repr(rule))
+    if mix not in self.MIXES:
+      raise tools.UserException("Unknown pre-aggregation " + repr(mix))
     self.rule, self.n, self.f, self.m, self.beta = rule, int(n), int(f), int(m), int(beta)
     self.iterations, self.nu, self.tau = int(iterations), float(nu), float(tau)
+    self.mix = mix
 
   @property
   def rule_id(self):
     return self.RULES.index(self.rule)
 
+  @property
+  def mix_id(self):
+    return self.MIXES.index(self.mix)
+
+  def with_mix(self, mix, f=None):
+    """The same rule with pre-aggregation `mix` (None or "nnm"), and declared f `f` (default: unchanged)."""
+    return FusedSpec(self.rule, self.n, self.f if f is None else f, self.m, self.beta, iterations=self.iterations, nu=self.nu, tau=self.tau,
+                     mix=mix)
+
   def __repr__(self):
     extra = {"geometric-median": ", iterations=%d, nu=%r" % (self.iterations, self.nu),
              "centered-clipping": ", iterations=%d, tau=%r" % (self.iterations, self.tau)}.get(self.rule, "")
+    if self.mix is not None:
+      extra += ", mix=%r" % self.mix
     return "FusedSpec(rule=%r, n=%d, f=%d, m=%d, beta=%d%s)" % (self.rule, self.n, self.f, self.m, self.beta, extra)
 
 

@@ -396,6 +396,86 @@ def torch_pairwise_distances(G):
   return dist
 
 
+# ---------------------------------------------------------------------------- #
+# Nearest-neighbour mixing (NNM; Allouah et al., "Fixing by Mixing", AISTATS 2023): a pre-aggregation run on the rows before the rule
+
+PRE_AGGREGATIONS = ("none", "nnm")
+
+
+def check_pre_aggregation(name):
+  """`--pre-aggregation` value -> the `FusedSpec.mix` it selects (None for "none")."""
+  if name is None or name == "none":
+    return None
+  if name not in PRE_AGGREGATIONS:
+    raise tools.UserException("Unknown pre-aggregation %r (expected one of %s)" % (name, ", ".join(PRE_AGGREGATIONS)))
+  return name
+
+
+def check_nnm(n, f):
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("Nearest-neighbour mixing needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+
+
+def nnm_select(dist, f):
+  """[n, n] distances -> [n, n] bool matrix, row i marking N_i: i itself and the n - f - 1 other rows first under the ordering
+  convention (finite ascending, non-finite last, ties -> lower index), whatever the ties at distance 0."""
+  n = dist.shape[0]
+  check_nnm(n, f)
+  key = _rank_key(dist.detach().to("cpu"))
+  member = torch.eye(n, dtype=torch.bool)
+  for i in range(n):
+    others = torch.tensor([j for j in range(n) if j != i], dtype=torch.int64)
+    order = torch.argsort(key[i, others], stable=True)
+    member[i, others[order[:n - f - 1]]] = True
+  return member
+
+
+def nnm_bits(member):
+  """[n, n] bool neighbourhoods (n <= 32) -> [n] int32 bit masks, the layout the sm_90a kernel reports."""
+  values = [sum(1 << j for j in range(member.shape[1]) if bool(member[i, j])) for i in range(member.shape[0])]
+  return torch.tensor([v - (1 << 32) if v >= 1 << 31 else v for v in values], dtype=torch.int32)
+
+
+def _nnm_members(masks, n):
+  """Neighbourhoods as an [n, n] bool matrix, from that matrix or from [n] int32 bit masks."""
+  masks = masks.detach().to("cpu")
+  if masks.dim() == 2:
+    return masks.bool()
+  return torch.tensor([[(int(masks[i]) >> j) & 1 == 1 for j in range(n)] for i in range(n)], dtype=torch.bool)
+
+
+def torch_nnm_mix(G, masks, f):
+  """y_i = (((x_a0 + x_a1) + x_a2) + ...) / (n - f) over the members of N_i in ascending worker order from +0, in G's dtype: one
+  `torch.add` per member and one division by a 0-d tensor (a sum over a gathered index may add in another order)."""
+  n = G.shape[0]
+  check_nnm(n, f)
+  member = _nnm_members(masks, n)
+  count = torch.tensor(float(n - f), dtype=G.dtype, device=G.device)
+  Y = torch.empty_like(G)
+  for i in range(n):
+    acc = torch.zeros_like(G[i])
+    for j in range(n):
+      if bool(member[i, j]):
+        acc = torch.add(acc, G[j])
+    Y[i] = torch.div(acc, count)
+  return Y
+
+
+def torch_nnm(G, f, return_details=False):
+  """NNM with the torch back-end: distances, selection, mixing; `return_details` also gives (distances, [n, n] neighbourhoods)."""
+  dist = torch_pairwise_distances(G)
+  member = nnm_select(dist, f)
+  Y = torch_nnm_mix(G, member, f)
+  return (Y, dist, member) if return_details else Y
+
+
+def host_nnm(G, f):
+  """NNM with the host library's distances; selection and mixing on CPU tensors. Returns the mixed rows on G's device."""
+  Gc = G.detach().to("cpu").contiguous()
+  member = nnm_select(host_pairwise_distances(Gc), f)
+  return torch_nnm_mix(Gc, member, f).to(G.device)
+
+
 def krum_select(dist, f, m):
   """[n, n] distances -> (scores [n], ids of the m best, ascending score / index-stable)."""
   n = dist.shape[0]

@@ -80,6 +80,7 @@ def make_parser():
   add("--authenticate", action="store_true", default=False, help="Sign every published gradient (ed25519) and verify before aggregating; slices failing the check become NaN")
   add("--worker-momentum", type=float, default=0.0, help="Worker momentum beta in [0, 1): every worker submits its momentum m <- beta m + (1 - dampening) g instead of its gradient (0 with a zero dampening: off)")
   add("--worker-momentum-dampening", type=float, default=0.0, help="Dampening of the worker momentum in [0, 1)")
+  add("--pre-aggregation", type=str, default="none", choices=("none", "nnm"), help="Pre-aggregation of the gathered rows before the rule: 'nnm' replaces every row by the mean of its n - f nearest rows (nearest-neighbour mixing, needs 0 <= 2 f < n), 'none' by default")
   return parser
 
 
@@ -130,7 +131,8 @@ def _validate(args):
       raise tools.UserException("Given cluster specification does not include a " + repr(missing[0]) + " job")
   fatal = (
     (n <= 0, "Expected at least one non-Byzantine worker"),
-    (n < real, "Got more real Byzantine workers (" + repr(real) + ") than total number of workers (" + repr(n) + ")"))
+    (n < real, "Got more real Byzantine workers (" + repr(real) + ") than total number of workers (" + repr(n) + ")"),
+    (args.pre_aggregation == "nnm" and not 0 <= 2 * f < n, "Nearest-neighbour mixing needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)))
   for failed, message in fatal:
     if failed:
       raise tools.UserException(message)
@@ -194,7 +196,7 @@ def main(argv=None):
     if not quiet:
       print("Using a total of " + repr(args.nb_workers) + " worker(s):")
       print("· " + repr(nb_nonbyz_workers) + " non-Byzantine worker(s)")
-      print("· " + repr(args.nb_decl_byz_workers) + " declared Byzantine worker(s)")
+      print("· " + repr(args.nb_decl_byz_workers) + " declared Byzantine worker(s)" + (", nearest-neighbour mixing (NNM) before the rule" if args.pre_aggregation == "nnm" else ""))
       print("  " + repr(args.nb_real_byz_workers) + " real Byzantine worker(s)")
       tools.print_args("experiment", args.experiment, args.experiment_args, head="")
       tools.print_args("gradient aggregation rule", args.aggregator, args.aggregator_args, head="")
@@ -252,6 +254,7 @@ def main(argv=None):
                         (args.l1_regularize, args.l2_regularize), trace=args.trace, attack=attack, nb_real_byz=args.nb_real_byz_workers if attacked else 0,
                         device=device, engine=engine, backend=args.nn_backend, seed=args.seed, placement=placement, debug_checksum=args.debug_checksum, authenticate=args.authenticate,
                         worker_momentum=args.worker_momentum, worker_momentum_dampening=args.worker_momentum_dampening,
+                        pre_aggregation=args.pre_aggregation, nb_decl_byz=args.nb_decl_byz_workers,
                         dtype={"bf16": torch.bfloat16, "tf32": torch.float32, "fp32": torch.float32}.get(args.dtype))
   if exit_pending:
     return 0

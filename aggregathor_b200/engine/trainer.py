@@ -15,7 +15,8 @@ One synchronous step on a rank:
      reads it — a real Byzantine worker keeps its honest momentum, the attack then transforms or replaces what is submitted;
   3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
      Byzantine rows from the honest ones, a collective call on every rank);
-  4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast);
+  4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast), after the optional pre-aggregation
+     (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing");
   5. the bf16 compute copy of the parameters is refreshed (unless the fused kernel already wrote it).
 """
 
@@ -46,8 +47,11 @@ class Manager:
   def __init__(self, experiment, aggregator, nbworkers, optimizer="sgd", optimizer_args=None, learning_rate="fixed", learning_rate_args=None,
                regularizations=(-1., -1.), trace=False, *, attack=None, nb_real_byz=0, device=None, group=None, engine="auto", backend="auto",
                dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False,
-               worker_momentum=0.0, worker_momentum_dampening=0.0):
+               worker_momentum=0.0, worker_momentum_dampening=0.0, pre_aggregation="none", nb_decl_byz=None):
+    """`pre_aggregation`: "none" or "nnm" (every row replaced by the mean of its n - f nearest rows before the rule), with f =
+    `nb_decl_byz`, the declared Byzantine workers (default: the rule's own f)."""
     from ..aggregators import _ops
+    self.pre_aggregation = _ops.check_pre_aggregation(pre_aggregation)   # None or "nnm"
     # (beta, c = 1 - dampening) in fp32; beta = dampening = 0 is off: no buffer, no kernel, the step is unchanged
     self.momentum = _ops.check_worker_momentum(worker_momentum, worker_momentum_dampening)
     self.momentum_on = self.momentum[0] != 0.0 or _ops.fp32(worker_momentum_dampening) != 0.0
@@ -80,8 +84,10 @@ class Manager:
     # -- aggregation engine (owns params + gradient rows) -------------------------- #
     engine_args = dict(engine_args or {})
     self._bucket_layers = {}
-    # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum)
-    plain_step = attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
+    # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum); with
+    # NNM the rule's distances are those of the mixed rows, which exist only once every row is complete
+    plain_step = (attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
+                  and self.pre_aggregation is None)
     if cuda and engine in ("auto", "fused") and aggregator.fused_spec() is not None:
       engine_args.setdefault("device_state", True)
       # The bucketed distance pass moves the gather + distance work of Krum / Bulyan under the backward pass (`gar_phase_a_kernel` on a side
@@ -94,10 +100,11 @@ class Manager:
         buckets, self._bucket_layers = self._plan_buckets()
         if len(buckets) > 1:
           engine_args["buckets"] = buckets
+    mix = dict(pre_aggregation=self.pre_aggregation, nb_decl_byz=nb_decl_byz)
     try:
-      self.aggregation = make_aggregation(engine, aggregator, self.layout, nbworkers, self.optimizer, group, self.device, **engine_args)
+      self.aggregation = make_aggregation(engine, aggregator, self.layout, nbworkers, self.optimizer, group, self.device, **mix, **engine_args)
     except TypeError:   # engines without these options (host, baseline)
-      self.aggregation = make_aggregation(engine, aggregator, self.layout, nbworkers, self.optimizer, group, self.device)
+      self.aggregation = make_aggregation(engine, aggregator, self.layout, nbworkers, self.optimizer, group, self.device, **mix)
     if not getattr(self.aggregation, "overlappable", False):
       self._bucket_layers = {}
     self._side_stream = None

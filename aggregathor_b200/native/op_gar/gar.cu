@@ -18,6 +18,9 @@
 //                    geometric median / centered clipping instead: T + 1 passes over the owned coordinates, with one exchange of
 //                    the n row distances per iteration (see `iterative_rule`)
 //
+// Nearest-neighbour mixing (NNM, `a.mix`) runs inside the finish kernel before any rule: raw distance pass (staging every row) and
+// exchange, one selection warp, then every row of the staged tile is replaced by the mean of its n - f nearest rows; the rule then
+// reads the mixed tile (see `nnm_pre_aggregation`).
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values.
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
@@ -47,7 +50,9 @@ constexpr int kSlotExit = kMaxSeg + 1;
 constexpr int kSlotCraft = kMaxSeg + 2;   // entry barrier of the Byzantine crafting kernel
 constexpr int kMaxIterations = 16;        // geometric median, centered clipping: iterations
 constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median, centered clipping: one exchange slot per iteration
-constexpr int kFlagSlots = kSlotGeoMedian + kMaxIterations;
+constexpr int kSlotMix = kSlotGeoMedian + kMaxIterations;   // NNM: exchange of the raw distances
+constexpr int kFlagSlots = kSlotMix + 1;
+constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
@@ -77,14 +82,15 @@ struct GarArgs {
     float* param_mc;                   // multicast address of the parameter buffers, or null
     __nv_bfloat16* param_bf16_dst[kMaxRanks]; // optional bf16 compute copy of the parameters
     uint32_t* signal[kMaxRanks];       // [kFlagSlots][R] flags of every rank
-    float* mailbox[kMaxRanks];         // [R][kMaxPairs + 1] partial distances (+ loss sum) of every rank
+    float* mailbox[kMaxRanks];         // 2 x [kMaxRanks][kMaxPairs + 1] partial distances (+ loss sum) of every rank; region 1: NNM
     uint32_t epoch;                    // immediate epoch, used when epoch_ptr is null
     uint32_t* epoch_ptr;               // device counter of completed steps: flags use *epoch_ptr + 1; the finish kernel increments it
     float* cta_partials;               // [grid][kMaxPairs]
     float* seg_partials;               // [kMaxSeg][seg_max_ctas][kMaxPairs]
     float* staging;                    // [n][owned length] or null
-    float* dist_out;                   // optional [n * n] (geometric median, centered clipping: [iterations][n])
-    int* info;                         // optional [64]: selection masks for tests/diagnostics
+    float* dist_out;                   // optional [n * n] (geometric median, centered clipping: [iterations][n]); with NNM: of the mixed rows
+    float* raw_dist_out;               // optional [n * n]: NNM's distances of the raw rows
+    int* info;                         // optional [128]: selection masks for tests/diagnostics; [64, 64 + n): NNM masks
     float const* loss_in;              // optional [nloss] local per-worker losses
     int nloss;
     float* loss_out;                   // [1]: total loss over all ranks (summed in rank order)
@@ -92,6 +98,7 @@ struct GarArgs {
     float nu;                          // geometric median: smoothing, finite and > 0
     float tau;                         // centered clipping: clipping radius, finite and > 0
     float* center;                     // centered clipping: [d] (local) center v, read and updated on the owned coordinates
+    int mix;                           // pre-aggregation: 0 none, 1 nearest-neighbour mixing (needs the staging buffer)
 };
 
 struct Shared {
@@ -112,6 +119,7 @@ struct Shared {
     float scores[kMaxWorkers];
     float warp_partials[16][kBlockRows * kBlockRows];
     unsigned selmask[kMaxWorkers];   // Krum, MDA: [0]; Bulyan: one per round
+    unsigned nnm_mask[kMaxWorkers];  // NNM: neighbourhood of every row (itself included); outlives the rule's phases
     int selcount[kMaxWorkers];
     int theta;
     float hyper[4];
@@ -547,7 +555,8 @@ __device__ __forceinline__ float sq_dist(float4 const& u, float4 const& v) {
     return (dx * dx + dy * dy) + (dz * dz + dw * dw);
 }
 
-template<bool CROSS>
+// STAGED_ONLY (NNM's distances of the mixed rows): every pass, block 0's diagonal included, reads the staged tile and stores nothing.
+template<bool CROSS, bool STAGED_ONLY = false>
 __device__ void phase_a_segment(GarArgs const& a, Shared& sh, int* pair_of, int seg, float* out, long long tid, long long nthreads) {
     constexpr int B = kBlockRows, NPB = B * (B - 1) / 2;
     int const n = a.n, nb = CROSS ? (n + B - 1) / B : 1;
@@ -556,7 +565,7 @@ __device__ void phase_a_segment(GarArgs const& a, Shared& sh, int* pair_of, int 
     auto staged = [&](int row, long long v) { return a.staging + row * owned + soff + (v << 2); };
     for (int bi = 0; bi < nb; ++bi) {
         int const i0 = bi * B;
-        bool const from_copy = a.staging != nullptr && bi > 0;   // blocks >= 1 were staged by the cross passes (0, b)
+        bool const from_copy = STAGED_ONLY || (a.staging != nullptr && bi > 0);   // blocks >= 1 were staged by the cross passes (0, b)
         if (threadIdx.x < NPB) {   // local pair index -> (i, j) -> global pair index
             int i = 0, rest = threadIdx.x;
             while (rest >= B - 1 - i) {
@@ -602,7 +611,7 @@ __device__ void phase_a_segment(GarArgs const& a, Shared& sh, int* pair_of, int 
         if (CROSS) {
             for (int bj = bi + 1; bj < nb; ++bj) {
                 int const j0 = bj * B;
-                bool const j_from_copy = a.staging != nullptr && bi > 0;   // first touch of block bj is the pass (0, bj)
+                bool const j_from_copy = STAGED_ONLY || (a.staging != nullptr && bi > 0);   // first touch of block bj is the pass (0, bj)
                 if (threadIdx.x < B * B) {
                     int const i = threadIdx.x / B, j = threadIdx.x % B;
                     pair_of[threadIdx.x] = (i0 + i < n && j0 + j < n) ? pair_index(i0 + i, j0 + j, n) : -1;
@@ -670,6 +679,158 @@ __global__ void __launch_bounds__(256, 1) gar_phase_a_kernel(GarArgs const a, in
     phase_a_segment<CROSS>(a, sh, pair_of, seg, out, tid, nthreads);
 }
 
+// ---- exchange of the pair distances: `cta_partials` (+ the pre-accumulated segments) -> every rank -> `sh.dist` ------------- //
+// Fixed order: pre-accumulated segments [0, first_seg) (ascending, their CTAs ascending), then this kernel's CTAs, then ranks
+// (ascending) => bit-identical matrix (and total loss) on every rank and in every CTA. `region`: float offset of the mailbox region,
+// `slot`: flag slot of this exchange; the rank's loss sum travels with the distances. Non-finite distances become +inf.
+__device__ void exchange_distances(GarArgs const& a, Shared& sh, cg::grid_group& grid, uint32_t epoch, int first_seg, int region, int slot,
+                                   float local_loss, float* dist_out) {
+    int const n = a.n, npairs = n * (n - 1) / 2;
+    bool const multi = a.R > 1;
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int p = threadIdx.x; p < npairs; p += blockDim.x) {
+            float s = 0.f;
+            for (int seg = 0; seg < first_seg; ++seg)
+                for (int b = 0; b < a.seg_ctas[seg]; ++b)
+                    s += ld_volatile_f(a.seg_partials + (static_cast<long long>(seg) * a.seg_max_ctas + b) * kMaxPairs + p);
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kMaxPairs + p);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][region + a.rank * (kMaxPairs + 1) + p] = s;
+        }
+        if (threadIdx.x == 0)
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][region + a.rank * (kMaxPairs + 1) + kMaxPairs] = local_loss;
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, slot, epoch);
+    }
+    if (multi) {
+        wait_all(a, slot, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    // -------- full distance matrix (rank order => identical everywhere) -------- //
+    for (int p = threadIdx.x; p < kMaxWorkers * (kMaxWorkers + 1); p += blockDim.x)
+        (&sh.dist[0][0])[p] = 0.f;
+    __syncthreads();
+    float const* const box = a.mailbox[a.rank] + region;
+    for (int p = threadIdx.x; p < npairs; p += blockDim.x) {
+        int i = 0, rest = p;
+        while (rest >= n - 1 - i) { // pair index -> (i, j) of the upper triangle
+            rest -= n - 1 - i;
+            ++i;
+        }
+        int const j = i + 1 + rest;
+        float s = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            s += ld_volatile_f(box + q * (kMaxPairs + 1) + p);
+        if (!is_finite(s))
+            s = __int_as_float(0x7f800000);
+        sh.dist[i][j] = s;
+        sh.dist[j][i] = s;
+        if (dist_out && blockIdx.x == 0) {
+            dist_out[i * n + j] = s;
+            dist_out[j * n + i] = s;
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
+        float total = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            total += ld_volatile_f(box + q * (kMaxPairs + 1) + kMaxPairs);
+        *a.loss_out = total;
+    }
+    __syncthreads();
+}
+
+// ---- nearest-neighbour mixing (Allouah et al., "Fixing by Mixing", AISTATS 2023) ------------------------------------------ //
+// D_ij = ||x_i - x_j||^2 (non-finite -> +inf); N_i = {i} and the n - f - 1 rows j != i first under the ordering convention;
+// y_i = (((x_a0 + x_a1) + x_a2) + ...) / (n - f), the members of N_i in ascending worker order from +0, every operation rounded once.
+//   1. raw distance pass over all owned segments: the rows cross NVLink once and land in the staged tile (block 0's diagonal and the
+//      cross passes (0, b) store every row they load); exchange through mailbox region 1 and flag slot kSlotMix, which no other
+//      exchange of the step touches (every CTA of every rank reads them, so a later exchange could not safely reuse them); the loss
+//      travels with it;
+//   2. warp 0 of every CTA builds the n masks from sh.dist (identical everywhere, so are the masks);
+//   3. mix pass, in place on the staged tile: a thread loads the n raw values of a coordinate, then stores its n mixed values over
+//      them. It uses the rules' own mapping (tid, VEC): a coordinate-wise or iterative rule's thread reads back only what it wrote
+//      itself, so no grid barrier follows; the distance rules add one before their own pass over the mixed tile.
+template<int N, int VEC>
+__device__ __forceinline__ void nnm_pre_aggregation(GarArgs const& a, Shared& sh, int* pair_of, cg::grid_group& grid, uint32_t epoch,
+                                                    float local_loss, long long tid, long long nthreads) {
+    int const n = a.n, npairs = n * (n - 1) / 2;
+    float* mine = a.cta_partials + static_cast<long long>(blockIdx.x) * kMaxPairs;
+    for (int p = threadIdx.x; p < npairs; p += blockDim.x)
+        mine[p] = 0.f;
+    __syncthreads();
+    for (int seg = 0; seg < a.nseg; ++seg)
+        phase_a_segment<(N > kBlockRows)>(a, sh, pair_of, seg, mine, tid, nthreads);
+    exchange_distances(a, sh, grid, epoch, 0, kMailboxRegion, kSlotMix, local_loss, a.raw_dist_out);
+    if (threadIdx.x < 32) {
+        int const lane = threadIdx.x, keep = n - a.f - 1;
+        if (lane < n) {
+            unsigned mask = 1u << lane;
+            for (int j = 0; j < n; ++j) {
+                if (j == lane)
+                    continue;
+                int rank = 0;
+                for (int k = 0; k < n; ++k)
+                    if (k != lane && k != j)
+                        rank += before(sh.dist[lane][k], k, sh.dist[lane][j], j) ? 1 : 0;
+                if (rank < keep)
+                    mask |= 1u << j;
+            }
+            sh.nnm_mask[lane] = mask;
+            if (a.info && blockIdx.x == 0)
+                a.info[64 + lane] = static_cast<int>(mask);
+        }
+    }
+    __syncthreads();
+    long long const owned = owned_length(a);
+    float const count = static_cast<float>(n - a.f);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            float* const tile = a.staging + soff + v * VEC;
+            float g[N][VEC];
+#pragma unroll
+            for (int i = 0; i < N; ++i) {
+                if (i < n) {
+                    V<VEC>::load(tile + i * owned, g[i]);
+                } else {
+#pragma unroll
+                    for (int c = 0; c < VEC; ++c)
+                        g[i][c] = 0.f;
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < VEC; ++c) {   // a component's n raw values are all read before any of them is replaced
+                float y[N];
+#pragma unroll
+                for (int i = 0; i < N; ++i) {
+                    unsigned const mask = i < n ? sh.nnm_mask[i] : 0u;
+                    float s = 0.f;
+#pragma unroll
+                    for (int j = 0; j < N; ++j)
+                        if ((mask >> j) & 1u)
+                            s = __fadd_rn(s, g[j][c]);
+                    y[i] = __fdiv_rn(s, count);
+                }
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    g[i][c] = y[i];
+            }
+#pragma unroll
+            for (int i = 0; i < N; ++i)
+                if (i < n)
+                    V<VEC>::store(tile + i * owned, g[i]);
+        }
+    }
+}
+
 // ---- iterative rules: geometric median (smoothed Weiszfeld, RFA) and centered clipping ---------- //
 // Geometric median: z_0 = coordinate-wise median; for t < T: D_i = ||z_t - x_i||^2, rows with a non-finite D_i are skipped,
 // beta_i = 1 / max(nu, sqrt(D_i)), S = sum beta_i and z_{t+1} = (sum beta_i x_i) / S, both sums over the kept rows in ascending worker
@@ -690,7 +851,8 @@ __global__ void __launch_bounds__(256, 1) gar_phase_a_kernel(GarArgs const a, in
 // Double buffering makes the mailbox safe to reuse: the half written at iteration t + 1 was last read at iteration t - 1; a rank
 // reads it before its block 0 reaches the grid barrier of iteration t, hence before it signals iteration t, and a writer stores
 // iteration t + 1 only after it has passed the barrier of iteration t, i.e. after every rank's iteration-t signal. With R = 1 a
-// second grid barrier takes the place of the flags. The loss travels through the exit barrier, as for the coordinate-wise rules.
+// second grid barrier takes the place of the flags. The loss travels through the exit barrier, as for the coordinate-wise rules
+// (with NNM: through NNM's exchange). With NNM, pass 0 reads the mixed tile too, with the mix pass's mapping (same thread).
 template<int N, int VEC>
 __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg::grid_group& grid, float const (&hyper)[4], uint32_t epoch,
                                                long long tid, long long nthreads) {
@@ -703,6 +865,7 @@ __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg:
     for (int t = 0; t <= T; ++t) {
         unsigned const mask = sh.geo.mask;
         float const S = sh.geo.sum;
+        bool const from_rows = !a.staging || (t == 0 && !a.mix);   // NNM: every pass reads the mixed tile
         float acc[N];
 #pragma unroll
         for (int i = 0; i < N; ++i)
@@ -716,7 +879,7 @@ __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg:
                 for (int i = 0; i < N; ++i) {
                     if (i < n) {
                         float* const staged = a.staging ? a.staging + i * owned + soff + v * VEC : nullptr;
-                        if (t == 0 || !staged) {
+                        if (from_rows) {
                             V<VEC>::load_stream(a.grad[i] + x, g[i]);
                             if (staged)
                                 V<VEC>::store(staged, g[i]);
@@ -849,6 +1012,92 @@ __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg:
     }
 }
 
+// ---- coordinate-wise rules: one streaming pass over the rows, or (STAGED, NNM) over the mixed tile, each thread reading what it
+// wrote in the mix pass ------------------------------------------------------------------------------------------------------ //
+template<int N, int VEC, bool STAGED>
+__device__ __forceinline__ void coordinate_rules(GarArgs const& a, float const (&hyper)[4], long long tid, long long nthreads) {
+    int const n = a.n;
+    long long const owned = STAGED ? owned_length(a) : 0;
+    bool const in_switch = a.rule == kAverage && a.grad_mc != nullptr && !STAGED;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = STAGED ? staged_offset(a, seg) : 0;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            auto row = [&](int i) -> float const* { return STAGED ? a.staging + i * owned + soff + v * VEC : a.grad[i] + x; };
+            float out[VEC];
+            if (a.rule == kAverage) {
+                float sum[VEC];
+#pragma unroll
+                for (int c = 0; c < VEC; ++c)
+                    sum[c] = 0.f;
+                if (VEC == 4 && in_switch) {   // NVLS: the switch adds the same row of every rank; rows of one rank are added here
+                    for (int j = 0; j < a.workers_per_rank; ++j) {
+                        float4 t = multimem_ld_reduce_add_f4(a.grad_mc + j * a.row_stride + x);
+                        sum[0] += t.x; sum[1 % VEC] += t.y; sum[2 % VEC] += t.z; sum[3 % VEC] += t.w;
+                    }
+                } else {
+                    if (N <= 16) {
+                        float g[N][VEC];
+#pragma unroll
+                        for (int i = 0; i < N; ++i)
+                            if (i < n)
+                                V<VEC>::load_stream(row(i), g[i]);
+#pragma unroll
+                        for (int i = 0; i < N; ++i)
+                            if (i < n) {
+#pragma unroll
+                                for (int c = 0; c < VEC; ++c)
+                                    sum[c] += g[i][c];
+                            }
+                    } else {
+                        for (int i = 0; i < n; ++i) {
+                            float g[VEC];
+                            V<VEC>::load_stream(row(i), g);
+#pragma unroll
+                            for (int c = 0; c < VEC; ++c)
+                                sum[c] += g[c];
+                        }
+                    }
+                }
+                float const count = static_cast<float>(n);
+#pragma unroll
+                for (int c = 0; c < VEC; ++c)
+                    out[c] = sum[c] / count;
+            } else {
+                float g[N][VEC];
+#pragma unroll
+                for (int i = 0; i < N; ++i) {
+                    if (i < n) {
+                        V<VEC>::load_stream(row(i), g[i]);
+                    } else {
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            g[i][c] = 0.f;
+                    }
+                }
+#pragma unroll
+                for (int c = 0; c < VEC; ++c) {
+                    float vals[N];
+#pragma unroll
+                    for (int i = 0; i < N; ++i)
+                        vals[i] = g[i][c];
+                    float r;
+                    if (a.rule == kAverageNan)
+                        r = coord_average_nan<N>(vals, n);
+                    else if (a.rule == kMedian)
+                        r = coord_median<N>(vals, n);
+                    else if (a.rule == kTrimmedMean)
+                        r = coord_trimmed_mean<N>(vals, n, a.f);
+                    else
+                        r = coord_averaged_median<N>(vals, n, a.beta);
+                    out[c] = r;
+                }
+            }
+            apply_update<VEC>(a, hyper, x, out);
+        }
+    }
+}
+
 // ---- the finish kernel -------------------------------------------------------------- //
 template<int N, int VEC>
 __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArgs const a) {
@@ -881,72 +1130,28 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
         for (int j = 0; j < a.nloss; ++j)
             local_loss += a.loss_in[j];
 
+    if (a.mix) {
+        nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
+        if (distance_rule) {
+            __threadfence();
+            grid.sync();   // the mix pass wrote the tile with the rule's (tid, VEC) mapping; the distance pass reads it by float4 blocks
+        }
+    }
+
     if (distance_rule) {
-        // -------- phase A of the segments that were not pre-accumulated -------- //
+        // -------- phase A of the segments that were not pre-accumulated (NNM: of the mixed tile) -------- //
         float* mine = a.cta_partials + static_cast<long long>(blockIdx.x) * kMaxPairs;
         for (int p = threadIdx.x; p < npairs; p += blockDim.x)
             mine[p] = 0.f;
         __syncthreads();
-        for (int seg = a.first_seg; seg < a.nseg; ++seg)
-            phase_a_segment<(N > kBlockRows)>(a, sh, pair_of, seg, mine, tid, nthreads);
-        __threadfence();
-        grid.sync();
-        // fixed order: pre-accumulated segments (ascending, their CTAs ascending), then this kernel's CTAs, then ranks (ascending)
-        if (blockIdx.x == 0) {
-            for (int p = threadIdx.x; p < npairs; p += blockDim.x) {
-                float s = 0.f;
-                for (int seg = 0; seg < a.first_seg; ++seg)
-                    for (int b = 0; b < a.seg_ctas[seg]; ++b)
-                        s += ld_volatile_f(a.seg_partials + (static_cast<long long>(seg) * a.seg_max_ctas + b) * kMaxPairs + p);
-                for (unsigned b = 0; b < gridDim.x; ++b)
-                    s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kMaxPairs + p);
-                for (int q = 0; q < a.R; ++q)
-                    a.mailbox[q][a.rank * (kMaxPairs + 1) + p] = s;
-            }
-            if (threadIdx.x == 0)
-                for (int q = 0; q < a.R; ++q)
-                    a.mailbox[q][a.rank * (kMaxPairs + 1) + kMaxPairs] = local_loss;
-            fence_sys();
-            __syncthreads();
-            if (multi)
-                signal_all(a, kSlotExchange, epoch);
+        for (int seg = a.first_seg; seg < a.nseg; ++seg) {
+            if (a.mix)
+                phase_a_segment<(N > kBlockRows), true>(a, sh, pair_of, seg, mine, tid, nthreads);
+            else
+                phase_a_segment<(N > kBlockRows)>(a, sh, pair_of, seg, mine, tid, nthreads);
         }
-        if (multi) {
-            wait_all(a, kSlotExchange, epoch);
-            __syncthreads();
-        } else {
-            grid.sync();
-        }
-        // -------- full distance matrix (rank order => identical everywhere) + selection -------- //
-        for (int p = threadIdx.x; p < kMaxWorkers * (kMaxWorkers + 1); p += blockDim.x)
-            (&sh.dist[0][0])[p] = 0.f;
-        __syncthreads();
-        for (int p = threadIdx.x; p < npairs; p += blockDim.x) {
-            int i = 0, rest = p;
-            while (rest >= n - 1 - i) { // pair index -> (i, j) of the upper triangle
-                rest -= n - 1 - i;
-                ++i;
-            }
-            int const j = i + 1 + rest;
-            float s = 0.f;
-            for (int q = 0; q < a.R; ++q)
-                s += ld_volatile_f(a.mailbox[a.rank] + q * (kMaxPairs + 1) + p);
-            if (!is_finite(s))
-                s = __int_as_float(0x7f800000);
-            sh.dist[i][j] = s;
-            sh.dist[j][i] = s;
-            if (a.dist_out && blockIdx.x == 0) {
-                a.dist_out[i * n + j] = s;
-                a.dist_out[j * n + i] = s;
-            }
-        }
-        if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
-            float total = 0.f;
-            for (int q = 0; q < a.R; ++q)
-                total += ld_volatile_f(a.mailbox[a.rank] + q * (kMaxPairs + 1) + kMaxPairs);
-            *a.loss_out = total;
-        }
-        __syncthreads();
+        // -------- full distance matrix + selection -------- //
+        exchange_distances(a, sh, grid, epoch, a.first_seg, 0, kSlotExchange, local_loss, a.dist_out);
         if (a.rule == kMda) {
             select_mda(a, sh, grid);
         } else if (threadIdx.x < 32) {
@@ -1047,91 +1252,18 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
     } else if (a.rule == kGeoMedian || a.rule == kCenteredClipping) {
         iterative_rule<N, VEC>(a, sh, grid, hyper, epoch, tid, nthreads);
     } else {
-        // -------- coordinate-wise rules: one streaming pass -------- //
-        bool const in_switch = a.rule == kAverage && a.grad_mc != nullptr;
-        for (int seg = 0; seg < a.nseg; ++seg) {
-            long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC;
-            for (long long v = tid; v < lenv; v += nthreads) {
-                long long const x = lo + v * VEC;
-                float out[VEC];
-                if (a.rule == kAverage) {
-                    float sum[VEC];
-#pragma unroll
-                    for (int c = 0; c < VEC; ++c)
-                        sum[c] = 0.f;
-                    if (VEC == 4 && in_switch) {   // NVLS: the switch adds the same row of every rank; rows of one rank are added here
-                        for (int j = 0; j < a.workers_per_rank; ++j) {
-                            float4 t = multimem_ld_reduce_add_f4(a.grad_mc + j * a.row_stride + x);
-                            sum[0] += t.x; sum[1 % VEC] += t.y; sum[2 % VEC] += t.z; sum[3 % VEC] += t.w;
-                        }
-                    } else {
-                        if (N <= 16) {
-                            float g[N][VEC];
-#pragma unroll
-                            for (int i = 0; i < N; ++i)
-                                if (i < n)
-                                    V<VEC>::load_stream(a.grad[i] + x, g[i]);
-#pragma unroll
-                            for (int i = 0; i < N; ++i)
-                                if (i < n) {
-#pragma unroll
-                                    for (int c = 0; c < VEC; ++c)
-                                        sum[c] += g[i][c];
-                                }
-                        } else {
-                            for (int i = 0; i < n; ++i) {
-                                float g[VEC];
-                                V<VEC>::load_stream(a.grad[i] + x, g);
-#pragma unroll
-                                for (int c = 0; c < VEC; ++c)
-                                    sum[c] += g[c];
-                            }
-                        }
-                    }
-                    float const count = static_cast<float>(n);
-#pragma unroll
-                    for (int c = 0; c < VEC; ++c)
-                        out[c] = sum[c] / count;
-                } else {
-                    float g[N][VEC];
-#pragma unroll
-                    for (int i = 0; i < N; ++i) {
-                        if (i < n) {
-                            V<VEC>::load_stream(a.grad[i] + x, g[i]);
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < VEC; ++c)
-                                g[i][c] = 0.f;
-                        }
-                    }
-#pragma unroll
-                    for (int c = 0; c < VEC; ++c) {
-                        float vals[N];
-#pragma unroll
-                        for (int i = 0; i < N; ++i)
-                            vals[i] = g[i][c];
-                        float r;
-                        if (a.rule == kAverageNan)
-                            r = coord_average_nan<N>(vals, n);
-                        else if (a.rule == kMedian)
-                            r = coord_median<N>(vals, n);
-                        else if (a.rule == kTrimmedMean)
-                            r = coord_trimmed_mean<N>(vals, n, a.f);
-                        else
-                            r = coord_averaged_median<N>(vals, n, a.beta);
-                        out[c] = r;
-                    }
-                }
-                apply_update<VEC>(a, hyper, x, out);
-            }
-        }
+        if (a.mix)
+            coordinate_rules<N, VEC, true>(a, hyper, tid, nthreads);
+        else
+            coordinate_rules<N, VEC, false>(a, hyper, tid, nthreads);
     }
 
+    bool const exchanged_loss = distance_rule || a.mix;   // the loss went through an exchange of distances (distance rules, NNM)
     if (multi) { // exit barrier: all slices have landed on all ranks, gradient buffers are free again
         fence_sys();
         grid.sync();
         if (blockIdx.x == 0) {
-            if (!distance_rule && threadIdx.x == 0) {   // rules without an exchange stage carry the loss through the exit barrier
+            if (!exchanged_loss && threadIdx.x == 0) {   // steps without an exchange stage carry the loss through the exit barrier
                 for (int q = 0; q < a.R; ++q)
                     a.mailbox[q][a.rank * (kMaxPairs + 1) + kMaxPairs] = local_loss;
                 fence_sys();
@@ -1140,14 +1272,14 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
             signal_all(a, kSlotExit, epoch);
             wait_all(a, kSlotExit, epoch);
             __syncthreads();
-            if (!distance_rule && threadIdx.x == 0 && a.loss_out) {
+            if (!exchanged_loss && threadIdx.x == 0 && a.loss_out) {
                 float total = 0.f;
                 for (int q = 0; q < a.R; ++q)
                     total += ld_volatile_f(a.mailbox[a.rank] + q * (kMaxPairs + 1) + kMaxPairs);
                 *a.loss_out = total;
             }
         }
-    } else if (!distance_rule && blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
+    } else if (!exchanged_loss && blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
         *a.loss_out = local_loss;
     }
     if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
@@ -1371,9 +1503,9 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t strea
 //   [0..32) gradient rows | [32] agg_out | [33] param | [34] slot0 | [35] slot1 | [36] param_mc | [37] cta_partials | [38] staging
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
+//   [47] center (centered clipping) | [112] raw_dist_out (NNM)
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-//   [47] center (centered clipping)
-//       [25] iterations
+//       [25] iterations | [26] mix (0 none, 1 NNM)
 // longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
@@ -1381,6 +1513,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.workers_per_rank = ints[10];
     a.nseg = ints[11]; a.first_seg = ints[12]; a.nloss = ints[13]; a.seg_max_ctas = ints[14];
     a.iterations = ints[25];
+    a.mix = ints[26];
     a.row_stride = longs[0];
     a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4]; a.tau = floats[5];
     a.center = reinterpret_cast<float*>(ptrs[47]);
@@ -1397,6 +1530,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     }
     if (a.rule < 0 || a.rule > kCenteredClipping)
         return 102;
+    if (a.mix < 0 || a.mix > 1 || (a.mix && (a.f < 0 || 2 * a.f >= a.n)))
+        return 117;
     if (a.rule == kCenteredClipping && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.tau > 0.f) ||
                                         !std::isfinite(a.tau) || !a.center))
         return 116;
@@ -1434,6 +1569,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.seg_partials = reinterpret_cast<float*>(ptrs[44]);
     a.loss_in = reinterpret_cast<float const*>(ptrs[45]);
     a.loss_out = reinterpret_cast<float*>(ptrs[46]);
+    a.raw_dist_out = reinterpret_cast<float*>(ptrs[112]);
     for (int q = 0; q < a.R; ++q) {
         a.param_dst[q] = reinterpret_cast<float*>(ptrs[48 + q]);
         a.signal[q] = reinterpret_cast<uint32_t*>(ptrs[64 + q]);
@@ -1452,6 +1588,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)
         return 108;
+    if (a.mix && (!a.cta_partials || !a.mailbox[0] || !a.staging))
+        return 108;   // NNM mixes the staged tile in place
+    if (a.mix && a.first_seg > 0)
+        return 111;   // NNM's raw distance pass covers every segment: nothing is pre-accumulated
     if (a.R > 1 && !a.signal[0])
         return 109;
     if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && !a.staging)
@@ -1483,7 +1623,7 @@ int agb_gar_max_ctas() {
 // Sizes of the per-rank communication regions (bytes): signal pad, mailbox.
 int agb_gar_region_bytes(long long* out) {
     out[0] = static_cast<long long>(kFlagSlots) * kMaxRanks * 4;
-    out[1] = static_cast<long long>(kMaxRanks) * (kMaxPairs + 1) * 4;
+    out[1] = 2ll * kMailboxRegion * 4;
     return 0;
 }
 
@@ -1515,7 +1655,8 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     if (status)
         return status;
     int const ctas = ints[15];
-    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda))
+    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda) ||
+        a.mix)
         return 111;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // small CTAs: a 64-thread CTA (8 K registers, 13 KB of static shared memory) fits beside a persistent GEMM CTA of the backward pass

@@ -20,9 +20,12 @@ MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS   # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration
+# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 1
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
-MAILBOX_BYTES = MAX_RANKS * (MAX_PAIRS + 1) * 4
+MAILBOX_BYTES = 2 * MAX_RANKS * (MAX_PAIRS + 1) * 4   # two regions: the rule's exchanges, NNM's exchange
+PTRS = 113
+INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
 
 _ERRORS = {
@@ -33,7 +36,8 @@ _ERRORS = {
   112: "invalid trimmed-mean parameters (0 <= 2 f < n)", 113: "invalid MDA parameters (0 <= 2 f < n and C(n, f) <= 2^20)",
   114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)",
   115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)",
-  116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)"}
+  116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)",
+  117: "invalid NNM parameters (0 <= 2 f < n)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1}
 
@@ -75,8 +79,9 @@ class FusedLauncher:
     self.local_mailbox = torch.zeros(MAILBOX_BYTES // 4, dtype=torch.float32, device=self.device)
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
     self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
-    self.info = torch.zeros(64, dtype=torch.int32, device=self.device)
-    self._ptrs = (ctypes.c_ulonglong * 112)()
+    self.raw_dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)   # NNM: distances of the raw rows
+    self.info = torch.zeros(INFO_INTS, dtype=torch.int32, device=self.device)
+    self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
     self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS))()
     self._floats = (ctypes.c_float * 6)()
@@ -93,7 +98,7 @@ class FusedLauncher:
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
             first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None):
     ptrs = self._ptrs
-    for i in range(112):
+    for i in range(PTRS):
       ptrs[i] = 0
     if len(rows) != spec.n:
       raise tools.UserException("Expected %d gradient rows, got %d" % (spec.n, len(rows)))
@@ -106,7 +111,7 @@ class FusedLauncher:
     dist_out = self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dist_out
     ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
     ptrs[42], ptrs[43], ptrs[44], ptrs[45], ptrs[46] = addr(epoch_ptr), addr(hyper_ptr), self.seg_partials.data_ptr(), addr(loss_in), addr(loss_out)
-    ptrs[47] = addr(center)
+    ptrs[47], ptrs[112] = addr(center), self.raw_dist_out.data_ptr()
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -116,7 +121,7 @@ class FusedLauncher:
     ints[0], ints[1], ints[2], ints[3], ints[4] = spec.n, spec.f, spec.m, spec.beta, spec.rule_id
     ints[5], ints[6], ints[7], ints[8], ints[9] = R, rank, OPTIMIZERS[opt], epoch & 0x7fffffff, max_ctas_limit
     ints[10], ints[11], ints[12], ints[13] = workers_per_rank, len(segments), first_seg, (loss_in.numel() if loss_in is not None else 0)
-    ints[14], ints[15], ints[24], ints[25] = self.phase_a_ctas, self.phase_a_ctas, self.phase_a_threads, spec.iterations
+    ints[14], ints[15], ints[24], ints[25], ints[26] = self.phase_a_ctas, self.phase_a_ctas, self.phase_a_threads, spec.iterations, spec.mix_id
     self._longs[0] = row_stride
     for s in range(MAX_SEGMENTS):
       lo, hi = segments[s] if s < len(segments) else (0, 0)
@@ -153,39 +158,67 @@ def _torch_rules(spec):
 def aggregate(spec, G, return_details=False, center=None):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
-  iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place."""
+  iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
+  With `spec.mix == "nnm"` the rule runs on the mixed rows (its distances and masks are those of the mixed rows), and
+  `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32)."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   n, d = G.shape
   if n != spec.n:
-    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau)
+    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau, mix=spec.mix)
   if spec.rule == "centered-clipping":
     return _aggregate_centered_clipping(spec, G, return_details, center)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
-    return _torch_rules(spec)(G)
+    return _torch_rules(spec)(_torch_mixed(spec, G))
   if G.dtype != torch.float32:
     out = aggregate(spec, G.float(), return_details)
     return (out[0].to(G.dtype),) + out[1:] if return_details else out.to(G.dtype)
   if n > MAX_WORKERS:  # beyond the kernels' worker limit: torch ops on the same device
-    return _torch_rules(spec)(G)
+    return _torch_rules(spec)(_torch_mixed(spec, G))
+  G, dp = _aligned_rows(G)
+  launcher = _launcher(G.device, n)
+  out = torch.empty(dp, dtype=torch.float32, device=G.device)
+  rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=_staging(spec, n, dp, G.device))
+  out = out[:d]
+  if return_details:
+    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule in ITERATIVE_RULES else launcher.dist_out.view(n, n)
+    return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
+  return out
+
+
+def _aligned_rows(G):
+  """Contiguous [n, dp] rows, dp the next multiple of 4, on a 16-byte boundary (zero padding) -> (rows, dp)."""
+  n, d = G.shape
   G = G.contiguous()
   pad = (-d) % 4
   if pad or G.data_ptr() % 16:
     Gp = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
     Gp[:, :d] = G
     G = Gp
-  dp = d + pad
-  launcher = _launcher(G.device, n)
-  out = torch.empty(dp, dtype=torch.float32, device=G.device)
-  rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher.launch(spec, rows, 0, dp, agg_out=out)
-  out = out[:d]
-  if return_details:
-    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule in ITERATIVE_RULES else launcher.dist_out.view(n, n)
-    return out, dist.clone(), launcher.info.clone()
-  return out
+  return G, d + pad
+
+
+def _staging(spec, n, dp, device):
+  """NNM mixes the rows in place in a local [n, dp] tile: the stand-alone op has to provide one."""
+  return torch.empty((n, dp), dtype=torch.float32, device=device) if spec.mix is not None else None
+
+
+def _mix_details(spec, launcher, n):
+  """The fourth `return_details` element with NNM: (raw distances [n, n], NNM masks [n] int32)."""
+  if spec.mix is None:
+    return ()
+  return ((launcher.raw_dist_out.view(n, n).clone(), launcher.info[64:64 + n].clone()),)
+
+
+def _torch_mixed(spec, G):
+  """The fall-backs' pre-aggregation: `spec.mix` with the torch reference on G's device."""
+  if spec.mix is None:
+    return G
+  from ..aggregators import _ops
+  return _ops.torch_nnm(G, spec.f)
 
 
 def _launcher(device, n):
@@ -207,16 +240,11 @@ def _aggregate_centered_clipping(spec, G, return_details, center):
       raise tools.UserException("Centered clipping needs a center of type %s (got %s)" % (G.dtype, center.dtype))
     if return_details:
       raise tools.UserException("Centered clipping returns its details from the sm_90a kernel only (fp32, n <= %d)" % MAX_WORKERS)
-    return _ops.torch_centered_clipping(G, spec.iterations, spec.tau, center)
+    return _ops.torch_centered_clipping(_torch_mixed(spec, G), spec.iterations, spec.tau, center)
   if G.dtype != torch.float32 or center.dtype != torch.float32:
     raise tools.UserException("Centered clipping on the device needs fp32 rows and center (got %s, %s)" % (G.dtype, center.dtype))
-  G = G.contiguous()
-  pad = (-d) % 4
-  if pad or G.data_ptr() % 16:
-    Gp = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
-    Gp[:, :d] = G
-    G = Gp
-  dp = d + pad
+  G, dp = _aligned_rows(G)
+  pad = dp - d
   work = center
   if pad or not center.is_contiguous() or center.data_ptr() % 16:
     work = torch.zeros(dp, dtype=torch.float32, device=G.device)
@@ -224,13 +252,13 @@ def _aggregate_centered_clipping(spec, G, return_details, center):
   launcher = _launcher(G.device, n)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher.launch(spec, rows, 0, dp, agg_out=out, center=work)
+  launcher.launch(spec, rows, 0, dp, agg_out=out, center=work, staging=_staging(spec, n, dp, G.device))
   if work is not center:
     center.copy_(work[:d])
   out = out[:d]
   if return_details:
     dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n)
-    return out, dist.clone(), launcher.info.clone()
+    return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
   return out
 
 

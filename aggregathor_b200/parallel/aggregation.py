@@ -17,6 +17,10 @@ Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always 
 Every engine also has `craft_byzantine(byz_slots, mode, coef)`, the omniscient attacks (`attacks/omniscient.py`): the rows at the
 given slots of the gathered matrix are overwritten with the ALIE / IPM row of the others, on every rank (a collective call).
 Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
+`pre_aggregation="nnm"` (nearest-neighbour mixing, `aggregators/_ops.py`) replaces every gathered row by the mean of its n - f
+nearest rows before the rule runs, on every engine: inside the fused kernel, in the stand-alone kernel of the baseline engine, with
+the host library's distances on the host engine and with the torch reference for plug-ins without a fused spec. The GAR object
+itself does not mix.
 """
 
 import os
@@ -35,11 +39,30 @@ def _world(group=None):
   return 0, 1
 
 
+def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz):
+  """-> (mix, f of the mix, fused spec or None). NNM mixes with the declared f: `nb_decl_byz`, or by default the rule's own f. Rules
+  whose spec ignores f (average, average-nan, median, averaged-median) carry the declared f in their spec for the kernel's mix."""
+  from ..aggregators import FusedSpec, _ops
+  mix = _ops.check_pre_aggregation(pre_aggregation)   # None or "nnm"
+  spec = gar.fused_spec()
+  own = spec.f if spec is not None and spec.rule in FusedSpec.RULES_WITH_F else getattr(gar, "_f", None)
+  f = own if nb_decl_byz is None else int(nb_decl_byz)
+  if mix is None:
+    return None, f, spec
+  if f is None:
+    raise tools.UserException("Nearest-neighbour mixing needs the declared number of Byzantine workers f of GAR " + type(gar).__name__)
+  if own is not None and own != f:
+    raise tools.UserException("Nearest-neighbour mixing runs with the rule's f = %d (got f = %d)" % (own, f))
+  _ops.check_nnm(nbworkers, f)
+  return mix, f, (spec.with_mix(mix, f) if spec is not None else None)
+
+
 class _AggregationBase:
   """Common state: layout, optimizer spec and slots, update counter."""
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None):
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, pre_aggregation=None, nb_decl_byz=None):
     self.gar = gar
+    self.mix, self.f, self.spec = _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz)
     self.layout = layout
     self.n = nbworkers
     self.optimizer = optimizer
@@ -55,7 +78,7 @@ class _AggregationBase:
 
   def _make_center(self):
     """Allocate the center (+0) when the rule is centered clipping; it lives as long as the engine and travels in checkpoints."""
-    spec = self.gar.fused_spec()
+    spec = self.spec
     if spec is not None and spec.rule == "centered-clipping":
       self.center = torch.zeros(self.d, dtype=torch.float32, device=self.device)
 
@@ -106,8 +129,8 @@ class HostAggregation(_AggregationBase):
 
   name = "host"
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cpu"):
-    super().__init__(gar, layout, nbworkers, optimizer, group)
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
     self.device = torch.device(device)
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
@@ -130,7 +153,11 @@ class HostAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
-    aggregated = self.gar.aggregate(self._gathered) if self.center is None else self.gar.aggregate(self._gathered, center=self.center)
+    rows = self._gathered
+    if self.mix is not None:
+      from ..aggregators import _ops
+      rows = _ops.host_nnm(rows, self.f) if rows.device.type == "cpu" else _ops.torch_nnm(rows, self.f)
+    aggregated = self.gar.aggregate(rows) if self.center is None else self.gar.aggregate(rows, center=self.center)
     self.updates += 1
     self.optimizer.apply_torch(self.params, aggregated, self.slots, rate, self.updates)
     self.last_aggregate = aggregated
@@ -141,10 +168,9 @@ class BaselineAggregation(_AggregationBase):
 
   name = "baseline"
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda"):
-    super().__init__(gar, layout, nbworkers, optimizer, group)
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", pre_aggregation=None, nb_decl_byz=None):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
     self.device = torch.device(device)
-    self.spec = gar.fused_spec()
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
     self.slots = optimizer.make_slots(self.params)
@@ -167,9 +193,13 @@ class BaselineAggregation(_AggregationBase):
     self._gather()
     state = {} if self.center is None else {"center": self.center}
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
-      aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)
+      aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)   # mixes inside the kernel
     else:
-      aggregated = self.gar.aggregate(self._gathered, **state)
+      rows = self._gathered
+      if self.mix is not None:
+        from ..aggregators import _ops
+        rows = _ops.torch_nnm(rows, self.f)
+      aggregated = self.gar.aggregate(rows, **state)
     self.updates += 1
     if self.optimizer.name == "sgd":
       gar_ops.sgd_(self.params, aggregated, rate)
@@ -191,10 +221,10 @@ class FusedAggregation(_AggregationBase):
 
   name = "fused"
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", keep_aggregate=False, bf16_copy=False, max_ctas=0, buckets=None, device_state=False):
-    super().__init__(gar, layout, nbworkers, optimizer, group)
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", keep_aggregate=False, bf16_copy=False, max_ctas=0, buckets=None, device_state=False,
+               pre_aggregation=None, nb_decl_byz=None):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
     self.device = torch.device(device)
-    self.spec = gar.fused_spec()
     if self.spec is None:
       raise tools.UserException("GAR " + type(gar).__name__ + " has no fused kernel; use the baseline/host engine")
     if self.spec.n != nbworkers:
@@ -220,8 +250,10 @@ class FusedAggregation(_AggregationBase):
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
-    # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows
-    need_staging = (self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
+    # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; NNM mixes the staged tile in place
+    # and every rule then reads it (n * owned * 4 bytes, also with R = 1)
+    need_staging = ((self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
+                    or self.mix is not None)
     self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     self.max_ctas = max_ctas
@@ -242,9 +274,9 @@ class FusedAggregation(_AggregationBase):
     self._mailboxes = [heap.peer(q, "mailbox") for q in range(R)]
     self._param_mc = heap.multicast("params") if R > 1 else 0
     # in-switch (NVLS) reduction of the gradients for the `average` rule instead of 7 P2P loads (0.241 vs 0.312 ms at 8 GPUs); AGB_NVLS_REDUCE=0 disables
-    self._grad_mc = heap.multicast("grads") if (R > 1 and self.spec.rule == "average" and os.environ.get("AGB_NVLS_REDUCE", "1") not in ("", "0")) else 0
-    tools.info("Fused aggregation: rule %r, n = %d (%d per rank), d = %d, %d bucket(s), %d owned coordinates, provider %s, NVLS multicast %s" % (
-      self.spec.rule, self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
+    self._grad_mc = heap.multicast("grads") if (R > 1 and self.spec.rule == "average" and self.mix is None and os.environ.get("AGB_NVLS_REDUCE", "1") not in ("", "0")) else 0
+    tools.info("Fused aggregation: rule %r%s, n = %d (%d per rank), d = %d, %d bucket(s), %d owned coordinates, provider %s, NVLS multicast %s" % (
+      self.spec.rule, " after NNM" if self.mix else "", self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
 
   @staticmethod
   def _check_buckets(buckets, d):
@@ -269,8 +301,9 @@ class FusedAggregation(_AggregationBase):
 
   @property
   def overlappable(self):
-    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates)."""
-    return self.distance_rule and len(self.buckets) > 1
+    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates); not with NNM,
+    whose raw distance pass runs in the finish kernel over every segment."""
+    return self.distance_rule and len(self.buckets) > 1 and self.mix is None
 
   def visible_rows(self):
     """Every worker's row through the peer mapping — the very addresses the fused kernel dereferences."""
@@ -367,9 +400,11 @@ def _single_host(group=None):
   return len(set(hosts)) == 1
 
 
-def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device="cpu", **kwargs):
+def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None, **kwargs):
   """`kind` in {"auto", "fused", "baseline", "host"}; "auto" = fused on CUDA when the rule has a kernel and all ranks share one
-  machine, the NCCL baseline engine on CUDA otherwise, host on CPU."""
+  machine, the NCCL baseline engine on CUDA otherwise, host on CPU. `pre_aggregation`: None / "none" or "nnm", on every engine, with
+  `nb_decl_byz` declared Byzantine workers (default: the rule's f)."""
+  mix = dict(pre_aggregation=pre_aggregation, nb_decl_byz=nb_decl_byz)
   device = torch.device(device)
   if kind == "auto":
     if device.type != "cuda":
@@ -382,9 +417,9 @@ def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device
     else:
       kind = "baseline"
   if kind == "fused":
-    return FusedAggregation(gar, layout, nbworkers, optimizer, group, device, **kwargs)
+    return FusedAggregation(gar, layout, nbworkers, optimizer, group, device, **mix, **kwargs)
   if kind == "baseline":
-    return BaselineAggregation(gar, layout, nbworkers, optimizer, group, device)
+    return BaselineAggregation(gar, layout, nbworkers, optimizer, group, device, **mix)
   if kind == "host":
-    return HostAggregation(gar, layout, nbworkers, optimizer, group, device)
+    return HostAggregation(gar, layout, nbworkers, optimizer, group, device, **mix)
   raise tools.UserException("Unknown aggregation engine " + repr(kind))

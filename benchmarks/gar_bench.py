@@ -15,6 +15,9 @@ the crafting kernel is also timed alone, next to the torch reference on the same
 `geometric-median` and `centered-clipping` entries also report their T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
 `--gar-worker-momentum beta` also times the worker-momentum kernel alone on the [w, d] rows of a rank (`ops.gar.worker_momentum_`,
 dampening 0), with the 16 * w * d bytes it must move (G and M read and written once).
+`--gar-pre-aggregation nnm` runs both engines with nearest-neighbour mixing before every rule (the checks above then hold for the
+mixed step), and also times the fused step of each rule without NNM, alternating with and without in the same process, to report
+the measured cost of the mix (`nnm_ms`, `plain_ms`, `nnm_overhead_ms`: medians over the alternated rounds).
 """
 
 import argparse
@@ -50,6 +53,8 @@ def main():
                       help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
   parser.add_argument("--gar-worker-momentum", dest="worker_momentum", type=float, default=None, metavar="BETA",
                       help="also time the worker-momentum kernel with this beta on the [w, d] rows of a rank")
+  parser.add_argument("--gar-pre-aggregation", dest="pre_aggregation", choices=("none", "nnm"), default="none",
+                      help="pre-aggregation of both engines (nnm: nearest-neighbour mixing, with the rule's f); nnm also times each rule without it")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -104,8 +109,9 @@ def main():
     name = {"krum": "krum", "bulyan": "bulyan"}.get(rule, rule)
     gar = aggregators.instantiate(name, n, f, args.rule_args or [])
     sgd = build(optimizers, "optimizer", "sgd", [])
-    fused = FusedAggregation(gar, layout, n, sgd, device=device, keep_aggregate=True)
-    base = BaselineAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device)
+    mix = dict(pre_aggregation=args.pre_aggregation, nb_decl_byz=f)
+    fused = FusedAggregation(gar, layout, n, sgd, device=device, keep_aggregate=True, **mix)
+    base = BaselineAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, **mix)
     gen = torch.Generator(device=device).manual_seed(1234)
     init = torch.randn(d, device=device, generator=gen)
     fused.params.copy_(init)
@@ -170,6 +176,27 @@ def main():
         engine.step(0.1)
     fused_ms = time_engine(fused)
     base_ms = time_engine(base)
+    mix_entry = {}
+    if fused.mix is not None:
+      # the same rule without NNM on the same rows, alternated with the NNM engine round by round (clock and thermal drift hit both)
+      plain = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True)
+      plain.params.copy_(init)
+      plain.grads.copy_(fused.grads)
+      for _ in range(3):
+        craft(plain)
+        plain.step(0.1)
+      rounds = {"nnm": [], "plain": []}
+      for _ in range(5):
+        rounds["nnm"].append(time_engine(fused))
+        rounds["plain"].append(time_engine(plain))
+      median = lambda values: sorted(values)[len(values) // 2]
+      nnm_ms, plain_ms = median(rounds["nnm"]), median(rounds["plain"])
+      mix_entry = {"pre_aggregation": fused.mix, "nnm_ms": nnm_ms, "plain_ms": plain_ms, "nnm_overhead_ms": nnm_ms - plain_ms,
+                   "nnm_rounds_ms": rounds["nnm"], "plain_rounds_ms": rounds["plain"],
+                   # local HBM bytes the mix adds: the staging store, the mix pass (read + write), the rule's read of the tile, and one more
+                   # read for the distance pass of the mixed rows (Krum / Bulyan / MDA)
+                   "nnm_tile_hbm_bytes": (4 + (1 if rule in ("krum", "bulyan", "mda") else 0)) * n * (fused.hi - fused.lo) * 4}
+      del plain
     attack_entry = {}
     if attack is not None:
       def time_craft(fn):
@@ -199,7 +226,7 @@ def main():
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
-    if rule in ("krum", "bulyan", "mda"):
+    if rule in ("krum", "bulyan", "mda") and fused.mix is None:   # no bucketed distance pass with NNM
       c1, c2, c3 = (d // 2) // 8 * 8, (d // 5) // 8 * 8, (d // 16) // 8 * 8
       over = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True,
                               buckets=[(c1, d), (c2, c1), (c3, c2), (0, c3)], device_state=True)
@@ -250,6 +277,7 @@ def main():
                      "bucketed_total_ms": bucketed_ms, "finish_kernel_exposed_ms": exposed_ms,
                      "local_hbm_bytes": hbm, "hbm_gbs": hbm / fused_ms / 1e6 if world == 1 else None}
     results[rule].update(attack_entry)
+    results[rule].update(mix_entry)
     if args.rule_args is not None:
       results[rule]["rule_args"] = args.rule_args
     if rule in ("geometric-median", "centered-clipping"):
@@ -262,7 +290,7 @@ def main():
       print(rule, json.dumps(results[rule]))
     del fused, base
     torch.cuda.empty_cache()
-  report = {"world": world, "n": n, "d": args.d, "results": results}
+  report = {"world": world, "n": n, "d": args.d, "pre_aggregation": args.pre_aggregation, "results": results}
   if args.worker_momentum is not None:
     beta, c = _ops.check_worker_momentum(args.worker_momentum, 0.0)
     rows = torch.randn((w, d), device=device)
