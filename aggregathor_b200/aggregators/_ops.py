@@ -539,17 +539,55 @@ def torch_bulyan(G, f, m, return_weights=False):
 # ---------------------------------------------------------------------------- #
 # Omniscient Byzantine rows (`attacks/omniscient.py`): the literal definition, the CPU back-end and the oracle of the sm_90a kernel
 
+OPTIMIZED_MODES = ("min-max", "min-sum")   # Shejwalkar & Houmansadr, NDSS 2021: gamma solved from whole-vector sums
+DEVIATIONS = ("unit-vec", "sign", "std")
+
+
 def check_byzantine_slots(n, byz_slots, mode):
-  """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("alie" needs 2 honest rows, "ipm" one)."""
-  if mode not in ("alie", "ipm"):
+  """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("ipm" needs 1 honest row, the others 2)."""
+  if mode not in ("alie", "ipm") + OPTIMIZED_MODES:
     raise tools.UserException("Unknown omniscient attack mode " + repr(mode))
   slots = sorted({int(i) for i in byz_slots})
   if not slots or slots[0] < 0 or slots[-1] >= n:
     raise tools.UserException("Byzantine slots must be a non-empty subset of [0, %d) (got %r)" % (n, list(byz_slots)))
-  need = 2 if mode == "alie" else 1
+  need = 1 if mode == "ipm" else 2
   if n - len(slots) < need:
     raise tools.UserException("%s needs at least %d honest row(s) (n = %d, %d Byzantine)" % (mode.upper(), need, n, len(slots)))
   return slots
+
+
+def check_deviation(mode, deviation):
+  """The deviation of Min-Max / Min-Sum: "unit-vec" (default), "sign" or "std"."""
+  if deviation is None:
+    return "unit-vec"
+  if deviation not in DEVIATIONS:
+    raise tools.UserException("%s: unknown deviation %r (expected one of %s)" % (mode, deviation, ", ".join(DEVIATIONS)))
+  return deviation
+
+
+def _scalar(G):
+  # divisors are device tensors: a Python-number divisor may be turned into a multiplication by its reciprocal on the GPU
+  return lambda value: torch.tensor(value, dtype=torch.float32, device=G.device)
+
+
+def _honest_mean(honest, scalar):
+  """mu = ((h0 + h1) + ...) / H, fp32, one rounded operation at a time."""
+  mu = honest[0]
+  for h in honest[1:]:
+    mu = mu + h
+  return mu / scalar(len(honest))
+
+
+def _honest_sigma(honest, mu, scalar):
+  """sqrt(sum_i (h_i - mu)^2 / (H - 1)), same order and rounding as `_honest_mean`."""
+  var = None
+  for h in honest:
+    dev = h - mu
+    square = dev * dev
+    var = square if var is None else var + square
+  # torch's vectorised fp32 sqrt on the CPU is not always correctly rounded: the square root of an fp32 value taken in fp64 and
+  # rounded once to fp32 is (fp64 carries more than 2 * 24 + 2 bits)
+  return torch.sqrt((var / scalar(len(honest) - 1)).double()).float()
 
 
 def torch_byzantine_row(G, byz_slots, mode, coef):
@@ -558,34 +596,100 @@ def torch_byzantine_row(G, byz_slots, mode, coef):
   time (separate torch calls, nothing that may fuse into an FMA)."""
   byz = set(check_byzantine_slots(G.shape[0], byz_slots, mode))
   honest = [G[i] for i in range(G.shape[0]) if i not in byz]
-  # divisors are device tensors: a Python-number divisor may be turned into a multiplication by its reciprocal on the GPU
-  scalar = lambda value: torch.tensor(value, dtype=torch.float32, device=G.device)
+  scalar = _scalar(G)
   coef = scalar(coef)
-  mu = honest[0]
-  for h in honest[1:]:
-    mu = mu + h
-  mu = mu / scalar(len(honest))
+  mu = _honest_mean(honest, scalar)
   if mode == "ipm":
     return torch.neg(coef) * mu
-  var = None
+  return mu + coef * _honest_sigma(honest, mu, scalar)
+
+
+def optimized_deviation(G, byz_slots, mode, deviation):
+  """(mu, p) of Min-Max / Min-Sum, fp32 per coordinate: ALIE's mu, and p = mu (unit-vec), sign(mu) (+1, -1, +0 for +-0, NaN for NaN)
+  or ALIE's sigma (std)."""
+  byz = set(check_byzantine_slots(G.shape[0], byz_slots, mode))
+  honest = [G[i] for i in range(G.shape[0]) if i not in byz]
+  scalar = _scalar(G)
+  mu = _honest_mean(honest, scalar)
+  deviation = check_deviation(mode, deviation)
+  if deviation == "std":
+    return mu, _honest_sigma(honest, mu, scalar)
+  if deviation == "sign":
+    one = torch.ones_like(mu)
+    return mu, torch.where(mu > 0, one, torch.where(mu < 0, -one, torch.where(mu == 0, torch.zeros_like(mu), mu)))
+  return mu, mu
+
+
+def optimized_statistics(G, byz_slots, mode, deviation):
+  """(mu, p, A, B, C, T) of Min-Max / Min-Sum: A_i = sum (mu - h_i)^2 and B_i = sum (mu - h_i) p over the honest rows (ascending slots),
+  C = sum p^2 and, for Min-Max, T = max_{j<k} sum (h_j - h_k)^2 (None for Min-Sum). The sums are taken in float64 from the fp32 mu, p and
+  rows, then rounded once to fp32 (Python floats); a non-finite sum stays non-finite."""
+  byz = set(check_byzantine_slots(G.shape[0], byz_slots, mode))
+  honest = [G[i] for i in range(G.shape[0]) if i not in byz]
+  mu, p = optimized_deviation(G, byz_slots, mode, deviation)
+  mu64, p64 = mu.double(), p.double()
+  A, B = [], []
   for h in honest:
-    dev = h - mu
-    square = dev * dev
-    var = square if var is None else var + square
-  # torch's vectorised fp32 sqrt on the CPU is not always correctly rounded: the square root of an fp32 value taken in fp64 and
-  # rounded once to fp32 is (fp64 carries more than 2 * 24 + 2 bits)
-  sigma = torch.sqrt((var / scalar(len(honest) - 1)).double()).float()
-  return mu + coef * sigma
+    dev = mu64 - h.double()
+    A.append(fp32(float((dev * dev).sum())))
+    B.append(fp32(float((dev * p64).sum())))
+  C = fp32(float((p64 * p64).sum()))
+  T = None
+  if mode == "min-max":
+    X = torch.stack(honest).double()
+    dist = torch.cat([((X[j + 1:] - X[j]) ** 2).sum(dim=1) for j in range(len(honest) - 1)])
+    T = fp32(float(dist.max())) if bool(torch.isfinite(dist).all()) else math.nan
+  return mu, p, A, B, C, T
 
 
-def torch_craft_byzantine_(G, byz_slots, mode, coef):
-  """In place on the [n, d] fp32 matrix G: every Byzantine row <- `torch_byzantine_row`; honest rows are not written."""
+def optimized_gamma(mode, A, B, C, T=None):
+  """gamma of Min-Max / Min-Sum from the fp32 sums (Python floats), in float64 with one rounding per operation, rounded once to fp32:
+  Min-Max: min_i gamma_i, E_i = max(T - A_i, 0), S_i = sqrt(B_i^2 + C E_i), gamma_i = (B_i + S_i) / C if B_i >= 0 else E_i / (S_i - B_i);
+  Min-Sum: sqrt(max_i A_i / C). 0 when C == 0 or any sum is not finite. The sm_90a kernel runs the same operations."""
+  values = list(A) + list(B) + [C] + ([T] if mode == "min-max" else [])
+  if C == 0 or not all(math.isfinite(v) for v in values):
+    return 0.0
+  if mode == "min-sum":
+    return fp32(math.sqrt(max(A) / C))
+  gamma = None
+  for a, b in zip(A, B):
+    e = max(T - a, 0.0)
+    s = math.sqrt(b * b + C * e)
+    g = (b + s) / C if b >= 0 else e / (s - b)
+    gamma = g if gamma is None else min(gamma, g)
+  return fp32(gamma)
+
+
+def optimized_coefficient(deviation, gamma, C):
+  """The push along the deviation's direction: gamma * sqrt(C) for unit-vec (p = mu / ||mu|| in the paper), gamma otherwise."""
+  return gamma * math.sqrt(C) if deviation == "unit-vec" and math.isfinite(C) else gamma
+
+
+def torch_optimized_row(G, byz_slots, mode, deviation, gamma):
+  """The Min-Max / Min-Sum row for a given fp32 `gamma`: mu - gamma * p, one rounded fp32 operation at a time (the kernel's arithmetic)."""
+  mu, p = optimized_deviation(G, byz_slots, mode, deviation)
+  return mu - _scalar(G)(gamma) * p
+
+
+def torch_craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False):
+  """In place on the [n, d] fp32 matrix G: every Byzantine row <- `torch_byzantine_row` (ALIE, IPM) or, for Min-Max / Min-Sum, the row
+  of `torch_optimized_row` with the gamma of `optimized_gamma`; honest rows are not written. Min-Max / Min-Sum with `return_details`
+  return (gamma, A, B, C, T) instead of G."""
   if G.dtype != torch.float32:
     raise tools.UserException("Omniscient attacks craft fp32 rows (got %s)" % G.dtype)
-  row = torch_byzantine_row(G, byz_slots, mode, coef)
+  details = None
+  if mode in OPTIMIZED_MODES:
+    mu, p, A, B, C, T = optimized_statistics(G, byz_slots, mode, deviation)
+    gamma = optimized_gamma(mode, A, B, C, T)
+    row = mu - _scalar(G)(gamma) * p
+    details = (gamma, A, B, C, T)
+  elif return_details:
+    raise tools.UserException("return_details is for Min-Max / Min-Sum only")
+  else:
+    row = torch_byzantine_row(G, byz_slots, mode, coef)
   for i in check_byzantine_slots(G.shape[0], byz_slots, mode):
     G[i].copy_(row)
-  return G
+  return details if return_details else G
 
 
 # ---------------------------------------------------------------------------- #

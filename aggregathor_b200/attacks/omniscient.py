@@ -4,10 +4,17 @@
           standard deviation of the honest rows. `z` defaults to z_max = Phi^-1((n - s) / n), s = floor(n / 2 + 1) - k, the largest shift
           that keeps the Byzantine rows inside the crowd the rule is supposed to trust.
 * `ipm`   inner-product manipulation ("Fall of Empires", Xie, Koyejo, Gupta, UAI 2019): b = -epsilon * mu (`epsilon` defaults to 0.1).
+* `min-max`, `min-sum`  the AGR-agnostic attacks of Shejwalkar & Houmansadr ("Manipulating the Byzantine: Optimizing Model Poisoning
+          Attacks and Defenses for Federated Learning", NDSS 2021): b = mu - gamma * p along the deviation p (`deviation:unit-vec`, the
+          default: p = mu, whose normalisation is folded into gamma; `sign`: sign(mu); `std`: ALIE's sigma), with the largest gamma that
+          keeps b inside the spread of the honest rows: Min-Max bounds max_i ||b - h_i||^2 by the largest honest distance
+          max_jk ||h_j - h_k||^2, Min-Sum bounds sum_i ||b - h_i||^2 by max_i sum_j ||h_i - h_j||^2. gamma is solved in closed form
+          (`aggregators._ops.optimized_gamma`) instead of the authors' search, and is not capped (their search stays below 20).
 
 The rows are crafted by the aggregation engine (`craft_byzantine`), not per worker: on the fused engine every rank computes its owned
 coordinates of every Byzantine row from the honest values it already reads for the rule, and stores them into the Byzantine rows over
-NVLink. The exact arithmetic is `aggregators._ops.torch_byzantine_row`. The Byzantine workers are the last k logical workers.
+NVLink (Min-Max / Min-Sum first exchange their whole-vector sums between the ranks). The exact arithmetic is
+`aggregators._ops.torch_byzantine_row` and `torch_optimized_row`. The Byzantine workers are the last k logical workers.
 """
 
 import math
@@ -37,6 +44,7 @@ def default_z(nbworkers, nbbyzwrks):
 class _Omniscient(_Attack):
   omniscient = True
   mode = None
+  deviation = None   # Min-Max / Min-Sum: "unit-vec", "sign" or "std"
   min_honest = 1
 
   def __init__(self, nbworkers, nbbyzwrks, args):
@@ -76,5 +84,29 @@ class IpmAttack(_Omniscient):
     self.coef = self._coefficient("epsilon", lambda: _fp32(0.1))
 
 
+class _OptimizedAttack(_Omniscient):
+  """Min-Max / Min-Sum: no coefficient (gamma is solved every step from the honest rows), only the deviation."""
+  min_honest = 2
+
+  def __init__(self, nbworkers, nbbyzwrks, args):
+    super().__init__(nbworkers, nbbyzwrks, args)
+    from ..aggregators import _ops
+    unknown = set(self.args) - {"deviation"}
+    if unknown:
+      raise tools.UserException("%s: unknown argument(s) %s (expected 'deviation:unit-vec|sign|std')" % (self.mode, ", ".join(sorted(unknown))))
+    self.deviation = _ops.check_deviation(self.mode, self.args.get("deviation"))
+    self.coef = None
+
+
+class MinMaxAttack(_OptimizedAttack):
+  mode = "min-max"
+
+
+class MinSumAttack(_OptimizedAttack):
+  mode = "min-sum"
+
+
 register("alie", AlieAttack)
 register("ipm", IpmAttack)
+register("min-max", MinMaxAttack)
+register("min-sum", MinSumAttack)

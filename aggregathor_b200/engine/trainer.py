@@ -381,7 +381,9 @@ class Manager:
       self._apply_momentum()
     if getattr(self.attack, "omniscient", False):
       if self.byzantine_slots:   # collective: every rank crafts its share, whether or not it hosts a Byzantine worker
-        self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef)
+        deviation = getattr(self.attack, "deviation", None)   # Min-Max / Min-Sum only: other engines' signatures stay as they were
+        extra = {} if deviation is None else {"deviation": deviation}
+        self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef, **extra)
       return losses
     forging = self.authenticator is not None and getattr(self.attack, "forges", False)
     for j, i in enumerate(self.local_workers):

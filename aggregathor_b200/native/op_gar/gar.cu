@@ -22,7 +22,8 @@
 // exchange, one selection warp, then every row of the staged tile is replaced by the mean of its n - f nearest rows; the rule then
 // reads the mixed tile (see `nnm_pre_aggregation`).
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
-// every Byzantine row from the honest values.
+// every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
+// whole-vector sums between the ranks, then the same per-coordinate write.
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
 // registers at a time; more rows are processed in 8-row blocks (diagonal + cross passes over the staged copy).
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
@@ -51,8 +52,15 @@ constexpr int kSlotCraft = kMaxSeg + 2;   // entry barrier of the Byzantine craf
 constexpr int kMaxIterations = 16;        // geometric median, centered clipping: iterations
 constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median, centered clipping: one exchange slot per iteration
 constexpr int kSlotMix = kSlotGeoMedian + kMaxIterations;   // NNM: exchange of the raw distances
-constexpr int kFlagSlots = kSlotMix + 1;
+constexpr int kSlotCraftStats = kSlotMix + 1;   // Min-Max / Min-Sum: exchange of the crafting statistics
+constexpr int kFlagSlots = kSlotCraftStats + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
+// Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
+// They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
+constexpr int kStatA = kMaxPairs, kStatB = kStatA + kMaxWorkers, kStatC = kStatB + kMaxWorkers;
+constexpr int kCraftStats = kStatC + 1;   // 561
+constexpr int kCraftRegion = 2 * kMailboxRegion;
+constexpr int kMailboxFloats = kCraftRegion + kMaxRanks * kCraftStats;
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
@@ -321,13 +329,13 @@ __device__ __forceinline__ int pair_index(int i, int j, int n) {
 }
 
 // offset of segment `seg` inside the staged copy (segments are stored back to back)
-__device__ __forceinline__ long long staged_offset(GarArgs const& a, int seg) {
+template<class Args> __device__ __forceinline__ long long staged_offset(Args const& a, int seg) {
     long long off = 0;
     for (int s = 0; s < seg; ++s)
         off += a.seg_hi[s] - a.seg_lo[s];
     return off;
 }
-__device__ __forceinline__ long long owned_length(GarArgs const& a) {
+template<class Args> __device__ __forceinline__ long long owned_length(Args const& a) {
     return staged_offset(a, a.nseg);
 }
 
@@ -556,8 +564,9 @@ __device__ __forceinline__ float sq_dist(float4 const& u, float4 const& v) {
 }
 
 // STAGED_ONLY (NNM's distances of the mixed rows): every pass, block 0's diagonal included, reads the staged tile and stores nothing.
-template<bool CROSS, bool STAGED_ONLY = false>
-__device__ void phase_a_segment(GarArgs const& a, Shared& sh, int* pair_of, int seg, float* out, long long tid, long long nthreads) {
+// `Args`: GarArgs, or ByzArgs for the honest distances of Min-Max (n, grad, staging and the segments, as GarArgs names them).
+template<bool CROSS, bool STAGED_ONLY = false, class Args>
+__device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg, float* out, long long tid, long long nthreads) {
     constexpr int B = kBlockRows, NPB = B * (B - 1) / 2;
     int const n = a.n, nb = CROSS ? (n + B - 1) / B : 1;
     long long const lo = a.seg_lo[seg], len4 = (a.seg_hi[seg] - lo) >> 2;
@@ -1315,8 +1324,17 @@ struct ByzArgs {
     uint32_t* signal[kMaxRanks];
     uint32_t epoch;
     uint32_t* epoch_ptr;
+    // Min-Max / Min-Sum only (`gar_optimized_kernel`)
+    int deviation;                     // 0: unit-vec (p = mu), 1: sign (p = sign(mu)), 2: std (p = sigma)
+    int n;                             // the honest rows as `phase_a_segment` reads them: n = H rows grad[0, H), ascending slots,
+    float const* grad[kMaxWorkers];    // no staging
+    float* staging;
+    float* mailbox[kMaxRanks];         // every rank's mailbox; region 2 (float offset kCraftRegion) carries the statistics
+    float* partials;                   // [grid][kCraftStats] CTA partials of this rank
+    float* stats_out;                  // optional [1 + kCraftStats]: gamma, then the statistics summed over the ranks
 };
-enum ByzMode { kAlie = 0, kIpm = 1 };
+enum ByzMode { kAlie = 0, kIpm = 1, kMinMax = 2, kMinSum = 3 };
+enum Deviation { kUnitVec = 0, kSign = 1, kStd = 2 };
 
 template<int N>
 __global__ void __launch_bounds__(256) gar_byzantine_kernel(ByzArgs const a) {
@@ -1396,6 +1414,277 @@ __global__ void __launch_bounds__(256) gar_byzantine_kernel(ByzArgs const a) {
                 for (int c = 0; c < 4; ++c)
                     out[c] = __fadd_rn(mu[c], __fmul_rn(a.coef, __fsqrt_rn(__fdiv_rn(var[c], dof))));
             }
+            for (int k = 0; k < a.K; ++k)
+                V<4>::store_stream(a.rows[a.byz[k]] + x, out);
+        }
+    }
+    fence_sys();
+}
+
+// ---- Min-Max / Min-Sum (Shejwalkar & Houmansadr, NDSS 2021) ------------------------------------ //
+// Every Byzantine row is b = mu - gamma * p, one rounded operation at a time, with ALIE's mu and the deviation p: mu (unit-vec), sign(mu)
+// (+1, -1, 0 for +-0, NaN for NaN) or ALIE's sigma (std). gamma is one fp32 scalar per step, solved in closed form from sums over all
+// d coordinates: A_i = sum (mu - h_i)^2, B_i = sum (mu - h_i) p, C = sum p^2 and, for Min-Max, the honest distances
+// D_jk = sum (h_j - h_k)^2, T = max D_jk:
+//   Min-Max: gamma = min_i gamma_i, E_i = max(T - A_i, 0), S_i = sqrt(B_i^2 + C E_i), gamma_i = (B_i + S_i) / C if B_i >= 0, else
+//            E_i / (S_i - B_i) (the largest gamma >= 0 with max_i ||b - h_i||^2 <= T);
+//   Min-Sum: gamma = sqrt(max_i A_i / C) (the summed constraint, reduced with sum_i B_i = 0 and sum_j D_ij = H A_i + sum A);
+// in float64 from the fp32 sums, rounded once; gamma = 0 when C == 0 or any of T, A_i, B_i, C is not finite.
+//
+// One cooperative launch per rank:
+//   1. entry barrier (slot kSlotCraft), as for ALIE / IPM;
+//   2. statistics pass over the owned segments: mu and p per coordinate, A_i / B_i / C accumulated per thread for 8 honest rows at a time
+//      (H <= 8: the H values stay in registers; above, one pass per 8-row block, mu and p recomputed from memory); Min-Max adds the
+//      honest distances with `phase_a_segment` on the honest rows. Every pass folds lanes -> warps -> CTA (`fold_pass`) into the CTA's
+//      slot of `partials`;
+//   3. grid barrier; block 0 adds the CTA slots in index order and posts the rank's sums into mailbox region 2 of every rank, then
+//      signals slot kSlotCraftStats; every CTA of every rank adds the R posts in rank order: the same bits, hence the same gamma,
+//      everywhere;
+//   4. write pass: mu and p recomputed from the honest rows (read a second time: staging them would cost 4 or 8 bytes of local HBM per
+//      owned coordinate for a pass that is bound by the honest reads either way), b stored into every Byzantine row (P2P stores).
+// It ends with a system-scope fence and no exit barrier, as `gar_byzantine_kernel` (same argument). Region 2 and slot kSlotCraftStats
+// are touched by no other kernel: a fast rank's finish kernel writes regions 0 / 1 of a slow rank's mailbox while the slow rank's
+// crafting CTAs may still be reading region 2. The next step's crafting does not race with this one: a rank posts into region 2 only
+// after the next entry barrier, i.e. after every rank has started its next crafting kernel, so after every rank's current crafting
+// kernel (same stream) has finished reading.
+
+// mu and p of the 4 coordinates at x. N > 0: the H <= N honest values are in g; N == 0: they are read from memory. mu and sigma are
+// computed exactly as in `gar_byzantine_kernel`.
+template<int N>
+__device__ __forceinline__ void mean_and_deviation(ByzArgs const& a, long long x, float const (&g)[N > 0 ? N : 1][4], float (&mu)[4], float (&p)[4]) {
+    int const H = a.H;
+    if constexpr (N > 0) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            mu[c] = g[0][c];
+#pragma unroll
+        for (int i = 1; i < N; ++i)
+            if (i < H) {
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    mu[c] = __fadd_rn(mu[c], g[i][c]);
+            }
+    } else {
+        V<4>::load(a.rows[a.honest[0]] + x, mu);
+        for (int i = 1; i < H; ++i) {
+            float h[4];
+            V<4>::load(a.rows[a.honest[i]] + x, h);
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                mu[c] = __fadd_rn(mu[c], h[c]);
+        }
+    }
+    float const count = static_cast<float>(H);
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+        mu[c] = __fdiv_rn(mu[c], count);
+    if (a.deviation == kStd) {
+        float var[4];
+        auto add_square = [&](int i, float const (&h)[4]) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                float const dev = __fsub_rn(h[c], mu[c]);
+                float const sq = __fmul_rn(dev, dev);
+                var[c] = i == 0 ? sq : __fadd_rn(var[c], sq);
+            }
+        };
+        if constexpr (N > 0) {
+#pragma unroll
+            for (int i = 0; i < N; ++i)
+                if (i < H)
+                    add_square(i, g[i]);
+        } else {
+            for (int i = 0; i < H; ++i) {
+                float h[4];
+                V<4>::load(a.rows[a.honest[i]] + x, h);
+                add_square(i, h);
+            }
+        }
+        float const dof = static_cast<float>(H - 1);
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            p[c] = __fsqrt_rn(__fdiv_rn(var[c], dof));
+    } else if (a.deviation == kSign) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            p[c] = mu[c] > 0.f ? 1.f : mu[c] < 0.f ? -1.f : mu[c] == 0.f ? 0.f : mu[c];
+    } else {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            p[c] = mu[c];
+    }
+}
+
+// A_i and B_i of the honest rows [i0, i0 + 8) (and C with the first block) over every owned segment, folded into `out`
+template<int N>
+__device__ void optimized_stats_pass(ByzArgs const& a, Shared& sh, int* pair_of, int i0, float* out, long long tid, long long nthreads) {
+    constexpr int B = kBlockRows, COUNT = 2 * B + 1;
+    static_assert(N == 0 || N == B, "registers hold one block of honest rows");
+    int const H = a.H;
+    if (threadIdx.x < COUNT) {
+        int const t = threadIdx.x, i = i0 + t % B;
+        pair_of[t] = t == 2 * B ? (i0 == 0 ? kStatC : -1) : i < H ? (t < B ? kStatA : kStatB) + i : -1;
+    }
+    __syncthreads();
+    float acc[COUNT];
+#pragma unroll
+    for (int k = 0; k < COUNT; ++k)
+        acc[k] = 0.f;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4];
+            mean_and_deviation<N>(a, x, g, mu, p);
+#pragma unroll
+            for (int i = 0; i < B; ++i) {
+                if (i0 + i < H) {
+                    float h[4];
+                    if constexpr (N > 0) {
+#pragma unroll
+                        for (int c = 0; c < 4; ++c)
+                            h[c] = g[i][c];
+                    } else {
+                        V<4>::load(a.rows[a.honest[i0 + i]] + x, h);
+                    }
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        float const dev = __fsub_rn(mu[c], h[c]);
+                        acc[i] = __fmaf_rn(dev, dev, acc[i]);
+                        acc[B + i] = __fmaf_rn(dev, p[c], acc[B + i]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                acc[2 * B] = __fmaf_rn(p[c], p[c], acc[2 * B]);
+        }
+    }
+    fold_pass<COUNT>(sh, acc, out, pair_of);
+}
+
+// gamma from the statistics summed over the ranks (see above), float64 with explicit roundings (no FMA contraction), rounded once to fp32
+__device__ float optimized_gamma(int mode, int H, float const* st) {
+    bool ok = is_finite(st[kStatC]) && st[kStatC] != 0.f;
+    double const C = st[kStatC];
+    double amax = 0.0, T = 0.0;
+    for (int i = 0; i < H; ++i) {
+        ok = ok && is_finite(st[kStatA + i]) && is_finite(st[kStatB + i]);
+        amax = fmax(amax, static_cast<double>(st[kStatA + i]));
+    }
+    if (mode == kMinMax) {
+        for (int k = 0; k < H * (H - 1) / 2; ++k) {
+            ok = ok && is_finite(st[k]);
+            T = fmax(T, static_cast<double>(st[k]));
+        }
+    }
+    if (!ok)
+        return 0.f;
+    if (mode == kMinSum)
+        return __double2float_rn(__dsqrt_rn(__ddiv_rn(amax, C)));
+    double gamma = 0.0;
+    for (int i = 0; i < H; ++i) {
+        double const A = st[kStatA + i], Bi = st[kStatB + i];
+        double const E = fmax(__dsub_rn(T, A), 0.0);
+        double const S = __dsqrt_rn(__dadd_rn(__dmul_rn(Bi, Bi), __dmul_rn(C, E)));
+        double const gi = Bi >= 0.0 ? __ddiv_rn(__dadd_rn(Bi, S), C) : __ddiv_rn(E, __dsub_rn(S, Bi));
+        gamma = i == 0 ? gi : fmin(gamma, gi);
+    }
+    return __double2float_rn(gamma);
+}
+
+template<int N>
+__global__ void __launch_bounds__(256) gar_optimized_kernel(ByzArgs const a) {
+    __shared__ Shared sh;
+    __shared__ int pair_of[kBlockRows * kBlockRows];
+    __shared__ float stats[kCraftStats];
+    __shared__ float gamma_sh;
+    cg::grid_group grid = cg::this_grid();
+    bool const multi = a.R > 1;
+    uint32_t const epoch = current_epoch(a);
+    if (multi) {
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const H = a.H;
+    float* const mine = a.partials + static_cast<long long>(blockIdx.x) * kCraftStats;
+    for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x)
+        mine[k] = 0.f;
+    __syncthreads();
+    // -------- statistics of the owned coordinates -------- //
+    for (int i0 = 0; i0 < H; i0 += kBlockRows)
+        optimized_stats_pass<N>(a, sh, pair_of, i0, mine, tid, nthreads);
+    if (a.mode == kMinMax) {
+        for (int seg = 0; seg < a.nseg; ++seg)
+            phase_a_segment<(N == 0)>(a, sh, pair_of, seg, mine, tid, nthreads);
+    }
+    // -------- exchange: CTAs in index order, then ranks in rank order -------- //
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.partials + static_cast<long long>(b) * kCraftStats + k);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kCraftRegion + a.rank * kCraftStats + k] = s;
+        }
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, kSlotCraftStats, epoch);
+    }
+    if (multi) {
+        wait_all(a, kSlotCraftStats, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    float const* const box = a.mailbox[a.rank] + kCraftRegion;
+    for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x) {
+        float s = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            s += ld_volatile_f(box + q * kCraftStats + k);
+        stats[k] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+        gamma_sh = optimized_gamma(a.mode, H, stats);
+    __syncthreads();
+    float const gamma = gamma_sh;
+    if (a.stats_out && blockIdx.x == 0) {
+        for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x)
+            a.stats_out[1 + k] = stats[k];
+        if (threadIdx.x == 0)
+            a.stats_out[0] = gamma;
+    }
+    // -------- b = mu - gamma * p into every Byzantine row -------- //
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4], out[4];
+            mean_and_deviation<N>(a, x, g, mu, p);
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                out[c] = __fsub_rn(mu[c], __fmul_rn(gamma, p[c]));
             for (int k = 0; k < a.K; ++k)
                 V<4>::store_stream(a.rows[a.byz[k]] + x, out);
         }
@@ -1604,7 +1893,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
 extern "C" {
 
 char const* agb_op_list() {
-    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,sgd,worker_momentum,drop_chunks,checksum,cast_bf16";
+    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,gar_byzantine_optimized,sgd,worker_momentum,drop_chunks,checksum,cast_bf16";
 }
 
 // Wall-clock bound (seconds, 0 = none) of the cross-GPU flag waits of this library's kernels.
@@ -1623,7 +1912,7 @@ int agb_gar_max_ctas() {
 // Sizes of the per-rank communication regions (bytes): signal pad, mailbox.
 int agb_gar_region_bytes(long long* out) {
     out[0] = static_cast<long long>(kFlagSlots) * kMaxRanks * 4;
-    out[1] = 2ll * kMailboxRegion * 4;
+    out[1] = static_cast<long long>(kMailboxFloats) * 4;
     return 0;
 }
 
@@ -1726,6 +2015,86 @@ int agb_gar_byzantine(unsigned long long const* rows, int n, long long const* se
     else
         gar_byzantine_kernel<0><<<static_cast<int>(grid), threads, 0, s>>>(a);
     AGB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// Min-Max (mode 2) / Min-Sum (mode 3) with deviation 0 unit-vec, 1 sign, 2 std, over this rank's owned segments; see
+// `gar_optimized_kernel`. Arguments as `agb_gar_byzantine`, plus: `mailboxes`: R mailbox addresses (every rank's, its own at `rank`);
+// `partials`: [partial_ctas][561] floats of scratch (the grid never exceeds partial_ctas CTAs); `stats_out`: optional [562] floats,
+// gamma then the statistics summed over the ranks ([0, 496) honest pair distances, [496, 528) A_i, [528, 560) B_i, [560] C).
+// Cooperative launch; collective when R > 1.
+int agb_gar_byzantine_optimized(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                                unsigned byzantine, int mode, int deviation, int R, int rank, unsigned long long const* signals,
+                                unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long stats_out,
+                                unsigned epoch, unsigned long long epoch_ptr, void* stream) {
+    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
+        return 100;
+    if (nseg < 1 || nseg > kMaxSeg)
+        return 101;
+    if ((mode != kMinMax && mode != kMinSum) || deviation < kUnitVec || deviation > kStd)
+        return 118;
+    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
+    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < 2)
+        return 114;
+    ByzArgs a{};
+    a.H = H;
+    a.K = K;
+    a.n = H;
+    for (int i = 0, h = 0, b = 0; i < n; ++i) {
+        a.rows[i] = reinterpret_cast<float*>(rows[i]);
+        if ((honest >> i) & 1u) {
+            a.grad[h] = a.rows[i];
+            a.honest[h++] = i;
+        }
+        if ((byzantine >> i) & 1u)
+            a.byz[b++] = i;
+    }
+    a.mode = mode;
+    a.deviation = deviation;
+    a.nseg = nseg;
+    long long work = 0;
+    for (int s = 0; s < nseg; ++s) {
+        a.seg_lo[s] = seg_lo[s];
+        a.seg_hi[s] = seg_hi[s];
+        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
+            return 101;
+        work += (seg_hi[s] - seg_lo[s]) / 4;
+    }
+    a.R = R;
+    a.rank = rank;
+    for (int q = 0; q < R; ++q) {
+        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
+        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
+        if (R > 1 && !a.signal[q])
+            return 109;
+        if (!a.mailbox[q])
+            return 108;
+    }
+    a.partials = reinterpret_cast<float*>(partials);
+    a.stats_out = reinterpret_cast<float*>(stats_out);
+    if (!a.partials || partial_ctas < 1)
+        return 108;
+    a.epoch = epoch;
+    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
+    // the grid depends only on the owned work (and the device): the fused engine at R = 1 and the stand-alone op on the same rows fold
+    // the same partials in the same order
+    int const threads = 256;
+    bool const in_registers = H <= kBlockRows;
+    int per_sm = 0;
+    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_optimized_kernel<kBlockRows> : gar_optimized_kernel<0>,
+                                                              threads, 0));
+    if (per_sm < 1)
+        return 2;
+    long long grid = (work + threads - 1) / threads;
+    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
+    cap = cap > partial_ctas ? partial_ctas : cap;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
+    void* params[] = {&a};
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_optimized_kernel<kBlockRows>)
+                                                         : reinterpret_cast<void*>(gar_optimized_kernel<0>),
+                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
     return 0;
 }
 

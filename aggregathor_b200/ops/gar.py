@@ -20,10 +20,13 @@ MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
-# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 1
+# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 2
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
-MAILBOX_BYTES = 2 * MAX_RANKS * (MAX_PAIRS + 1) * 4   # two regions: the rule's exchanges, NNM's exchange
+# Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]
+CRAFT_STATS = MAX_PAIRS + 2 * MAX_WORKERS + 1
+# three regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics
+MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS) * 4
 PTRS = 113
 INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
@@ -37,9 +40,11 @@ _ERRORS = {
   114: "invalid Byzantine crafting parameters (disjoint slot masks, at least one Byzantine slot, H >= 2 for ALIE, H >= 1 for IPM)",
   115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)",
   116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)",
-  117: "invalid NNM parameters (0 <= 2 f < n)"}
+  117: "invalid NNM parameters (0 <= 2 f < n)",
+  118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
-BYZANTINE_MODES = {"alie": 0, "ipm": 1}
+BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
+DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
 
 
 def _lib():
@@ -81,6 +86,10 @@ class FusedLauncher:
     self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
     self.raw_dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)   # NNM: distances of the raw rows
     self.info = torch.zeros(INFO_INTS, dtype=torch.int32, device=self.device)
+    # Min-Max / Min-Sum: CTA partials of the statistics pass, and gamma followed by the statistics summed over the ranks
+    self.craft_ctas = ctas
+    self.craft_partials = torch.zeros(ctas * CRAFT_STATS, dtype=torch.float32, device=self.device)
+    self.craft_stats = torch.zeros(1 + CRAFT_STATS, dtype=torch.float32, device=self.device)
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
     self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS))()
@@ -283,10 +292,14 @@ def worker_momentum_(G, M, beta, c):
   return G
 
 
-def craft(rows, segments, honest, byzantine, mode, coef, *, R=1, rank=0, signals=None, epoch=1, epoch_ptr=None, stream=None):
+def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, launcher=None, mailboxes=None, R=1, rank=0, signals=None, epoch=1,
+          epoch_ptr=None, stream=None):
   """Craft the omniscient Byzantine rows (`attacks/omniscient.py`) over the owned `segments` of the n rows at device addresses `rows`
-  (raw ints, local or peer-mapped): every slot of `byzantine` receives the ALIE / IPM value of the `honest` slots. Collective when R > 1
-  (entry barrier through the signal pads, at flag value `epoch`, or `*epoch_ptr + 1` when given)."""
+  (raw ints, local or peer-mapped): every slot of `byzantine` receives the ALIE / IPM / Min-Max / Min-Sum value of the `honest` slots.
+  Collective when R > 1 (entry barrier through the signal pads, at flag value `epoch`, or `*epoch_ptr + 1` when given).
+  Min-Max and Min-Sum (`coef` unused) take the `deviation` (default "unit-vec") and the `FusedLauncher` whose scratch holds the CTA
+  partials and receives gamma and the summed statistics (`launcher.craft_stats`); their statistics are exchanged through `mailboxes`
+  (R addresses, every rank's; default: the launcher's local mailbox when R = 1)."""
   n = len(rows)
   if n > MAX_WORKERS:
     raise tools.UserException("The sm_90a crafting kernel supports n <= %d workers (got %d)" % (MAX_WORKERS, n))
@@ -298,6 +311,25 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, R=1, rank=0, signals
   lo = (ctypes.c_longlong * len(segments))(*[int(a) for a, _ in segments])
   hi = (ctypes.c_longlong * len(segments))(*[int(b) for _, b in segments])
   c_signals = (ctypes.c_ulonglong * R)(*[addr(signals[q]) for q in range(R)]) if signals is not None else None
+  if mode in ("min-max", "min-sum"):
+    if deviation is None:
+      deviation = "unit-vec"
+    if deviation not in DEVIATIONS:
+      raise tools.UserException("Unknown deviation %r for %s (expected one of %s)" % (deviation, mode, ", ".join(DEVIATIONS)))
+    if launcher is None:
+      raise tools.UserException("%s needs the scratch of a FusedLauncher" % mode)
+    if mailboxes is None:
+      if R != 1:
+        raise tools.UserException("%s over %d ranks needs every rank's mailbox" % (mode, R))
+      mailboxes = [launcher.local_mailbox]
+    c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
+    func = _lib().agb_gar_byzantine_optimized
+    func.restype = ctypes.c_int
+    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
+                ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_int(DEVIATIONS[deviation]), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+                ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(launcher.craft_stats.data_ptr()),
+                ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_optimized")
+    return
   func = _lib().agb_gar_byzantine
   func.restype = ctypes.c_int
   _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
@@ -305,14 +337,30 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, R=1, rank=0, signals
               ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine")
 
 
-def craft_byzantine_(G, byz_slots, mode, coef):
-  """Stand-alone omniscient attack on the [n, d] fp32 matrix `G`, in place: rows `byz_slots` <- the ALIE (`coef` = z) or IPM
-  (`coef` = epsilon) row of the other rows. CUDA tensors with n <= 32 run the sm_90a kernel; others the torch reference."""
+def craft_details(launcher, mode, H):
+  """(gamma, A [H], B [H], C, T) of the last Min-Max / Min-Sum crafting run with `launcher`: Python floats (fp32 values), as the kernel
+  solved them; T is None for Min-Sum."""
+  stats = launcher.craft_stats.cpu().tolist()
+  st = stats[1:]
+  a, b, c = MAX_PAIRS, MAX_PAIRS + MAX_WORKERS, MAX_PAIRS + 2 * MAX_WORKERS
+  T = max(st[:H * (H - 1) // 2]) if mode == "min-max" else None
+  return stats[0], st[a:a + H], st[b:b + H], st[c], T
+
+
+def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False):
+  """Stand-alone omniscient attack on the [n, d] fp32 matrix `G`, in place: rows `byz_slots` <- the ALIE (`coef` = z), IPM
+  (`coef` = epsilon), Min-Max or Min-Sum (`deviation`) row of the other rows. CUDA tensors with n <= 32 run the sm_90a kernel; others
+  the torch reference. Min-Max / Min-Sum with `return_details` return (gamma, A, B, C, T) instead of G (see `craft_details`)."""
   from ..aggregators import _ops
   n, d = G.shape
   byz_slots = _ops.check_byzantine_slots(n, byz_slots, mode)
+  optimized = mode in _ops.OPTIMIZED_MODES
+  if optimized:
+    deviation = _ops.check_deviation(mode, deviation)
+  elif return_details:
+    raise tools.UserException("return_details is for Min-Max / Min-Sum only")
   if not G.is_cuda or n > MAX_WORKERS:
-    return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef)
+    return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef, deviation=deviation, return_details=return_details)
   if G.dtype != torch.float32:
     raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
   pad = (-d) % 4
@@ -322,11 +370,14 @@ def craft_byzantine_(G, byz_slots, mode, coef):
     work[:, :d] = G
   dp = d + pad
   rows = [work.data_ptr() + i * dp * 4 for i in range(n)]
+  launcher = _launcher(G.device, n) if optimized else None
   with torch.cuda.device(G.device):
-    craft(rows, [(0, dp)], [i for i in range(n) if i not in byz_slots], byz_slots, mode, coef)
+    craft(rows, [(0, dp)], [i for i in range(n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation, launcher=launcher)
   if work is not G:
     index = torch.tensor(byz_slots, dtype=torch.int64, device=G.device)
     G[index] = work[index, :d]
+  if return_details:
+    return craft_details(launcher, mode, n - len(byz_slots))
   return G
 
 

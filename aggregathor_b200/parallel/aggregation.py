@@ -14,8 +14,9 @@ Three interchangeable engines share one interface (`params`, `grads`, `step()`):
   (`mnist` + `average`, 2 workers) and the fallback for user plug-in GARs without a fused spec.
 
 Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always sees n rows.
-Every engine also has `craft_byzantine(byz_slots, mode, coef)`, the omniscient attacks (`attacks/omniscient.py`): the rows at the
-given slots of the gathered matrix are overwritten with the ALIE / IPM row of the others, on every rank (a collective call).
+Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None)`, the omniscient attacks (`attacks/omniscient.py`): the
+rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM / Min-Max / Min-Sum row of the others, on every rank
+(a collective call); `last_craft` then holds Min-Max / Min-Sum's (gamma, A, B, C, T) of that call.
 Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
 `pre_aggregation="nnm"` (nearest-neighbour mixing, `aggregators/_ops.py`) replaces every gathered row by the mean of its n - f
 nearest rows before the rule runs, on every engine: inside the fused kernel, in the stand-alone kernel of the baseline engine, with
@@ -139,17 +140,21 @@ class HostAggregation(_AggregationBase):
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
+    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`
 
   def visible_rows(self):
     self._gather()
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef):
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None):
     """Gather, then the torch reference on the gathered matrix (every rank computes the same bits)."""
     from ..aggregators import _ops
     self.visible_rows()
-    _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef)
+    if mode in _ops.OPTIMIZED_MODES:
+      self.last_craft = _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
+    else:
+      _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef)
 
   def step(self, rate):
     self._gather()
@@ -178,16 +183,21 @@ class BaselineAggregation(_AggregationBase):
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
+    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`
 
   def visible_rows(self):
     self._gather()
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef):
-    """Gather, then the stand-alone crafting kernel on the gathered matrix (every rank computes the same bits)."""
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None):
+    """Gather, then the stand-alone crafting kernel (R = 1) on the gathered matrix (every rank computes the same bits)."""
+    from ..aggregators import _ops
     self.visible_rows()
-    gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef)
+    if mode in _ops.OPTIMIZED_MODES:
+      self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
+    else:
+      gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef)
 
   def step(self, rate):
     self._gather()
@@ -264,6 +274,7 @@ class FusedAggregation(_AggregationBase):
     self._hyper_host = torch.zeros(4, dtype=torch.float32).pin_memory() if device_state else None
     self.loss_out = torch.zeros(1, dtype=torch.float32, device=self.device)
     self._pre_accumulated = 0
+    self._craft_mode = None   # Min-Max / Min-Sum: (mode, H) of the last `craft_byzantine`
     self._prepared = False   # `prepare` ran for the step that has not been aggregated yet
     self._row_views = None
     heap = self.heap
@@ -339,14 +350,26 @@ class FusedAggregation(_AggregationBase):
       self._hyper_host[0], self._hyper_host[1], self._hyper_host[2], self._hyper_host[3] = lr, hyper[0], hyper[1], hyper[2]
       self.hyper_dev.copy_(self._hyper_host, non_blocking=True)
 
-  def craft_byzantine(self, byz_slots, mode, coef, stream=None):
+  def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None):
     """Collective: this rank crafts its owned segments of every Byzantine row, local or on a peer (`ops.gar.craft`), behind an entry
-    barrier at the epoch of the step about to be aggregated. Every rank calls it, including ranks that host no Byzantine worker."""
+    barrier at the epoch of the step about to be aggregated. Every rank calls it, including ranks that host no Byzantine worker.
+    Min-Max / Min-Sum exchange their statistics through the mailboxes; `last_craft` reads gamma and the sums back (a synchronisation)."""
     from ..aggregators import _ops
     byz_slots = _ops.check_byzantine_slots(self.n, byz_slots, mode)
+    optimized = mode in _ops.OPTIMIZED_MODES
+    if optimized:
+      deviation = _ops.check_deviation(mode, deviation)
     epoch = self.epoch if self._prepared else self.epoch + 1
-    gar_ops.craft(self._rows, self.segments, [i for i in range(self.n) if i not in byz_slots], byz_slots, mode, coef, R=self.world, rank=self.rank,
+    gar_ops.craft(self._rows, self.segments, [i for i in range(self.n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation,
+                  launcher=self.launcher if optimized else None, mailboxes=self._mailboxes if optimized else None, R=self.world, rank=self.rank,
                   signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream)
+    self._craft_mode = (mode, self.n - len(byz_slots)) if optimized else None
+
+  @property
+  def last_craft(self):
+    """Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`, as the kernel solved them (identical on every rank)."""
+    mode = self._craft_mode
+    return None if mode is None else gar_ops.craft_details(self.launcher, *mode)
 
   def phase_a(self, seg, stream=None):
     """Distance pass + staging of bucket `seg` (buckets must be pre-accumulated in order 0, 1, ...). Call between `prepare` and `step`."""

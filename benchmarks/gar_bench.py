@@ -11,6 +11,8 @@ fraction of the peer-copy rate measured at start-up; writes JSON to <--gar-out>/
 (`craft_byzantine`: the sm_90a kernel, sharded over the ranks on the fused engine, after the NCCL all-gather on the baseline one);
 the crafting kernel is also timed alone, next to the torch reference on the same device, with the (H + k) * d * 4 bytes it must move.
 `--gar-dump-rows` then saves, from the last rank, every row the fused engine aggregated (honest and crafted, all d coordinates).
+`--gar-attack min-max|min-sum` (Shejwalkar & Houmansadr, NDSS 2021; `--gar-attack-args deviation:unit-vec|sign|std`) also reports the
+gamma every rank solved, and times the crafting kernel alternated round by round with ALIE's on the same rows.
 `--gar-rule-args key:value ...` passes the same `--aggregator-args` to every rule (rules ignore keys they do not use). The
 `geometric-median` and `centered-clipping` entries also report their T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
 `--gar-worker-momentum beta` also times the worker-momentum kernel alone on the [w, d] rows of a rank (`ops.gar.worker_momentum_`,
@@ -47,7 +49,10 @@ def main():
   parser.add_argument("--gar-rules", dest="rules", type=str, default="average,average-nan,median,averaged-median,krum,bulyan")
   parser.add_argument("--gar-out", dest="out", type=str, default=".")
   parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
-  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm"), default=None, help="omniscient attack by the last f workers, crafted every step")
+  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm", "min-max", "min-sum"), default=None,
+                      help="omniscient attack by the last f workers, crafted every step")
+  parser.add_argument("--gar-attack-args", dest="attack_args", nargs="*", default=None, metavar="KEY:VALUE",
+                      help="`--attack-args` of --gar-attack (e.g. deviation:std for min-max / min-sum)")
   parser.add_argument("--gar-dump-rows", dest="dump_rows", action="store_true", help="with --gar-attack: save the last rank's view of every row to <--gar-out>")
   parser.add_argument("--gar-rule-args", dest="rule_args", nargs="*", default=None, metavar="KEY:VALUE",
                       help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
@@ -124,12 +129,13 @@ def main():
         grads[j].mul_(20.0).add_(3.0)  # the last f workers are outliers
     fused.grads.copy_(grads)
     base.grads.copy_(grads)
-    attack = attacks.instantiate(args.attack, n, f, []) if args.attack else None
+    attack = attacks.instantiate(args.attack, n, f, args.attack_args or []) if args.attack else None
     byz_slots = list(range(n - f, n))
+    extra = {"deviation": attack.deviation} if attack is not None and attack.deviation is not None else {}
 
     def craft(engine):
       if attack is not None:
-        engine.craft_byzantine(byz_slots, attack.mode, attack.coef)
+        engine.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra)
 
     torch.cuda.synchronize()
     if world > 1:
@@ -139,10 +145,21 @@ def main():
     craft(base)
     base.step(0.1)
     torch.cuda.synchronize()
+    gamma_entry = {}
+    if attack is not None and attack.deviation is not None:
+      # gamma as every rank solved it (fused engine), and as the baseline engine's stand-alone kernel solved it on the gathered rows
+      gamma = torch.tensor([fused.last_craft[0]], dtype=torch.float32, device=device)
+      gammas = [torch.zeros_like(gamma) for _ in range(world)]
+      if world > 1:
+        dist.all_gather(gammas, gamma)
+      else:
+        gammas = [gamma]
+      gamma_entry = {"deviation": attack.deviation, "gamma_per_rank": [float(x.item()) for x in gammas], "baseline_gamma": base.last_craft[0]}
     if attack is not None and args.dump_rows and rank == world - 1:
       rows = fused.visible_rows()
       os.makedirs(args.out, exist_ok=True)
-      torch.save({"rows": torch.stack([rows[i].cpu() for i in range(n)]), "byzantine": byz_slots, "mode": attack.mode, "coef": attack.coef},
+      torch.save({"rows": torch.stack([rows[i].cpu() for i in range(n)]), "byzantine": byz_slots, "mode": attack.mode, "coef": attack.coef,
+                  "deviation": attack.deviation, "gamma": fused.last_craft[0] if attack.deviation is not None else None},
                  os.path.join(args.out, "gar_rows_%s_%d.pt" % (rule, world)))
     diff = float((fused.params - base.params).abs().max())
     digest = gar_ops.checksum(fused.params)
@@ -216,13 +233,28 @@ def main():
         if world > 1:
           dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
-      craft_ms = time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef))
+      craft_ms = time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra))
       # the torch reference on this device, over the full [n, d] matrix (what a torch attack would run after an all-gather)
-      reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef))
+      reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef, **extra))
       craft_bytes = n * d * 4   # (H + k) * d * 4: every honest value read once, every Byzantine value written once (over all ranks)
+      if attack.deviation is not None:
+        # Min-Max / Min-Sum read the honest values again in the write pass, and Min-Max once more in its honest-distance pass
+        craft_bytes += (2 if attack.mode == "min-max" else 1) * (n - f) * d * 4
       attack_entry = {"attack": attack.mode, "coef": attack.coef, "k": f, "craft_ms": craft_ms, "torch_reference_ms": reference_ms,
                       "craft_bytes": craft_bytes, "craft_gbs": craft_bytes / craft_ms / 1e6,
                       "torch_reference_gbs": craft_bytes / reference_ms / 1e6}
+      attack_entry.update(gamma_entry)
+      if attack.deviation is not None:
+        # ALIE's crafting kernel on the same rows, alternated with this attack's round by round (clock and thermal drift hit both).
+        # Repeated calls at one step's epoch pass the flag barriers at once: with R > 1 they time the kernels, their gamma is not checked.
+        alie = attacks.instantiate("alie", n, f, [])
+        rounds = {"craft": [], "alie": []}
+        for _ in range(5):
+          rounds["craft"].append(time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra)))
+          rounds["alie"].append(time_craft(lambda: fused.craft_byzantine(byz_slots, "alie", alie.coef)))
+        median = lambda values: sorted(values)[len(values) // 2]
+        attack_entry.update({"craft_rounds_ms": rounds["craft"], "alie_craft_rounds_ms": rounds["alie"], "craft_median_ms": median(rounds["craft"]),
+                             "alie_craft_median_ms": median(rounds["alie"])})
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
