@@ -14,6 +14,7 @@ gather+aggregate+update kernel (`parallel/fused.py`); rules returning `None`
 optimizer path.
 """
 
+import math
 import pathlib
 
 from .. import tools
@@ -25,14 +26,15 @@ class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
   RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
-           "centered-clipping")
+           "centered-clipping", "dnc")
 
-  RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping")   # the others ignore f
+  RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc")   # the others ignore f
   MIXES = (None, "nnm")
 
-  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None):
+  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None, subsample=10000, c=1.0, seed=0):
     """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing, `iterations` and `tau` centered
-    clipping's iterations and clipping radius; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
+    clipping's iterations and clipping radius, `iterations`, `subsample`, `c` and `seed` DnC's iterations, sampled coordinates,
+    filtering fraction and sampling seed; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
     rule: None, or "nnm" (nearest-neighbour mixing with the same f)."""
     if rule not in self.RULES:
       raise tools.UserException("Unknown fused rule " + repr(rule))
@@ -41,6 +43,7 @@ class FusedSpec:
     self.rule, self.n, self.f, self.m, self.beta = rule, int(n), int(f), int(m), int(beta)
     self.iterations, self.nu, self.tau = int(iterations), float(nu), float(tau)
     self.mix = mix
+    self.subsample, self.c, self.seed = int(subsample), float(c), int(seed)
 
   @property
   def rule_id(self):
@@ -53,11 +56,17 @@ class FusedSpec:
   def with_mix(self, mix, f=None):
     """The same rule with pre-aggregation `mix` (None or "nnm"), and declared f `f` (default: unchanged)."""
     return FusedSpec(self.rule, self.n, self.f if f is None else f, self.m, self.beta, iterations=self.iterations, nu=self.nu, tau=self.tau,
-                     mix=mix)
+                     mix=mix, subsample=self.subsample, c=self.c, seed=self.seed)
+
+  @property
+  def removed(self):
+    """DnC: the rows every iteration removes, r = floor(c f) in float64."""
+    return math.floor(self.c * self.f)
 
   def __repr__(self):
     extra = {"geometric-median": ", iterations=%d, nu=%r" % (self.iterations, self.nu),
-             "centered-clipping": ", iterations=%d, tau=%r" % (self.iterations, self.tau)}.get(self.rule, "")
+             "centered-clipping": ", iterations=%d, tau=%r" % (self.iterations, self.tau),
+             "dnc": ", iterations=%d, subsample=%d, c=%r, seed=%d" % (self.iterations, self.subsample, self.c, self.seed)}.get(self.rule, "")
     if self.mix is not None:
       extra += ", mix=%r" % self.mix
     return "FusedSpec(rule=%r, n=%d, f=%d, m=%d, beta=%d%s)" % (self.rule, self.n, self.f, self.m, self.beta, extra)

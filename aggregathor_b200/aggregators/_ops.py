@@ -15,6 +15,7 @@ import ctypes
 import itertools
 import math
 
+import numpy as np
 import torch
 
 from .. import tools
@@ -534,6 +535,219 @@ def torch_bulyan(G, f, m, return_weights=False):
   inter = torch.stack([G[weights[k] != 0].sum(dim=0) / int((weights[k] != 0).sum()) for k in range(theta)], dim=0)
   out = torch_averaged_median(inter, beta)
   return (out, weights) if return_weights else out
+
+
+# ---------------------------------------------------------------------------- #
+# Divide-and-conquer (DnC; Shejwalkar & Houmansadr, "Manipulating the Byzantine", NDSS 2021): the sampler, the selection (a float64
+# transcription of the sm_90a kernel's, bit for bit), the torch and host back-ends
+
+DNC_MAX_ITERATIONS = 8
+DNC_MAX_SUBSAMPLE = 1 << 20
+DNC_MAX_DOMAIN = 1 << 48
+DNC_JACOBI_SWEEPS = 32
+DNC_JACOBI_TOL = 1e-26
+_U64 = (1 << 64) - 1
+
+
+def check_dnc(n, f, iterations, subsample, c, seed):
+  """Validate DnC's parameters -> (iterations, subsample, c, seed, r) with r = floor(c f) computed in float64."""
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("DnC needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+  if isinstance(iterations, bool) or int(iterations) != iterations or not 1 <= iterations <= DNC_MAX_ITERATIONS:
+    raise tools.UserException("DnC needs 1 <= iterations <= %d (got %r)" % (DNC_MAX_ITERATIONS, iterations))
+  if isinstance(subsample, bool) or int(subsample) != subsample or not 1 <= subsample <= DNC_MAX_SUBSAMPLE:
+    raise tools.UserException("DnC needs 1 <= subsample <= 2^20 (got %r)" % (subsample,))
+  c = float(c)
+  if not (math.isfinite(c) and c >= 0):
+    raise tools.UserException("DnC needs a finite filtering fraction c >= 0 (got %r)" % (c,))
+  if isinstance(seed, bool) or int(seed) != seed or not 0 <= seed <= _U64:
+    raise tools.UserException("DnC needs a seed in [0, 2^64) (got %r)" % (seed,))
+  r = math.floor(c * f)
+  if n - int(iterations) * r < 1:
+    raise tools.UserException("DnC removes r = floor(c f) = %d rows per iteration: n - iterations * r = %d must be >= 1" % (r, n - int(iterations) * r))
+  return int(iterations), int(subsample), c, int(seed), int(r)
+
+
+def check_dnc_step(step):
+  """DnC's step key: an integer in [0, 2^63) (the kernels take it as a signed 64-bit value)."""
+  if isinstance(step, bool) or int(step) != step or not 0 <= step < 1 << 63:
+    raise tools.UserException("DnC needs a step key in [0, 2^63) (got %r)" % (step,))
+  return int(step)
+
+
+def _splitmix64(z):
+  z = z + np.uint64(0x9E3779B97F4A7C15)
+  z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+  z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+  return z ^ (z >> np.uint64(31))
+
+
+def dnc_sample(domain, subsample, seed, step, t):
+  """The b' = min(subsample, domain) coordinates of [0, domain) that iteration t of step `step` samples: P(0), ..., P(b' - 1), P a
+  4-round Feistel permutation on w bits (w the smallest even number >= max(2, bit length of domain - 1)) with round function
+  F_r(R) = splitmix64(K ^ (r << 48) ^ R) mod 2^(w/2), K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ t), cycle-walked into
+  [0, domain). -> int64 array."""
+  domain, step = int(domain), check_dnc_step(step)
+  if not 1 <= domain <= DNC_MAX_DOMAIN:
+    raise tools.UserException("DnC samples a domain of 1 to 2^48 coordinates (got %d)" % domain)
+  with np.errstate(over="ignore"):
+    key = _splitmix64(np.array([seed & _U64], dtype=np.uint64))
+    key = _splitmix64(key ^ np.uint64(step))
+    key = _splitmix64(key ^ np.uint64(t))
+    width = max(2, (domain - 1).bit_length())
+    half = np.uint64((width + (width & 1)) // 2)
+    mask = np.uint64((1 << int(half)) - 1)
+
+    def feistel(x):
+      L, R = x >> half, x & mask
+      for r in range(4):
+        L, R = R, L ^ (_splitmix64(key ^ np.uint64(r << 48) ^ R) & mask)
+      return (L << half) | R
+
+    y = feistel(np.arange(min(int(subsample), domain), dtype=np.uint64))
+    out = y >= np.uint64(domain)
+    while out.any():
+      y[out] = feistel(y[out])
+      out = y >= np.uint64(domain)
+  return y.astype(np.int64)
+
+
+def _serial_sum(values):
+  """Left-to-right float64 sum from +0 (np.sum adds pairwise)."""
+  return float(np.cumsum(np.concatenate([[0.0], values]))[-1])
+
+
+def dnc_eigh(B):
+  """Float64 cyclic Jacobi on the symmetric [m, m] matrix B (m >= 2) -> (eigenvalues, eigenvectors as columns), the sm_90a kernel's
+  operations one for one: before each sweep (at most 32) stop when sum_{i != j} B_ij^2 <= 1e-26 sum_i B_ii^2 (both added row-major);
+  a sweep is m' - 1 rounds (m' = m rounded up to even) of m' / 2 disjoint pairs (circle method); a round computes every pair's rotation
+  from B as it stands (tau = (B_qq - B_pp) / (2 B_pq), t = sign(tau) / (|tau| + sqrt(1 + tau^2)), c = 1 / sqrt(1 + t^2), s = t c; none
+  when B_pq = 0), rotates rows p, q, then columns p, q of B and V, then zeroes B_pq and B_qp."""
+  A = np.array(B, dtype=np.float64, copy=True)
+  m = A.shape[0]
+  V = np.eye(m)
+  mm = m + (m & 1)
+  offdiag = ~np.eye(m, dtype=bool)
+  player = lambda pos, rnd: 0 if pos == 0 else 1 + (pos - 1 + rnd) % (mm - 1)
+  with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
+    for _ in range(DNC_JACOBI_SWEEPS):
+      sq = A * A
+      if _serial_sum(sq[offdiag]) <= DNC_JACOBI_TOL * _serial_sum(np.diag(sq)):
+        break
+      for rnd in range(mm - 1):
+        pairs = [sorted((player(k, rnd), player(mm - 1 - k, rnd))) for k in range(mm // 2)]
+        pairs = [(p, q) for p, q in pairs if q < m]
+        P = np.array([p for p, _ in pairs])
+        Q = np.array([q for _, q in pairs])
+        apq = A[P, Q]
+        tau = (A[Q, Q] - A[P, P]) / (2.0 * apq)
+        t = np.where(tau >= 0, 1.0, -1.0) / (np.abs(tau) + np.sqrt(1.0 + tau * tau))
+        c = 1.0 / np.sqrt(1.0 + t * t)
+        s = t * c
+        zero = apq == 0
+        c, s = np.where(zero, 1.0, c)[:, None], np.where(zero, 0.0, s)[:, None]
+        bp, bq = A[P, :].copy(), A[Q, :].copy()
+        A[P, :], A[Q, :] = c * bp - s * bq, s * bp + c * bq
+        c, s = c.T, s.T
+        bp, bq, vp, vq = A[:, P].copy(), A[:, Q].copy(), V[:, P].copy(), V[:, Q].copy()
+        A[:, P], A[:, Q] = c * bp - s * bq, s * bp + c * bq
+        V[:, P], V[:, Q] = c * vp - s * vq, s * vp + c * vq
+        A[P, Q] = 0.0
+        A[Q, P] = 0.0
+  return np.diag(A).copy(), V
+
+
+def dnc_scores(dist):
+  """Scores u_i^2 of the m rows of the finite [m, m] distance matrix `dist`: u the top eigenvector of the classical double centring
+  B = -1/2 (D_ij - r_i - r_j + g) (r_i the row means, g the mean of the r_i, both added in ascending index, float64), from `dnc_eigh`;
+  a tie in the top eigenvalue goes to the lower column. m <= 1: zeros."""
+  D = np.asarray(dist, dtype=np.float64)
+  m = D.shape[0]
+  if m <= 1:
+    return np.zeros(m)
+  r = np.cumsum(np.concatenate([np.zeros((m, 1)), D], axis=1), axis=1)[:, -1] / float(m)
+  g = _serial_sum(r) / float(m)
+  B = -0.5 * (((D - r[:, None]) - r[None, :]) + g)
+  lam, V = dnc_eigh(B)
+  u = V[:, int(np.argmax(lam))]
+  return u * u
+
+
+def dnc_select(dists, r):
+  """[T, n, n] sampled distances -> ([T, n] bool: the rows iteration t keeps, [n] bool: the rows every iteration kept). Iteration t
+  drops the rows with the most non-finite distances to the other remaining rows, the highest index first, until every remaining
+  distance is finite (they score +inf); the others score `dnc_scores`; it keeps the n - r rows first under the ordering convention."""
+  dists = np.asarray(dists.detach().to("cpu") if isinstance(dists, torch.Tensor) else dists, dtype=np.float64)
+  T, n = dists.shape[0], dists.shape[1]
+  masks = np.zeros((T, n), dtype=bool)
+  for t in range(T):
+    D = dists[t]
+    bad = ~np.isfinite(D)
+    remaining = list(range(n))
+    while True:
+      counts = [int(bad[i, remaining].sum()) for i in remaining]
+      most = max(counts)
+      if most == 0:
+        break
+      remaining.pop(max(k for k, value in enumerate(counts) if value == most))
+    scores = np.full(n, np.inf)
+    scores[remaining] = dnc_scores(D[np.ix_(remaining, remaining)])
+    order = sorted(range(n), key=lambda i: (not np.isfinite(scores[i]), scores[i] if np.isfinite(scores[i]) else 0.0, i))
+    masks[t, order[:n - r]] = True
+  return masks, masks.all(axis=0)
+
+
+def selection_mean(G, good):
+  """Mean of the rows `good` ([n] bool) of G, added in ascending order from +0 and divided once, in G's dtype (Krum's phase D)."""
+  acc = torch.zeros_like(G[0])
+  for i in range(G.shape[0]):
+    if bool(good[i]):
+      acc = torch.add(acc, G[i])
+  return torch.div(acc, torch.tensor(float(int(np.sum(good))), dtype=G.dtype, device=G.device))
+
+
+def torch_dnc(G, f, iterations, subsample, c, seed, step, domain=None, return_details=False):
+  """DnC with torch ops in G's dtype and on its device (double inputs, more than 32 workers, the test oracle); `domain` defaults to
+  G's row length. `return_details` also gives the [T, n, n] sampled distances and the masks of `dnc_select`."""
+  n, d = G.shape
+  T, b, _, seed, r = check_dnc(n, f, iterations, subsample, c, seed)
+  step = check_dnc_step(step)
+  domain = d if domain is None else int(domain)
+  if domain > d:
+    raise tools.UserException("DnC samples [0, %d) from rows of %d coordinates" % (domain, d))
+  dists = []
+  for t in range(T):
+    index = torch.from_numpy(dnc_sample(domain, b, seed, step, t)).to(G.device)
+    dists.append(torch_pairwise_distances(G[:, index]))
+  dists = torch.stack(dists)
+  masks, good = dnc_select(dists, r)
+  out = selection_mean(G, good)
+  return (out, dists, (masks, good)) if return_details else out
+
+
+def host_dnc(G, f, iterations, subsample, c, seed, step, domain=None, return_details=False):
+  """DnC with the host library: its sampled distances (`agb_cpu_dnc_sample_distances`), the selection of `dnc_select` and its
+  selection mean. Returns the output on G's device."""
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  T, b, _, seed, r = check_dnc(n, f, iterations, subsample, c, seed)
+  step = check_dnc_step(step)
+  domain = d if domain is None else int(domain)
+  if not 1 <= domain <= min(d, DNC_MAX_DOMAIN):
+    raise tools.UserException("DnC samples [0, %d) from rows of %d coordinates" % (domain, d))
+  dists = torch.empty((T, n, n), dtype=Gc.dtype)
+  status = _host("dnc_sample_distances", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), ctypes.c_size_t(T), ctypes.c_size_t(b),
+                                                   ctypes.c_uint64(seed), ctypes.c_uint64(step), ctypes.c_size_t(domain), _ptr(dists))
+  if status != 0:
+    raise tools.UserException("Host DnC rejected its arguments (n = %d, d = %d, iterations = %d, subsample = %d)" % (n, d, T, b))
+  masks, good = dnc_select(dists, r)
+  selected = torch.tensor([i for i in range(n) if good[i]], dtype=torch.int64)
+  out = torch.empty(d, dtype=Gc.dtype)
+  status = _host("selection_mean", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(selected), ctypes.c_size_t(selected.numel()), _ptr(out))
+  if status != 0:
+    raise tools.UserException("Host selection mean rejected its arguments")
+  out = out.to(G.device)
+  return (out, dists, (masks, good)) if return_details else out
 
 
 # ---------------------------------------------------------------------------- #

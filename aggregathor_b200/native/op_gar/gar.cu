@@ -24,6 +24,8 @@
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
 // whole-vector sums between the ranks, then the same per-coordinate write.
+// DnC (rule kDnc) has a finish kernel of its own, `gar_dnc_kernel`: a sampled distance pass, one exchange, a float64 Jacobi per CTA,
+// then Krum's phase D (see `dnc_selection`).
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
 // registers at a time; more rows are processed in 8-row blocks (diagonal + cross passes over the staged copy).
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
@@ -53,19 +55,25 @@ constexpr int kMaxIterations = 16;        // geometric median, centered clipping
 constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median, centered clipping: one exchange slot per iteration
 constexpr int kSlotMix = kSlotGeoMedian + kMaxIterations;   // NNM: exchange of the raw distances
 constexpr int kSlotCraftStats = kSlotMix + 1;   // Min-Max / Min-Sum: exchange of the crafting statistics
-constexpr int kFlagSlots = kSlotCraftStats + 1;
+constexpr int kSlotDnc = kSlotCraftStats + 1;   // DnC: exchange of the sampled distances
+constexpr int kFlagSlots = kSlotDnc + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 // Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
 // They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
 constexpr int kStatA = kMaxPairs, kStatB = kStatA + kMaxWorkers, kStatC = kStatB + kMaxWorkers;
 constexpr int kCraftStats = kStatC + 1;   // 561
 constexpr int kCraftRegion = 2 * kMailboxRegion;
-constexpr int kMailboxFloats = kCraftRegion + kMaxRanks * kCraftStats;
+constexpr int kDncIterations = 8;         // DnC: iterations T in [1, kDncIterations]
+constexpr int kDncStride = kDncIterations * kMaxPairs + 1;   // DnC post of one rank: T x [kMaxPairs] sampled distances, then the loss
+constexpr int kDncRegion = kCraftRegion + kMaxRanks * kCraftStats;   // mailbox region 3: kMaxRanks x kDncStride floats
+constexpr int kMailboxFloats = kDncRegion + kMaxRanks * kDncStride;
+constexpr int kJacobiSweeps = 32;         // DnC: sweep budget of the cyclic Jacobi
+constexpr double kJacobiTol = 1e-26;      // DnC: stop once sum_{i != j} B_ij^2 <= kJacobiTol * sum_i B_ii^2
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
 enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8,
-           kCenteredClipping = 9 };
+           kCenteredClipping = 9, kDnc = 10 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -107,6 +115,21 @@ struct GarArgs {
     float tau;                         // centered clipping: clipping radius, finite and > 0
     float* center;                     // centered clipping: [d] (local) center v, read and updated on the owned coordinates
     int mix;                           // pre-aggregation: 0 none, 1 nearest-neighbour mixing (needs the staging buffer)
+    // DnC (T = iterations)
+    int dnc_r;                         // rows removed per iteration, r = floor(c f)
+    long long dnc_b, dnc_domain;       // subsample b and sample domain D: b' = min(b, D) coordinates of [0, D) per iteration
+    unsigned long long dnc_seed;
+    long long dnc_step;                // step key, used when dnc_step_ptr is null
+    long long const* dnc_step_ptr;     // device step key (graph replay), or null
+    float* dnc_scratch;                // [grid][kDncIterations][kMaxPairs] CTA partials, then the samples [T][n][b'4]
+};
+
+// the rows `phase_a_segment` reads in DnC's sampled pass: one segment [0, b'4) of the gathered samples of one iteration, no staging
+struct SampleRows {
+    int n, nseg;
+    long long seg_lo[1], seg_hi[1];
+    float const* grad[kMaxWorkers];
+    float* staging;
 };
 
 struct Shared {
@@ -132,6 +155,20 @@ struct Shared {
     int theta;
     float hyper[4];
     uint32_t epoch;
+};
+
+// DnC's selection state, declared by `gar_dnc_kernel` alone (the other kernels' shared memory does not grow)
+struct DncShared {
+    double B[kMaxWorkers][kMaxWorkers + 1];       // double-centred Gram matrix of the m remaining rows
+    double V[kMaxWorkers][kMaxWorkers + 1];       // Jacobi eigenvectors
+    double rot[kMaxWorkers / 2][2];               // (c, s) of every pair of the current round
+    double rmean[kMaxWorkers];
+    double score[kMaxWorkers];                    // by worker; +inf for the rows dropped for non-finite distances
+    double grand;
+    int idx[kMaxWorkers];                         // the remaining rows, ascending
+    unsigned remaining, keep;
+    int converged;
+    SampleRows rows;
 };
 
 // ---- VEC-wide (4 or 1) coordinate accesses ----------------------------------- //
@@ -1021,6 +1058,341 @@ __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg:
     }
 }
 
+// ---- divide-and-conquer (DnC; Shejwalkar & Houmansadr, "Manipulating the Byzantine", NDSS 2021) ----------------------------- //
+// Iteration t < T of step `step` samples b' = min(b, D) distinct coordinates s_k = P(k) of [0, D), P a keyed permutation: a 4-round
+// Feistel network on w bits (w the smallest even number >= max(2, bit length of D - 1), halves of h = w / 2 bits), round function
+// F_r(R) = splitmix64(K ^ (r << 48) ^ R) mod 2^h with K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ t), cycle-walked into
+// [0, D). D^t_ij = sum_k (x_i[s_k] - x_j[s_k])^2 (fp32). The rows with the most non-finite distances to the other remaining rows are
+// dropped one at a time (the highest index first) until every remaining distance is finite; they score +inf. The m remaining rows
+// score u_i^2, u the top eigenvector of B = -1/2 (D_ij - r_i - r_j + g) (classical double centring, float64), which ranks them as the
+// paper's <x_i - mu, v>^2 = lambda_1 u_i^2 does. Iteration t keeps the n - r rows first under the ordering convention; the output is
+// the mean of the rows every iteration kept (Krum's phase D).
+//   1. gather: every thread evaluates P for its share of the T b'4 sample slots and copies the n values of the slots this rank owns
+//      (P2P from the rows, or the mixed tile under NNM) into the compact scratch [T][n][b'4]; other slots hold +0, which adds exactly +0
+//      to every distance;
+//   2. grid barrier, then `phase_a_segment` over the scratch of every iteration, folded into the CTA's [T][kMaxPairs] partials;
+//   3. one exchange: block 0 adds the CTA partials in index order and posts them with the loss into mailbox region 3 of every rank
+//      (flag slot kSlotDnc, touched by no other exchange of the step); every CTA adds the R posts in rank order;
+//   4. every CTA runs the same selection (same bits everywhere): a float64 cyclic Jacobi with round-robin pair ordering, every operation
+//      rounded once (explicit _rn intrinsics: no FMA), which `_ops.dnc_scores` transcribes bit for bit.
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ long long dnc_permute(unsigned long long key, int h, long long domain, long long x) {
+    unsigned long long const mask = (1ull << h) - 1ull;
+    unsigned long long y = static_cast<unsigned long long>(x);
+    do {
+        unsigned long long L = y >> h, R = y & mask;
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            unsigned long long const F = splitmix64(key ^ (static_cast<unsigned long long>(r) << 48) ^ R) & mask;
+            unsigned long long const next = L ^ F;
+            L = R;
+            R = next;
+        }
+        y = (L << h) | R;
+    } while (y >= static_cast<unsigned long long>(domain));
+    return static_cast<long long>(y);
+}
+
+__device__ __forceinline__ bool before_d(double a, int ia, double b, int ib) {
+    bool const fa = isfinite(a), fb = isfinite(b);
+    if (fa != fb)
+        return fa;
+    if (fa && a != b)
+        return a < b;
+    return ia < ib;
+}
+
+// eigenvectors of ds.B[0, m)^2 (m >= 2) into ds.V; B ends (nearly) diagonal. A sweep is m' - 1 rounds (m' = m rounded up to
+// even) of m' / 2 disjoint pairs (circle method: position 0 fixed, the others rotated); a round computes every pair's rotation from
+// B as it stands, then rotates the rows, then the columns of B and V, then zeroes B_pq and B_qp.
+__device__ void dnc_jacobi(DncShared& ds, int m) {
+    int const mm = m + (m & 1), half = mm / 2;
+    auto player = [&](int pos, int round) { return pos == 0 ? 0 : 1 + (pos - 1 + round) % (mm - 1); };
+    for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
+        if (threadIdx.x == 0) {
+            double off = 0.0, diag = 0.0;
+            for (int i = 0; i < m; ++i)
+                for (int j = 0; j < m; ++j) {
+                    double const sq = __dmul_rn(ds.B[i][j], ds.B[i][j]);
+                    if (i == j)
+                        diag = __dadd_rn(diag, sq);
+                    else
+                        off = __dadd_rn(off, sq);
+                }
+            ds.converged = off <= __dmul_rn(kJacobiTol, diag);
+        }
+        __syncthreads();
+        if (ds.converged)
+            break;
+        for (int round = 0; round < mm - 1; ++round) {
+            if (threadIdx.x < half) {
+                int const u = player(threadIdx.x, round), v = player(mm - 1 - threadIdx.x, round);
+                int const p = u < v ? u : v, q = u < v ? v : u;
+                double c = 1.0, s = 0.0;
+                if (q < m && ds.B[p][q] != 0.0) {
+                    double const apq = ds.B[p][q];
+                    double const tau = __ddiv_rn(__dsub_rn(ds.B[q][q], ds.B[p][p]), __dmul_rn(2.0, apq));
+                    double const t = __ddiv_rn(tau >= 0.0 ? 1.0 : -1.0, __dadd_rn(fabs(tau), __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(tau, tau)))));
+                    c = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(t, t))));
+                    s = __dmul_rn(t, c);
+                }
+                ds.rot[threadIdx.x][0] = c;
+                ds.rot[threadIdx.x][1] = s;
+            }
+            __syncthreads();
+            for (int task = threadIdx.x; task < half * m; task += blockDim.x) {   // rows p, q of B
+                int const k = task / m, j = task % m;
+                int const u = player(k, round), v = player(mm - 1 - k, round);
+                int const p = u < v ? u : v, q = u < v ? v : u;
+                if (q < m) {
+                    double const c = ds.rot[k][0], s = ds.rot[k][1], bp = ds.B[p][j], bq = ds.B[q][j];
+                    ds.B[p][j] = __dsub_rn(__dmul_rn(c, bp), __dmul_rn(s, bq));
+                    ds.B[q][j] = __dadd_rn(__dmul_rn(s, bp), __dmul_rn(c, bq));
+                }
+            }
+            __syncthreads();
+            for (int task = threadIdx.x; task < half * m; task += blockDim.x) {   // columns p, q of B and V
+                int const k = task / m, i = task % m;
+                int const u = player(k, round), v = player(mm - 1 - k, round);
+                int const p = u < v ? u : v, q = u < v ? v : u;
+                if (q < m) {
+                    double const c = ds.rot[k][0], s = ds.rot[k][1];
+                    double const bp = ds.B[i][p], bq = ds.B[i][q], vp = ds.V[i][p], vq = ds.V[i][q];
+                    ds.B[i][p] = __dsub_rn(__dmul_rn(c, bp), __dmul_rn(s, bq));
+                    ds.B[i][q] = __dadd_rn(__dmul_rn(s, bp), __dmul_rn(c, bq));
+                    ds.V[i][p] = __dsub_rn(__dmul_rn(c, vp), __dmul_rn(s, vq));
+                    ds.V[i][q] = __dadd_rn(__dmul_rn(s, vp), __dmul_rn(c, vq));
+                }
+            }
+            __syncthreads();
+            if (threadIdx.x < half) {
+                int const u = player(threadIdx.x, round), v = player(mm - 1 - threadIdx.x, round);
+                int const p = u < v ? u : v, q = u < v ? v : u;
+                if (q < m) {
+                    ds.B[p][q] = 0.0;
+                    ds.B[q][p] = 0.0;
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// the rows iteration t keeps, from its distances in sh.dist (whole CTA; every thread returns the same mask)
+__device__ unsigned dnc_keep(GarArgs const& a, Shared& sh, DncShared& ds) {
+    int const n = a.n, lane = threadIdx.x & 31;
+    unsigned const full = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    if (threadIdx.x < 32) {   // drop the rows with the most non-finite distances, the highest index first
+        unsigned bad = 0u;
+        if (lane < n)
+            for (int j = 0; j < n; ++j)
+                bad |= is_finite(sh.dist[lane][j]) ? 0u : 1u << j;
+        unsigned remaining = full;
+        for (;;) {
+            int count = lane < n && ((remaining >> lane) & 1u) ? __popc(bad & remaining) : 0;
+            int most = count;
+            for (int o = 16; o > 0; o >>= 1)
+                most = max(most, __shfl_xor_sync(0xffffffffu, most, o));
+            if (most == 0)
+                break;
+            unsigned const candidates = __ballot_sync(0xffffffffu, count == most);
+            remaining &= ~(1u << (31 - __clz(candidates)));
+        }
+        if (lane == 0)
+            ds.remaining = remaining;
+        if (lane < n && ((remaining >> lane) & 1u))
+            ds.idx[__popc(remaining & ((1u << lane) - 1u))] = lane;
+        if (lane < n)
+            ds.score[lane] = ((remaining >> lane) & 1u) ? 0.0 : __longlong_as_double(0x7ff0000000000000ll);
+    }
+    __syncthreads();
+    int const m = __popc(ds.remaining);
+    if (m >= 2) {
+        if (threadIdx.x < m) {   // row means, ascending index
+            int const i = ds.idx[threadIdx.x];
+            double sum = 0.0;
+            for (int j = 0; j < m; ++j)
+                sum = __dadd_rn(sum, static_cast<double>(sh.dist[i][ds.idx[j]]));
+            ds.rmean[threadIdx.x] = __ddiv_rn(sum, static_cast<double>(m));
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double sum = 0.0;
+            for (int i = 0; i < m; ++i)
+                sum = __dadd_rn(sum, ds.rmean[i]);
+            ds.grand = __ddiv_rn(sum, static_cast<double>(m));
+        }
+        __syncthreads();
+        for (int e = threadIdx.x; e < m * m; e += blockDim.x) {
+            int const i = e / m, j = e % m;
+            double const dij = static_cast<double>(sh.dist[ds.idx[i]][ds.idx[j]]);
+            ds.B[i][j] = __dmul_rn(-0.5, __dadd_rn(__dsub_rn(__dsub_rn(dij, ds.rmean[i]), ds.rmean[j]), ds.grand));
+            ds.V[i][j] = i == j ? 1.0 : 0.0;
+        }
+        __syncthreads();
+        dnc_jacobi(ds, m);
+        if (threadIdx.x < m) {   // top eigenpair: the largest diagonal entry, ties -> lower column
+            int best = 0;
+            for (int k = 1; k < m; ++k)
+                if (ds.B[k][k] > ds.B[best][best])
+                    best = k;
+            double const u = ds.V[threadIdx.x][best];
+            ds.score[ds.idx[threadIdx.x]] = __dmul_rn(u, u);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        bool keep = false;
+        if (lane < n) {
+            int rank = 0;
+            for (int j = 0; j < n; ++j)
+                if (j != lane)
+                    rank += before_d(ds.score[j], j, ds.score[lane], lane) ? 1 : 0;
+            keep = rank < n - a.dnc_r;
+        }
+        unsigned const mask = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0)
+            ds.keep = mask;
+    }
+    __syncthreads();
+    unsigned const keep = ds.keep;
+    __syncthreads();
+    return keep;
+}
+
+template<int N>
+__device__ void dnc_selection(GarArgs const& a, Shared& sh, DncShared& ds, int* pair_of, cg::grid_group& grid, uint32_t epoch,
+                              float local_loss, long long tid, long long nthreads) {
+    int const n = a.n, T = a.iterations, npairs = n * (n - 1) / 2;
+    bool const multi = a.R > 1;
+    long long const domain = a.dnc_domain, b = a.dnc_b < domain ? a.dnc_b : domain, b4 = (b + 3) & ~3ll;
+    float* const partials = a.dnc_scratch;
+    float* const samples = a.dnc_scratch + static_cast<long long>(gridDim.x) * kDncIterations * kMaxPairs;
+    long long const owned = owned_length(a);
+    unsigned long long const step = static_cast<unsigned long long>(a.dnc_step_ptr ? *a.dnc_step_ptr : a.dnc_step);
+    int const width = 64 - __clzll(static_cast<unsigned long long>(domain - 1));
+    int const h = (width < 2 ? 2 : width + (width & 1)) / 2;
+    unsigned long long const base_key = splitmix64(splitmix64(a.dnc_seed) ^ step);
+    // -------- 1. gather the owned samples -------- //
+    for (long long k = tid; k < T * b4; k += nthreads) {
+        int const t = static_cast<int>(k / b4);
+        long long const slot = k - t * b4;
+        float* const dst = samples + static_cast<long long>(t) * n * b4 + slot;
+        long long x = -1, soff = 0;
+        int seg = -1;
+        if (slot < b) {
+            x = dnc_permute(splitmix64(base_key ^ static_cast<unsigned long long>(t)), h, domain, slot);
+            for (int s = 0; s < a.nseg; ++s) {
+                if (x >= a.seg_lo[s] && x < a.seg_hi[s]) {
+                    seg = s;
+                    break;
+                }
+                soff += a.seg_hi[s] - a.seg_lo[s];
+            }
+        }
+        for (int i = 0; i < n; ++i) {
+            float value = 0.f;
+            if (seg >= 0)
+                value = a.mix ? a.staging[i * owned + soff + (x - a.seg_lo[seg])] : a.grad[i][x];
+            dst[i * b4] = value;
+        }
+    }
+    __threadfence();
+    grid.sync();
+    // -------- 2. sampled distances of every iteration -------- //
+    float* const mine = partials + static_cast<long long>(blockIdx.x) * kDncIterations * kMaxPairs;
+    for (int p = threadIdx.x; p < T * kMaxPairs; p += blockDim.x)
+        mine[p] = 0.f;
+    for (int t = 0; t < T; ++t) {
+        if (threadIdx.x == 0) {
+            ds.rows.n = n;
+            ds.rows.nseg = 1;
+            ds.rows.seg_lo[0] = 0;
+            ds.rows.seg_hi[0] = b4;
+            ds.rows.staging = nullptr;
+        }
+        if (threadIdx.x < n)
+            ds.rows.grad[threadIdx.x] = samples + (static_cast<long long>(t) * n + threadIdx.x) * b4;
+        __syncthreads();
+        phase_a_segment<(N > kBlockRows)>(ds.rows, sh, pair_of, 0, mine + t * kMaxPairs, tid, nthreads);
+    }
+    // -------- 3. one exchange: T x npairs partial distances and the loss -------- //
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int k = threadIdx.x; k < T * npairs; k += blockDim.x) {
+            int const t = k / npairs, p = k - t * npairs;
+            float s = 0.f;
+            for (unsigned c = 0; c < gridDim.x; ++c)
+                s += ld_volatile_f(partials + static_cast<long long>(c) * kDncIterations * kMaxPairs + t * kMaxPairs + p);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kDncRegion + a.rank * kDncStride + t * kMaxPairs + p] = s;
+        }
+        if (threadIdx.x == 0)
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kDncRegion + a.rank * kDncStride + kDncIterations * kMaxPairs] = local_loss;
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, kSlotDnc, epoch);
+    }
+    if (multi) {
+        wait_all(a, kSlotDnc, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    float const* const box = a.mailbox[a.rank] + kDncRegion;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
+        float total = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            total += ld_volatile_f(box + q * kDncStride + kDncIterations * kMaxPairs);
+        *a.loss_out = total;
+    }
+    // -------- 4. selection, identical in every CTA of every rank -------- //
+    unsigned good = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    for (int t = 0; t < T; ++t) {
+        for (int p = threadIdx.x; p < kMaxWorkers * (kMaxWorkers + 1); p += blockDim.x)
+            (&sh.dist[0][0])[p] = 0.f;
+        __syncthreads();
+        for (int p = threadIdx.x; p < npairs; p += blockDim.x) {
+            int i = 0, rest = p;
+            while (rest >= n - 1 - i) {
+                rest -= n - 1 - i;
+                ++i;
+            }
+            int const j = i + 1 + rest;
+            float s = 0.f;
+            for (int q = 0; q < a.R; ++q)
+                s += ld_volatile_f(box + q * kDncStride + t * kMaxPairs + p);
+            if (!is_finite(s))
+                s = __int_as_float(0x7f800000);
+            sh.dist[i][j] = s;
+            sh.dist[j][i] = s;
+            if (a.dist_out && blockIdx.x == 0) {
+                a.dist_out[(t * n + i) * n + j] = s;
+                a.dist_out[(t * n + j) * n + i] = s;
+            }
+        }
+        __syncthreads();
+        unsigned const keep = dnc_keep(a, sh, ds);
+        good &= keep;
+        if (a.info && blockIdx.x == 0 && threadIdx.x == 0)
+            a.info[96 + t] = static_cast<int>(keep);
+    }
+    if (threadIdx.x == 0) {
+        sh.selmask[0] = good;
+        sh.selcount[0] = __popc(good);
+        sh.theta = 1;
+    }
+}
+
 // ---- coordinate-wise rules: one streaming pass over the rows, or (STAGED, NNM) over the mixed tile, each thread reading what it
 // wrote in the mix pass ------------------------------------------------------------------------------------------------------ //
 template<int N, int VEC, bool STAGED>
@@ -1290,6 +1662,111 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
         }
     } else if (!exchanged_loss && blockIdx.x == 0 && threadIdx.x == 0 && a.loss_out) {
         *a.loss_out = local_loss;
+    }
+    if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
+        *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
+}
+
+// ---- the DnC finish kernel ------------------------------------------------------------- //
+// The finish kernel of rule kDnc: the same steps as `gar_fused_kernel` (entry barrier, NNM, selection, Krum's phase D, exit barrier),
+// with `dnc_selection` in place of the distance rules' phase A and selection. A kernel of its own keeps the sampled pass and the
+// Jacobi out of the register allocation of the other rules' coordinate loops, and DncShared out of their shared memory.
+template<int N, int VEC>
+__global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs const a) {
+    __shared__ Shared sh;
+    __shared__ DncShared ds;
+    __shared__ int pair_of[kBlockRows * kBlockRows];
+    cg::grid_group grid = cg::this_grid();
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    bool const multi = a.R > 1;
+    if (threadIdx.x == 0) {
+        sh.epoch = current_epoch(a);
+        for (int i = 0; i < 4; ++i)
+            sh.hyper[i] = a.hyper_ptr ? a.hyper_ptr[i] : (i == 0 ? a.lr : i == 1 ? a.h0 : i == 2 ? a.h1 : a.h2);
+    }
+    __syncthreads();
+    uint32_t const epoch = sh.epoch;
+    float const hyper[4] = {sh.hyper[0], sh.hyper[1], sh.hyper[2], sh.hyper[3]};
+    long long const owned = owned_length(a);
+    if (multi) {   // entry barrier: every rank's gradients are published (nothing is pre-accumulated for DnC)
+        if (blockIdx.x == 0)
+            signal_all(a, 0, epoch);
+        wait_all(a, 0, epoch);
+        __syncthreads();
+    }
+    float local_loss = 0.f;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_in)
+        for (int j = 0; j < a.nloss; ++j)
+            local_loss += a.loss_in[j];
+    if (a.mix) {
+        nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
+        __threadfence();
+        grid.sync();   // the mix pass wrote the tile with the rule's (tid, VEC) mapping; the gather reads any coordinate of it
+    }
+    dnc_selection<N>(a, sh, ds, pair_of, grid, epoch, local_loss, tid, nthreads);   // carries the loss
+    __syncthreads();
+    if (a.info && blockIdx.x == 0 && threadIdx.x == 0) {
+        a.info[0] = 1;
+        a.info[1] = static_cast<int>(sh.selmask[0]);
+    }
+    // -------- phase D: mean of the kept rows, update, broadcast (Krum's) -------- //
+    unsigned const mask = sh.selmask[0];
+    float const count = static_cast<float>(sh.selcount[0]);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            float sum[VEC];
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                sum[c] = 0.f;
+            auto load_row = [&](int i, float (&dst)[VEC]) {
+                if (a.staging)
+                    V<VEC>::load(a.staging + i * owned + soff + v * VEC, dst);
+                else
+                    V<VEC>::load_stream(a.grad[i] + x, dst);
+            };
+            if (N <= 16) {   // all kept rows in flight at once, added in ascending worker order
+                float g[N][VEC];
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u)
+                        load_row(i, g[i]);
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u) {
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            sum[c] += g[i][c];
+                    }
+            } else {
+                for (int i = 0; i < a.n; ++i) {
+                    if ((mask >> i) & 1u) {
+                        float g[VEC];
+                        load_row(i, g);
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            sum[c] += g[c];
+                    }
+                }
+            }
+            float out[VEC];
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                out[c] = sum[c] / count;
+            apply_update<VEC>(a, hyper, x, out);
+        }
+    }
+    if (multi) {   // exit barrier, as in `gar_fused_kernel` (the loss went through DnC's exchange)
+        fence_sys();
+        grid.sync();
+        if (blockIdx.x == 0) {
+            __syncthreads();
+            signal_all(a, kSlotExit, epoch);
+            wait_all(a, kSlotExit, epoch);
+            __syncthreads();
+        }
     }
     if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
         *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
@@ -1766,12 +2243,13 @@ __global__ void cast_bf16_kernel(float const* __restrict__ src, __nv_bfloat16* _
     }
 }
 
-template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t stream) {
+template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_floats, cudaStream_t stream) {
     int const threads = N <= 8 ? 512 : 256;
     int device = 0, sms = 0, per_sm = 0;
+    auto const kernel = a.rule == kDnc ? gar_dnc_kernel<N, VEC> : gar_fused_kernel<N, VEC>;
     AGB_CUDA_OK(cudaGetDevice(&device));
     AGB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gar_fused_kernel<N, VEC>, threads, 0));
+    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0));
     if (per_sm < 1)
         return 2;
     long long work = 0;
@@ -1783,8 +2261,13 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t strea
         grid = max_ctas;
     if (want < grid)
         grid = want < 1 ? 1 : static_cast<int>(want);
+    if (a.rule == kDnc) {   // CTA partials of this grid, then the samples
+        long long const b = a.dnc_b < a.dnc_domain ? a.dnc_b : a.dnc_domain;
+        if (static_cast<long long>(grid) * kDncIterations * kMaxPairs + a.iterations * a.n * ((b + 3) & ~3ll) > scratch_floats)
+            return 108;
+    }
     void* params[] = {&a};
-    AGB_CUDA_OK(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(gar_fused_kernel<N, VEC>), dim3(grid), dim3(threads), params, 0, stream));
+    AGB_CUDA_OK(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(threads), params, 0, stream));
     return 0;
 }
 
@@ -1792,10 +2275,11 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, cudaStream_t strea
 //   [0..32) gradient rows | [32] agg_out | [33] param | [34] slot0 | [35] slot1 | [36] param_mc | [37] cta_partials | [38] staging
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
-//   [47] center (centered clipping) | [112] raw_dist_out (NNM)
+//   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-//       [25] iterations | [26] mix (0 none, 1 NNM)
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi ; floats: lr h0 h1 h2 nu tau
+//       [25] iterations | [26] mix (0 none, 1 NNM) | [27] DnC r
+// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step [21] scratch floats
+// floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
     a.R = ints[5]; a.rank = ints[6]; a.opt = ints[7]; a.epoch = static_cast<uint32_t>(ints[8]);
@@ -1806,6 +2290,13 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.row_stride = longs[0];
     a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4]; a.tau = floats[5];
     a.center = reinterpret_cast<float*>(ptrs[47]);
+    a.dnc_r = ints[27];
+    a.dnc_b = longs[17];
+    a.dnc_domain = longs[18];
+    a.dnc_seed = static_cast<unsigned long long>(longs[19]);
+    a.dnc_step = longs[20];
+    a.dnc_step_ptr = reinterpret_cast<long long const*>(ptrs[113]);
+    a.dnc_scratch = reinterpret_cast<float*>(ptrs[114]);
     if (a.n < 1 || a.n > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
@@ -1817,7 +2308,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kCenteredClipping)
+    if (a.rule < 0 || a.rule > kDnc)
         return 102;
     if (a.mix < 0 || a.mix > 1 || (a.mix && (a.f < 0 || 2 * a.f >= a.n)))
         return 117;
@@ -1826,6 +2317,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 116;
     if (a.rule == kGeoMedian && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.nu > 0.f) || !std::isfinite(a.nu)))
         return 115;
+    if (a.rule == kDnc && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kDncIterations || a.dnc_r < 0 ||
+                           a.n - a.iterations * a.dnc_r < 1 || a.dnc_b < 1 || a.dnc_b > (1ll << 20) || a.dnc_domain < 1 ||
+                           a.dnc_domain > (1ll << 48) || a.dnc_step < 0))
+        return 119;
     if ((a.rule == kTrimmedMean || a.rule == kMda) && (a.f < 0 || 2 * a.f >= a.n))
         return a.rule == kTrimmedMean ? 112 : 113;
     if (a.rule == kMda) {
@@ -1877,6 +2372,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)
         return 108;
+    if (a.rule == kDnc && (!a.mailbox[0] || !a.dnc_scratch))
+        return 108;
+    if (a.rule == kDnc && a.first_seg > 0)
+        return 111;   // DnC's sampled pass runs in its finish kernel: nothing is pre-accumulated
     if (a.mix && (!a.cta_partials || !a.mailbox[0] || !a.staging))
         return 108;   // NNM mixes the staged tile in place
     if (a.mix && a.first_seg > 0)
@@ -1930,10 +2429,10 @@ int agb_gar_fused(unsigned long long const* ptrs, int const* ints, long long con
         return 0;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (a.n <= 8)
-        return launch<8, 4>(a, max_ctas, s);
+        return launch<8, 4>(a, max_ctas, longs[21], s);
     if (a.n <= 16)
-        return launch<16, 4>(a, max_ctas, s);
-    return launch<32, 1>(a, max_ctas, s);
+        return launch<16, 4>(a, max_ctas, longs[21], s);
+    return launch<32, 1>(a, max_ctas, longs[21], s);
 }
 
 // Phase A (partial pairwise distances + local staging) of owned segment `seg` alone, on `ctas` CTAs: launched on a side stream as soon as

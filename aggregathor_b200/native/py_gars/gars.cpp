@@ -719,6 +719,76 @@ template<class T> int bulyan(T const* g, size_t n, size_t d, size_t f, size_t m,
     return 0;
 }
 
+// ------------------------------------------------------------------------ //
+// DnC's sampled distances (`native/op_gar/gar.cu` defines the sampler): for t < T, D^t_ij = sum_k (x_i[s_k] - x_j[s_k])^2 over the
+// b' = min(b, domain) coordinates s_k = P(k) of iteration t, added in ascending k; non-finite -> +inf. The selection runs in Python
+// (`_ops.dnc_select`), so that its float64 Jacobi exists once on the host.
+inline uint64_t splitmix64(uint64_t z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+template<class T> int dnc_sample_distances(T const* g, size_t n, size_t d, size_t iterations, size_t b, uint64_t seed, uint64_t step,
+                                           size_t domain, T* dist /* [T, n, n] */) {
+    if (n < 1 || iterations < 1 || iterations > 8 || b < 1 || b > (size_t(1) << 20) || domain < 1 || domain > d || domain > (size_t(1) << 48))
+        return 1;
+    size_t const count = std::min(b, domain);
+    int width = 0;
+    while (width < 64 && ((domain - 1) >> width) != 0)
+        ++width;
+    int const h = (width < 2 ? 2 : width + (width & 1)) / 2;
+    uint64_t const mask = (uint64_t(1) << h) - 1;
+    std::vector<T> sample(n * count);
+    for (size_t t = 0; t < iterations; ++t) {
+        uint64_t const key = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ t);
+        for (size_t k = 0; k < count; ++k) {
+            uint64_t y = k;
+            do {
+                uint64_t L = y >> h, R = y & mask;
+                for (uint64_t r = 0; r < 4; ++r) {
+                    uint64_t const next = L ^ (splitmix64(key ^ (r << 48) ^ R) & mask);
+                    L = R;
+                    R = next;
+                }
+                y = (L << h) | R;
+            } while (y >= domain);
+            for (size_t i = 0; i < n; ++i)
+                sample[i * count + k] = g[i * d + y];
+        }
+        T* out = dist + t * n * n;
+        for (size_t i = 0; i < n; ++i) {
+            out[i * n + i] = T(0);
+            for (size_t j = i + 1; j < n; ++j) {
+                T sum = T(0);
+                for (size_t k = 0; k < count; ++k) {
+                    T const delta = sample[i * count + k] - sample[j * count + k];
+                    sum += delta * delta;
+                }
+                if (!std::isfinite(sum))
+                    sum = std::numeric_limits<T>::infinity();
+                out[i * n + j] = sum;
+                out[j * n + i] = sum;
+            }
+        }
+    }
+    return 0;
+}
+
+template<class T> int selection_mean_of(T const* g, size_t n, size_t d, int64_t const* selected, size_t count, T* out) {
+    if (count < 1)
+        return 1;
+    std::vector<size_t> sel(count);
+    for (size_t k = 0; k < count; ++k) {
+        if (selected[k] < 0 || static_cast<size_t>(selected[k]) >= n)
+            return 1;
+        sel[k] = static_cast<size_t>(selected[k]);
+    }
+    selection_mean<T>(g, d, sel, out);
+    return 0;
+}
+
 template<class T> T squared_distance(T const* a, T const* b, size_t d) {
     size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
     std::vector<T> partial(chunks, T(0));
@@ -774,6 +844,8 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_centered_clipping_##S(T const* g, size_t n, size_t d, size_t iterations, double tau, T* center, T* dist) { return centered_clipping<T>(g, n, d, iterations, tau, center, dist); } \
     extern "C" int agb_cpu_pairwise_distances_##S(T const* g, size_t n, size_t d, T* dist) { if (n < 1) return 1; pairwise_distances<T>(g, n, d, dist); return 0; } \
     extern "C" int agb_cpu_weighted_sum_##S(T const* g, size_t n, size_t d, T const* w, T* out) { weighted_sum<T>(g, n, d, w, out); return 0; } \
+    extern "C" int agb_cpu_dnc_sample_distances_##S(T const* g, size_t n, size_t d, size_t iterations, size_t b, uint64_t seed, uint64_t step, size_t domain, T* dist) { return dnc_sample_distances<T>(g, n, d, iterations, b, seed, step, domain, dist); } \
+    extern "C" int agb_cpu_selection_mean_##S(T const* g, size_t n, size_t d, int64_t const* selected, size_t count, T* out) { return selection_mean_of<T>(g, n, d, selected, count, out); } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }
 
 AGB_EXPORT(float, float)

@@ -20,15 +20,19 @@ MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
-# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 2
+# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange;
+# DnC's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 3
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 # Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]
 CRAFT_STATS = MAX_PAIRS + 2 * MAX_WORKERS + 1
-# three regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics
-MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS) * 4
-PTRS = 113
-INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks
+DNC_MAX_ITERATIONS = 8
+# DnC's post of one rank: the sampled distances of every iteration ([DNC_MAX_ITERATIONS][MAX_PAIRS]), then the loss
+DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
+# four regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances
+MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS) * 4
+PTRS = 115
+INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks; [96, 96 + T): DnC's mask of every iteration
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
 
 _ERRORS = {
@@ -41,7 +45,8 @@ _ERRORS = {
   115: "invalid geometric-median parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite nu > 0)",
   116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)",
   117: "invalid NNM parameters (0 <= 2 f < n)",
-  118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)"}
+  118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)",
+  119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
@@ -85,6 +90,9 @@ class FusedLauncher:
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
     self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
     self.raw_dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)   # NNM: distances of the raw rows
+    self.dnc_dist_out = torch.zeros(DNC_MAX_ITERATIONS * n * n, dtype=torch.float32, device=self.device)   # DnC: [T, n, n] sampled distances
+    self.ctas = ctas
+    self._dnc_scratch = None
     self.info = torch.zeros(INFO_INTS, dtype=torch.int32, device=self.device)
     # Min-Max / Min-Sum: CTA partials of the statistics pass, and gamma followed by the statistics summed over the ranks
     self.craft_ctas = ctas
@@ -92,7 +100,7 @@ class FusedLauncher:
     self.craft_stats = torch.zeros(1 + CRAFT_STATS, dtype=torch.float32, device=self.device)
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
-    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS))()
+    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 5))()
     self._floats = (ctypes.c_float * 6)()
     self._func = _lib().agb_gar_fused
     self._func.restype = ctypes.c_int
@@ -105,7 +113,7 @@ class FusedLauncher:
 
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
-            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None):
+            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None):
     ptrs = self._ptrs
     for i in range(PTRS):
       ptrs[i] = 0
@@ -117,10 +125,14 @@ class FusedLauncher:
       ptrs[i] = row
     addr = lambda t: 0 if t is None else (t if isinstance(t, int) else t.data_ptr())
     ptrs[32], ptrs[33], ptrs[34], ptrs[35], ptrs[36] = addr(agg_out), addr(param), addr(slot0), addr(slot1), int(param_mc or 0)
-    dist_out = self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dist_out
+    dist_out = self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dnc_dist_out if spec.rule == "dnc" else self.dist_out
     ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
     ptrs[42], ptrs[43], ptrs[44], ptrs[45], ptrs[46] = addr(epoch_ptr), addr(hyper_ptr), self.seg_partials.data_ptr(), addr(loss_in), addr(loss_out)
     ptrs[47], ptrs[112] = addr(center), self.raw_dist_out.data_ptr()
+    if domain is None:
+      domain = max(hi for _, hi in segments)
+    scratch = self.dnc_scratch(spec, domain) if spec.rule == "dnc" else None
+    ptrs[113], ptrs[114] = addr(step_ptr), addr(scratch)
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -138,6 +150,19 @@ class FusedLauncher:
       ints[16 + s] = self.phase_a_ctas if s < first_seg else 0
     self._floats[0], self._floats[1], self._floats[2], self._floats[3], self._floats[4] = lr, hyper[0], hyper[1], hyper[2], spec.nu
     self._floats[5] = spec.tau
+    ints[27] = spec.removed if spec.rule == "dnc" else 0
+    longs = self._longs
+    longs[17], longs[18], longs[19], longs[20] = spec.subsample, domain, spec.seed - (1 << 64) if spec.seed >= 1 << 63 else spec.seed, step
+    longs[21] = scratch.numel() if scratch is not None else 0
+
+  def dnc_scratch(self, spec, domain):
+    """DnC's scratch for rule `spec` over `domain` coordinates: the CTA partials of the sampled distances of the largest grid, then the
+    gathered samples [T][n][b' rounded up to 4] (grown on demand)."""
+    count = min(spec.subsample, int(domain))
+    need = self.ctas * DNC_MAX_ITERATIONS * MAX_PAIRS + spec.iterations * spec.n * ((count + 3) // 4 * 4)
+    if self._dnc_scratch is None or self._dnc_scratch.numel() < need:
+      self._dnc_scratch = torch.zeros(need, dtype=torch.float32, device=self.device)
+    return self._dnc_scratch
 
   def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
@@ -156,44 +181,56 @@ class FusedLauncher:
 _launchers = {}
 
 
-def _torch_rules(spec):
+def _torch_rules(spec, step=0):
   from ..aggregators import _ops
   return {"average": _ops.torch_average, "average-nan": _ops.torch_average_nan, "median": _ops.torch_median,
           "averaged-median": lambda M: _ops.torch_averaged_median(M, spec.beta), "krum": lambda M: _ops.torch_krum(M, spec.f, spec.m),
           "bulyan": lambda M: _ops.torch_bulyan(M, spec.f, spec.m), "trimmed-mean": lambda M: _ops.torch_trimmed_mean(M, spec.f),
-          "mda": lambda M: _ops.torch_mda(M, spec.f), "geometric-median": lambda M: _ops.torch_geometric_median(M, spec.iterations, spec.nu)}[spec.rule]
+          "mda": lambda M: _ops.torch_mda(M, spec.f), "geometric-median": lambda M: _ops.torch_geometric_median(M, spec.iterations, spec.nu),
+          "dnc": lambda M: _ops.torch_dnc(M, spec.f, spec.iterations, spec.subsample, spec.c, spec.seed, step)}[spec.rule]
 
 
-def aggregate(spec, G, return_details=False, center=None):
+def aggregate(spec, G, return_details=False, center=None, step=0):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
   iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
+  DnC draws its samples with step key `step` over the d coordinates of G's rows; its details are the [T, n, n] sampled distances and
+  `info` with [0] = 1, [1] = the final mask (bit i: row i kept) and [96 + t] = the mask of iteration t.
   With `spec.mix == "nnm"` the rule runs on the mixed rows (its distances and masks are those of the mixed rows), and
   `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32)."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   n, d = G.shape
   if n != spec.n:
-    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau, mix=spec.mix)
+    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau, mix=spec.mix,
+                     subsample=spec.subsample, c=spec.c, seed=spec.seed)
   if spec.rule == "centered-clipping":
     return _aggregate_centered_clipping(spec, G, return_details, center)
+  if spec.rule == "dnc":
+    from ..aggregators import _ops
+    step = _ops.check_dnc_step(step)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
-    return _torch_rules(spec)(_torch_mixed(spec, G))
+    return _torch_rules(spec, step)(_torch_mixed(spec, G))
   if G.dtype != torch.float32:
-    out = aggregate(spec, G.float(), return_details)
+    out = aggregate(spec, G.float(), return_details, step=step)
     return (out[0].to(G.dtype),) + out[1:] if return_details else out.to(G.dtype)
   if n > MAX_WORKERS:  # beyond the kernels' worker limit: torch ops on the same device
-    return _torch_rules(spec)(_torch_mixed(spec, G))
+    return _torch_rules(spec, step)(_torch_mixed(spec, G))
   G, dp = _aligned_rows(G)
   launcher = _launcher(G.device, n)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=_staging(spec, n, dp, G.device))
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=_staging(spec, n, dp, G.device), step=step, domain=d)
   out = out[:d]
   if return_details:
-    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n) if spec.rule in ITERATIVE_RULES else launcher.dist_out.view(n, n)
+    if spec.rule in ITERATIVE_RULES:
+      dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n)
+    elif spec.rule == "dnc":
+      dist = launcher.dnc_dist_out[:spec.iterations * n * n].view(spec.iterations, n, n)
+    else:
+      dist = launcher.dist_out.view(n, n)
     return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
   return out
 

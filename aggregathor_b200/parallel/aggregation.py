@@ -18,6 +18,8 @@ Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None)`, 
 rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM / Min-Max / Min-Sum row of the others, on every rank
 (a collective call); `last_craft` then holds Min-Max / Min-Sum's (gamma, A, B, C, T) of that call.
 Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
+`dnc` draws its samples with the number of the optimizer update the aggregation feeds as step key (`updates` once it is counted,
+checkpointed with it) over the padded flat size `layout.padded_size`, on every engine.
 `pre_aggregation="nnm"` (nearest-neighbour mixing, `aggregators/_ops.py`) replaces every gathered row by the mean of its n - f
 nearest rows before the rule runs, on every engine: inside the fused kernel, in the stand-alone kernel of the baseline engine, with
 the host library's distances on the host engine and with the torch reference for plug-ins without a fused spec. The GAR object
@@ -104,6 +106,15 @@ class _AggregationBase:
         tools.warning("The checkpoint holds no center for centered clipping: it starts from zero", context="restore")
         self.center.zero_()
 
+  def _rule_kwargs(self):
+    """Keywords of the rule's `aggregate` (and of `ops.gar.aggregate`) for the step about to be counted: centered clipping's center,
+    DnC's step key."""
+    if self.center is not None:
+      return {"center": self.center}
+    if self.spec is not None and self.spec.rule == "dnc":
+      return {"step": self.updates + 1}
+    return {}
+
   def full_slots(self):
     return self.slots
 
@@ -162,7 +173,7 @@ class HostAggregation(_AggregationBase):
     if self.mix is not None:
       from ..aggregators import _ops
       rows = _ops.host_nnm(rows, self.f) if rows.device.type == "cpu" else _ops.torch_nnm(rows, self.f)
-    aggregated = self.gar.aggregate(rows) if self.center is None else self.gar.aggregate(rows, center=self.center)
+    aggregated = self.gar.aggregate(rows, **self._rule_kwargs())
     self.updates += 1
     self.optimizer.apply_torch(self.params, aggregated, self.slots, rate, self.updates)
     self.last_aggregate = aggregated
@@ -201,7 +212,7 @@ class BaselineAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
-    state = {} if self.center is None else {"center": self.center}
+    state = self._rule_kwargs()
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
       aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)   # mixes inside the kernel
     else:
@@ -266,12 +277,17 @@ class FusedAggregation(_AggregationBase):
                     or self.mix is not None)
     self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
+    if self.spec.rule == "dnc":
+      self.launcher.dnc_scratch(self.spec, d)   # allocated before any graph capture
     self.max_ctas = max_ctas
     self.epoch = 0
     self.device_state = bool(device_state)
     self.epoch_dev = torch.zeros(1, dtype=torch.int32, device=self.device) if device_state else None
     self.hyper_dev = torch.zeros(4, dtype=torch.float32, device=self.device) if device_state else None
     self._hyper_host = torch.zeros(4, dtype=torch.float32).pin_memory() if device_state else None
+    dnc = self.spec.rule == "dnc"
+    # DnC: the step key of its samples, refreshed by `prepare` so that graph replays draw new samples
+    self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device) if device_state and dnc else None
     self.loss_out = torch.zeros(1, dtype=torch.float32, device=self.device)
     self._pre_accumulated = 0
     self._craft_mode = None   # Min-Max / Min-Sum: (mode, H) of the last `craft_byzantine`
@@ -349,6 +365,8 @@ class FusedAggregation(_AggregationBase):
       lr, hyper = self._rate_args
       self._hyper_host[0], self._hyper_host[1], self._hyper_host[2], self._hyper_host[3] = lr, hyper[0], hyper[1], hyper[2]
       self.hyper_dev.copy_(self._hyper_host, non_blocking=True)
+      if self.step_dev is not None:   # the value travels as a kernel argument of the fill, fixed when it is enqueued
+        self.step_dev.fill_(self.updates)
 
   def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None):
     """Collective: this rank crafts its owned segments of every Byzantine row, local or on a peer (`ops.gar.craft`), behind an entry
@@ -385,7 +403,8 @@ class FusedAggregation(_AggregationBase):
     self._prepared = False
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
-                         loss_in=loss_in, loss_out=self.loss_out, center=self.center, **self._common(self._rate_args))
+                         loss_in=loss_in, loss_out=self.loss_out, center=self.center, step=self.updates, step_ptr=self.step_dev, domain=self.d,
+                         **self._common(self._rate_args))
 
   def _assemble(self, vector):
     """Full copy of a [d] vector maintained on the owned segments only (collective when R > 1)."""

@@ -20,6 +20,9 @@ dampening 0), with the 16 * w * d bytes it must move (G and M read and written o
 `--gar-pre-aggregation nnm` runs both engines with nearest-neighbour mixing before every rule (the checks above then hold for the
 mixed step), and also times the fused step of each rule without NNM, alternating with and without in the same process, to report
 the measured cost of the mix (`nnm_ms`, `plain_ms`, `nnm_overhead_ms`: medians over the alternated rounds).
+`dnc` (divide-and-conquer) takes `--gar-rule-args iterations:<T> subsample:<b> c:<c> seed:<s>`; both engines draw the same samples (the
+step key is the update count), so the fused-vs-baseline check holds for it as for the other rules; its entry also reports the rows
+each engine kept in the checked step (`fused_mask`, `baseline_mask`, `masks_agree`).
 """
 
 import argparse
@@ -145,6 +148,11 @@ def main():
     craft(base)
     base.step(0.1)
     torch.cuda.synchronize()
+    mask_entry = {}
+    if rule == "dnc":   # the rows each engine kept in the checked step (bit i: row i)
+      fused_mask = int(fused.launcher.info[1].item()) & 0xffffffff
+      base_mask = int(gar_ops._launcher(base._gathered.device, n).info[1].item()) & 0xffffffff
+      mask_entry = {"fused_mask": fused_mask, "baseline_mask": base_mask, "masks_agree": fused_mask == base_mask}
     gamma_entry = {}
     if attack is not None and attack.deviation is not None:
       # gamma as every rank solved it (fused engine), and as the baseline engine's stand-alone kernel solved it on the gathered rows
@@ -310,6 +318,7 @@ def main():
                      "local_hbm_bytes": hbm, "hbm_gbs": hbm / fused_ms / 1e6 if world == 1 else None}
     results[rule].update(attack_entry)
     results[rule].update(mix_entry)
+    results[rule].update(mask_entry)
     if args.rule_args is not None:
       results[rule]["rule_args"] = args.rule_args
     if rule in ("geometric-median", "centered-clipping"):
