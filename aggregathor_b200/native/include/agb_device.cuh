@@ -152,6 +152,19 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// max / min that return NaN when either input is NaN (fmaxf / fminf return the other operand): a ReLU or clamp built on them
+// lets a NaN activation reach the loss instead of turning it into a number.
+__device__ __forceinline__ float max_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+__device__ __forceinline__ float min_nan(float a, float b) {
+    float r;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
 __device__ __forceinline__ bool is_finite(float v) {
     return (__float_as_uint(v) & 0x7f800000u) != 0x7f800000u;
 }

@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(kThreads) relu6_kernel(bf16 const* __restrict_
         } else {
 #pragma unroll
             for (int j = 0; j < 8; ++j)
-                v[j] = fminf(fmaxf(v[j], 0.f), 6.f);
+                v[j] = min_nan(max_nan(v[j], 0.f), 6.f);
         }
         reinterpret_cast<uint4*>(out)[i] = pack8(v);
     }

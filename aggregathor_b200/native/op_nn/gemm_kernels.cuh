@@ -152,8 +152,8 @@ __device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap
                     v1 += b1;
                 }
                 if (p.relu) {
-                    v0 = fmaxf(v0, 0.f);
-                    v1 = fmaxf(v1, 0.f);
+                    v0 = max_nan(v0, 0.f);
+                    v1 = max_nan(v1, 0.f);
                 }
                 uint8_t* dst = buf + row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15);
                 if constexpr (kFp32)
@@ -211,8 +211,8 @@ __device__ __forceinline__ void epilogue_slab(GemmParams const& p, float (&acc)[
                     v1 += __ldg(p.bias + col + 1);
             }
             if (p.relu) {
-                v0 = fmaxf(v0, 0.f);
-                v1 = fmaxf(v1, 0.f);
+                v0 = max_nan(v0, 0.f);
+                v1 = max_nan(v1, 0.f);
             }
             if (p.out_fp32) {
                 float* dst = static_cast<float*>(p.C) + offset + col;

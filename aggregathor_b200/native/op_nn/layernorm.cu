@@ -44,20 +44,24 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) layernorm_fwd_kernel(bf16 c
         return;
     int const octets = C >> 3;
     bf16 const* xr = x + row * C;
+    // sums of (x - pivot) with the row's first element as pivot: sumsq / C - shifted^2 stays well conditioned when |mean| >> std
+    float const pivot = __bfloat162float(xr[0]);
     float sum = 0.f, sumsq = 0.f;
     for (int o = lane; o < octets; o += 32) {
         float v[8];
         unpack8(*reinterpret_cast<uint4 const*>(xr + o * 8), v);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            sum += v[j];
-            sumsq += v[j] * v[j];
+            float const d = v[j] - pivot;
+            sum += d;
+            sumsq += d * d;
         }
     }
     sum = warp_sum(sum);
     sumsq = warp_sum(sumsq);
-    float const mean = sum / C;
-    float const var = fmaxf(sumsq / C - mean * mean, 0.f);
+    float const shifted = sum / C;
+    float const mean = pivot + shifted;
+    float const var = fmaxf(sumsq / C - shifted * shifted, 0.f);
     float const rstd = rsqrtf(var + eps);
     if (lane == 0) {
         mean_out[row] = mean;

@@ -66,7 +66,8 @@ template<> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 constexpr int kThreads = 256;
 
 // ---------------------------------------------------------------------------- //
-// Per-channel (and per-group) sums: out[g][c] += sum_r f(...). MODE 0: (x, x^2); MODE 1: (dy', dy' * xhat) with
+// Per-channel (and per-group) sums: out[g][c] += sum_r f(...). MODE 0: (x - p, (x - p)^2) with the pivot p = the group's first row,
+// so that E[x^2] - E[x]^2 stays well conditioned in fp32 even when |mean| >> std; MODE 1: (dy', dy' * xhat) with
 // dy' = dy masked by (y > 0) when y != null; MODE 2: (dy') only (bias gradient). C % 8 == 0.
 // 2-D decomposition: blockIdx.x = row chunk, blockIdx.y = strip of STRIP octets (8 * STRIP channels), blockIdx.z = group.
 // Inside a CTA, STRIP lanes cover the strip's octets (up to 512 contiguous bytes per row: whole DRAM bursts instead of
@@ -92,8 +93,8 @@ struct SumsFinalize {
     float eps, decay;
 };
 
-template<int MODE>
-__device__ void finalize_sums(double* sums, SumsFinalize const& f, int C, long long rows_per_group) {
+template<int MODE, typename T>
+__device__ void finalize_sums(double* sums, SumsFinalize const& f, int C, long long rows_per_group, T const* x) {
     double const n = static_cast<double>(rows_per_group), inv_n = 1.0 / n;
     for (int i = threadIdx.x; i < C * f.groups; i += blockDim.x) {
         int const c = i % C, g = i / C;
@@ -101,8 +102,9 @@ __device__ void finalize_sums(double* sums, SumsFinalize const& f, int C, long l
         sums[2 * i] = 0.;       // leave the workspace zeroed for the next statistics kernel (no memset between launches)
         sums[2 * i + 1] = 0.;
         if (MODE == 0) {
-            double const mean = s0 * inv_n;
-            double var = fma(-mean, mean, s1 * inv_n);
+            double const shifted = s0 * inv_n;
+            double const mean = shifted + static_cast<double>(to_f(x[g * rows_per_group * C + c]));
+            double var = fma(-shifted, shifted, s1 * inv_n);
             if (var < 0.)
                 var = 0.;
             float const rstd = rsqrtf(static_cast<float>(var) + f.eps);
@@ -162,6 +164,8 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
             rs[j] = rstd[group * C + o * 8 + j];
         }
     }
+    if (MODE == 0 && active)
+        unpack8(load_oct(a + base * C + o * 8), mu);
     if (active) {
         constexpr int U = MODE == 1 ? 2 : kRowUnroll;
         for (long long r0 = row_begin + tr; r0 < row_end; r0 += kRowLanes * U) {
@@ -187,8 +191,9 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
                     if (MODE == 0) {
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
-                            s0[j] += va[j];
-                            s1[j] += va[j] * va[j];
+                            float const d = va[j] - mu[j];
+                            s0[j] += d;
+                            s1[j] += d * d;
                         }
                     } else {
                         if (y) {
@@ -248,7 +253,7 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
     __syncthreads();
     if (is_last) {
         __threadfence();
-        finalize_sums<MODE>(out, fin, C, rows_per_group);
+        finalize_sums<MODE>(out, fin, C, rows_per_group, a);
     }
 }
 
@@ -287,7 +292,7 @@ __global__ void __launch_bounds__(kThreads) bn_apply_kernel(T const* __restrict_
         for (int j = 0; j < 8; ++j) {
             v[j] = v[j] * sc[j] + sh[j] + r[j];
             if (relu)
-                v[j] = fmaxf(v[j], 0.f);
+                v[j] = max_nan(v[j], 0.f);
         }
         return pack_oct<T>(v);
     };
@@ -434,7 +439,7 @@ __global__ void add_relu_kernel(T const* __restrict__ a, T const* __restrict__ b
         if (relu) {
 #pragma unroll
             for (int j = 0; j < 8; ++j)
-                va[j] = fmaxf(va[j], 0.f);
+                va[j] = max_nan(va[j], 0.f);
         }
         store_oct(out + i * 8, pack_oct<T>(va));
     }
@@ -459,7 +464,8 @@ __global__ void relu_bwd_kernel(T const* __restrict__ dy, T const* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------- //
-// Max pooling (k x k, stride s, explicit pads, -inf padding), NHWC. Forward also records the argmax (window-relative index).
+// Max pooling (k x k, stride s, explicit pads, -inf padding), NHWC. Forward also records the argmax (window-relative index): the
+// first maximal tap in row-major window order, or the last NaN tap of a window holding NaN (NaN propagates, as in torch).
 // K > 0: window size known at compile time — the K * K taps are loaded first (all in flight), then compared; K = 0: any window.
 template<typename T, int K>
 __global__ void maxpool_fwd_kernel(T const* __restrict__ x, T* __restrict__ y, unsigned char* __restrict__ arg, int N, int H, int W, int C, int OH, int OW,
@@ -501,7 +507,7 @@ __global__ void maxpool_fwd_kernel(T const* __restrict__ x, T* __restrict__ y, u
                 unpack8(taps[t], v);
 #pragma unroll
                 for (int j = 0; j < 8; ++j)
-                    if (valid[t] && v[j] > best[j]) {
+                    if (valid[t] && (v[j] > best[j] || v[j] != v[j])) {   // a NaN wins its window
                         best[j] = v[j];
                         where[j] = static_cast<unsigned char>(t);
                     }
@@ -519,7 +525,7 @@ __global__ void maxpool_fwd_kernel(T const* __restrict__ x, T* __restrict__ y, u
                     unpack8(load_oct(x + ((static_cast<long long>(n) * H + h) * W + w) * C + o * 8), v);
 #pragma unroll
                     for (int j = 0; j < 8; ++j)
-                        if (v[j] > best[j]) {
+                        if (v[j] > best[j] || v[j] != v[j]) {
                             best[j] = v[j];
                             where[j] = static_cast<unsigned char>(kh * k + kw);
                         }
@@ -956,7 +962,7 @@ inline SumsPlan plan_sums(long long rows_per_group, int C, int groups) {
 
 constexpr int kFusedThreads = 512;
 constexpr int kFusedScratchBytes = kFusedThreads * 16 * 4;      // CTA reduction scratch: [lanes][octets * 16] floats
-constexpr int kFusedPivotBytes = 12 * 1024;                     // the forward pivot per channel, kept from phase 0 to phase 2
+constexpr int kFusedMovingBytes = 12 * 1024;                    // the moving mean per channel, kept from phase 0 to phase 2
 constexpr int kFusedStashBytes = 180 * 1024;                    // resident tile(s)
 // fp64 accumulation of the CTAs' fp32 partial sums is exact (53-bit mantissa vs <= 132 addends of 24 bits), hence independent of
 // the arrival order: statistics are bit-reproducible from run to run. To keep the atomics off a handful of hot L2 lines when C
@@ -1001,8 +1007,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
     pdl_wait();
     extern __shared__ __align__(16) unsigned char fused_smem[];
     float* red = reinterpret_cast<float*>(fused_smem);
-    float* pivot_s = reinterpret_cast<float*>(fused_smem + kFusedScratchBytes);
-    uint4* stash_a = reinterpret_cast<uint4*>(fused_smem + kFusedScratchBytes + kFusedPivotBytes);
+    float* moving_s = reinterpret_cast<float*>(fused_smem + kFusedScratchBytes);
+    uint4* stash_a = reinterpret_cast<uint4*>(fused_smem + kFusedScratchBytes + kFusedMovingBytes);
     uint4* stash_b = stash_a + p.stash_vecs;
     int const octets = p.C >> 3;
     // Per-channel vectors (pivot / saved statistics, later the coefficients) are fetched by ONE thread per channel and handed to
@@ -1018,9 +1024,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
         for (int u = 0; u < 4; ++u) {
             int const c = c0 + u * kFusedThreads;
             first[u] = second[u] = 0.f;
-            if (c < p.C) {
-                first[u] = BWD ? p.save_mean[group * p.C + c] : (p.moving_mean ? p.moving_mean[c] : 0.f);
-                second[u] = BWD ? p.save_rstd[group * p.C + c] : 0.f;
+            if (c < p.C) {   // forward: the statistics pivot (the group's first row) and the moving mean
+                first[u] = BWD ? p.save_mean[group * p.C + c] : __bfloat162float(p.a[static_cast<long long>(group) * p.rows_per_group * p.C + c]);
+                second[u] = BWD ? p.save_rstd[group * p.C + c] : (p.moving_mean ? p.moving_mean[c] : 0.f);
             }
         }
 #pragma unroll
@@ -1030,7 +1036,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
                 chan[c] = first[u];
                 chan[p.C + c] = second[u];
                 if (!BWD)
-                    pivot_s[c] = first[u];   // phase 2 must use the value read HERE: by then another CTA has updated the moving mean
+                    moving_s[c] = second[u];   // phase 2 must use the value read HERE: by then another CTA has updated the moving mean
             }
         }
     }
@@ -1058,8 +1064,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
     bool const active = static_cast<int>(threadIdx.x) < stride;
     int const o = threadIdx.x % octets, lane = threadIdx.x / octets;
     int const cbase = group * p.C + o * 8;
-    // forward: `mu` is a per-channel pivot (the moving mean): sums of (x - pivot) and (x - pivot)^2 keep E[x^2] - E[x]^2 well
-    // conditioned in fp32 even when |mean| >> std; backward: the saved batch statistics.
+    // forward: `mu` is a per-channel pivot (the group's first row, a sample of the batch, so also right on the first step when the
+    // moving mean is still zero): sums of (x - pivot) and (x - pivot)^2 keep E[x^2] - E[x]^2 well conditioned in fp32 even when
+    // |mean| >> std; backward: the saved batch statistics.
     float s0[8], s1[8], mu[8], rs[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -1183,7 +1190,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
                 t1 += part[r].y;
             }
             if (!BWD) {
-                float const pivot = pivot_s[c];
+                float const pivot = __bfloat162float(p.a[static_cast<long long>(group) * p.rows_per_group * p.C + c]);
                 double const shifted = t0 * inv_n;
                 double const mean = shifted + static_cast<double>(pivot);
                 double var = fma(-shifted, shifted, t1 * inv_n);
@@ -1197,7 +1204,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
                     p.save_rstd[idx] = rstd;
                     if (p.moving_mean && group == 0) {   // unbiased variance in the moving average, as TF's fused batch norm
                         double const unbiased = n > 1. ? var * n / (n - 1.) : var;
-                        p.moving_mean[c] = p.decay * pivot + (1.f - p.decay) * static_cast<float>(mean);
+                        p.moving_mean[c] = p.decay * moving_s[c] + (1.f - p.decay) * static_cast<float>(mean);
                         p.moving_var[c] = p.decay * p.moving_var[c] + (1.f - p.decay) * static_cast<float>(unbiased);
                     }
                 }
@@ -1231,7 +1238,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
             for (int j = 0; j < 8; ++j) {
                 va[j] = va[j] * c0[j] + c1[j] + vx[j];
                 if (p.relu)
-                    va[j] = fmaxf(va[j], 0.f);
+                    va[j] = max_nan(va[j], 0.f);
             }
         } else {
 #pragma unroll
@@ -1315,10 +1322,10 @@ long long g_fused_min_rows = 4096;
 template<bool BWD>
 int launch_bn_fused(BnFused p, long long rows, cudaStream_t s) {
     int const octets = p.C >> 3;
-    if ((p.C & 7) || 3 * p.C * 4 > kFusedScratchBytes || p.C * 4 > kFusedPivotBytes || p.groups < 1 || p.groups > agb::sm_count() || rows % p.groups || static_cast<long long>(p.C) * p.groups > 16384)
+    if ((p.C & 7) || 3 * p.C * 4 > kFusedScratchBytes || p.C * 4 > kFusedMovingBytes || p.groups < 1 || p.groups > agb::sm_count() || rows % p.groups || static_cast<long long>(p.C) * p.groups > 16384)
         return 399;
     static bool configured = false;
-    int const smem = kFusedScratchBytes + kFusedPivotBytes + kFusedStashBytes;
+    int const smem = kFusedScratchBytes + kFusedMovingBytes + kFusedStashBytes;
     if (!configured) {
         AGB_CUDA_OK(cudaFuncSetAttribute(bn_fused_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;

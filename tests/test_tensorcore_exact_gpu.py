@@ -411,11 +411,15 @@ def test_strided_operands(dtype):
 
 @gpu
 @pytest.mark.parametrize("dtype", [BF16, FP32], ids=["bf16", "tf32"])
-@pytest.mark.parametrize("layout", ["nt", "nn", "tn"])
+@pytest.mark.parametrize("layout", ["nt", "nn", "tn", "nt+relu"])
 def test_nonfinite_inputs_stay_in_their_row_and_column(layout, dtype):
-  """Inf in one row of A and NaN in one column of B (no ReLU): exactly the outputs in that row or column are non-finite, and every other
-  output is still exact. Catches contamination across tiles, k-splits or work items through the reused shared-memory ring."""
+  """Inf in one row of A and NaN in one column of B: exactly the outputs in that row or column are non-finite, and every other
+  output is still exact. Catches contamination across tiles, k-splits or work items through the reused shared-memory ring.
+  `nt+relu`: the epilogue ReLU keeps NaN and +inf and maps -inf to 0, so in the inf row only the outputs whose B entry is
+  positive (+inf) or zero (inf * 0 = NaN) stay non-finite."""
   from aggregathor_b200.ops import nn_native as nat
+  relu = layout == "nt+relu"
+  layout = "nt" if relu else layout
   m, n, k = 300, 260, 1000
   row, col, k_inf, k_nan = 131, 70, 5, 900
   sa, sb = _gemm_shapes(layout, m, n, k)
@@ -433,6 +437,13 @@ def test_nonfinite_inputs_stay_in_their_row_and_column(layout, dtype):
   expect[row, :] = True
   expect[:, col] = True
   ref = _on_grid(ref.masked_fill(expect, 0))
+  nonfinite = expect
+  if relu:
+    ref = torch.relu(ref)
+    inf_row = float("inf") * b[:, k_inf].double()   # the inf term of each output of the row; the finite terms cannot change it
+    nonfinite = expect.clone()
+    nonfinite[row, :] = torch.isnan(inf_row) | (inf_row > 0)
+    nonfinite[:, col] = True
   for persistent in (True, False):
     for bn, wide in BN_VARIANTS:
       with _gemm_mode(persistent, wide):
@@ -441,9 +452,9 @@ def test_nonfinite_inputs_stay_in_their_row_and_column(layout, dtype):
           if layout == "tn":
             out = nat.mm_tn(a, b, splits=splits, bn=bn)
           else:
-            out = (nat.mm_nt if layout == "nt" else nat.mm_nn)(a, b, bn=bn, out_dtype=FP32)
+            out = nat.mm_nt(a, b, relu=relu, bn=bn, out_dtype=FP32) if layout == "nt" else nat.mm_nn(a, b, bn=bn, out_dtype=FP32)
           bad = ~torch.isfinite(out)
-          assert torch.equal(bad, expect), (what, int((bad != expect).sum()), bad.nonzero()[:8].tolist())
+          assert torch.equal(bad, nonfinite), (what, int((bad != nonfinite).sum()), (bad != nonfinite).nonzero()[:8].tolist())
           _assert_exact(out.masked_fill(expect, 0), ref, what)
 
 
