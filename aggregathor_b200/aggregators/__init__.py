@@ -29,13 +29,15 @@ class FusedSpec:
            "centered-clipping", "dnc")
 
   RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc")   # the others ignore f
-  MIXES = (None, "nnm")
+  MIXES = (None, "nnm", "arc", "arc+nnm")   # the index is the kernel's bit mask: MIX_NNM | MIX_ARC
+  MIX_NNM, MIX_ARC = 1, 2
 
   def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None, subsample=10000, c=1.0, seed=0):
     """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing, `iterations` and `tau` centered
     clipping's iterations and clipping radius, `iterations`, `subsample`, `c` and `seed` DnC's iterations, sampled coordinates,
     filtering fraction and sampling seed; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
-    rule: None, or "nnm" (nearest-neighbour mixing with the same f)."""
+    rule, with the same f: None, "nnm" (nearest-neighbour mixing), "arc" (adaptive robust clipping) or "arc+nnm" (ARC, then NNM on
+    the clipped rows)."""
     if rule not in self.RULES:
       raise tools.UserException("Unknown fused rule " + repr(rule))
     if mix not in self.MIXES:
@@ -54,7 +56,7 @@ class FusedSpec:
     return self.MIXES.index(self.mix)
 
   def with_mix(self, mix, f=None):
-    """The same rule with pre-aggregation `mix` (None or "nnm"), and declared f `f` (default: unchanged)."""
+    """The same rule with pre-aggregation `mix` (one of `MIXES`), and declared f `f` (default: unchanged)."""
     return FusedSpec(self.rule, self.n, self.f if f is None else f, self.m, self.beta, iterations=self.iterations, nu=self.nu, tau=self.tau,
                      mix=mix, subsample=self.subsample, c=self.c, seed=self.seed)
 

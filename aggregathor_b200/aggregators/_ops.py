@@ -400,7 +400,7 @@ def torch_pairwise_distances(G):
 # ---------------------------------------------------------------------------- #
 # Nearest-neighbour mixing (NNM; Allouah et al., "Fixing by Mixing", AISTATS 2023): a pre-aggregation run on the rows before the rule
 
-PRE_AGGREGATIONS = ("none", "nnm")
+PRE_AGGREGATIONS = ("none", "nnm", "arc", "arc+nnm")   # "arc+nnm": adaptive robust clipping, then NNM on the clipped rows
 
 
 def check_pre_aggregation(name):
@@ -475,6 +475,78 @@ def host_nnm(G, f):
   Gc = G.detach().to("cpu").contiguous()
   member = nnm_select(host_pairwise_distances(Gc), f)
   return torch_nnm_mix(Gc, member, f).to(G.device)
+
+
+# Adaptive robust clipping (ARC; Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"): the k rows of
+# largest norm are clipped to the norm of the largest row left alone
+
+def check_arc(n, f):
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("Adaptive robust clipping needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+
+
+def arc_clip_count(n, f):
+  """k = floor(2 f (n - f) / n), in integer arithmetic: the number of rows ARC clips."""
+  check_arc(n, f)
+  return (2 * f * (n - f)) // n
+
+
+def arc_factors(N, f):
+  """[n] squared row norms -> ([n] factors in N's dtype, [n] bool mask of the clipped rows). The rows are ordered by N (finite ascending,
+  non-finite last, ties -> lower index); the last k are clipped, C = sqrt(N) of the row at position n - k - 1, and a clipped row's
+  factor is 1 if sqrt(N_i) <= C else C / sqrt(N_i) (every square root and the division rounded once); every factor is 1 and no row
+  is clipped when k = 0 or C is not finite."""
+  N = N.detach().to("cpu")
+  n = N.shape[0]
+  k = arc_clip_count(n, f)
+  one = torch.tensor(1.0, dtype=N.dtype)
+  factors = torch.ones(n, dtype=N.dtype)
+  clipped = torch.zeros(n, dtype=torch.bool)
+  if k == 0:
+    return factors, clipped
+  order = torch.argsort(_rank_key(N), stable=True)
+  # the square root of an fp32 value taken in fp64 and rounded once is correctly rounded
+  root = torch.sqrt(N.double()).to(N.dtype)
+  C = root[order[n - k - 1]]
+  if not math.isfinite(float(C)):
+    return factors, clipped
+  for i in order[n - k:].tolist():
+    clipped[i] = True
+    factors[i] = one if bool(root[i] <= C) else torch.div(C, root[i])
+  return factors, clipped
+
+
+def torch_arc_clip(G, factors):
+  """y_i = x_i * c_i, one `torch.mul` per row whose factor is not 1 (NaN included); the other rows are copied unchanged."""
+  Y = G.clone()
+  factors = factors.detach().to("cpu")
+  for i in range(G.shape[0]):
+    c = factors[i]
+    if not bool(c == 1):
+      Y[i] = torch.mul(G[i], c.to(device=G.device, dtype=G.dtype))
+  return Y
+
+
+def torch_arc(G, f, return_details=False):
+  """ARC with the torch back-end in G's dtype: squared norms, factors, clipping; `return_details` also gives (N, factors, clipped)."""
+  N = (G * G).sum(dim=1)
+  factors, clipped = arc_factors(N, f)
+  Y = torch_arc_clip(G, factors)
+  return (Y, N, factors, clipped) if return_details else Y
+
+
+def torch_pre_aggregate(G, mix, f, host=False):
+  """The pre-aggregation `mix` (a `FusedSpec.MIXES` value) of the [n, d] rows G with the torch reference: ARC, then NNM; `host`: NNM
+  takes the host library's distances for CPU rows (`host_nnm`)."""
+  if mix is None:
+    return G
+  if mix not in PRE_AGGREGATIONS:
+    raise tools.UserException("Unknown pre-aggregation %r (expected one of %s)" % (mix, ", ".join(PRE_AGGREGATIONS)))
+  if mix in ("arc", "arc+nnm"):
+    G = torch_arc(G, f)
+  if mix in ("nnm", "arc+nnm"):
+    G = host_nnm(G, f) if host and G.device.type == "cpu" else torch_nnm(G, f)
+  return G
 
 
 def krum_select(dist, f, m):

@@ -80,7 +80,7 @@ def make_parser():
   add("--authenticate", action="store_true", default=False, help="Sign every published gradient (ed25519) and verify before aggregating; slices failing the check become NaN")
   add("--worker-momentum", type=float, default=0.0, help="Worker momentum beta in [0, 1): every worker submits its momentum m <- beta m + (1 - dampening) g instead of its gradient (0 with a zero dampening: off)")
   add("--worker-momentum-dampening", type=float, default=0.0, help="Dampening of the worker momentum in [0, 1)")
-  add("--pre-aggregation", type=str, default="none", choices=("none", "nnm"), help="Pre-aggregation of the gathered rows before the rule: 'nnm' replaces every row by the mean of its n - f nearest rows (nearest-neighbour mixing, needs 0 <= 2 f < n), 'none' by default")
+  add("--pre-aggregation", type=str, default="none", choices=("none", "nnm", "arc", "arc+nnm"), help="Pre-aggregation of the gathered rows before the rule: 'nnm' replaces every row by the mean of its n - f nearest rows (nearest-neighbour mixing), 'arc' clips the floor(2 f (n - f) / n) rows of largest norm to the norm of the largest row left alone (adaptive robust clipping), 'arc+nnm' clips then mixes; all need 0 <= 2 f < n; 'none' by default")
   return parser
 
 
@@ -132,7 +132,8 @@ def _validate(args):
   fatal = (
     (n <= 0, "Expected at least one non-Byzantine worker"),
     (n < real, "Got more real Byzantine workers (" + repr(real) + ") than total number of workers (" + repr(n) + ")"),
-    (args.pre_aggregation == "nnm" and not 0 <= 2 * f < n, "Nearest-neighbour mixing needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)))
+    (args.pre_aggregation == "nnm" and not 0 <= 2 * f < n, "Nearest-neighbour mixing needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)),
+    (args.pre_aggregation in ("arc", "arc+nnm") and not 0 <= 2 * f < n, "Adaptive robust clipping needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)))
   for failed, message in fatal:
     if failed:
       raise tools.UserException(message)
@@ -196,7 +197,9 @@ def main(argv=None):
     if not quiet:
       print("Using a total of " + repr(args.nb_workers) + " worker(s):")
       print("· " + repr(nb_nonbyz_workers) + " non-Byzantine worker(s)")
-      print("· " + repr(args.nb_decl_byz_workers) + " declared Byzantine worker(s)" + (", nearest-neighbour mixing (NNM) before the rule" if args.pre_aggregation == "nnm" else ""))
+      pre = {"nnm": ", nearest-neighbour mixing (NNM) before the rule", "arc": ", adaptive robust clipping (ARC) before the rule",
+             "arc+nnm": ", adaptive robust clipping (ARC) then nearest-neighbour mixing (NNM) before the rule"}
+      print("· " + repr(args.nb_decl_byz_workers) + " declared Byzantine worker(s)" + pre.get(args.pre_aggregation, ""))
       print("  " + repr(args.nb_real_byz_workers) + " real Byzantine worker(s)")
       tools.print_args("experiment", args.experiment, args.experiment_args, head="")
       tools.print_args("gradient aggregation rule", args.aggregator, args.aggregator_args, head="")

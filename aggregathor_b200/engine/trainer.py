@@ -16,7 +16,8 @@ One synchronous step on a rank:
   3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
      Byzantine rows from the honest ones, a collective call on every rank);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast), after the optional pre-aggregation
-     (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing");
+     (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing"; "arc": adaptive
+     robust clipping, Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"; "arc+nnm": both);
   5. the bf16 compute copy of the parameters is refreshed (unless the fused kernel already wrote it).
 """
 
@@ -48,10 +49,11 @@ class Manager:
                regularizations=(-1., -1.), trace=False, *, attack=None, nb_real_byz=0, device=None, group=None, engine="auto", backend="auto",
                dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False,
                worker_momentum=0.0, worker_momentum_dampening=0.0, pre_aggregation="none", nb_decl_byz=None):
-    """`pre_aggregation`: "none" or "nnm" (every row replaced by the mean of its n - f nearest rows before the rule), with f =
-    `nb_decl_byz`, the declared Byzantine workers (default: the rule's own f)."""
+    """`pre_aggregation`: "none", "nnm" (every row replaced by the mean of its n - f nearest rows before the rule), "arc" (adaptive
+    robust clipping: the floor(2 f (n - f) / n) rows of largest norm clipped to the norm of the largest row left alone) or "arc+nnm"
+    (ARC, then NNM), with f = `nb_decl_byz`, the declared Byzantine workers (default: the rule's own f)."""
     from ..aggregators import _ops
-    self.pre_aggregation = _ops.check_pre_aggregation(pre_aggregation)   # None or "nnm"
+    self.pre_aggregation = _ops.check_pre_aggregation(pre_aggregation)   # None, "nnm", "arc" or "arc+nnm"
     # (beta, c = 1 - dampening) in fp32; beta = dampening = 0 is off: no buffer, no kernel, the step is unchanged
     self.momentum = _ops.check_worker_momentum(worker_momentum, worker_momentum_dampening)
     self.momentum_on = self.momentum[0] != 0.0 or _ops.fp32(worker_momentum_dampening) != 0.0
@@ -85,7 +87,7 @@ class Manager:
     engine_args = dict(engine_args or {})
     self._bucket_layers = {}
     # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum); with
-    # NNM the rule's distances are those of the mixed rows, which exist only once every row is complete
+    # a pre-aggregation the rule's distances are those of the mixed or clipped rows, which exist only once every row is complete
     plain_step = (attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
                   and self.pre_aggregation is None)
     if cuda and engine in ("auto", "fused") and aggregator.fused_spec() is not None:

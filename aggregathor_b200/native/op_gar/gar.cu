@@ -20,7 +20,9 @@
 //
 // Nearest-neighbour mixing (NNM, `a.mix`) runs inside the finish kernel before any rule: raw distance pass (staging every row) and
 // exchange, one selection warp, then every row of the staged tile is replaced by the mean of its n - f nearest rows; the rule then
-// reads the mixed tile (see `nnm_pre_aggregation`).
+// reads the mixed tile (see `nnm_pre_aggregation`). Adaptive robust clipping (ARC, bit kMixArc of `a.mix`) runs before NNM: a norm pass
+// (staging every row), one exchange of the squared norms, one selection warp, then the clipped rows of the tile are rescaled in
+// place (see `arc_pre_aggregation`).
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
 // whole-vector sums between the ranks, then the same per-coordinate write.
@@ -56,7 +58,8 @@ constexpr int kSlotGeoMedian = kMaxSeg + 3;   // geometric median, centered clip
 constexpr int kSlotMix = kSlotGeoMedian + kMaxIterations;   // NNM: exchange of the raw distances
 constexpr int kSlotCraftStats = kSlotMix + 1;   // Min-Max / Min-Sum: exchange of the crafting statistics
 constexpr int kSlotDnc = kSlotCraftStats + 1;   // DnC: exchange of the sampled distances
-constexpr int kFlagSlots = kSlotDnc + 1;
+constexpr int kSlotArc = kSlotDnc + 1;   // ARC: exchange of the squared row norms
+constexpr int kFlagSlots = kSlotArc + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 // Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
 // They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
@@ -66,7 +69,10 @@ constexpr int kCraftRegion = 2 * kMailboxRegion;
 constexpr int kDncIterations = 8;         // DnC: iterations T in [1, kDncIterations]
 constexpr int kDncStride = kDncIterations * kMaxPairs + 1;   // DnC post of one rank: T x [kMaxPairs] sampled distances, then the loss
 constexpr int kDncRegion = kCraftRegion + kMaxRanks * kCraftStats;   // mailbox region 3: kMaxRanks x kDncStride floats
-constexpr int kMailboxFloats = kDncRegion + kMaxRanks * kDncStride;
+constexpr int kArcStride = kMaxWorkers + 1;   // ARC post of one rank: the n partial squared norms, then the loss
+constexpr int kArcRegion = kDncRegion + kMaxRanks * kDncStride;   // mailbox region 4: kMaxRanks x kArcStride floats
+constexpr int kMailboxFloats = kArcRegion + kMaxRanks * kArcStride;
+constexpr int kMixNnm = 1, kMixArc = 2;   // GarArgs::mix bits
 constexpr int kJacobiSweeps = 32;         // DnC: sweep budget of the cyclic Jacobi
 constexpr double kJacobiTol = 1e-26;      // DnC: stop once sum_{i != j} B_ij^2 <= kJacobiTol * sum_i B_ii^2
 constexpr int kBlockRows = 8;             // rows held in registers at a time
@@ -114,7 +120,9 @@ struct GarArgs {
     float nu;                          // geometric median: smoothing, finite and > 0
     float tau;                         // centered clipping: clipping radius, finite and > 0
     float* center;                     // centered clipping: [d] (local) center v, read and updated on the owned coordinates
-    int mix;                           // pre-aggregation: 0 none, 1 nearest-neighbour mixing (needs the staging buffer)
+    int mix;                           // pre-aggregation bits (need the staging buffer): kMixNnm nearest-neighbour mixing, kMixArc adaptive
+                                       // robust clipping; both: ARC, then NNM
+    float* arc_out;                    // optional [2n]: ARC's squared norms N, then its factors c
     // DnC (T = iterations)
     int dnc_r;                         // rows removed per iteration, r = floor(c f)
     long long dnc_b, dnc_domain;       // subsample b and sample domain D: b' = min(b, D) coordinates of [0, D) per iteration
@@ -151,6 +159,8 @@ struct Shared {
     float warp_partials[16][kBlockRows * kBlockRows];
     unsigned selmask[kMaxWorkers];   // Krum, MDA: [0]; Bulyan: one per round
     unsigned nnm_mask[kMaxWorkers];  // NNM: neighbourhood of every row (itself included); outlives the rule's phases
+    float arc_c[kMaxWorkers];        // ARC: clipping factor of every row
+    unsigned arc_clipped;            // ARC: the rows the clip pass rescales
     int selcount[kMaxWorkers];
     int theta;
     float hyper[4];
@@ -797,7 +807,8 @@ __device__ void exchange_distances(GarArgs const& a, Shared& sh, cg::grid_group&
 // D_ij = ||x_i - x_j||^2 (non-finite -> +inf); N_i = {i} and the n - f - 1 rows j != i first under the ordering convention;
 // y_i = (((x_a0 + x_a1) + x_a2) + ...) / (n - f), the members of N_i in ascending worker order from +0, every operation rounded once.
 //   1. raw distance pass over all owned segments: the rows cross NVLink once and land in the staged tile (block 0's diagonal and the
-//      cross passes (0, b) store every row they load); exchange through mailbox region 1 and flag slot kSlotMix, which no other
+//      cross passes (0, b) store every row they load; after ARC, which staged and clipped every row, a STAGED_ONLY pass over the
+//      tile, behind a grid barrier); exchange through mailbox region 1 and flag slot kSlotMix, which no other
 //      exchange of the step touches (every CTA of every rank reads them, so a later exchange could not safely reuse them); the loss
 //      travels with it;
 //   2. warp 0 of every CTA builds the n masks from sh.dist (identical everywhere, so are the masks);
@@ -812,8 +823,12 @@ __device__ __forceinline__ void nnm_pre_aggregation(GarArgs const& a, Shared& sh
     for (int p = threadIdx.x; p < npairs; p += blockDim.x)
         mine[p] = 0.f;
     __syncthreads();
-    for (int seg = 0; seg < a.nseg; ++seg)
-        phase_a_segment<(N > kBlockRows)>(a, sh, pair_of, seg, mine, tid, nthreads);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        if (a.mix & kMixArc)   // after ARC the rows are staged (and clipped): the distances of the tile
+            phase_a_segment<(N > kBlockRows), true>(a, sh, pair_of, seg, mine, tid, nthreads);
+        else
+            phase_a_segment<(N > kBlockRows)>(a, sh, pair_of, seg, mine, tid, nthreads);
+    }
     exchange_distances(a, sh, grid, epoch, 0, kMailboxRegion, kSlotMix, local_loss, a.raw_dist_out);
     if (threadIdx.x < 32) {
         int const lane = threadIdx.x, keep = n - a.f - 1;
@@ -877,6 +892,154 @@ __device__ __forceinline__ void nnm_pre_aggregation(GarArgs const& a, Shared& sh
     }
 }
 
+// ---- adaptive robust clipping (ARC; Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning") ------- //
+// k = floor(2 f (n - f) / n); N_i = ||x_i||^2 (fp32); the k rows last under the ordering convention (by N) are clipped to the norm of
+// the row at position n - k - 1, C = sqrt_rn(N_thr): c_i = 1 if s_i <= C else C / s_i (s_i = sqrt_rn(N_i), centered clipping's
+// factor with radius C), y_i = x_i * c_i, one rounding each. c_i = 1 for every row when k = 0 or C is not finite.
+//   1. norm pass over all owned segments, with the rules' (tid, VEC) mapping: the rows cross NVLink once and land in the staged tile,
+//      N_i accumulates in registers (one FMA per value, as centered clipping's D_i);
+//   2. lanes -> warps -> CTA -> `cta_partials` -> grid barrier; block 0 folds the CTAs in order and posts the rank's partials and its
+//      loss into mailbox region 4 of every rank, then signals slot kSlotArc. Every CTA of every rank reads region 4 after the wait, so
+//      no later exchange of the step may reuse it; the next write into it comes from the next step's ARC exchange, which a rank
+//      reaches only after every rank's exit barrier of this step, hence after every CTA has finished reading;
+//   3. warp 0 of every CTA sums the R posts in rank order and selects (identical everywhere): sh.arc_c, sh.arc_clipped;
+//   4. clip pass, in place on the staged tile over the clipped rows only, with the same (tid, VEC) mapping: a coordinate-wise or
+//      iterative rule's thread reads back only values it staged and clipped itself, so no grid barrier follows; the distance rules,
+//      DnC's gather and NNM add one.
+template<int N, int VEC>
+__device__ __forceinline__ void arc_pre_aggregation(GarArgs const& a, Shared& sh, cg::grid_group& grid, uint32_t epoch, float local_loss,
+                                                    long long tid, long long nthreads) {
+    int const n = a.n, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    bool const multi = a.R > 1;
+    long long const owned = owned_length(a);
+    float acc[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i)
+        acc[i] = 0.f;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+#pragma unroll
+            for (int i0 = 0; i0 < N; i0 += kBlockRows) {   // 8 rows in flight at a time: the pass stays within the rules' register budget
+                float g[kBlockRows][VEC];
+#pragma unroll
+                for (int i = 0; i < kBlockRows; ++i)
+                    if (i0 + i < n)
+                        V<VEC>::load_stream(a.grad[i0 + i] + x, g[i]);
+#pragma unroll
+                for (int i = 0; i < kBlockRows; ++i) {
+                    if (i0 + i < n) {
+                        V<VEC>::store(a.staging + (i0 + i) * owned + soff + v * VEC, g[i]);
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            acc[i0 + i] = __fmaf_rn(g[i][c], g[i][c], acc[i0 + i]);
+                    }
+                }
+            }
+        }
+    }
+    // -------- exchange of the n partial squared norms (and the loss) -------- //
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        if (i < n) {
+            float const s = warp_sum(acc[i]);
+            if (lane == 0)
+                sh.warp_partials[warp][i] = s;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < n) {
+        float s = 0.f;
+        for (int w = 0; w < nwarps; ++w)
+            s += sh.warp_partials[w][threadIdx.x];
+        a.cta_partials[static_cast<long long>(blockIdx.x) * kMaxPairs + threadIdx.x] = s;
+    }
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        if (threadIdx.x < n) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kMaxPairs + threadIdx.x);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kArcRegion + a.rank * kArcStride + threadIdx.x] = s;
+        }
+        if (threadIdx.x == 0)
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kArcRegion + a.rank * kArcStride + kMaxWorkers] = local_loss;
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, kSlotArc, epoch);
+    }
+    if (multi) {
+        wait_all(a, kSlotArc, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    // -------- selection: warp 0 of every CTA -------- //
+    if (warp == 0) {
+        float const* const box = a.mailbox[a.rank] + kArcRegion;
+        float N2 = 0.f;
+        if (lane < n)
+            for (int q = 0; q < a.R; ++q)
+                N2 += ld_volatile_f(box + q * kArcStride + lane);
+        int const k = (2 * a.f * (n - a.f)) / n;
+        int rank = 0;
+        for (int j = 0; j < n; ++j) {
+            float const Nj = __shfl_sync(0xffffffffu, N2, j);
+            if (j != lane)
+                rank += before(Nj, j, N2, lane) ? 1 : 0;
+        }
+        unsigned const thr = __ballot_sync(0xffffffffu, lane < n && rank == n - k - 1);
+        float const C = __fsqrt_rn(__shfl_sync(0xffffffffu, N2, __ffs(thr) - 1));
+        bool const clipped = lane < n && k > 0 && is_finite(C) && rank >= n - k;
+        float const s = __fsqrt_rn(N2);
+        float const c = clipped ? (s <= C ? 1.f : __fdiv_rn(C, s)) : 1.f;
+        sh.arc_c[lane] = c;
+        unsigned const mask = __ballot_sync(0xffffffffu, clipped);
+        if (lane == 0)
+            sh.arc_clipped = mask;
+        if (blockIdx.x == 0) {
+            if (a.arc_out && lane < n) {
+                a.arc_out[lane] = N2;
+                a.arc_out[n + lane] = c;
+            }
+            if (lane == 0 && a.loss_out) {
+                float total = 0.f;
+                for (int q = 0; q < a.R; ++q)
+                    total += ld_volatile_f(box + q * kArcStride + kMaxWorkers);
+                *a.loss_out = total;
+            }
+        }
+    }
+    __syncthreads();
+    // -------- clip pass over the clipped rows of the staged tile -------- //
+    unsigned const mask = sh.arc_clipped;
+    if (mask == 0u)
+        return;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            float* const tile = a.staging + soff + v * VEC;
+#pragma unroll
+            for (int i = 0; i < N; ++i) {
+                if ((mask >> i) & 1u) {
+                    float const c = sh.arc_c[i];
+                    float y[VEC];
+                    V<VEC>::load(tile + i * owned, y);
+#pragma unroll
+                    for (int e = 0; e < VEC; ++e)
+                        y[e] = __fmul_rn(y[e], c);
+                    V<VEC>::store(tile + i * owned, y);
+                }
+            }
+        }
+    }
+}
+
 // ---- iterative rules: geometric median (smoothed Weiszfeld, RFA) and centered clipping ---------- //
 // Geometric median: z_0 = coordinate-wise median; for t < T: D_i = ||z_t - x_i||^2, rows with a non-finite D_i are skipped,
 // beta_i = 1 / max(nu, sqrt(D_i)), S = sum beta_i and z_{t+1} = (sum beta_i x_i) / S, both sums over the kept rows in ascending worker
@@ -898,7 +1061,8 @@ __device__ __forceinline__ void nnm_pre_aggregation(GarArgs const& a, Shared& sh
 // reads it before its block 0 reaches the grid barrier of iteration t, hence before it signals iteration t, and a writer stores
 // iteration t + 1 only after it has passed the barrier of iteration t, i.e. after every rank's iteration-t signal. With R = 1 a
 // second grid barrier takes the place of the flags. The loss travels through the exit barrier, as for the coordinate-wise rules
-// (with NNM: through NNM's exchange). With NNM, pass 0 reads the mixed tile too, with the mix pass's mapping (same thread).
+// (with a pre-aggregation: through its exchange). After a pre-aggregation, pass 0 reads the staged tile too (mixed or clipped), with
+// the mix and clip passes' mapping (same thread).
 template<int N, int VEC>
 __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg::grid_group& grid, float const (&hyper)[4], uint32_t epoch,
                                                long long tid, long long nthreads) {
@@ -911,7 +1075,7 @@ __device__ __forceinline__ void iterative_rule(GarArgs const& a, Shared& sh, cg:
     for (int t = 0; t <= T; ++t) {
         unsigned const mask = sh.geo.mask;
         float const S = sh.geo.sum;
-        bool const from_rows = !a.staging || (t == 0 && !a.mix);   // NNM: every pass reads the mixed tile
+        bool const from_rows = !a.staging || (t == 0 && !a.mix);   // NNM, ARC: every pass reads the pre-aggregated tile
         float acc[N];
 #pragma unroll
         for (int i = 0; i < N; ++i)
@@ -1393,8 +1557,8 @@ __device__ void dnc_selection(GarArgs const& a, Shared& sh, DncShared& ds, int* 
     }
 }
 
-// ---- coordinate-wise rules: one streaming pass over the rows, or (STAGED, NNM) over the mixed tile, each thread reading what it
-// wrote in the mix pass ------------------------------------------------------------------------------------------------------ //
+// ---- coordinate-wise rules: one streaming pass over the rows, or (STAGED, NNM / ARC) over the pre-aggregated tile, each thread
+// reading what it wrote in the mix or clip pass ------------------------------------------------------------------------------ //
 template<int N, int VEC, bool STAGED>
 __device__ __forceinline__ void coordinate_rules(GarArgs const& a, float const (&hyper)[4], long long tid, long long nthreads) {
     int const n = a.n;
@@ -1512,15 +1676,24 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
             local_loss += a.loss_in[j];
 
     if (a.mix) {
-        nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
-        if (distance_rule) {
-            __threadfence();
-            grid.sync();   // the mix pass wrote the tile with the rule's (tid, VEC) mapping; the distance pass reads it by float4 blocks
+        if (a.mix & kMixArc) {
+            arc_pre_aggregation<N, VEC>(a, sh, grid, epoch, local_loss, tid, nthreads);
+            if (distance_rule || (a.mix & kMixNnm)) {
+                __threadfence();
+                grid.sync();   // the clip pass wrote the tile with the rule's (tid, VEC) mapping; distance passes read it by float4 blocks
+            }
+        }
+        if (a.mix & kMixNnm) {
+            nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
+            if (distance_rule) {
+                __threadfence();
+                grid.sync();   // the mix pass wrote the tile with the rule's (tid, VEC) mapping; the distance pass reads it by float4 blocks
+            }
         }
     }
 
     if (distance_rule) {
-        // -------- phase A of the segments that were not pre-accumulated (NNM: of the mixed tile) -------- //
+        // -------- phase A of the segments that were not pre-accumulated (pre-aggregation: of the staged tile) -------- //
         float* mine = a.cta_partials + static_cast<long long>(blockIdx.x) * kMaxPairs;
         for (int p = threadIdx.x; p < npairs; p += blockDim.x)
             mine[p] = 0.f;
@@ -1700,9 +1873,17 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs 
         for (int j = 0; j < a.nloss; ++j)
             local_loss += a.loss_in[j];
     if (a.mix) {
-        nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
+        if (a.mix & kMixArc) {
+            arc_pre_aggregation<N, VEC>(a, sh, grid, epoch, local_loss, tid, nthreads);
+            if (a.mix & kMixNnm) {
+                __threadfence();
+                grid.sync();   // the clip pass wrote the tile with the rule's (tid, VEC) mapping; NNM's distance pass reads float4 blocks
+            }
+        }
+        if (a.mix & kMixNnm)
+            nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
         __threadfence();
-        grid.sync();   // the mix pass wrote the tile with the rule's (tid, VEC) mapping; the gather reads any coordinate of it
+        grid.sync();   // the clip or mix pass wrote the tile with the rule's (tid, VEC) mapping; the gather reads any coordinate of it
     }
     dnc_selection<N>(a, sh, ds, pair_of, grid, epoch, local_loss, tid, nthreads);   // carries the loss
     __syncthreads();
@@ -2276,8 +2457,9 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 //   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
+//   [115] arc_out (ARC: [2n] squared norms, then factors)
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-//       [25] iterations | [26] mix (0 none, 1 NNM) | [27] DnC r
+//       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC) | [27] DnC r
 // longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step [21] scratch floats
 // floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
@@ -2310,7 +2492,11 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     }
     if (a.rule < 0 || a.rule > kDnc)
         return 102;
-    if (a.mix < 0 || a.mix > 1 || (a.mix && (a.f < 0 || 2 * a.f >= a.n)))
+    if (a.mix < 0 || a.mix > (kMixNnm | kMixArc))
+        return 117;
+    if ((a.mix & kMixArc) && (a.f < 0 || 2 * a.f >= a.n))
+        return 120;
+    if ((a.mix & kMixNnm) && (a.f < 0 || 2 * a.f >= a.n))
         return 117;
     if (a.rule == kCenteredClipping && (a.f < 0 || 2 * a.f >= a.n || a.iterations < 1 || a.iterations > kMaxIterations || !(a.tau > 0.f) ||
                                         !std::isfinite(a.tau) || !a.center))
@@ -2354,6 +2540,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.loss_in = reinterpret_cast<float const*>(ptrs[45]);
     a.loss_out = reinterpret_cast<float*>(ptrs[46]);
     a.raw_dist_out = reinterpret_cast<float*>(ptrs[112]);
+    a.arc_out = reinterpret_cast<float*>(ptrs[115]);
     for (int q = 0; q < a.R; ++q) {
         a.param_dst[q] = reinterpret_cast<float*>(ptrs[48 + q]);
         a.signal[q] = reinterpret_cast<uint32_t*>(ptrs[64 + q]);
@@ -2377,9 +2564,9 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     if (a.rule == kDnc && a.first_seg > 0)
         return 111;   // DnC's sampled pass runs in its finish kernel: nothing is pre-accumulated
     if (a.mix && (!a.cta_partials || !a.mailbox[0] || !a.staging))
-        return 108;   // NNM mixes the staged tile in place
+        return 108;   // NNM mixes, ARC clips the staged tile in place
     if (a.mix && a.first_seg > 0)
-        return 111;   // NNM's raw distance pass covers every segment: nothing is pre-accumulated
+        return 111;   // NNM's raw distance pass and ARC's norm pass cover every segment: nothing is pre-accumulated
     if (a.R > 1 && !a.signal[0])
         return 109;
     if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && !a.staging)

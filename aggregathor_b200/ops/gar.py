@@ -21,17 +21,19 @@ MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
 # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange;
-# DnC's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 3
+# DnC's exchange; ARC's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 4
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 # Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]
 CRAFT_STATS = MAX_PAIRS + 2 * MAX_WORKERS + 1
 DNC_MAX_ITERATIONS = 8
 # DnC's post of one rank: the sampled distances of every iteration ([DNC_MAX_ITERATIONS][MAX_PAIRS]), then the loss
 DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
-# four regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances
-MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS) * 4
-PTRS = 115
+# ARC's post of one rank: the partial squared norms of the rows ([MAX_WORKERS]), then the loss
+ARC_STATS = MAX_WORKERS + 1
+# five regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms
+MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS) * 4
+PTRS = 116
 INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks; [96, 96 + T): DnC's mask of every iteration
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
 
@@ -46,7 +48,8 @@ _ERRORS = {
   116: "invalid centered-clipping parameters (0 <= 2 f < n, 1 <= iterations <= 16, finite tau > 0, a center buffer)",
   117: "invalid NNM parameters (0 <= 2 f < n)",
   118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)",
-  119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)"}
+  119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)",
+  120: "invalid ARC parameters (0 <= 2 f < n)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
@@ -90,6 +93,7 @@ class FusedLauncher:
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
     self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
     self.raw_dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)   # NNM: distances of the raw rows
+    self.arc_out = torch.zeros(2 * n, dtype=torch.float32, device=self.device)   # ARC: squared norms N [n], then factors c [n]
     self.dnc_dist_out = torch.zeros(DNC_MAX_ITERATIONS * n * n, dtype=torch.float32, device=self.device)   # DnC: [T, n, n] sampled distances
     self.ctas = ctas
     self._dnc_scratch = None
@@ -132,7 +136,7 @@ class FusedLauncher:
     if domain is None:
       domain = max(hi for _, hi in segments)
     scratch = self.dnc_scratch(spec, domain) if spec.rule == "dnc" else None
-    ptrs[113], ptrs[114] = addr(step_ptr), addr(scratch)
+    ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch), self.arc_out.data_ptr()
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -197,7 +201,9 @@ def aggregate(spec, G, return_details=False, center=None, step=0):
   DnC draws its samples with step key `step` over the d coordinates of G's rows; its details are the [T, n, n] sampled distances and
   `info` with [0] = 1, [1] = the final mask (bit i: row i kept) and [96 + t] = the mask of iteration t.
   With `spec.mix == "nnm"` the rule runs on the mixed rows (its distances and masks are those of the mixed rows), and
-  `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32)."""
+  `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32). With "arc" the rule runs on the
+  clipped rows and `return_details` adds (squared norms N [n], factors c [n]); with "arc+nnm" NNM mixes the clipped rows (its
+  distances are theirs) and both elements follow, NNM's first."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   n, d = G.shape
@@ -248,23 +254,26 @@ def _aligned_rows(G):
 
 
 def _staging(spec, n, dp, device):
-  """NNM mixes the rows in place in a local [n, dp] tile: the stand-alone op has to provide one."""
+  """NNM mixes and ARC clips the rows in place in a local [n, dp] tile: the stand-alone op has to provide one."""
   return torch.empty((n, dp), dtype=torch.float32, device=device) if spec.mix is not None else None
 
 
 def _mix_details(spec, launcher, n):
-  """The fourth `return_details` element with NNM: (raw distances [n, n], NNM masks [n] int32)."""
-  if spec.mix is None:
-    return ()
-  return ((launcher.raw_dist_out.view(n, n).clone(), launcher.info[64:64 + n].clone()),)
+  """The `return_details` elements of the pre-aggregation: with NNM (raw distances [n, n], NNM masks [n] int32), then with ARC
+  (squared norms [n], factors [n])."""
+  details = ()
+  if spec.mix_id & FusedSpec.MIX_NNM:
+    details += ((launcher.raw_dist_out.view(n, n).clone(), launcher.info[64:64 + n].clone()),)
+  if spec.mix_id & FusedSpec.MIX_ARC:
+    arc = launcher.arc_out.clone()
+    details += ((arc[:n], arc[n:]),)
+  return details
 
 
 def _torch_mixed(spec, G):
   """The fall-backs' pre-aggregation: `spec.mix` with the torch reference on G's device."""
-  if spec.mix is None:
-    return G
   from ..aggregators import _ops
-  return _ops.torch_nnm(G, spec.f)
+  return _ops.torch_pre_aggregate(G, spec.mix, spec.f)
 
 
 def _launcher(device, n):

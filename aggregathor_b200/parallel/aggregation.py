@@ -23,7 +23,8 @@ checkpointed with it) over the padded flat size `layout.padded_size`, on every e
 `pre_aggregation="nnm"` (nearest-neighbour mixing, `aggregators/_ops.py`) replaces every gathered row by the mean of its n - f
 nearest rows before the rule runs, on every engine: inside the fused kernel, in the stand-alone kernel of the baseline engine, with
 the host library's distances on the host engine and with the torch reference for plug-ins without a fused spec. The GAR object
-itself does not mix.
+itself does not mix. `pre_aggregation="arc"` (adaptive robust clipping) clips the k = floor(2 f (n - f) / n) rows of largest norm to
+the norm of the largest row left alone, in the same places (the host engine with the torch reference); "arc+nnm" clips, then mixes.
 """
 
 import os
@@ -42,21 +43,27 @@ def _world(group=None):
   return 0, 1
 
 
+_MIX_NAMES = {"nnm": "Nearest-neighbour mixing", "arc": "Adaptive robust clipping", "arc+nnm": "Adaptive robust clipping with nearest-neighbour mixing"}
+
+
 def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz):
-  """-> (mix, f of the mix, fused spec or None). NNM mixes with the declared f: `nb_decl_byz`, or by default the rule's own f. Rules
-  whose spec ignores f (average, average-nan, median, averaged-median) carry the declared f in their spec for the kernel's mix."""
+  """-> (mix, f of the mix, fused spec or None). The pre-aggregation (NNM, ARC or both) runs with the declared f: `nb_decl_byz`, or by
+  default the rule's own f. Rules whose spec ignores f (average, average-nan, median, averaged-median) carry the declared f in their
+  spec for the kernel's pre-aggregation."""
   from ..aggregators import FusedSpec, _ops
-  mix = _ops.check_pre_aggregation(pre_aggregation)   # None or "nnm"
+  mix = _ops.check_pre_aggregation(pre_aggregation)   # None, "nnm", "arc" or "arc+nnm"
   spec = gar.fused_spec()
   own = spec.f if spec is not None and spec.rule in FusedSpec.RULES_WITH_F else getattr(gar, "_f", None)
   f = own if nb_decl_byz is None else int(nb_decl_byz)
   if mix is None:
     return None, f, spec
+  name = _MIX_NAMES[mix]
   if f is None:
-    raise tools.UserException("Nearest-neighbour mixing needs the declared number of Byzantine workers f of GAR " + type(gar).__name__)
+    raise tools.UserException(name + " needs the declared number of Byzantine workers f of GAR " + type(gar).__name__)
   if own is not None and own != f:
-    raise tools.UserException("Nearest-neighbour mixing runs with the rule's f = %d (got f = %d)" % (own, f))
-  _ops.check_nnm(nbworkers, f)
+    raise tools.UserException(name + " runs with the rule's f = %d (got f = %d)" % (own, f))
+  if not 0 <= 2 * f < nbworkers:
+    raise tools.UserException(name + " needs 0 <= 2 f < n (got n = %d, f = %d)" % (nbworkers, f))
   return mix, f, (spec.with_mix(mix, f) if spec is not None else None)
 
 
@@ -172,7 +179,7 @@ class HostAggregation(_AggregationBase):
     rows = self._gathered
     if self.mix is not None:
       from ..aggregators import _ops
-      rows = _ops.host_nnm(rows, self.f) if rows.device.type == "cpu" else _ops.torch_nnm(rows, self.f)
+      rows = _ops.torch_pre_aggregate(rows, self.mix, self.f, host=True)
     aggregated = self.gar.aggregate(rows, **self._rule_kwargs())
     self.updates += 1
     self.optimizer.apply_torch(self.params, aggregated, self.slots, rate, self.updates)
@@ -214,12 +221,12 @@ class BaselineAggregation(_AggregationBase):
     self._gather()
     state = self._rule_kwargs()
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
-      aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)   # mixes inside the kernel
+      aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)   # pre-aggregates inside the kernel
     else:
       rows = self._gathered
       if self.mix is not None:
         from ..aggregators import _ops
-        rows = _ops.torch_nnm(rows, self.f)
+        rows = _ops.torch_pre_aggregate(rows, self.mix, self.f)
       aggregated = self.gar.aggregate(rows, **state)
     self.updates += 1
     if self.optimizer.name == "sgd":
@@ -271,8 +278,8 @@ class FusedAggregation(_AggregationBase):
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
-    # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; NNM mixes the staged tile in place
-    # and every rule then reads it (n * owned * 4 bytes, also with R = 1)
+    # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; a pre-aggregation (NNM mixes, ARC
+    # clips) rewrites the staged tile in place and every rule then reads it (n * owned * 4 bytes, also with R = 1)
     need_staging = ((self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
                     or self.mix is not None)
     self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
@@ -303,7 +310,7 @@ class FusedAggregation(_AggregationBase):
     # in-switch (NVLS) reduction of the gradients for the `average` rule instead of 7 P2P loads (0.241 vs 0.312 ms at 8 GPUs); AGB_NVLS_REDUCE=0 disables
     self._grad_mc = heap.multicast("grads") if (R > 1 and self.spec.rule == "average" and self.mix is None and os.environ.get("AGB_NVLS_REDUCE", "1") not in ("", "0")) else 0
     tools.info("Fused aggregation: rule %r%s, n = %d (%d per rank), d = %d, %d bucket(s), %d owned coordinates, provider %s, NVLS multicast %s" % (
-      self.spec.rule, " after NNM" if self.mix else "", self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
+      self.spec.rule, {"nnm": " after NNM", "arc": " after ARC", "arc+nnm": " after ARC and NNM"}.get(self.mix, ""), self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
 
   @staticmethod
   def _check_buckets(buckets, d):
@@ -328,8 +335,8 @@ class FusedAggregation(_AggregationBase):
 
   @property
   def overlappable(self):
-    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates); not with NNM,
-    whose raw distance pass runs in the finish kernel over every segment."""
+    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates); not with a
+    pre-aggregation, whose first pass (NNM's raw distances, ARC's norms) runs in the finish kernel over every segment."""
     return self.distance_rule and len(self.buckets) > 1 and self.mix is None
 
   def visible_rows(self):
@@ -444,7 +451,7 @@ def _single_host(group=None):
 
 def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None, **kwargs):
   """`kind` in {"auto", "fused", "baseline", "host"}; "auto" = fused on CUDA when the rule has a kernel and all ranks share one
-  machine, the NCCL baseline engine on CUDA otherwise, host on CPU. `pre_aggregation`: None / "none" or "nnm", on every engine, with
+  machine, the NCCL baseline engine on CUDA otherwise, host on CPU. `pre_aggregation`: None / "none", "nnm", "arc" or "arc+nnm", on every engine, with
   `nb_decl_byz` declared Byzantine workers (default: the rule's f)."""
   mix = dict(pre_aggregation=pre_aggregation, nb_decl_byz=nb_decl_byz)
   device = torch.device(device)

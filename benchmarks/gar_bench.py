@@ -20,6 +20,8 @@ dampening 0), with the 16 * w * d bytes it must move (G and M read and written o
 `--gar-pre-aggregation nnm` runs both engines with nearest-neighbour mixing before every rule (the checks above then hold for the
 mixed step), and also times the fused step of each rule without NNM, alternating with and without in the same process, to report
 the measured cost of the mix (`nnm_ms`, `plain_ms`, `nnm_overhead_ms`: medians over the alternated rounds).
+`--gar-pre-aggregation arc` (adaptive robust clipping) and `arc+nnm` (ARC, then NNM) do the same, with keys `arc_ms`,
+`arc_overhead_ms` and `arc_nnm_ms`, `arc_nnm_overhead_ms`.
 `dnc` (divide-and-conquer) takes `--gar-rule-args iterations:<T> subsample:<b> c:<c> seed:<s>`; both engines draw the same samples (the
 step key is the update count), so the fused-vs-baseline check holds for it as for the other rules; its entry also reports the rows
 each engine kept in the checked step (`fused_mask`, `baseline_mask`, `masks_agree`).
@@ -61,8 +63,9 @@ def main():
                       help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
   parser.add_argument("--gar-worker-momentum", dest="worker_momentum", type=float, default=None, metavar="BETA",
                       help="also time the worker-momentum kernel with this beta on the [w, d] rows of a rank")
-  parser.add_argument("--gar-pre-aggregation", dest="pre_aggregation", choices=("none", "nnm"), default="none",
-                      help="pre-aggregation of both engines (nnm: nearest-neighbour mixing, with the rule's f); nnm also times each rule without it")
+  parser.add_argument("--gar-pre-aggregation", dest="pre_aggregation", choices=("none", "nnm", "arc", "arc+nnm"), default="none",
+                      help="pre-aggregation of both engines, with the rule's f (nnm: nearest-neighbour mixing, arc: adaptive robust clipping, "
+                           "arc+nnm: both); also times each rule without it")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -203,24 +206,32 @@ def main():
     base_ms = time_engine(base)
     mix_entry = {}
     if fused.mix is not None:
-      # the same rule without NNM on the same rows, alternated with the NNM engine round by round (clock and thermal drift hit both)
+      # the same rule without the pre-aggregation on the same rows, alternated with the pre-aggregating engine round by round (clock and
+      # thermal drift hit both); keys are prefixed by the pre-aggregation: nnm_ms, arc_ms, arc_nnm_ms, ...
       plain = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True)
       plain.params.copy_(init)
       plain.grads.copy_(fused.grads)
       for _ in range(3):
         craft(plain)
         plain.step(0.1)
-      rounds = {"nnm": [], "plain": []}
+      rounds = {"pre": [], "plain": []}
       for _ in range(5):
-        rounds["nnm"].append(time_engine(fused))
+        rounds["pre"].append(time_engine(fused))
         rounds["plain"].append(time_engine(plain))
       median = lambda values: sorted(values)[len(values) // 2]
-      nnm_ms, plain_ms = median(rounds["nnm"]), median(rounds["plain"])
-      mix_entry = {"pre_aggregation": fused.mix, "nnm_ms": nnm_ms, "plain_ms": plain_ms, "nnm_overhead_ms": nnm_ms - plain_ms,
-                   "nnm_rounds_ms": rounds["nnm"], "plain_rounds_ms": rounds["plain"],
-                   # local HBM bytes the mix adds: the staging store, the mix pass (read + write), the rule's read of the tile, and one more
-                   # read for the distance pass of the mixed rows (Krum / Bulyan / MDA)
-                   "nnm_tile_hbm_bytes": (4 + (1 if rule in ("krum", "bulyan", "mda") else 0)) * n * (fused.hi - fused.lo) * 4}
+      pre_ms, plain_ms = median(rounds["pre"]), median(rounds["plain"])
+      key = fused.mix.replace("+", "_")
+      slice_rows = n * (fused.hi - fused.lo) * 4
+      # local HBM bytes of the staged tile: the staging store; ARC's clip pass (read + write of its k rows); NNM's mix pass (read + write)
+      # after its distance pass (a read of the tile when ARC staged it); the rule's read of the tile; and one more read for the distance
+      # pass of the pre-aggregated rows (Krum / Bulyan / MDA)
+      k = _ops.arc_clip_count(n, f) if "arc" in fused.mix else 0
+      tile_reads = 2 + (1 if rule in ("krum", "bulyan", "mda") else 0) + (2 if "nnm" in fused.mix else 0) + (1 if fused.mix == "arc+nnm" else 0)
+      mix_entry = {"pre_aggregation": fused.mix, key + "_ms": pre_ms, "plain_ms": plain_ms, key + "_overhead_ms": pre_ms - plain_ms,
+                   key + "_rounds_ms": rounds["pre"], "plain_rounds_ms": rounds["plain"],
+                   key + "_tile_hbm_bytes": tile_reads * slice_rows + 2 * k * (fused.hi - fused.lo) * 4}
+      if k:
+        mix_entry["arc_clipped_rows"] = k
       del plain
     attack_entry = {}
     if attack is not None:
