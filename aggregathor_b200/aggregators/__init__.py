@@ -26,9 +26,9 @@ class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
   RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
-           "centered-clipping", "dnc")
+           "centered-clipping", "dnc", "smea")
 
-  RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc")   # the others ignore f
+  RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc", "smea")   # the others ignore f
   MIXES = (None, "nnm", "arc", "arc+nnm")   # the index is the kernel's bit mask: MIX_NNM | MIX_ARC
   MIX_NNM, MIX_ARC = 1, 2
 

@@ -689,44 +689,66 @@ def _serial_sum(values):
   return float(np.cumsum(np.concatenate([[0.0], values]))[-1])
 
 
+def _serial_sums(values):
+  """Left-to-right float64 sums from +0 of the rows of the [S, k] array `values` -> [S]."""
+  return np.cumsum(np.concatenate([np.zeros((values.shape[0], 1)), values], axis=1), axis=1)[:, -1]
+
+
+def _jacobi(A, V=None):
+  """In place on the stack of symmetric [S, m, m] float64 matrices A (m >= 2) and, when given, their [S, m, m] eigenvector matrices V:
+  the cyclic Jacobi of `dnc_eigh`, applied to every matrix on its own. A matrix that passes its stop test is frozen (left out of the
+  later sweeps), exactly as if it had been run alone."""
+  m = A.shape[1]
+  mm = m + (m & 1)
+  offdiag = ~np.eye(m, dtype=bool)
+  diag = np.arange(m)
+  player = lambda pos, rnd: 0 if pos == 0 else 1 + (pos - 1 + rnd) % (mm - 1)
+  active = np.arange(A.shape[0])
+  with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
+    for _ in range(DNC_JACOBI_SWEEPS):
+      sq = A[active] * A[active]
+      active = active[~(_serial_sums(sq[:, offdiag]) <= DNC_JACOBI_TOL * _serial_sums(sq[:, diag, diag]))]
+      if active.size == 0:
+        break
+      X = A[active]
+      W = V[active] if V is not None else None
+      for rnd in range(mm - 1):
+        pairs = [sorted((player(k, rnd), player(mm - 1 - k, rnd))) for k in range(mm // 2)]
+        pairs = [(p, q) for p, q in pairs if q < m]
+        P = np.array([p for p, _ in pairs])
+        Q = np.array([q for _, q in pairs])
+        apq = X[:, P, Q]
+        tau = (X[:, Q, Q] - X[:, P, P]) / (2.0 * apq)
+        t = np.where(tau >= 0, 1.0, -1.0) / (np.abs(tau) + np.sqrt(1.0 + tau * tau))
+        c = 1.0 / np.sqrt(1.0 + t * t)
+        s = t * c
+        zero = apq == 0
+        c, s = np.where(zero, 1.0, c)[:, :, None], np.where(zero, 0.0, s)[:, :, None]
+        bp, bq = X[:, P, :].copy(), X[:, Q, :].copy()
+        X[:, P, :], X[:, Q, :] = c * bp - s * bq, s * bp + c * bq
+        c, s = c.transpose(0, 2, 1), s.transpose(0, 2, 1)
+        bp, bq = X[:, :, P].copy(), X[:, :, Q].copy()
+        X[:, :, P], X[:, :, Q] = c * bp - s * bq, s * bp + c * bq
+        if W is not None:
+          vp, vq = W[:, :, P].copy(), W[:, :, Q].copy()
+          W[:, :, P], W[:, :, Q] = c * vp - s * vq, s * vp + c * vq
+        X[:, P, Q] = 0.0
+        X[:, Q, P] = 0.0
+      A[active] = X
+      if V is not None:
+        V[active] = W
+
+
 def dnc_eigh(B):
   """Float64 cyclic Jacobi on the symmetric [m, m] matrix B (m >= 2) -> (eigenvalues, eigenvectors as columns), the sm_90a kernel's
   operations one for one: before each sweep (at most 32) stop when sum_{i != j} B_ij^2 <= 1e-26 sum_i B_ii^2 (both added row-major);
   a sweep is m' - 1 rounds (m' = m rounded up to even) of m' / 2 disjoint pairs (circle method); a round computes every pair's rotation
   from B as it stands (tau = (B_qq - B_pp) / (2 B_pq), t = sign(tau) / (|tau| + sqrt(1 + tau^2)), c = 1 / sqrt(1 + t^2), s = t c; none
   when B_pq = 0), rotates rows p, q, then columns p, q of B and V, then zeroes B_pq and B_qp."""
-  A = np.array(B, dtype=np.float64, copy=True)
-  m = A.shape[0]
-  V = np.eye(m)
-  mm = m + (m & 1)
-  offdiag = ~np.eye(m, dtype=bool)
-  player = lambda pos, rnd: 0 if pos == 0 else 1 + (pos - 1 + rnd) % (mm - 1)
-  with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
-    for _ in range(DNC_JACOBI_SWEEPS):
-      sq = A * A
-      if _serial_sum(sq[offdiag]) <= DNC_JACOBI_TOL * _serial_sum(np.diag(sq)):
-        break
-      for rnd in range(mm - 1):
-        pairs = [sorted((player(k, rnd), player(mm - 1 - k, rnd))) for k in range(mm // 2)]
-        pairs = [(p, q) for p, q in pairs if q < m]
-        P = np.array([p for p, _ in pairs])
-        Q = np.array([q for _, q in pairs])
-        apq = A[P, Q]
-        tau = (A[Q, Q] - A[P, P]) / (2.0 * apq)
-        t = np.where(tau >= 0, 1.0, -1.0) / (np.abs(tau) + np.sqrt(1.0 + tau * tau))
-        c = 1.0 / np.sqrt(1.0 + t * t)
-        s = t * c
-        zero = apq == 0
-        c, s = np.where(zero, 1.0, c)[:, None], np.where(zero, 0.0, s)[:, None]
-        bp, bq = A[P, :].copy(), A[Q, :].copy()
-        A[P, :], A[Q, :] = c * bp - s * bq, s * bp + c * bq
-        c, s = c.T, s.T
-        bp, bq, vp, vq = A[:, P].copy(), A[:, Q].copy(), V[:, P].copy(), V[:, Q].copy()
-        A[:, P], A[:, Q] = c * bp - s * bq, s * bp + c * bq
-        V[:, P], V[:, Q] = c * vp - s * vq, s * vp + c * vq
-        A[P, Q] = 0.0
-        A[Q, P] = 0.0
-  return np.diag(A).copy(), V
+  A = np.array(B, dtype=np.float64, copy=True)[None]
+  V = np.eye(A.shape[1])[None].copy()
+  _jacobi(A, V)
+  return np.diag(A[0]).copy(), V[0]
 
 
 def dnc_scores(dist):
@@ -820,6 +842,91 @@ def host_dnc(G, f, iterations, subsample, c, seed, step, domain=None, return_det
     raise tools.UserException("Host selection mean rejected its arguments")
   out = out.to(G.device)
   return (out, dists, (masks, good)) if return_details else out
+
+
+# ---------------------------------------------------------------------------- #
+# Smallest maximum eigenvalue averaging (SMEA; Allouah et al., "Robust Distributed Learning: Tight Error Bounds and Breakdown Point
+# under Data Heterogeneity", NeurIPS 2023): the selection (the sm_90a kernel's, bit for bit), the torch and host back-ends
+
+# the selection costs about 3.4 ms per set of 28 rows and warp on an H100 (every warp of the grid searches its share of the sets): the
+# bound keeps it below 50 ms; C(32, 4) = 35960 sets took 114 ms
+SMEA_MAX_SETS = 1 << 14
+
+
+def check_smea(n, f):
+  if not 0 <= 2 * f < n:
+    raise tools.UserException("SMEA needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f))
+  if math.comb(n, f) > SMEA_MAX_SETS:
+    raise tools.UserException("SMEA runs one eigenvalue search per subset of removed workers: C(%d, %d) = %d is above the bound 2^14" % (n, f, math.comb(n, f)))
+
+
+def smea_scores(dist, f, chunk=2048):
+  """[n, n] distances -> float64 scores of the C(n, f) kept sets S (|S| = m = n - f), in lexicographic kept-set order
+  (`itertools.combinations`): the largest diagonal entry of B_S = -1/2 (D_ij - r_i - r_j + g) over S (`dnc_scores`' double centring)
+  after `dnc_eigh`'s Jacobi, i.e. m times the largest eigenvalue of the covariance of S; +inf when a distance between two members of S
+  is not finite; 0 for m = 1. Vectorised over the sets (`chunk` at a time); every value has the bits of `dnc_eigh` on that set alone."""
+  D = np.asarray(dist.detach().to("cpu") if isinstance(dist, torch.Tensor) else dist, dtype=np.float64)
+  n = D.shape[0]
+  check_smea(n, f)
+  m = n - f
+  sets = np.array(list(itertools.combinations(range(n), m)), dtype=np.int64).reshape(-1, m)
+  scores = np.zeros(sets.shape[0])
+  for lo in range(0, sets.shape[0], chunk):
+    part = sets[lo:lo + chunk]
+    DS = D[part[:, :, None], part[:, None, :]]
+    finite = np.isfinite(DS).all(axis=(1, 2))
+    scores[lo:lo + chunk][~finite] = np.inf
+    if m < 2 or not finite.any():
+      continue
+    DS = DS[finite]
+    r = _serial_sums(DS.reshape(-1, m)).reshape(-1, m) / float(m)
+    g = _serial_sums(r) / float(m)
+    B = -0.5 * (((DS - r[:, :, None]) - r[:, None, :]) + g[:, None, None])
+    _jacobi(B)
+    with np.errstate(invalid="ignore"):
+      scores[lo:lo + chunk][finite] = np.max(np.diagonal(B, axis1=1, axis2=2), axis=1)
+  return scores
+
+
+def smea_select(dist, f, return_score=False):
+  """[n, n] distances -> ascending ids of the n - f kept workers whose score (`smea_scores`) is smallest, compared as doubles with
+  non-finite scores last and -0 == +0; ties -> the lexicographically smallest id list (`argmin` returns the first minimum of the
+  lexicographic enumeration). `return_score` also gives the winning score (+0 for a zero, +inf for a non-finite score)."""
+  n = dist.shape[0]
+  scores = smea_scores(dist, f)
+  key = np.where(np.isfinite(scores), scores, np.inf)
+  best = int(np.argmin(key))
+  ids = torch.tensor(next(itertools.islice(itertools.combinations(range(n), n - f), best, None)), dtype=torch.int64)
+  return (ids, float(key[best]) + 0.0) if return_score else ids
+
+
+def torch_smea(G, f, return_details=False):
+  """SMEA with torch ops in G's dtype and on its device (double inputs, more than 32 workers, the test oracle): distances, the selection
+  of `smea_select`, the selection mean. `return_details` also gives (distances, selected ids, winning score)."""
+  n = G.shape[0]
+  check_smea(n, f)
+  dist = torch_pairwise_distances(G)
+  ids, score = smea_select(dist, f, return_score=True)
+  good = np.zeros(n, dtype=bool)
+  good[ids.numpy()] = True
+  out = selection_mean(G, good)
+  return (out, dist, ids, score) if return_details else out
+
+
+def host_smea(G, f, return_details=False):
+  """SMEA with the host library: its distances (`agb_cpu_pairwise_distances`), the selection of `smea_select` and its selection mean.
+  Returns the output on G's device; `return_details` also gives (distances, selected ids, winning score)."""
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  check_smea(n, f)
+  dist = host_pairwise_distances(Gc)
+  ids, score = smea_select(dist, f, return_score=True)
+  out = torch.empty(d, dtype=Gc.dtype)
+  status = _host("selection_mean", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(ids), ctypes.c_size_t(ids.numel()), _ptr(out))
+  if status != 0:
+    raise tools.UserException("Host selection mean rejected its arguments")
+  out = out.to(G.device)
+  return (out, dist, ids, score) if return_details else out
 
 
 # ---------------------------------------------------------------------------- #

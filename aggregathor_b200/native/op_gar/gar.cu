@@ -11,8 +11,8 @@
 //                    distances with direct differences, stage the tile locally
 //   finish kernel    (cooperative) phase A of whatever was not pre-accumulated; partial matrices go to every peer's mailbox together
 //                    with the rank's loss sum; summed in rank order => bit-identical distance matrix (and total loss) on every rank;
-//                    one warp: Krum scores / Bulyan iterative selection, or the whole grid: MDA's minimum-diameter search
-//                    (replicated on all ranks); phase D: aggregate the owned coordinates (mean of selected / coordinate-wise
+//                    one warp: Krum scores / Bulyan iterative selection, or the whole grid: MDA's minimum-diameter search or
+//                    SMEA's smallest-largest-eigenvalue search (replicated on all ranks); phase D: aggregate the owned coordinates (mean of selected / coordinate-wise
 //                    trimmed mean / median / NaN-aware mean), apply the optimizer,
 //                    store the new parameters into every rank's buffer (P2P stores or one NVLS multimem.st); exit barrier
 //                    geometric median / centered clipping instead: T + 1 passes over the owned coordinates, with one exchange of
@@ -78,8 +78,9 @@ constexpr double kJacobiTol = 1e-26;      // DnC: stop once sum_{i != j} B_ij^2 
 constexpr int kBlockRows = 8;             // rows held in registers at a time
 
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
+constexpr long long kSmeaMaxSets = 1 << 14;   // SMEA runs one float64 Jacobi per removal set (`_ops.SMEA_MAX_SETS`)
 enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8,
-           kCenteredClipping = 9, kDnc = 10 };
+           kCenteredClipping = 9, kDnc = 10, kSmea = 11 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -130,6 +131,7 @@ struct GarArgs {
     long long dnc_step;                // step key, used when dnc_step_ptr is null
     long long const* dnc_step_ptr;     // device step key (graph replay), or null
     float* dnc_scratch;                // [grid][kDncIterations][kMaxPairs] CTA partials, then the samples [T][n][b'4]
+    double* smea_scratch;              // SMEA: one [m][m] slab per warp of the grid (m = n - f), the double-centred matrix of its set
 };
 
 // the rows `phase_a_segment` reads in DnC's sampled pass: one segment [0, b'4) of the gathered samples of one iteration, no staging
@@ -149,6 +151,10 @@ struct Shared {
             unsigned binom[kMaxWorkers + 1][kMaxWorkers / 2 + 1];
             unsigned long long best[16];                  // per-warp minimum keys
         } mda;
+        struct {                                          // SMEA
+            unsigned binom[kMaxWorkers + 1][kMaxWorkers / 2 + 1];
+            unsigned long long best[16][2];               // per-warp minimum keys (score key, set key)
+        } smea;
         struct {                                          // geometric median, centered clipping: weights of the current iterate
             float beta[kMaxWorkers];                      // 1 / max(nu, sqrt(D_i)) (CC: the clipping factors c_i) of the kept rows
             float sum;                                    // geometric median: their sum, in ascending worker order
@@ -489,17 +495,43 @@ __device__ void select_bulyan(GarArgs const& a, Shared& sh) {
 // is the distance of the first pair, in descending distance order, whose ends are both kept: at most f (n - 1) + 1 steps. Keys
 // (diameter bits, ~__brev(mask)) are exact, so their minimum does not depend on the reduction order: every CTA and every rank (same
 // distance matrix) selects the same set. The per-CTA minima go through `cta_partials`, free again once the distances are exchanged.
-__device__ void select_mda(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
+// binom[m][k] = C(m, k) for m <= 32, k <= 16 (whole CTA; the caller synchronises)
+__device__ __forceinline__ void fill_binomials(unsigned (&binom)[kMaxWorkers + 1][kMaxWorkers / 2 + 1]) {
     constexpr int K = kMaxWorkers / 2 + 1;
-    int const n = a.n, f = a.f, npairs = n * (n - 1) / 2;
-    int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     for (int p = threadIdx.x; p < (kMaxWorkers + 1) * K; p += blockDim.x) {
         int const m = p / K, k = p % K;
         unsigned long long c = 1;   // C(m, k) < 2^32 for m <= 32; every partial product is an exact binomial times (m - t)
         for (int t = 0; t < k && t < m; ++t)
             c = c * (m - t) / (t + 1);
-        sh.mda.binom[m][k] = k > m ? 0u : static_cast<unsigned>(c);
+        binom[m][k] = k > m ? 0u : static_cast<unsigned>(c);
     }
+}
+
+// the removal set of rank r among the f-subsets of [0, n) in colexicographic order (= ascending masks): the combinatorial number
+// system, r = sum_k C(c_k, k), c_f > ... > c_1
+__device__ __forceinline__ unsigned unrank_removal(unsigned const (&binom)[kMaxWorkers + 1][kMaxWorkers / 2 + 1], int n, int f, long long r) {
+    unsigned removed = 0;
+    long long rest = r;
+    for (int k = f; k >= 1; --k) {
+        int c = n - 1;
+        while (binom[c][k] > rest)
+            --c;
+        removed |= 1u << c;
+        rest -= binom[c][k];
+    }
+    return removed;
+}
+
+// Gosper's hack: the next mask with as many bits as `removed` (removed != 0)
+__device__ __forceinline__ unsigned next_removal(unsigned removed) {
+    unsigned const low = removed & (0u - removed), up = removed + low;
+    return (((up ^ removed) >> 2) >> (__ffs(low) - 1)) | up;
+}
+
+__device__ void select_mda(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
+    int const n = a.n, f = a.f, npairs = n * (n - 1) / 2;
+    int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    fill_binomials(sh.mda.binom);
     for (int p = threadIdx.x; p < npairs; p += blockDim.x) {   // rank of pair p by (distance descending, pair index ascending)
         int i = 0, rest = p;
         while (rest >= n - 1 - i) {
@@ -526,15 +558,7 @@ __device__ void select_mda(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
     unsigned const full = n == 32 ? 0xffffffffu : (1u << n) - 1u;
     unsigned long long best = ~0ull;
     if (r < end) {
-        unsigned removed = 0;   // combinatorial number system: r = sum_k C(c_k, k), c_f > ... > c_1
-        long long rest = r;
-        for (int k = f; k >= 1; --k) {
-            int c = n - 1;
-            while (sh.mda.binom[c][k] > rest)
-                --c;
-            removed |= 1u << c;
-            rest -= sh.mda.binom[c][k];
-        }
+        unsigned removed = unrank_removal(sh.mda.binom, n, f, r);
         for (;;) {
             unsigned const keep = full & ~removed;
             float diam = 0.f;
@@ -549,8 +573,7 @@ __device__ void select_mda(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
             best = key < best ? key : best;
             if (++r >= end)
                 break;
-            unsigned const low = removed & (0u - removed), up = removed + low;   // Gosper's hack: next mask with f bits
-            removed = (((up ^ removed) >> 2) >> (__ffs(low) - 1)) | up;
+            removed = next_removal(removed);
         }
     }
     for (int o = 16; o > 0; o >>= 1) {
@@ -1272,6 +1295,15 @@ __device__ __forceinline__ bool before_d(double a, int ia, double b, int ib) {
     return ia < ib;
 }
 
+// the rotation (c, s) that zeroes B_pq != 0: tau = (B_qq - B_pp) / (2 B_pq), t = sign(tau) / (|tau| + sqrt(1 + tau^2)), c = 1 / sqrt(1 + t^2),
+// s = t c, every operation rounded once (DnC's and SMEA's Jacobi, and `_ops.dnc_eigh`)
+__device__ __forceinline__ void jacobi_rotation(double bpp, double bqq, double apq, double& c, double& s) {
+    double const tau = __ddiv_rn(__dsub_rn(bqq, bpp), __dmul_rn(2.0, apq));
+    double const t = __ddiv_rn(tau >= 0.0 ? 1.0 : -1.0, __dadd_rn(fabs(tau), __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(tau, tau)))));
+    c = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(t, t))));
+    s = __dmul_rn(t, c);
+}
+
 // eigenvectors of ds.B[0, m)^2 (m >= 2) into ds.V; B ends (nearly) diagonal. A sweep is m' - 1 rounds (m' = m rounded up to
 // even) of m' / 2 disjoint pairs (circle method: position 0 fixed, the others rotated); a round computes every pair's rotation from
 // B as it stands, then rotates the rows, then the columns of B and V, then zeroes B_pq and B_qp.
@@ -1299,13 +1331,8 @@ __device__ void dnc_jacobi(DncShared& ds, int m) {
                 int const u = player(threadIdx.x, round), v = player(mm - 1 - threadIdx.x, round);
                 int const p = u < v ? u : v, q = u < v ? v : u;
                 double c = 1.0, s = 0.0;
-                if (q < m && ds.B[p][q] != 0.0) {
-                    double const apq = ds.B[p][q];
-                    double const tau = __ddiv_rn(__dsub_rn(ds.B[q][q], ds.B[p][p]), __dmul_rn(2.0, apq));
-                    double const t = __ddiv_rn(tau >= 0.0 ? 1.0 : -1.0, __dadd_rn(fabs(tau), __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(tau, tau)))));
-                    c = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(1.0, __dmul_rn(t, t))));
-                    s = __dmul_rn(t, c);
-                }
+                if (q < m && ds.B[p][q] != 0.0)
+                    jacobi_rotation(ds.B[p][p], ds.B[q][q], ds.B[p][q], c, s);
                 ds.rot[threadIdx.x][0] = c;
                 ds.rot[threadIdx.x][1] = s;
             }
@@ -1344,6 +1371,176 @@ __device__ void dnc_jacobi(DncShared& ds, int m) {
                 }
             }
             __syncthreads();
+        }
+    }
+}
+
+// SMEA (every thread of the grid): the kept set S, |S| = m = n - f, whose double-centred matrix B_S = -1/2 (D_ij - r_i - r_j + g) (r_i
+// the row means over S, g their mean, both added in ascending index) has the smallest largest eigenvalue; the score is the largest
+// diagonal entry after the Jacobi of `dnc_jacobi` (same rounds, rotations, stop test and sweep budget; no eigenvectors), +inf for a set
+// with a non-finite distance between two members, 0 for m = 1; ties -> the lexicographically smallest sorted index list. The C(n, f)
+// removal sets are split over the warps of the grid, unranked and stepped as in `select_mda`; a warp keeps B_S in its own [m][m] slab of
+// `smea_scratch` and runs every round warp-synchronously. Keys (the score's ordered bits with -0 -> +0 and non-finite -> +inf, then
+// ~__brev(keep)) are exact, so their minimum does not depend on the reduction order. The per-CTA minima go through `cta_partials`;
+// block 0 writes the winning score's bits to info[32, 34).
+__device__ void select_smea(GarArgs const& a, Shared& sh, cg::grid_group& grid) {
+    int const n = a.n, f = a.f, m = n - f, mm = m + (m & 1), half = mm / 2;
+    int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    unsigned const all = 0xffffffffu, full = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    double const inf = __longlong_as_double(0x7ff0000000000000ll);
+    fill_binomials(sh.smea.binom);
+    __syncthreads();
+    unsigned bad = 0u;   // lane i < n: the workers j with a non-finite D_ij
+    if (lane < n)
+        for (int j = 0; j < n; ++j)
+            bad |= is_finite(sh.dist[lane][j]) ? 0u : 1u << j;
+    long long const total = sh.smea.binom[n][f];
+    long long const gwarps = static_cast<long long>(gridDim.x) * nwarps, gw = static_cast<long long>(blockIdx.x) * nwarps + warp;
+    long long const per = (total + gwarps - 1) / gwarps;
+    long long r = gw * per;
+    long long const end = r + per < total ? r + per : total;
+    double* const B = a.smea_scratch + gw * m * m;
+    auto player = [&](int pos, int round) { return pos == 0 ? 0 : 1 + (pos - 1 + round) % (mm - 1); };
+    unsigned long long best_score = ~0ull, best_set = ~0ull;
+    if (r < end) {
+        unsigned removed = unrank_removal(sh.smea.binom, n, f, r);
+        for (;;) {
+            unsigned const keep = full & ~removed;
+            double score = 0.0;
+            if (__any_sync(all, lane < n && ((keep >> lane) & 1u) && (bad & keep))) {
+                score = inf;
+            } else if (m >= 2) {
+                int const i = lane < m ? static_cast<int>(__fns(keep, 0, lane + 1)) : 0;   // lane k < m: row k, the k-th kept worker
+                double rmean = 0.0;
+                if (lane < m) {
+                    double sum = 0.0;
+                    for (unsigned rest = keep; rest; rest &= rest - 1)
+                        sum = __dadd_rn(sum, static_cast<double>(sh.dist[i][__ffs(rest) - 1]));
+                    rmean = __ddiv_rn(sum, static_cast<double>(m));
+                }
+                double grand = 0.0;
+                for (int k = 0; k < m; ++k)
+                    grand = __dadd_rn(grand, __shfl_sync(all, rmean, k));
+                grand = __ddiv_rn(grand, static_cast<double>(m));
+                unsigned rest = keep;
+                for (int j = 0; j < m; ++j, rest &= rest - 1) {
+                    double const rj = __shfl_sync(all, rmean, j);
+                    if (lane < m) {
+                        double const dij = static_cast<double>(sh.dist[i][__ffs(rest) - 1]);
+                        B[lane * m + j] = __dmul_rn(-0.5, __dadd_rn(__dsub_rn(__dsub_rn(dij, rmean), rj), grand));
+                    }
+                }
+                __syncwarp();
+                for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
+                    int converged = 0;
+                    if (lane == 0) {
+                        double off = 0.0, diag = 0.0;
+                        for (int p = 0; p < m; ++p)
+                            for (int q = 0; q < m; ++q) {
+                                double const sq = __dmul_rn(B[p * m + q], B[p * m + q]);
+                                if (p == q)
+                                    diag = __dadd_rn(diag, sq);
+                                else
+                                    off = __dadd_rn(off, sq);
+                            }
+                        converged = off <= __dmul_rn(kJacobiTol, diag);
+                    }
+                    if (__shfl_sync(all, converged, 0))
+                        break;
+                    for (int round = 0; round < mm - 1; ++round) {
+                        double c = 1.0, s = 0.0;   // lane k < m' / 2: the rotation of pair k, from B as it stands
+                        if (lane < half) {
+                            int const u = player(lane, round), v = player(mm - 1 - lane, round);
+                            int const p = u < v ? u : v, q = u < v ? v : u;
+                            if (q < m && B[p * m + q] != 0.0)
+                                jacobi_rotation(B[p * m + p], B[q * m + q], B[p * m + q], c, s);
+                        }
+                        __syncwarp();
+                        for (int base = 0; base < half * m; base += 32) {   // rows p, q
+                            int const task = base + lane, k = task / m, j = task % m;
+                            double const ck = __shfl_sync(all, c, k & 31), sk = __shfl_sync(all, s, k & 31);
+                            int const u = player(k, round), v = player(mm - 1 - k, round);
+                            int const p = u < v ? u : v, q = u < v ? v : u;
+                            if (task < half * m && q < m) {
+                                double const bp = B[p * m + j], bq = B[q * m + j];
+                                B[p * m + j] = __dsub_rn(__dmul_rn(ck, bp), __dmul_rn(sk, bq));
+                                B[q * m + j] = __dadd_rn(__dmul_rn(sk, bp), __dmul_rn(ck, bq));
+                            }
+                        }
+                        __syncwarp();
+                        for (int base = 0; base < half * m; base += 32) {   // columns p, q
+                            int const task = base + lane, k = task / m, i2 = task % m;
+                            double const ck = __shfl_sync(all, c, k & 31), sk = __shfl_sync(all, s, k & 31);
+                            int const u = player(k, round), v = player(mm - 1 - k, round);
+                            int const p = u < v ? u : v, q = u < v ? v : u;
+                            if (task < half * m && q < m) {
+                                double const bp = B[i2 * m + p], bq = B[i2 * m + q];
+                                B[i2 * m + p] = __dsub_rn(__dmul_rn(ck, bp), __dmul_rn(sk, bq));
+                                B[i2 * m + q] = __dadd_rn(__dmul_rn(sk, bp), __dmul_rn(ck, bq));
+                            }
+                        }
+                        __syncwarp();
+                        if (lane < half) {
+                            int const u = player(lane, round), v = player(mm - 1 - lane, round);
+                            int const p = u < v ? u : v, q = u < v ? v : u;
+                            if (q < m) {
+                                B[p * m + q] = 0.0;
+                                B[q * m + p] = 0.0;
+                            }
+                        }
+                        __syncwarp();
+                    }
+                }
+                score = lane < m ? B[lane * (m + 1)] : -inf;   // the largest diagonal entry; a NaN wins
+                for (int o = 16; o > 0; o >>= 1) {
+                    double const other = __shfl_xor_sync(all, score, o);
+                    score = (other > score || other != other) ? other : score;
+                }
+            }
+            unsigned long long bits = !isfinite(score) ? 0x7ff0000000000000ull : score == 0.0 ? 0ull : static_cast<unsigned long long>(__double_as_longlong(score));
+            unsigned long long const skey = (bits >> 63) ? ~bits : bits | (1ull << 63), set = ~__brev(keep);
+            if (skey < best_score || (skey == best_score && set < best_set)) {
+                best_score = skey;
+                best_set = set;
+            }
+            if (++r >= end)
+                break;
+            removed = next_removal(removed);
+        }
+    }
+    if (lane == 0) {
+        sh.smea.best[warp][0] = best_score;
+        sh.smea.best[warp][1] = best_set;
+    }
+    __syncthreads();
+    unsigned long long* const slots = reinterpret_cast<unsigned long long*>(a.cta_partials);
+    if (threadIdx.x == 0) {
+        for (int w = 0; w < nwarps; ++w)
+            if (sh.smea.best[w][0] < best_score || (sh.smea.best[w][0] == best_score && sh.smea.best[w][1] < best_set)) {
+                best_score = sh.smea.best[w][0];
+                best_set = sh.smea.best[w][1];
+            }
+        slots[static_cast<long long>(blockIdx.x) * (kMaxPairs / 2)] = best_score;
+        slots[static_cast<long long>(blockIdx.x) * (kMaxPairs / 2) + 1] = best_set;
+    }
+    __threadfence();
+    grid.sync();
+    if (threadIdx.x == 0) {
+        for (unsigned b = 0; b < gridDim.x; ++b) {
+            unsigned long long volatile const* const slot = slots + static_cast<long long>(b) * (kMaxPairs / 2);
+            unsigned long long const score = slot[0], set = slot[1];
+            if (score < best_score || (score == best_score && set < best_set)) {
+                best_score = score;
+                best_set = set;
+            }
+        }
+        sh.selmask[0] = __brev(~static_cast<unsigned>(best_set));
+        sh.selcount[0] = m;
+        sh.theta = 1;
+        if (a.info && blockIdx.x == 0) {
+            unsigned long long const bits = (best_score >> 63) ? best_score & ~(1ull << 63) : ~best_score;
+            a.info[32] = static_cast<int>(static_cast<unsigned>(bits));
+            a.info[33] = static_cast<int>(static_cast<unsigned>(bits >> 32));
         }
     }
 }
@@ -1653,7 +1850,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
     long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
     bool const multi = a.R > 1;
-    bool const distance_rule = a.rule == kKrum || a.rule == kBulyan || a.rule == kMda;
+    bool const distance_rule = a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kSmea;
     if (threadIdx.x == 0) {
         sh.epoch = current_epoch(a);
         for (int i = 0; i < 4; ++i)
@@ -1708,6 +1905,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
         exchange_distances(a, sh, grid, epoch, a.first_seg, 0, kSlotExchange, local_loss, a.dist_out);
         if (a.rule == kMda) {
             select_mda(a, sh, grid);
+        } else if (a.rule == kSmea) {
+            select_smea(a, sh, grid);
         } else if (threadIdx.x < 32) {
             if (a.rule == kKrum)
                 select_krum(a, sh);
@@ -1732,7 +1931,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
                         V<VEC>::load_stream(a.grad[i] + x, dst);
                 };
                 float out[VEC];
-                if (a.rule != kBulyan) {   // Krum, MDA: mean of the selected rows
+                if (a.rule != kBulyan) {   // Krum, MDA, SMEA: mean of the selected rows
                     unsigned const mask = sh.selmask[0];
                     float sum[VEC];
 #pragma unroll
@@ -2447,6 +2646,8 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
         if (static_cast<long long>(grid) * kDncIterations * kMaxPairs + a.iterations * a.n * ((b + 3) & ~3ll) > scratch_floats)
             return 108;
     }
+    if (a.rule == kSmea && static_cast<long long>(grid) * (threads / 32) * (a.n - a.f) * (a.n - a.f) > scratch_floats)
+        return 108;   // one [m][m] slab of doubles per warp
     void* params[] = {&a};
     AGB_CUDA_OK(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(threads), params, 0, stream));
     return 0;
@@ -2457,10 +2658,11 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
 //   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 //   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
-//   [115] arc_out (ARC: [2n] squared norms, then factors)
+//   [115] arc_out (ARC: [2n] squared norms, then factors) | [116] SMEA scratch (doubles)
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
 //       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC) | [27] DnC r
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step [21] scratch floats
+// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step
+//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles)
 // floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
@@ -2479,6 +2681,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.dnc_step = longs[20];
     a.dnc_step_ptr = reinterpret_cast<long long const*>(ptrs[113]);
     a.dnc_scratch = reinterpret_cast<float*>(ptrs[114]);
+    a.smea_scratch = reinterpret_cast<double*>(ptrs[116]);
     if (a.n < 1 || a.n > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
@@ -2490,7 +2693,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kDnc)
+    if (a.rule < 0 || a.rule > kSmea)
         return 102;
     if (a.mix < 0 || a.mix > (kMixNnm | kMixArc))
         return 117;
@@ -2515,6 +2718,15 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
             sets = sets * (a.n - t) / (t + 1);
         if (sets > kMdaMaxSets)
             return 113;
+    }
+    if (a.rule == kSmea) {
+        if (a.f < 0 || 2 * a.f >= a.n)
+            return 122;
+        long long sets = 1;   // C(n, f), exact while it stays below the bound
+        for (int t = 0; t < a.f && sets <= kSmeaMaxSets; ++t)
+            sets = sets * (a.n - t) / (t + 1);
+        if (sets > kSmeaMaxSets)
+            return 122;
     }
     if ((a.rule == kKrum || a.rule == kBulyan) && (a.n - a.f - 2 < 1 || a.m < 1 || a.m > a.n))
         return 103;
@@ -2553,7 +2765,10 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 107;
     if (a.opt == kAdagrad && !a.slot0)
         return 107;
-    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kGeoMedian || a.rule == kCenteredClipping) && (!a.cta_partials || !a.mailbox[0]))
+    if ((a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kSmea || a.rule == kGeoMedian || a.rule == kCenteredClipping) &&
+        (!a.cta_partials || !a.mailbox[0]))
+        return 108;
+    if (a.rule == kSmea && !a.smea_scratch)
         return 108;
     if ((a.rule == kGeoMedian || a.rule == kCenteredClipping) && a.R > 1 && !a.staging)
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
@@ -2569,7 +2784,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 111;   // NNM's raw distance pass and ARC's norm pass cover every segment: nothing is pre-accumulated
     if (a.R > 1 && !a.signal[0])
         return 109;
-    if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda) && !a.staging)
+    if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kSmea) && !a.staging)
         return 110;   // blocked passes over remote rows need the staged copy
     return 0;
 }
@@ -2630,7 +2845,7 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     if (status)
         return status;
     int const ctas = ints[15];
-    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda) ||
+    if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda && a.rule != kSmea) ||
         a.mix)
         return 111;
     cudaStream_t s = static_cast<cudaStream_t>(stream);

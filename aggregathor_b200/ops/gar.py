@@ -33,8 +33,10 @@ DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
 ARC_STATS = MAX_WORKERS + 1
 # five regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms
 MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS) * 4
-PTRS = 116
-INFO_INTS = 128   # [0]: theta, [1, 1 + theta): selection masks; [64, 64 + n): NNM masks; [96, 96 + T): DnC's mask of every iteration
+PTRS = 117
+# [0]: theta, [1, 1 + theta): selection masks; [32, 34): SMEA's winning score (float64 bits); [64, 64 + n): NNM masks;
+# [96, 96 + T): DnC's mask of every iteration
+INFO_INTS = 128
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
 
 _ERRORS = {
@@ -49,7 +51,7 @@ _ERRORS = {
   117: "invalid NNM parameters (0 <= 2 f < n)",
   118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)",
   119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)",
-  120: "invalid ARC parameters (0 <= 2 f < n)"}
+  120: "invalid ARC parameters (0 <= 2 f < n)", 122: "invalid SMEA parameters (0 <= 2 f < n and C(n, f) <= 2^14)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
@@ -97,6 +99,7 @@ class FusedLauncher:
     self.dnc_dist_out = torch.zeros(DNC_MAX_ITERATIONS * n * n, dtype=torch.float32, device=self.device)   # DnC: [T, n, n] sampled distances
     self.ctas = ctas
     self._dnc_scratch = None
+    self._smea_scratch = None
     self.info = torch.zeros(INFO_INTS, dtype=torch.int32, device=self.device)
     # Min-Max / Min-Sum: CTA partials of the statistics pass, and gamma followed by the statistics summed over the ranks
     self.craft_ctas = ctas
@@ -136,7 +139,10 @@ class FusedLauncher:
     if domain is None:
       domain = max(hi for _, hi in segments)
     scratch = self.dnc_scratch(spec, domain) if spec.rule == "dnc" else None
-    ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch), self.arc_out.data_ptr()
+    if spec.rule == "smea":
+      scratch = self.smea_scratch(spec)
+    ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch) if spec.rule == "dnc" else 0, self.arc_out.data_ptr()
+    ptrs[116] = addr(scratch) if spec.rule == "smea" else 0
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -168,6 +174,14 @@ class FusedLauncher:
       self._dnc_scratch = torch.zeros(need, dtype=torch.float32, device=self.device)
     return self._dnc_scratch
 
+  def smea_scratch(self, spec):
+    """SMEA's workspace for rule `spec`: one [m][m] float64 slab (m = n - f) per warp of the largest grid."""
+    m = max(spec.n - spec.f, 0)
+    need = self.ctas * ((512 if spec.n <= 8 else 256) // 32) * m * m
+    if self._smea_scratch is None or self._smea_scratch.numel() < need:
+      self._smea_scratch = torch.zeros(need, dtype=torch.float64, device=self.device)
+    return self._smea_scratch
+
   def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
     `rows`: n device addresses of the workers' gradient rows (raw ints, local or peer-mapped); owned coordinates `[lo, hi)` or `segments`."""
@@ -191,7 +205,8 @@ def _torch_rules(spec, step=0):
           "averaged-median": lambda M: _ops.torch_averaged_median(M, spec.beta), "krum": lambda M: _ops.torch_krum(M, spec.f, spec.m),
           "bulyan": lambda M: _ops.torch_bulyan(M, spec.f, spec.m), "trimmed-mean": lambda M: _ops.torch_trimmed_mean(M, spec.f),
           "mda": lambda M: _ops.torch_mda(M, spec.f), "geometric-median": lambda M: _ops.torch_geometric_median(M, spec.iterations, spec.nu),
-          "dnc": lambda M: _ops.torch_dnc(M, spec.f, spec.iterations, spec.subsample, spec.c, spec.seed, step)}[spec.rule]
+          "dnc": lambda M: _ops.torch_dnc(M, spec.f, spec.iterations, spec.subsample, spec.c, spec.seed, step),
+          "smea": lambda M: _ops.torch_smea(M, spec.f)}[spec.rule]
 
 
 def aggregate(spec, G, return_details=False, center=None, step=0):
@@ -199,7 +214,8 @@ def aggregate(spec, G, return_details=False, center=None, step=0):
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
   iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
   DnC draws its samples with step key `step` over the d coordinates of G's rows; its details are the [T, n, n] sampled distances and
-  `info` with [0] = 1, [1] = the final mask (bit i: row i kept) and [96 + t] = the mask of iteration t.
+  `info` with [0] = 1, [1] = the final mask (bit i: row i kept) and [96 + t] = the mask of iteration t. SMEA's details are MDA's (the
+  [n, n] distances and `info`), then its winning score (a 0-d float64 tensor).
   With `spec.mix == "nnm"` the rule runs on the mixed rows (its distances and masks are those of the mixed rows), and
   `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32). With "arc" the rule runs on the
   clipped rows and `return_details` adds (squared norms N [n], factors c [n]); with "arc+nnm" NNM mixes the clipped rows (its
@@ -237,7 +253,9 @@ def aggregate(spec, G, return_details=False, center=None, step=0):
       dist = launcher.dnc_dist_out[:spec.iterations * n * n].view(spec.iterations, n, n)
     else:
       dist = launcher.dist_out.view(n, n)
-    return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
+    info = launcher.info.clone()
+    score = (info[32:34].cpu().view(torch.float64)[0],) if spec.rule == "smea" else ()
+    return (out, dist.clone(), info) + score + _mix_details(spec, launcher, n)
   return out
 
 

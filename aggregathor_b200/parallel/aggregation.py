@@ -258,7 +258,7 @@ class FusedAggregation(_AggregationBase):
     if self.spec.n != nbworkers:
       raise tools.UserException("GAR built for %d workers used with %d" % (self.spec.n, nbworkers))
     d, w, R = self.d, self.w, self.world
-    self.distance_rule = self.spec.rule in ("krum", "bulyan", "mda")
+    self.distance_rule = self.spec.rule in ("krum", "bulyan", "mda", "smea")
     self.buckets = self._check_buckets(buckets, d)
     self.segments_of = [[self._share(lo, hi, q, R) for lo, hi in self.buckets] for q in range(R)]
     self.segments = self.segments_of[self.rank]
@@ -286,6 +286,8 @@ class FusedAggregation(_AggregationBase):
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     if self.spec.rule == "dnc":
       self.launcher.dnc_scratch(self.spec, d)   # allocated before any graph capture
+    if self.spec.rule == "smea":
+      self.launcher.smea_scratch(self.spec)
     self.max_ctas = max_ctas
     self.epoch = 0
     self.device_state = bool(device_state)
@@ -335,7 +337,7 @@ class FusedAggregation(_AggregationBase):
 
   @property
   def overlappable(self):
-    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA is additive over coordinates); not with a
+    """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA / SMEA is additive over coordinates); not with a
     pre-aggregation, whose first pass (NNM's raw distances, ARC's norms) runs in the finish kernel over every segment."""
     return self.distance_rule and len(self.buckets) > 1 and self.mix is None
 

@@ -224,9 +224,9 @@ def main():
       slice_rows = n * (fused.hi - fused.lo) * 4
       # local HBM bytes of the staged tile: the staging store; ARC's clip pass (read + write of its k rows); NNM's mix pass (read + write)
       # after its distance pass (a read of the tile when ARC staged it); the rule's read of the tile; and one more read for the distance
-      # pass of the pre-aggregated rows (Krum / Bulyan / MDA)
+      # pass of the pre-aggregated rows (Krum / Bulyan / MDA / SMEA)
       k = _ops.arc_clip_count(n, f) if "arc" in fused.mix else 0
-      tile_reads = 2 + (1 if rule in ("krum", "bulyan", "mda") else 0) + (2 if "nnm" in fused.mix else 0) + (1 if fused.mix == "arc+nnm" else 0)
+      tile_reads = 2 + (1 if rule in ("krum", "bulyan", "mda", "smea") else 0) + (2 if "nnm" in fused.mix else 0) + (1 if fused.mix == "arc+nnm" else 0)
       mix_entry = {"pre_aggregation": fused.mix, key + "_ms": pre_ms, "plain_ms": plain_ms, key + "_overhead_ms": pre_ms - plain_ms,
                    key + "_rounds_ms": rounds["pre"], "plain_rounds_ms": rounds["plain"],
                    key + "_tile_hbm_bytes": tile_reads * slice_rows + 2 * k * (fused.hi - fused.lo) * 4}
@@ -277,7 +277,7 @@ def main():
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
-    if rule in ("krum", "bulyan", "mda") and fused.mix is None:   # no bucketed distance pass with NNM
+    if rule in ("krum", "bulyan", "mda", "smea") and fused.mix is None:   # no bucketed distance pass with NNM
       c1, c2, c3 = (d // 2) // 8 * 8, (d // 5) // 8 * 8, (d // 16) // 8 * 8
       over = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True,
                               buckets=[(c1, d), (c2, c1), (c3, c2), (0, c3)], device_state=True)
