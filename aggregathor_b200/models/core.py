@@ -139,13 +139,14 @@ class Conv2d(Module):
       self._saved_x, self._saved_y, self._saved_pads, self._saved_aux = x, (y if self.relu else None), pads, aux
     return y
 
-  def backward(self, dy, ctx):
+  def backward(self, dy, ctx, addend=None):
+    """`addend` (the input's shape): returns dx + addend (a gradient reaching the same input by another path)."""
     x, pads = self._saved_x, self._saved_pads
     weight = ctx.weights[self.name + "/weights"]
-    need_dx = ctx.need_input_grad or not getattr(self, "is_first", False)
+    need_dx = ctx.need_input_grad or not getattr(self, "is_first", False) or addend is not None
     dx, dw, db = nn_ops.conv2d_backward(ctx.backend, dy, x, weight, self._saved_y, self.stride, pads, self.relu, self.bias, need_dx,
                                         ctx.grads[self.name + "/weights"], ctx.grads[self.name + "/biases"] if self.bias else None, ctx.groups, ctx.group_stride,
-                                        self._saved_aux)
+                                        self._saved_aux, addend)
     self._saved_x = self._saved_y = self._saved_aux = None
     return dx
 
@@ -217,15 +218,16 @@ class BatchNorm(Module):
     mean, var = ctx.state[self.name + "/moving_mean"], ctx.state[self.name + "/moving_variance"]
     if not ctx.training:
       return nn_ops.batchnorm_inference(ctx.backend, x, gamma, beta, mean, var, self.epsilon, self.relu)
-    y, batch_mean, batch_rstd = nn_ops.batchnorm_forward(ctx.backend, x, gamma, beta, mean, var, self.decay, self.epsilon, self.relu, ctx.groups)
-    self._saved = (x, y if self.relu else None, batch_mean, batch_rstd)
+    # with ReLU, the coefficients applied let the backward recompute the mask y > 0 from x instead of reading y
+    y, batch_mean, batch_rstd, coef = nn_ops.batchnorm_forward(ctx.backend, x, gamma, beta, mean, var, self.decay, self.epsilon, self.relu, ctx.groups, coef=True)
+    self._saved = (x, y if self.relu else None, batch_mean, batch_rstd, coef if self.relu else None)
     return y
 
   def backward(self, dy, ctx):
-    x, y, batch_mean, batch_rstd = self._saved
+    x, y, batch_mean, batch_rstd, coef = self._saved
     gamma = ctx.master[self.name + "/gamma"] if self.scale else None
     dx = nn_ops.batchnorm_backward(ctx.backend, dy, x, y, gamma, batch_mean, batch_rstd, self.relu,
-                                   ctx.grads[self.name + "/gamma"] if self.scale else None, ctx.grads[self.name + "/beta"], ctx.groups, ctx.group_stride)
+                                   ctx.grads[self.name + "/gamma"] if self.scale else None, ctx.grads[self.name + "/beta"], ctx.groups, ctx.group_stride, mask_coef=coef)
     self._saved = None
     return dx
 
@@ -488,6 +490,8 @@ class Residual(Module):
     norm = self._closing_norm()
     if norm is not None:
       db, dy = norm.backward_add_relu(dy, ctx)
+      if ctx.backend == "native" and isinstance(self.residual.layers[0], Conv2d) and len(self.residual.layers) > 2:
+        return self._backward_summed(db, dy, ctx)
       for layer in reversed(self.residual.layers[:-1]):
         db = layer.backward(db, ctx)
       da = self.shortcut.backward(dy, ctx)
@@ -498,6 +502,18 @@ class Residual(Module):
     da = self.shortcut.backward(dy, ctx)
     db = self.residual.backward(dy, ctx)
     return nn_ops.add_forward(ctx.backend, da, db)
+
+
+  def _backward_summed(self, db, dy, ctx):
+    """Backward below the closing norm with the two gradients of x summed where the residual branch's first convolution writes its
+    data gradient (the epilogue of a 1x1 stride-1 one), instead of by a separate pass over a tensor the size of x. A strided
+    `Subsample` shortcut is added in place at the sampled pixels only. Same values as `add_forward(da, db)` under `torch.equal`."""
+    strided = isinstance(self.shortcut, Subsample) and self.shortcut.stride > 1
+    da = None if strided else self.shortcut.backward(dy, ctx)
+    for layer in reversed(self.residual.layers[1:-1]):
+      db = layer.backward(db, ctx)
+    dx = self.residual.layers[0].backward(db, ctx, addend=da)
+    return nn_ops.subsample_accumulate(ctx.backend, dx, dy, self.shortcut.stride) if strided else dx
 
 
 class Identity(Module):

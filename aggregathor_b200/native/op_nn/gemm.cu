@@ -47,17 +47,22 @@ int agb_gemm_epilogue_staged() {
 // lda/ldb must be multiples of 8 elements, bases 16-byte aligned. splits > 1 => fp32 atomic accumulation into C
 // (caller zeroes C). bn in {64, 128, 256} or 0 for an automatic choice.
 int agb_gemm_bf16_grouped(void const* A, void const* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-                          int a_mn, int b_mn, void const* bias, int relu, int out_fp32, int splits, int bn, int groups, long long c_group_stride, void* stream);
+                          int a_mn, int b_mn, void const* bias, int relu, int out_fp32, int splits, int bn, int groups, long long c_group_stride, void const* addend,
+                          void* stream);
 
 int agb_gemm_bf16(void const* A, void const* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                   int a_mn, int b_mn, void const* bias, int relu, int out_fp32, int splits, int bn, void* stream) {
-    return agb_gemm_bf16_grouped(A, B, C, M, N, K, lda, ldb, ldc, a_mn, b_mn, bias, relu, out_fp32, splits, bn, 1, 0, stream);
+    return agb_gemm_bf16_grouped(A, B, C, M, N, K, lda, ldb, ldc, a_mn, b_mn, bias, relu, out_fp32, splits, bn, 1, 0, nullptr, stream);
 }
 
 // Grouped form (weight gradients of several logical workers in one launch): A and B hold `groups` consecutive blocks of K rows
 // (a_mn = b_mn = 1 required when groups > 1), group g accumulates into C + g * c_group_stride. K is the per-group depth.
+// `addend` (null = none): a tensor with C's element type and row stride; C = round(round(product) + addend), bit for bit what a
+// separate element-wise add of the stored product and the addend gives (a data gradient summed with a shortcut gradient). Only
+// for data gradients (a_mn = 0, b_mn = 1), without split-K, on tiles up to 128 wide (the automatic choice keeps to them).
 int agb_gemm_bf16_grouped(void const* A, void const* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-                          int a_mn, int b_mn, void const* bias, int relu, int out_fp32, int splits, int bn, int groups, long long c_group_stride, void* stream) {
+                          int a_mn, int b_mn, void const* bias, int relu, int out_fp32, int splits, int bn, int groups, long long c_group_stride, void const* addend,
+                          void* stream) {
     if (M <= 0 || N <= 0 || K <= 0)
         return 0;
     if ((lda & 7) || (ldb & 7) || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(B) & 15))
@@ -70,10 +75,12 @@ int agb_gemm_bf16_grouped(void const* A, void const* B, void* C, int M, int N, i
         splits = 1;
     if (splits > 1 && !out_fp32)
         return 205;
+    if (splits > 1 && addend)
+        return 207;
     if (bn == 0) {
         // 128 x 256 tiles halve the B re-reads per flop whenever there are enough of them to occupy the chip
         long long const wide_tiles = static_cast<long long>((M + kBM - 1) / kBM) * ((N + 255) / 256) * (groups > 1 ? groups : 1) * (splits > 1 ? splits : 1);
-        bn = N <= 64 ? 64 : (N >= 256 && g_wide_tiles && wide_tiles >= 96 ? 256 : 128);
+        bn = N <= 64 ? 64 : (N >= 256 && g_wide_tiles && wide_tiles >= 96 && !addend ? 256 : 128);
     }
     int const total_kblocks = (K + kBK - 1) / kBK;
     if (splits > total_kblocks)
@@ -85,6 +92,7 @@ int agb_gemm_bf16_grouped(void const* A, void const* B, void* C, int M, int N, i
     p.groups = groups; p.c_group_stride = c_group_stride;
     p.kblocks_per_split = (total_kblocks + splits - 1) / splits;
     splits = (total_kblocks + p.kblocks_per_split - 1) / p.kblocks_per_split;
+    p.addend = addend;
     CUtensorMap ta, tb;
     int status;
     if (a_mn && b_mn)
@@ -110,9 +118,9 @@ int agb_gemm_bf16_grouped(void const* A, void const* B, void* C, int M, int N, i
 }
 
 // fp32 operands multiplied as TF32, fp32 accumulation and output: same layouts and options as agb_gemm_bf16_grouped;
-// lda / ldb multiples of 4 elements, bases 16-byte aligned, bn in {64, 128} (0 = automatic), C is fp32.
+// lda / ldb multiples of 4 elements, bases 16-byte aligned, bn in {64, 128} (0 = automatic), C (and `addend`) fp32.
 int agb_gemm_tf32_grouped(void const* A, void const* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-                          int a_mn, int b_mn, void const* bias, int relu, int splits, int bn, int groups, long long c_group_stride, void* stream) {
+                          int a_mn, int b_mn, void const* bias, int relu, int splits, int bn, int groups, long long c_group_stride, void const* addend, void* stream) {
     using E = ElemTF32;
     if (M <= 0 || N <= 0 || K <= 0)
         return 0;
@@ -129,6 +137,8 @@ int agb_gemm_tf32_grouped(void const* A, void const* B, void* C, int M, int N, i
     int const total_kblocks = (K + E::kBK - 1) / E::kBK;
     if (splits > total_kblocks)
         splits = total_kblocks;
+    if (splits > 1 && addend)
+        return 207;
     GemmParams p{};
     p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.C = C;
     p.bias = static_cast<float const*>(bias);
@@ -136,6 +146,7 @@ int agb_gemm_tf32_grouped(void const* A, void const* B, void* C, int M, int N, i
     p.groups = groups; p.c_group_stride = c_group_stride;
     p.kblocks_per_split = (total_kblocks + splits - 1) / splits;
     splits = (total_kblocks + p.kblocks_per_split - 1) / p.kblocks_per_split;
+    p.addend = addend;
     CUtensorMap ta, tb;
     int status;
     uint64_t const m = static_cast<uint64_t>(M), n = static_cast<uint64_t>(N), k = static_cast<uint64_t>(K), g = static_cast<uint64_t>(groups);

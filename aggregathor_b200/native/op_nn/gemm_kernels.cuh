@@ -91,6 +91,7 @@ struct GemmParams {
     int groups;              // grouped weight gradients: independent K ranges (one per logical worker) ...
     long long c_group_stride; // ... each accumulating into C + group * c_group_stride
     int staged;              // 1: epilogue through shared memory and TMA stores / reductions (the output tensor map), 0: from registers
+    void const* addend;      // null, or a tensor laid out like C added to the rounded product: C = round(round(acc) + addend) (no split-K)
 };
 
 // 4-D tensor map over the epilogue output, 128-byte swizzle, box = one warp's piece: 128 bytes of columns x `box` (16 rows in all)
@@ -118,8 +119,11 @@ inline bool make_tmap_out(CUtensorMap* map, void const* base, bool fp32, uint64_
 // 16-row box whose coordinates `coords(col, c)` gives. The two buffers of a warp alternate; a buffer is rewritten only once the bulk
 // group that read it has finished reading (`issued` counts this warp's pieces across work items). Rows past M and columns past N
 // are clipped by the map.
-template<int BN, bool kFp32, bool kReduce, typename CoordFn>
-__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords) {
+// kAdd: the addend's box (same geometry, map `tmap_d`) is first brought into the buffer by a TMA load on the warp's mbarrier `dbar`
+// (one load per piece, so its phase is `issued & 1`); every lane reads its addend pair from the very bytes it then overwrites.
+template<int BN, bool kFp32, bool kReduce, bool kAdd, typename CoordFn>
+__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords,
+                                                CUtensorMap const* tmap_d, uint64_t* dbar) {
     constexpr int kCols = kFp32 ? 32 : 64;
     int const lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll
@@ -128,9 +132,20 @@ __device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap
         if (col0 >= p.N)
             break;
         uint8_t* buf = staging + (issued & 1) * kPieceBytes;
-        if (lane == 0)
+        if (lane == 0) {
             bulk_wait_read<1>();
+            if constexpr (kAdd) {
+                int c[4];
+                coords(col0, c);
+                mbar_expect_tx(dbar, kPieceBytes);
+                tma_load_4d(buf, tmap_d, dbar, c[0], c[1], c[2], c[3]);
+            }
+        }
         __syncwarp();
+        if constexpr (kAdd) {   // a plain spin: the bounded wait's timer and message cost the 256-wide tile registers it has none to spare of
+            while (!mbar_try_wait(dbar, issued & 1)) {
+            }
+        }
 #pragma unroll
         for (int jj = 0; jj < kCols / 8; ++jj) {
             int const j = q * (kCols / 8) + jj;
@@ -156,10 +171,22 @@ __device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap
                     v1 = max_nan(v1, 0.f);
                 }
                 uint8_t* dst = buf + row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15);
-                if constexpr (kFp32)
+                if constexpr (kFp32) {
+                    if constexpr (kAdd) {
+                        float2 const d = *reinterpret_cast<float2 const*>(dst);
+                        v0 += d.x;
+                        v1 += d.y;
+                    }
                     *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
-                else
+                } else {
+                    if constexpr (kAdd) {   // the product is rounded to bf16 first, as a separate add of two bf16 tensors sees it
+                        float2 const d = __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 const*>(dst));
+                        float2 const r = __bfloat1622float2(__floats2bfloat162_rn(v0, v1));
+                        v0 = r.x + d.x;
+                        v1 = r.y + d.y;
+                    }
                     *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+                }
             }
         }
         fence_proxy_async_smem();
@@ -174,23 +201,33 @@ __device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap
     }
 }
 
-template<int BN, typename CoordFn>
-__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords) {
-    if (!p.out_fp32)
-        epilogue_staged<BN, false, false>(p, tmap_c, acc, staging, issued, n0, coords);
-    else if (p.atomic)
-        epilogue_staged<BN, true, true>(p, tmap_c, acc, staging, issued, n0, coords);
-    else
-        epilogue_staged<BN, true, false>(p, tmap_c, acc, staging, issued, n0, coords);
+// kMayAdd: the caller passes the addend's map and the warp's mbarrier (plain GEMMs); the convolution kernels never take an addend.
+template<int BN, bool kMayAdd = false, typename CoordFn>
+__device__ __forceinline__ void epilogue_staged(GemmParams const& p, CUtensorMap const* tmap_c, float (&acc)[BN / 2], uint8_t* staging, uint32_t& issued, int n0, CoordFn const& coords,
+                                                CUtensorMap const* tmap_d = nullptr, uint64_t* dbar = nullptr) {
+    if (kMayAdd && p.addend) {   // never with split-K (rejected by the entry points)
+        if (!p.out_fp32)
+            epilogue_staged<BN, false, false, kMayAdd>(p, tmap_c, acc, staging, issued, n0, coords, tmap_d, dbar);
+        else
+            epilogue_staged<BN, true, false, kMayAdd>(p, tmap_c, acc, staging, issued, n0, coords, tmap_d, dbar);
+    } else if (!p.out_fp32) {
+        epilogue_staged<BN, false, false, false>(p, tmap_c, acc, staging, issued, n0, coords, tmap_d, dbar);
+    } else if (p.atomic) {
+        epilogue_staged<BN, true, true, false>(p, tmap_c, acc, staging, issued, n0, coords, tmap_d, dbar);
+    } else {
+        epilogue_staged<BN, true, false, false>(p, tmap_c, acc, staging, issued, n0, coords, tmap_d, dbar);
+    }
 }
 
 // Epilogue of one warp's 16 x BN slab of the accumulator (fragment layout: agb_sm90.cuh). `row_at(r, valid, offset)` tells whether
 // tile row r is a real output row and the element offset of that row in C (lets implicit-GEMM convolutions scatter pixel-box rows to
 // NHWC addresses). Pairs of adjacent columns go out as one 8-byte (fp32, also for the split-K reductions) or 4-byte (bf16) access.
-template<int BN, typename RowFn>
+template<int BN, bool kMayAdd = false, typename RowFn>
 __device__ __forceinline__ void epilogue_slab(GemmParams const& p, float (&acc)[BN / 2], int slab_row, int n0, RowFn const& row_at) {
     int const lane = threadIdx.x & 31;
-    bool const pairs = (p.ldc & 1) == 0 && (p.c_group_stride & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & (p.out_fp32 ? 7 : 3)) == 0;
+    uintptr_t const align = p.out_fp32 ? 7 : 3;
+    bool const pairs = (p.ldc & 1) == 0 && (p.c_group_stride & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & align) == 0
+                       && (!kMayAdd || (reinterpret_cast<uintptr_t>(p.addend) & align) == 0);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         bool valid;
@@ -216,6 +253,12 @@ __device__ __forceinline__ void epilogue_slab(GemmParams const& p, float (&acc)[
             }
             if (p.out_fp32) {
                 float* dst = static_cast<float*>(p.C) + offset + col;
+                if (kMayAdd && p.addend) {   // same order as epilogue_staged: the bias and ReLU first, then the addend
+                    float const* src = static_cast<float const*>(p.addend) + offset + col;
+                    v0 += src[0];
+                    if (both)
+                        v1 += src[1];
+                }
                 if (p.atomic) {
                     if (both && pairs) {
                         atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));   // vector reduction (sm_90+)
@@ -233,6 +276,12 @@ __device__ __forceinline__ void epilogue_slab(GemmParams const& p, float (&acc)[
                 }
             } else {
                 __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.C) + offset + col;
+                if (kMayAdd && p.addend) {   // round the product to bf16 first, as epilogue_staged does
+                    __nv_bfloat16 const* src = static_cast<__nv_bfloat16 const*>(p.addend) + offset + col;
+                    v0 = __bfloat162float(__float2bfloat16(v0)) + __bfloat162float(src[0]);
+                    if (both)
+                        v1 = __bfloat162float(__float2bfloat16(v1)) + __bfloat162float(src[1]);
+                }
                 if (both && pairs) {
                     *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
                 } else {
@@ -348,14 +397,22 @@ __device__ __forceinline__ void produce_stage(CUtensorMap const* tmap_a, CUtenso
     }
 }
 
+// The kernels that take an addend: data gradients (A K-major, B MN-major) with tiles up to 128 wide. At 256 the accumulator leaves the
+// epilogue no registers for it (it would spill).
+template<int BN, bool A_MN, bool B_MN>
+constexpr bool kAddendKernel = !A_MN && B_MN && BN <= 128;
+
 template<int BN, bool A_MN, bool B_MN, typename E = ElemBF16>
 __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                                                                 const __grid_constant__ CUtensorMap tmap_c, GemmParams const p, int m_tiles, int n_tiles, int splits) {
+                                                                 const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_d, GemmParams const p,
+                                                                 int m_tiles, int n_tiles, int splits) {
     using Cfg = Config<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kRingBytes + kStagingBytes);
     uint64_t* empty = full + Cfg::kStages;
+    uint64_t* addend_bar = empty + Cfg::kStages;   // one per consumer warp: its staged addend loads
+    static_assert((2 * Cfg::kStages + kConsumerWarps) * 8 <= 256, "barriers outgrow their shared-memory slot");
 
     int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     int const total_kblocks = (p.K + E::kBK - 1) / E::kBK;
@@ -368,10 +425,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
             mbar_init(full + s, 1);
             mbar_init(empty + s, kConsumerWarps);   // one arrival per consumer warp
         }
+        for (int w = 0; w < kConsumerWarps; ++w)
+            mbar_init(addend_bar + w, 1);
         mbar_fence_init();
     }
-    if (p.staged && warp == 0 && lane == 0)
+    if (p.staged && warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmap_c);
+        if (p.addend)
+            tma_prefetch_desc(&tmap_d);
+    }
     __syncthreads();
     pdl_trigger();   // set-up done: the next kernel may start its own; ...
     pdl_wait();      // ... our inputs are complete only once the previous kernel has finished
@@ -421,12 +483,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         decode(item, m0, n0, kb_begin, nkb, group);
         mainloop<BN, A_MN, B_MN, E>(smem, full, empty, ring, nkb, warp, acc);
         if (p.staged) {   // output map (N, M, groups, 1)
-            epilogue_staged<BN>(p, &tmap_c, acc, staging, issued, n0, [&](int col, int (&c)[4]) {
+            epilogue_staged<BN, kAddendKernel<BN, A_MN, B_MN>>(p, &tmap_c, acc, staging, issued, n0, [&](int col, int (&c)[4]) {
                 c[0] = col; c[1] = m0 + 16 * warp; c[2] = group; c[3] = 0;
-            });
+            }, &tmap_d, addend_bar + warp);
             continue;
         }
-        epilogue_slab<BN>(p, acc, 16 * warp, n0, [&](int r, bool& valid, long long& offset) {
+        epilogue_slab<BN, kAddendKernel<BN, A_MN, B_MN>>(p, acc, 16 * warp, n0, [&](int r, bool& valid, long long& offset) {
             int const row = m0 + r;
             valid = row < p.M;
             offset = static_cast<long long>(row) * p.ldc + group * p.c_group_stride;
@@ -455,10 +517,18 @@ int launch_gemm(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& 
         char const* env = std::getenv("AGB_GEMM_PERSISTENT");
         g_persistent = env ? std::atoi(env) : 1;
     }
+    if (params.addend && !kAddendKernel<BN, A_MN, B_MN>)
+        return 207;
     GemmParams p = params;
-    CUtensorMap tc;
+    CUtensorMap tc, td;
     std::memset(&tc, 0, sizeof(tc));
+    std::memset(&td, 0, sizeof(td));
     p.staged = agb_gemm_epilogue_staged() && gemm_out_map(&tc, p);
+    if (p.staged && p.addend) {   // the addend's map: the output's geometry over the addend's base
+        GemmParams q = p;
+        q.C = const_cast<void*>(p.addend);
+        p.staged = gemm_out_map(&td, q);
+    }
     int const m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + BN - 1) / BN;
     auto kernel = gemm_sm90_kernel<BN, A_MN, B_MN, E>;
     static bool configured = false;
@@ -470,7 +540,7 @@ int launch_gemm(CUtensorMap const& ta, CUtensorMap const& tb, GemmParams const& 
     long long const items = static_cast<long long>(m_tiles) * n_tiles * splits * (p.groups > 1 ? p.groups : 1);
     long long const cap = g_persistent ? sm_count() : 0x7fffffffll;
     int const grid = static_cast<int>(items < cap ? items : cap);
-    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, tc, p, m_tiles, n_tiles, splits));
+    AGB_CUDA_OK(launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, ta, tb, tc, td, p, m_tiles, n_tiles, splits));
     return 0;
 }
 

@@ -63,12 +63,19 @@ template<typename T> __device__ __forceinline__ T from_f(float v);
 template<> __device__ __forceinline__ bf16 from_f<bf16>(float v) { return __float2bfloat16(v); }
 template<> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 
+// ReLU mask of a batch norm recomputed from its input. The forward stored y = T(max_nan(fma(x, scale, shift) + residual, 0)) with
+// no residual, so y > 0 exactly when T(fma(x, scale, shift)) > 0: NaN is masked, and so is a positive value that rounds to zero in T.
+template<typename T> __device__ __forceinline__ bool relu_kept(float x, float scale, float shift) {
+    return to_f(from_f<T>(fmaf(x, scale, shift))) > 0.f;
+}
+
 constexpr int kThreads = 256;
 
 // ---------------------------------------------------------------------------- //
 // Per-channel (and per-group) sums: out[g][c] += sum_r f(...). MODE 0: (x - p, (x - p)^2) with the pivot p = the group's first row,
 // so that E[x^2] - E[x]^2 stays well conditioned in fp32 even when |mean| >> std; MODE 1: (dy', dy' * xhat) with
-// dy' = dy masked by (y > 0) when y != null; MODE 2: (dy') only (bias gradient). C % 8 == 0.
+// dy' = dy masked by (y > 0) when y != null, or by the mask recomputed from x with the forward's coefficients `msc` / `msh`
+// (relu_kept) when those are given; MODE 2: (dy') only (bias gradient). C % 8 == 0.
 // 2-D decomposition: blockIdx.x = row chunk, blockIdx.y = strip of STRIP octets (8 * STRIP channels), blockIdx.z = group.
 // Inside a CTA, STRIP lanes cover the strip's octets (up to 512 contiguous bytes per row: whole DRAM bursts instead of
 // 128-byte columns) and 256 / STRIP lanes cover rows, several rows in flight per thread; one fp64 atomic per channel and
@@ -138,7 +145,8 @@ __device__ void finalize_sums(double* sums, SumsFinalize const& f, int C, long l
 
 template<typename T, int MODE, int STRIP>
 __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restrict__ a, T const* __restrict__ b, T const* __restrict__ y, float const* __restrict__ mean,
-                                    float const* __restrict__ rstd, double* __restrict__ out, long long rows_per_group, int C, int rows_per_cta, SumsFinalize const fin) {
+                                    float const* __restrict__ rstd, float const* __restrict__ msc, float const* __restrict__ msh, double* __restrict__ out,
+                                    long long rows_per_group, int C, int rows_per_cta, SumsFinalize const fin) {
     pdl_trigger();
     pdl_wait();
     constexpr int kStripOctets = STRIP, kRowLanes = kThreads / STRIP;
@@ -152,16 +160,23 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
     long long const row_begin = static_cast<long long>(blockIdx.x) * rows_per_cta;
     long long const row_end = min(rows_per_group, row_begin + rows_per_cta);
     long long const base = static_cast<long long>(group) * rows_per_group;
-    float s0[8], s1[8], mu[8], rs[8];
+    float s0[8], s1[8], mu[8], rs[8], sc[8], sh[8];
+    bool const recompute = MODE == 1 && msc != nullptr;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         s0[j] = 0.f;
         s1[j] = 0.f;
         mu[j] = 0.f;
         rs[j] = 0.f;
+        sc[j] = 0.f;
+        sh[j] = 0.f;
         if (MODE == 1 && active) {
             mu[j] = mean[group * C + o * 8 + j];
             rs[j] = rstd[group * C + o * 8 + j];
+            if (recompute) {
+                sc[j] = msc[group * C + o * 8 + j];
+                sh[j] = msh[group * C + o * 8 + j];
+            }
         }
     }
     if (MODE == 0 && active)
@@ -206,6 +221,11 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
                         if (MODE == 1) {
                             float vx[8];
                             unpack8(rb[u], vx);
+                            if (recompute) {
+#pragma unroll
+                                for (int j = 0; j < 8; ++j)
+                                    va[j] = relu_kept<T>(vx[j], sc[j], sh[j]) ? va[j] : 0.f;
+                            }
 #pragma unroll
                             for (int j = 0; j < 8; ++j) {
                                 s0[j] += va[j];
@@ -317,10 +337,12 @@ __global__ void __launch_bounds__(kThreads) bn_apply_kernel(T const* __restrict_
     }
 }
 
-// dx = a * dy' + b * x + c0 with per-(group, channel) coefficients prepared by the statistics kernel's last CTA.
+// dx = a * dy' + b * x + c0 with per-(group, channel) coefficients prepared by the statistics kernel's last CTA; dy' = dy masked by
+// y > 0, or by the mask recomputed from x (`msc` / `msh`: the forward's coefficients, relu_kept), or dy when neither is given.
 template<typename T>
 __global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restrict__ dy, T const* __restrict__ x, T const* __restrict__ y, T* __restrict__ dx, T* __restrict__ dmasked,
-                                    float const* __restrict__ coef, long long total_octets, int C, long long rows_per_group) {
+                                    float const* __restrict__ coef, float const* __restrict__ msc, float const* __restrict__ msh, long long total_octets, int C,
+                                    long long rows_per_group) {
     pdl_trigger();
     pdl_wait();
     unsigned const octets = static_cast<unsigned>(C >> 3);
@@ -333,7 +355,8 @@ __global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restr
     long long const octets_per_group = rows_per_group * octets;
     bool const single_group = octets_per_group >= total_octets;
     int cached_group = -1;
-    float ca[8], cb[8], cc[8];
+    float ca[8], cb[8], cc[8], sc[8], sh[8];
+    bool const recompute = msc != nullptr;
     auto load_coefficients = [&](int g) {
         cached_group = g;
         float const* cf = coef + (static_cast<long long>(g) * C + o * 8) * 3;
@@ -342,13 +365,19 @@ __global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restr
             ca[j] = cf[3 * j];
             cb[j] = cf[3 * j + 1];
             cc[j] = cf[3 * j + 2];
+            sc[j] = recompute ? msc[g * C + o * 8 + j] : 0.f;
+            sh[j] = recompute ? msh[g * C + o * 8 + j] : 0.f;
         }
     };
     auto transform = [&](Oct<T> rd, Oct<T> rx, Oct<T> ry, bool masked, long long index) {
         float vd[8], vx[8];
         unpack8(rd, vd);
         unpack8(rx, vx);
-        if (masked) {
+        if (recompute) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                vd[j] = relu_kept<T>(vx[j], sc[j], sh[j]) ? vd[j] : 0.f;
+        } else if (masked) {
             float vy[8];
             unpack8(ry, vy);
 #pragma unroll
@@ -416,6 +445,29 @@ __global__ void subsample_bwd_kernel(T const* __restrict__ dy, T* __restrict__ d
         int const w = i / octets, o = i - w * octets;
         bool const hit = row_hit && w % s == 0 && w / s < OW;
         dst[i] = hit ? src[static_cast<long long>(w / s) * octets + o] : zero_oct<T>();
+    }
+}
+
+// The same gradient added in place to an existing dx: dx[n, oh*s, ow*s, :] += dy[n, oh, ow, :], the other pixels untouched. This is
+// add(dx, subsample_backward(dy)) reading and writing only the sampled quarter of dx; the one difference is that the separate add
+// turns a -0 of dx into +0 (-0 + +0) at the pixels this kernel skips. grid.y = n * OH + oh, threads along (ow, channel octet).
+template<typename T>
+__global__ void subsample_add_kernel(T const* __restrict__ dy, T* __restrict__ dx, int H, int W, int OH, int OW, int octets, int s) {
+    pdl_trigger();
+    pdl_wait();   // dx is the output of the previous kernel (see launch_pdl)
+    int const n = blockIdx.y / OH, oh = blockIdx.y % OH;
+    Oct<T> const* src = reinterpret_cast<Oct<T> const*>(dy) + static_cast<long long>(blockIdx.y) * OW * octets;
+    T* dst = dx + (static_cast<long long>(n) * H + static_cast<long long>(oh) * s) * W * octets * 8;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < OW * octets; i += gridDim.x * blockDim.x) {
+        int const ow = i / octets, o = i - ow * octets;
+        T* p = dst + (static_cast<long long>(ow) * s * octets + o) * 8;
+        float va[8], vb[8];
+        unpack8(load_oct(p), va);
+        unpack8(src[i], vb);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            va[j] += vb[j];
+        store_oct(p, pack_oct<T>(va));
     }
 }
 
@@ -982,6 +1034,8 @@ struct BnFused {
     float* moving_var;
     float* save_mean;           // forward: out          backward: in
     float* save_rstd;
+    float* scale;               // forward: out, the coefficients applied (y = x * scale + shift), or null
+    float* shift;
     float* dgamma;
     float* dbeta;
     long long group_stride;
@@ -1197,11 +1251,16 @@ __global__ void __launch_bounds__(kFusedThreads, 1) bn_fused_kernel(BnFused cons
                 if (var < 0.)
                     var = 0.;
                 float const rstd = rsqrtf(static_cast<float>(var) + p.eps);
-                chan[c] = gmc * rstd;
-                chan[p.C + c] = aux0 - static_cast<float>(mean) * gmc * rstd;
+                float const scale = gmc * rstd, shift = aux0 - static_cast<float>(mean) * gmc * rstd;
+                chan[c] = scale;
+                chan[p.C + c] = shift;
                 if (chunk == 0) {
                     p.save_mean[idx] = static_cast<float>(mean);
                     p.save_rstd[idx] = rstd;
+                    if (p.scale) {   // a backward pass may recompute the ReLU mask from x with them
+                        p.scale[idx] = scale;
+                        p.shift[idx] = shift;
+                    }
                     if (p.moving_mean && group == 0) {   // unbiased variance in the moving average, as TF's fused batch norm
                         double const unbiased = n > 1. ? var * n / (n - 1.) : var;
                         p.moving_mean[c] = p.decay * moving_s[c] + (1.f - p.decay) * static_cast<float>(mean);
@@ -1354,14 +1413,14 @@ int launch_bn_fused(BnFused p, long long rows, cudaStream_t s) {
 }
 
 template<int MODE, typename T>
-int launch_sums(SumsPlan const& plan, cudaStream_t s, T const* a, T const* b, T const* y, float const* mean, float const* rstd, double* out,
-                 long long rows_per_group, int C, SumsFinalize const& fin) {
+int launch_sums(SumsPlan const& plan, cudaStream_t s, T const* a, T const* b, T const* y, float const* mean, float const* rstd, float const* msc, float const* msh,
+                 double* out, long long rows_per_group, int C, SumsFinalize const& fin) {
     if (plan.strip == 32)
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 32>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 32>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     else if (plan.strip == 16)
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 16>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 16>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     else
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 8>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 8>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     return 0;
 }
 
@@ -1381,7 +1440,7 @@ int bn_forward_impl(void const* x, void const* residual, void* y, void const* ga
     fin.moving_mean = static_cast<float*>(moving_mean); fin.moving_var = static_cast<float*>(moving_var);
     fin.groups = groups; fin.eps = eps; fin.decay = decay;
     SumsPlan plan = plan_sums(rpg, C, groups);
-    if (int status = launch_sums<0, T>(plan, s, static_cast<T const*>(x), nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rpg, C, fin))
+    if (int status = launch_sums<0, T>(plan, s, static_cast<T const*>(x), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rpg, C, fin))
         return status;
     long long const octets = rows * (C >> 3);
     AGB_CUDA_OK(launch_pdl(bn_apply_kernel<T>, dim3(grid_for(octets)), dim3(kThreads), 0, s, static_cast<T const*>(x), static_cast<T const*>(residual), static_cast<T*>(y), static_cast<float const*>(scale), static_cast<float const*>(shift), octets, C, rpg, relu));
@@ -1390,10 +1449,14 @@ int bn_forward_impl(void const* x, void const* residual, void* y, void const* ga
 }
 
 template<typename T>
-int bn_backward_impl(void const* dy, void const* x, void const* y, void const* gamma, void const* save_mean, void const* save_rstd, void* dx, void* dmasked, void* dgamma, void* dbeta,
-                    void* sums, void* coef, long long rows, int C, int groups, long long group_stride, void* stream) {
+int bn_backward_impl(void const* dy, void const* x, void const* y, void const* mask_scale, void const* mask_shift, void const* gamma, void const* save_mean, void const* save_rstd,
+                    void* dx, void* dmasked, void* dgamma, void* dbeta, void* sums, void* coef, long long rows, int C, int groups, long long group_stride, void* stream) {
     if ((C & 7) || groups < 1 || rows % groups)
         return 301;
+    if ((mask_scale == nullptr) != (mask_shift == nullptr) || (mask_scale && (y || dmasked)))
+        return 302;
+    float const* msc = static_cast<float const*>(mask_scale);
+    float const* msh = static_cast<float const*>(mask_shift);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     long long const rpg = rows / groups;
     SumsFinalize fin{};
@@ -1405,11 +1468,11 @@ int bn_backward_impl(void const* dy, void const* x, void const* y, void const* g
     fin.groups = groups; fin.group_stride = group_stride;
     SumsPlan plan = plan_sums(rpg, C, groups);
     if (int status = launch_sums<1, T>(plan, s, static_cast<T const*>(dy), static_cast<T const*>(x), static_cast<T const*>(y), static_cast<float const*>(save_mean),
-                   static_cast<float const*>(save_rstd), static_cast<double*>(sums), rpg, C, fin))
+                   static_cast<float const*>(save_rstd), msc, msh, static_cast<double*>(sums), rpg, C, fin))
         return status;
     long long const octets = rows * (C >> 3);
     AGB_CUDA_OK(launch_pdl(bn_bwd_apply_kernel<T>, dim3(grid_for(octets)), dim3(kThreads), 0, s, static_cast<T const*>(dy), static_cast<T const*>(x), static_cast<T const*>(y), static_cast<T*>(dx),
-        static_cast<T*>(dmasked), static_cast<float const*>(coef), octets, C, rpg));
+        static_cast<T*>(dmasked), static_cast<float const*>(coef), msc, msh, octets, C, rpg));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1424,7 +1487,7 @@ int colsum_impl(void const* dy, void const* y, void* out, void* sums, long long 
     fin.dbeta = static_cast<float*>(out);
     fin.groups = groups; fin.group_stride = group_stride;
     SumsPlan plan = plan_sums(rows / groups, C, groups);
-    if (int status = launch_sums<2, T>(plan, s, static_cast<T const*>(dy), nullptr, static_cast<T const*>(y), nullptr, nullptr, static_cast<double*>(sums), rows / groups, C, fin))
+    if (int status = launch_sums<2, T>(plan, s, static_cast<T const*>(dy), nullptr, static_cast<T const*>(y), nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rows / groups, C, fin))
         return status;
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
@@ -1461,6 +1524,19 @@ int subsample_backward_impl(void const* dy, void* dx, int N, int H, int W, int C
         return 399;
     int const per_row = W * octets;
     AGB_CUDA_OK(launch_pdl(subsample_bwd_kernel<T>, dim3((per_row + kThreads - 1) / kThreads, N * H), dim3(kThreads), 0, static_cast<cudaStream_t>(stream), static_cast<T const*>(dy), static_cast<T*>(dx), H, W, OH, OW, octets, s));
+    AGB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+template<typename T>
+int subsample_add_impl(void const* dy, void* dx, int N, int H, int W, int C, int s, void* stream) {
+    if ((C & 7) || s < 1)
+        return 301;
+    int const OH = (H + s - 1) / s, OW = (W + s - 1) / s, octets = C >> 3;
+    if (static_cast<long long>(N) * OH > 65535)
+        return 399;
+    int const per_row = OW * octets;
+    AGB_CUDA_OK(launch_pdl(subsample_add_kernel<T>, dim3((per_row + kThreads - 1) / kThreads, N * OH), dim3(kThreads), 0, static_cast<cudaStream_t>(stream), static_cast<T const*>(dy), static_cast<T*>(dx), H, W, OH, OW, octets, s));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1590,6 +1666,9 @@ extern "C" {
 // Workspace layout for BN (caller provides, zeroed `sums` not required: it is cleared here):
 //   sums  double [groups*C*2] | save_mean, save_rstd, scale, shift float [groups*C] each (forward)
 //   sums  double [groups*C*2] | coef float [groups*C*3]                              (backward)
+// Backward: the ReLU mask is y > 0 when `y` is given, or is recomputed from x with the forward's `scale` / `shift` ([groups*C]
+// each, what agb_bn_forward(_fused) stored) when `mask_scale` / `mask_shift` are given instead: one activation fewer to read in
+// each of the two passes, same result bit for bit. Neither: no ReLU. `dmasked` needs `y`.
 int agb_bn_forward(void const* x, void const* residual, void* y, void const* gamma, void const* beta, void* moving_mean, void* moving_var, void* save_mean, void* save_rstd,
                    void* sums, void* scale, void* shift, long long rows, int C, int groups, float eps, float decay, int relu, void* stream) {
     return bn_forward_impl<bf16>(x, residual, y, gamma, beta, moving_mean, moving_var, save_mean, save_rstd, sums, scale, shift, rows, C, groups, eps, decay, relu, stream);
@@ -1600,13 +1679,15 @@ int agb_bn_forward_f32(void const* x, void const* residual, void* y, void const*
 }
 
 
-int agb_bn_backward(void const* dy, void const* x, void const* y, void const* gamma, void const* save_mean, void const* save_rstd, void* dx, void* dmasked, void* dgamma, void* dbeta,
-                    void* sums, void* coef, long long rows, int C, int groups, long long group_stride, void* stream) {
-    return bn_backward_impl<bf16>(dy, x, y, gamma, save_mean, save_rstd, dx, dmasked, dgamma, dbeta, sums, coef, rows, C, groups, group_stride, stream);
+int agb_bn_backward(void const* dy, void const* x, void const* y, void const* mask_scale, void const* mask_shift, void const* gamma, void const* save_mean,
+                    void const* save_rstd, void* dx, void* dmasked, void* dgamma, void* dbeta, void* sums, void* coef, long long rows, int C, int groups,
+                    long long group_stride, void* stream) {
+    return bn_backward_impl<bf16>(dy, x, y, mask_scale, mask_shift, gamma, save_mean, save_rstd, dx, dmasked, dgamma, dbeta, sums, coef, rows, C, groups, group_stride, stream);
 }
-int agb_bn_backward_f32(void const* dy, void const* x, void const* y, void const* gamma, void const* save_mean, void const* save_rstd, void* dx, void* dmasked, void* dgamma, void* dbeta,
-                    void* sums, void* coef, long long rows, int C, int groups, long long group_stride, void* stream) {
-    return bn_backward_impl<float>(dy, x, y, gamma, save_mean, save_rstd, dx, dmasked, dgamma, dbeta, sums, coef, rows, C, groups, group_stride, stream);
+int agb_bn_backward_f32(void const* dy, void const* x, void const* y, void const* mask_scale, void const* mask_shift, void const* gamma, void const* save_mean,
+                    void const* save_rstd, void* dx, void* dmasked, void* dgamma, void* dbeta, void* sums, void* coef, long long rows, int C, int groups,
+                    long long group_stride, void* stream) {
+    return bn_backward_impl<float>(dy, x, y, mask_scale, mask_shift, gamma, save_mean, save_rstd, dx, dmasked, dgamma, dbeta, sums, coef, rows, C, groups, group_stride, stream);
 }
 
 
@@ -1623,13 +1704,15 @@ long long agb_bn_fused_workspace_bytes() {
 }
 
 // `residual` (optional, same shape as x): y = relu?(bn(x) + residual) — the closing add + ReLU of a residual unit.
+// `scale` / `shift` (optional, [groups*C] each): the coefficients applied, as agb_bn_forward stores them.
 int agb_bn_forward_fused(void const* x, void const* residual, void* y, void const* gamma, void const* beta, void* moving_mean, void* moving_var, void* save_mean, void* save_rstd,
-                         void* ws, long long rows, int C, int groups, float eps, float decay, int relu, void* stream) {
+                         void* scale, void* shift, void* ws, long long rows, int C, int groups, float eps, float decay, int relu, void* stream) {
     BnFused p{};
     p.a = static_cast<bf16 const*>(x); p.b = static_cast<bf16 const*>(residual); p.out = static_cast<bf16*>(y);
     p.gamma = static_cast<float const*>(gamma); p.beta = static_cast<float const*>(beta);
     p.moving_mean = static_cast<float*>(moving_mean); p.moving_var = static_cast<float*>(moving_var);
     p.save_mean = static_cast<float*>(save_mean); p.save_rstd = static_cast<float*>(save_rstd);
+    p.scale = static_cast<float*>(scale); p.shift = static_cast<float*>(shift);
     p.state = static_cast<unsigned*>(ws); p.ws = static_cast<unsigned char*>(ws) + 16;
     p.C = C; p.groups = groups; p.eps = eps; p.decay = decay; p.relu = relu;
     return launch_bn_fused<false>(p, rows, static_cast<cudaStream_t>(stream));
@@ -1682,6 +1765,15 @@ int agb_subsample_backward(void const* dy, void* dx, int N, int H, int W, int C,
 }
 int agb_subsample_backward_f32(void const* dy, void* dx, int N, int H, int W, int C, int s, void* stream) {
     return subsample_backward_impl<float>(dy, dx, N, H, W, C, s, stream);
+}
+
+
+// dx[n, h*s, w*s, :] += dy[n, h, w, :] in place: the gradient of a strided shortcut summed into the residual branch's.
+int agb_subsample_add(void const* dy, void* dx, int N, int H, int W, int C, int s, void* stream) {
+    return subsample_add_impl<bf16>(dy, dx, N, H, W, C, s, stream);
+}
+int agb_subsample_add_f32(void const* dy, void* dx, int N, int H, int W, int C, int s, void* stream) {
+    return subsample_add_impl<float>(dy, dx, N, H, W, C, s, stream);
 }
 
 

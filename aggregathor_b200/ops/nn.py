@@ -82,9 +82,18 @@ def conv2d_forward(backend, x, weight, bias, stride, pads, relu, aux=None):
   return y.contiguous(memory_format=_CL)
 
 
-def conv2d_backward(backend, dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups=1, group_stride=0, aux=None):
+def conv2d_backward(backend, dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups=1, group_stride=0, aux=None, addend=None):
   """Writes dW into `grad_w` ([Cout, kh, kw, Cin] fp32 view) and db into `grad_b`; returns dx or None. With `groups` > 1 the batch
-  is `groups` consecutive per-worker batches and worker g's gradients go `g * group_stride` elements after worker 0's."""
+  is `groups` consecutive per-worker batches and worker g's gradients go `g * group_stride` elements after worker 0's.
+  `addend` (x's shape, with `need_dx`): returns `add_forward(addend, dx)` instead of dx; the native 1x1 stride-1 data gradient sums it
+  in its epilogue, every other case adds it separately."""
+  if addend is not None:
+    if backend == "native" and x.is_cuda:
+      out = _native().conv2d_backward(dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups, group_stride, aux, addend)
+      if out is not NotImplemented:
+        return out, None, None
+    dx, _, _ = conv2d_backward(backend, dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups, group_stride, aux)
+    return add_forward(backend, addend, dx), None, None
   if backend == "native" and x.is_cuda:
     out = _native().conv2d_backward(dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups, group_stride, aux)
     if out is not NotImplemented:
@@ -182,14 +191,17 @@ def linear_backward(backend, dy, x, weight, y, relu, need_dx, grad_w, grad_b, gr
 # ---------------------------------------------------------------------------- #
 # Batch normalisation
 
-def batchnorm_forward(backend, x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups=1):
+def batchnorm_forward(backend, x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups=1, coef=False):
   """Training-mode batch norm; with `groups` > 1 every consecutive batch slice (one logical worker) has its own statistics;
-  returns (y, mean [groups * C], rstd [groups * C])."""
+  returns (y, mean [groups * C], rstd [groups * C]), and with `coef` a fourth item: the native kernels' (scale, shift), what
+  `batchnorm_backward(mask_coef=)` takes (None from the torch provider)."""
   if backend == "native" and x.is_cuda:
-    out = _native().batchnorm_forward(x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups)
+    out = _native().batchnorm_forward(x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups, coef=coef)
     if out is not None:
       return out
     _fallback("batchnorm_forward")
+  if coef:
+    return batchnorm_forward(backend, x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups) + (None,)
   if groups > 1:
     outs = [batchnorm_forward(backend, x_g.contiguous(memory_format=_CL), gamma, beta, moving_mean if g == 0 else None, moving_var if g == 0 else None, decay, eps, relu)
             for g, x_g in enumerate(_chunks(x, groups))]
@@ -227,9 +239,10 @@ def batchnorm_inference(backend, x, gamma, beta, moving_mean, moving_var, eps, r
   return torch.relu_(y) if relu else y
 
 
-def batchnorm_backward(backend, dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups=1, group_stride=0):
+def batchnorm_backward(backend, dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups=1, group_stride=0, mask_coef=None):
+  """`mask_coef`: the fourth item of `batchnorm_forward(coef=True)` for the forward that produced `y`, or None."""
   if backend == "native" and x.is_cuda:
-    out = _native().batchnorm_backward(dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups, group_stride)
+    out = _native().batchnorm_backward(dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups, group_stride, mask_coef=mask_coef)
     if out is not None:
       return out
     _fallback("batchnorm_backward")
@@ -411,6 +424,16 @@ def subsample_forward(backend, x, stride):
       return out
     _fallback("subsample_forward")
   return x[:, :, ::stride, ::stride].contiguous(memory_format=_CL)
+
+
+def subsample_accumulate(backend, dx, dy, stride):
+  """dx + subsample_backward(dy), adding dy in place at the sampled pixels of dx (equal under `torch.equal`: a -0 of dx stays -0)."""
+  if backend == "native" and dx.is_cuda:
+    out = _native().subsample_accumulate(dx, dy, stride)
+    if out is not None:
+      return out
+    _fallback("subsample_accumulate")
+  return add_forward(backend, subsample_backward(backend, dy, dx.shape, stride), dx)
 
 
 def subsample_backward(backend, dy, shape, stride):

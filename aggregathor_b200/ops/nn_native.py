@@ -162,22 +162,25 @@ def alloc_out(m, n, dtype, device):
   return torch.empty((m, ld), dtype=dtype, device=device)[:, :n]
 
 
-def _gemm(a, b, out, M, N, K, a_mn, b_mn, bias, relu, splits, bn, groups=1, group_stride=0):
+def _gemm(a, b, out, M, N, K, a_mn, b_mn, bias, relu, splits, bn, groups=1, group_stride=0, addend=None):
   if out.stride(1) != 1:
     raise RuntimeError("GEMM output must have unit inner stride")
+  if addend is not None and (addend.dtype != out.dtype or addend.shape != out.shape or addend.stride() != out.stride() or splits != 1):
+    raise RuntimeError("GEMM addend must match the output's dtype, shape and strides, without split-K")
   if a.dtype == torch.float32:   # TF32 products, fp32 output
     if b.dtype != torch.float32 or out.dtype != torch.float32:
       raise RuntimeError("TF32 GEMM needs fp32 operands and output")
     status = _lib().agb_gemm_tf32_grouped(_ptr(a), _ptr(b), _ptr(out), ctypes.c_int(M), ctypes.c_int(N), ctypes.c_int(K), ctypes.c_longlong(a.stride(0)), ctypes.c_longlong(b.stride(0)),
                                           ctypes.c_longlong(out.stride(0)), ctypes.c_int(1 if a_mn else 0), ctypes.c_int(1 if b_mn else 0), _ptr(bias), ctypes.c_int(1 if relu else 0),
-                                          ctypes.c_int(splits), ctypes.c_int(128 if bn == 256 else bn), ctypes.c_int(groups), ctypes.c_longlong(group_stride), _stream())
+                                          ctypes.c_int(splits), ctypes.c_int(128 if bn == 256 else bn), ctypes.c_int(groups), ctypes.c_longlong(group_stride), _ptr(addend),
+                                          _stream())
     _check(status, "gemm_tf32")
     return out
   func = _lib().agb_gemm_bf16_grouped
   out_fp32 = 1 if out.dtype == torch.float32 else 0
   status = func(_ptr(a), _ptr(b), _ptr(out), ctypes.c_int(M), ctypes.c_int(N), ctypes.c_int(K), ctypes.c_longlong(a.stride(0)), ctypes.c_longlong(b.stride(0)),
                 ctypes.c_longlong(out.stride(0)), ctypes.c_int(1 if a_mn else 0), ctypes.c_int(1 if b_mn else 0), _ptr(bias), ctypes.c_int(1 if relu else 0),
-                ctypes.c_int(out_fp32), ctypes.c_int(splits), ctypes.c_int(bn), ctypes.c_int(groups), ctypes.c_longlong(group_stride), _stream())
+                ctypes.c_int(out_fp32), ctypes.c_int(splits), ctypes.c_int(bn), ctypes.c_int(groups), ctypes.c_longlong(group_stride), _ptr(addend), _stream())
   _check(status, "gemm_bf16")
   return out
 
@@ -195,15 +198,17 @@ def mm_nt(x, w, bias=None, relu=False, out=None, out_dtype=None, bn=0):
   return _gemm(x, w, out, M, N, K, False, False, bias, relu, 1, bn)
 
 
-def mm_nn(x, w, out=None, out_dtype=None, bn=0):
-  """x[M,K] @ w[K,N]."""
+def mm_nn(x, w, out=None, out_dtype=None, bn=0, addend=None):
+  """x[M,K] @ w[K,N] (+ `addend`, [M,N] with the output's dtype: the product is rounded to it before the add, as a separate add sees it)."""
   x = _rows(x)
   w = _rows(w, x.dtype)
   M, K = x.shape
   N = w.shape[1]
   if out is None:
     out = alloc_out(M, N, (out_dtype or x.dtype) if x.dtype == torch.bfloat16 else torch.float32, x.device)
-  return _gemm(x, w, out, M, N, K, False, True, None, False, 1, bn)
+  if addend is not None and addend.stride() != out.stride():
+    addend = addend.contiguous() if out.is_contiguous() else _rows(addend)
+  return _gemm(x, w, out, M, N, K, False, True, None, False, 1, bn, addend=addend)
 
 
 # Split-K weight gradients accumulate their partial products with fp32 reductions (red.global.add.v4.f32) whose arrival order varies
@@ -320,8 +325,13 @@ def conv2d_forward(x, weight, bias, stride, pads, relu, aux=None):
   return None
 
 
-def conv2d_backward(dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups=1, group_stride=0, aux=None):
+def conv2d_backward(dy, x, weight, y, stride, pads, relu, has_bias, need_dx, grad_w, grad_b, groups=1, group_stride=0, aux=None, addend=None):
+  """`addend` (optional, x's shape and dtype, needs `need_dx`): returns dx + addend summed in the epilogue of the data-gradient GEMM,
+  bit for bit `add_relu_forward(addend, dx, False)`. Only 1x1 stride-1 convolutions take one (NotImplemented otherwise)."""
   if not enabled("conv"):
+    return NotImplemented
+  if addend is not None and not (need_dx and _is_pointwise(weight, stride, pads) and addend.dtype == x.dtype and addend.shape == x.shape
+                                 and addend.is_contiguous(memory_format=torch.channels_last)):
     return NotImplemented
   if _is_pointwise(weight, stride, pads) and x.is_contiguous(memory_format=torch.channels_last) and x.shape[1] % 8 == 0 and weight.shape[0] % 8 == 0:
     n, c, h, w = x.shape
@@ -333,7 +343,7 @@ def conv2d_backward(dy, x, weight, y, stride, pads, relu, has_bias, need_dx, gra
       mm_tn(dy2d, _as_rows(x), out=grad_w.view(grad_w.shape[0], -1), groups=groups, group_stride=group_stride)
       if has_bias:
         colsum(dy2d, out=grad_b, groups=groups, group_stride=group_stride)
-    dx = _from_rows(mm_nn(dy2d, weight.reshape(weight.shape[0], -1)), n, h, w) if need_dx else None
+    dx = _from_rows(mm_nn(dy2d, weight.reshape(weight.shape[0], -1), addend=None if addend is None else _as_rows(addend)), n, h, w) if need_dx else None
     fork.join()
     return dx
   if _implicit_ok(x, weight, stride, pads) and dy.dtype == x.dtype:
@@ -546,8 +556,9 @@ def _bn_fused_workspace(device, name):
   return _workspace(device, name, int(lib.agb_bn_fused_workspace_bytes()), torch.uint8)
 
 
-def batchnorm_forward(x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups=1, residual=None):
-  """`residual`: y = relu?(bn(x) + residual), only through the single-launch kernel (None when it cannot take the shape)."""
+def batchnorm_forward(x, gamma, beta, moving_mean, moving_var, decay, eps, relu, groups=1, residual=None, coef=False):
+  """`residual`: y = relu?(bn(x) + residual), only through the single-launch kernel (None when it cannot take the shape).
+  `coef`: also return the per-(group, channel) (scale, shift) applied, [2, groups * C], what `batchnorm_backward(mask_coef=)` takes."""
   if not enabled("bn") or not _cl_ok(x, residual) or x.shape[1] % 8:
     return None
   n, c, h, w = x.shape
@@ -558,20 +569,24 @@ def batchnorm_forward(x, gamma, beta, moving_mean, moving_var, decay, eps, relu,
   stats = torch.empty((4, groups * c), dtype=torch.float32, device=x.device)  # save_mean, save_rstd, scale, shift
   if _BN_FUSED and x.dtype == torch.bfloat16:   # the resident-tile kernel is sized for 2-byte activations
     status = _lib().agb_bn_forward_fused(_ptr(x), _ptr(residual), _ptr(y), _ptr(gamma), _ptr(beta), _ptr(moving_mean), _ptr(moving_var), _ptr(stats[0]), _ptr(stats[1]),
-                                         _ptr(_bn_fused_workspace(x.device, "bn_fused_fwd")), ctypes.c_longlong(rows), ctypes.c_int(c), ctypes.c_int(groups),
-                                         ctypes.c_float(eps), ctypes.c_float(decay), ctypes.c_int(1 if relu else 0), _stream())
+                                         _ptr(stats[2] if coef else None), _ptr(stats[3] if coef else None), _ptr(_bn_fused_workspace(x.device, "bn_fused_fwd")),
+                                         ctypes.c_longlong(rows), ctypes.c_int(c), ctypes.c_int(groups), ctypes.c_float(eps), ctypes.c_float(decay), ctypes.c_int(1 if relu else 0),
+                                         _stream())
     if status != _BN_UNSUPPORTED:
       _check(status, "bn_forward_fused")
-      return y, stats[0], stats[1]
+      return (y, stats[0], stats[1], stats[2:]) if coef else (y, stats[0], stats[1])
   sums = _workspace(x.device, "bn_sums", 2 * groups * c + 1, torch.float64)
   _check(_fn("agb_bn_forward", x)(_ptr(x), _ptr(residual), _ptr(y), _ptr(gamma), _ptr(beta), _ptr(moving_mean), _ptr(moving_var), _ptr(stats[0]), _ptr(stats[1]), _ptr(sums),
                                _ptr(stats[2]), _ptr(stats[3]), ctypes.c_longlong(rows), ctypes.c_int(c), ctypes.c_int(groups), ctypes.c_float(eps),
                                ctypes.c_float(decay), ctypes.c_int(1 if relu else 0), _stream()), "bn_forward")
-  return y, stats[0], stats[1]
+  return (y, stats[0], stats[1], stats[2:]) if coef else (y, stats[0], stats[1])
 
 
-def batchnorm_backward(dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups=1, group_stride=0, want_masked=False):
-  """`want_masked` (needs `relu`): returns (dx, dy * (y > 0)) — single-launch kernel only (None when it cannot take the shape)."""
+def batchnorm_backward(dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta, groups=1, group_stride=0, want_masked=False, mask_coef=None):
+  """`want_masked` (needs `relu`): returns (dx, dy * (y > 0)) — single-launch kernel only (None when it cannot take the shape).
+  `mask_coef` (with `relu`, without `want_masked`): the forward's (scale, shift) from `batchnorm_forward(coef=True)`, y being that
+  forward's output. The statistics + apply pair then recomputes the mask y > 0 from x instead of reading y (same bits); the
+  single-launch kernel reads y."""
   if not enabled("bn") or not _cl_ok(x, dy, y) or x.shape[1] % 8 or (want_masked and not relu):
     return None
   if not dy.is_contiguous(memory_format=torch.channels_last):
@@ -589,8 +604,11 @@ def batchnorm_backward(dy, x, y, gamma, mean, rstd, relu, grad_gamma, grad_beta,
       return (dx, masked) if want_masked else dx
   sums = _workspace(x.device, "bn_sums", 2 * groups * c + 1, torch.float64)
   coef = _workspace(x.device, "bn_coef", 3 * groups * c, torch.float32)
-  _check(_fn("agb_bn_backward", x)(_ptr(dy), _ptr(x), _ptr(y if relu else None), _ptr(gamma), _ptr(mean), _ptr(rstd), _ptr(dx), _ptr(masked), _ptr(grad_gamma), _ptr(grad_beta),
-                                _ptr(sums), _ptr(coef), ctypes.c_longlong(rows), ctypes.c_int(c), ctypes.c_int(groups), ctypes.c_longlong(group_stride), _stream()), "bn_backward")
+  recompute = relu and mask_coef is not None and not want_masked
+  mask = (None, mask_coef[0], mask_coef[1]) if recompute else (y if relu else None, None, None)
+  _check(_fn("agb_bn_backward", x)(_ptr(dy), _ptr(x), *(_ptr(t) for t in mask), _ptr(gamma), _ptr(mean), _ptr(rstd), _ptr(dx), _ptr(masked), _ptr(grad_gamma),
+                                _ptr(grad_beta), _ptr(sums), _ptr(coef), ctypes.c_longlong(rows), ctypes.c_int(c), ctypes.c_int(groups), ctypes.c_longlong(group_stride),
+                                _stream()), "bn_backward")
   return (dx, masked) if want_masked else dx
 
 
@@ -726,6 +744,20 @@ def subsample_backward(dy, shape, stride):
     return None
   _check(status, "subsample_backward")
   return dx.permute(0, 3, 1, 2)
+
+
+def subsample_accumulate(dx, dy, stride):
+  """dx[:, :, ::stride, ::stride] += dy in place (dx channels_last); returns dx."""
+  n, c, h, w = dx.shape
+  if not enabled("eltwise") or not _cl_ok(dx, dy) or dy.dim() != 4 or c % 8 or dy.shape != (n, c, -(-h // stride), -(-w // stride)):
+    return None
+  if not dy.is_contiguous(memory_format=torch.channels_last):
+    dy = dy.contiguous(memory_format=torch.channels_last)
+  status = _fn("agb_subsample_add", dy)(_ptr(dy), _ptr(dx), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w), ctypes.c_int(c), ctypes.c_int(stride), _stream())
+  if status == _BN_UNSUPPORTED:
+    return None
+  _check(status, "subsample_add")
+  return dx
 
 
 def relu_backward(dy, y):

@@ -5,6 +5,7 @@
     python benchmarks/nn_bench.py --dry-run                # product table with FLOP and byte counts (no GPU needed)
     python benchmarks/nn_bench.py --out DIR                # time every product, staged vs register epilogue alternating in one process
     python benchmarks/nn_bench.py --profile --out DIR      # torch.profiler pass over the headline step (run it on its own)
+    python benchmarks/nn_bench.py --traffic                # HBM bytes of the batch-norm and residual passes (no GPU needed)
 
 The products are derived from the model: a CPU forward pass at batch 1 records every Conv2d / Dense input shape, and the same
 dispatch rules as `ops/nn_native.py` (1x1 stride-1 -> GEMM, implicit-GEMM conv, im2col + GEMM) turn each layer into its
@@ -31,6 +32,7 @@ SM_COUNT = 132   # H100 SXM: the split-K choice of the nn wrappers depends on it
 def parse():
   parser = argparse.ArgumentParser()
   parser.add_argument("--dry-run", action="store_true")
+  parser.add_argument("--traffic", action="store_true")
   parser.add_argument("--profile", action="store_true")
   parser.add_argument("--out", type=str, default="nn_bench_out")
   parser.add_argument("--workers", type=int, default=8)
@@ -180,6 +182,86 @@ def describe(p):
 
 
 # ---------------------------------------------------------------------------- #
+# Activation traffic of the batch-norm and residual passes
+
+FUSED_MB = (72, 40)   # single-launch batch norm envelope, forward / backward (`nn_native.set_bn_fused_limits` defaults; no ResNet-50 tensor is under its row minimum at these sizes)
+
+
+def traffic(workers, batch, image_size):
+  """HBM bytes per step of the batch-norm passes (single launch or statistics + apply pair, as the envelope picks) and of the
+  residual-gradient passes, before and after summing the shortcut gradient in the data-gradient epilogue and recomputing the ReLU
+  mask of the pair's backward from x. A pass counts every activation it reads or writes once (bf16); per-channel vectors, and
+  the single-launch kernel's L2 re-reads of rows past its on-chip stash, are left out. Returns {category: [tensors, before, after]}."""
+  from aggregathor_b200.engine.flat import FlatLayout
+  from aggregathor_b200.models import Context, get_network
+  from aggregathor_b200.models import core
+  model = get_network("resnet_v1_50", 1000)
+  layout, states = FlatLayout(), {}
+  model.declare(layout, states)
+  layout.freeze()
+  params = torch.zeros(layout.padded_size)
+  state = {k: torch.zeros(v) for k, v in states.items()}
+  model.initialize(layout.views(params), state, torch.Generator().manual_seed(0))
+  ctx = Context("torch", True, torch.float32, "cpu")
+  ctx.master = ctx.weights = layout.views(params)
+  ctx.state = state
+  norms, units = [], []
+  bn_forward, bn_closing, unit_forward = core.BatchNorm.forward, core.BatchNorm.forward_add_relu, core.Residual.forward
+
+  def norm(self, x, c):
+    norms.append((x[0].numel(), self.relu, False))
+    return bn_forward(self, x, c)
+
+  def closing(self, x, shortcut, c):
+    norms.append((x[0].numel(), True, True))
+    return bn_closing(self, x, shortcut, c)
+
+  def unit(self, x, c):
+    shortcut = self.shortcut
+    kind = ("subsample" if shortcut.stride > 1 else "identity") if isinstance(shortcut, core.Subsample) else "projection"
+    units.append((x[0].numel(), kind))
+    return unit_forward(self, x, c)
+
+  core.BatchNorm.forward, core.BatchNorm.forward_add_relu, core.Residual.forward = norm, closing, unit
+  try:
+    x = torch.zeros((1, 3, image_size, image_size)).contiguous(memory_format=torch.channels_last)
+    with torch.no_grad():
+      model.root.forward(x, ctx)
+  finally:
+    core.BatchNorm.forward, core.BatchNorm.forward_add_relu, core.Residual.forward = bn_forward, bn_closing, unit_forward
+  B = workers * batch
+  sums = collections.OrderedDict()
+
+  def add(category, before, after):
+    entry = sums.setdefault(category, [0, 0, 0])
+    entry[0] += 1
+    entry[1] += before
+    entry[2] += after
+
+  for numel, relu, closes in norms:
+    S = 2 * B * numel
+    extra = S if closes else 0   # forward: the shortcut read; backward: the masked gradient written for the shortcut
+    if S <= FUSED_MB[0] << 20:   # reads x (+ shortcut) once, writes y
+      add("bn forward, single launch", 2 * S + extra, 2 * S + extra)
+    else:                        # statistics read x, apply reads x (+ shortcut) and writes y
+      add("bn forward, pair", 3 * S + extra, 3 * S + extra)
+    reads = 3 if relu else 2     # dy, x (, y for the mask)
+    if S <= FUSED_MB[1] << 20:
+      add("bn backward, single launch", (reads + 1) * S + extra, (reads + 1) * S + extra)
+    elif relu and not closes:    # both passes recompute the mask from x: y is no longer read
+      add("bn backward, pair, ReLU", (2 * reads + 1) * S, (2 * reads - 1) * S)
+    else:
+      add("bn backward, pair, %s" % ("closing (keeps y)" if closes else "no ReLU"), (2 * reads + 1) * S + extra, (2 * reads + 1) * S + extra)
+  for numel, kind in units:
+    X = 2 * B * numel
+    if kind == "subsample":   # scatter into a full-size tensor (read X/4, write X) + add (2 reads, 1 write) -> in-place add of a quarter
+      add("residual grads, subsample units", X // 4 + X + 3 * X, 3 * (X // 4))
+    else:                     # add (2 reads, 1 write) -> the addend read by the data-gradient epilogue
+      add("residual grads, %s units" % kind, 3 * X, X)
+  return sums
+
+
+# ---------------------------------------------------------------------------- #
 # Timing
 
 def launcher(p, device):
@@ -315,6 +397,14 @@ def run_profile(args):
 
 def main():
   args = parse()
+  if args.traffic:
+    sums = traffic(args.workers, args.batch_size, args.image_size)
+    print("%-42s %7s %10s %10s %9s" % ("pass (%d images, bf16)" % (args.workers * args.batch_size), "tensors", "before GB", "after GB", "saved GB"))
+    for category, (count, before, after) in sums.items():
+      print("%-42s %7d %10.2f %10.2f %9.2f" % (category, count, before / 1e9, after / 1e9, (before - after) / 1e9))
+    before, after = sum(v[1] for v in sums.values()), sum(v[2] for v in sums.values())
+    print("%-42s %7s %10.2f %10.2f %9.2f" % ("total", "", before / 1e9, after / 1e9, (before - after) / 1e9))
+    return 0
   if args.dry_run:
     table = products(args.workers, args.batch_size, args.image_size)
     flop = sum(p["flop"] * p["calls"] for p in table)
