@@ -400,15 +400,19 @@ def torch_pairwise_distances(G):
 # ---------------------------------------------------------------------------- #
 # Nearest-neighbour mixing (NNM; Allouah et al., "Fixing by Mixing", AISTATS 2023): a pre-aggregation run on the rows before the rule
 
-PRE_AGGREGATIONS = ("none", "nnm", "arc", "arc+nnm")   # "arc+nnm": adaptive robust clipping, then NNM on the clipped rows
+# "arc+nnm": adaptive robust clipping, then NNM on the clipped rows; "bucketing": means of buckets of s rows, which needs the bucket size s
+PRE_AGGREGATIONS = ("none", "nnm", "arc", "arc+nnm", "bucketing")
 
 
-def check_pre_aggregation(name):
-  """`--pre-aggregation` value -> the `FusedSpec.mix` it selects (None for "none")."""
+def check_pre_aggregation(name, bucket_size=None):
+  """`--pre-aggregation` value -> the `FusedSpec.mix` it selects (None for "none"). "bucketing" is only complete with its bucket size
+  `bucket_size` (checked against n by `check_bucketing`)."""
   if name is None or name == "none":
     return None
   if name not in PRE_AGGREGATIONS:
     raise tools.UserException("Unknown pre-aggregation %r (expected one of %s)" % (name, ", ".join(PRE_AGGREGATIONS)))
+  if name == "bucketing" and bucket_size is None:
+    raise tools.UserException("Bucketing needs a bucket size s >= 1")
   return name
 
 
@@ -535,18 +539,96 @@ def torch_arc(G, f, return_details=False):
   return (Y, N, factors, clipped) if return_details else Y
 
 
-def torch_pre_aggregate(G, mix, f, host=False):
-  """The pre-aggregation `mix` (a `FusedSpec.MIXES` value) of the [n, d] rows G with the torch reference: ARC, then NNM; `host`: NNM
-  takes the host library's distances for CPU rows (`host_nnm`)."""
+def torch_pre_aggregate(G, mix, f, host=False, bucket_size=None, seed=0, step=0):
+  """The pre-aggregation `mix` (a `FusedSpec.MIXES` value, or "bucketing") of the [n, d] rows G with the torch reference: ARC, then
+  NNM; `host`: NNM takes the host library's distances for CPU rows (`host_nnm`). Bucketing (`bucket_size`, `seed`, `step`) returns
+  the n' = ceil(n / s) bucket means."""
   if mix is None:
     return G
   if mix not in PRE_AGGREGATIONS:
     raise tools.UserException("Unknown pre-aggregation %r (expected one of %s)" % (mix, ", ".join(PRE_AGGREGATIONS)))
+  if mix == "bucketing":
+    return torch_bucketing(G, bucket_size, seed, step)
   if mix in ("arc", "arc+nnm"):
     G = torch_arc(G, f)
   if mix in ("nnm", "arc+nnm"):
     G = host_nnm(G, f) if host and G.device.type == "cpu" else torch_nnm(G, f)
   return G
+
+
+# Bucketing (Karimireddy, He & Jaggi, "Byzantine-Robust Learning on Heterogeneous Datasets via Bucketing", ICLR 2022): the rows are
+# shuffled by a keyed permutation, cut into buckets of s rows and replaced by the n' = ceil(n / s) bucket means
+
+BUCKETING_TAG = 0x42554B54   # "BUKT": the third splitmix64 input of the key; >= 8, so it never equals one of DnC's iteration numbers
+_MASK64 = (1 << 64) - 1
+
+
+def _splitmix64_int(z):
+  """splitmix64 on a Python integer, mod 2^64 (the same function as `_splitmix64` and the kernels' `splitmix64`)."""
+  z = (z + 0x9E3779B97F4A7C15) & _MASK64
+  z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _MASK64
+  z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _MASK64
+  return z ^ (z >> 31)
+
+
+def check_bucketing(n, s):
+  """1 <= s <= n -> n' = ceil(n / s), the number of buckets (the rows the rule sees)."""
+  if isinstance(s, bool) or not isinstance(s, int) or not 1 <= s <= n:
+    raise tools.UserException("Bucketing needs a bucket size 1 <= s <= n (got n = %d, s = %r)" % (n, s))
+  return (n + s - 1) // s
+
+
+def check_bucketing_key(seed, step):
+  if isinstance(seed, bool) or int(seed) != seed or not 0 <= seed <= _MASK64:
+    raise tools.UserException("Bucketing needs a seed in [0, 2^64) (got %r)" % (seed,))
+  if isinstance(step, bool) or int(step) != step or not 0 <= step < 1 << 63:
+    raise tools.UserException("Bucketing needs a step key in [0, 2^63) (got %r)" % (step,))
+  return int(seed), int(step)
+
+
+def bucketing_permutation(n, seed, step):
+  """pi of step `step`, a list of the n worker indices: K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ TAG); from the identity,
+  for i = n - 1 down to 1, j = splitmix64(K ^ i) mod (i + 1) and pi[i], pi[j] are swapped (unsigned 64-bit arithmetic)."""
+  seed, step = check_bucketing_key(seed, step)
+  key = _splitmix64_int(_splitmix64_int(_splitmix64_int(seed) ^ step) ^ BUCKETING_TAG)
+  perm = list(range(n))
+  for i in range(n - 1, 0, -1):
+    j = _splitmix64_int(key ^ i) % (i + 1)
+    perm[i], perm[j] = perm[j], perm[i]
+  return perm
+
+
+def bucketing_masks(n, s, perm):
+  """The n' member sets as bit masks (Python ints): bucket b holds pi[b s], ..., pi[min((b + 1) s, n) - 1]."""
+  count = check_bucketing(n, s)
+  return [sum(1 << perm[p] for p in range(b * s, min((b + 1) * s, n))) for b in range(count)]
+
+
+def bucketing_mean(G, masks):
+  """y_b = (((x_a0 + x_a1) + ...) / |M_b| over the members of every mask in ascending worker order from +0, in G's dtype: one
+  `torch.add` per member and one division by a 0-d tensor (NNM's mixing arithmetic). `masks`: ints, or the kernel's int32 values."""
+  Y = torch.empty((len(masks),) + tuple(G.shape[1:]), dtype=G.dtype, device=G.device)
+  for b, mask in enumerate(masks):
+    mask = int(mask) + (1 << 32 if int(mask) < 0 else 0)
+    members = [j for j in range(G.shape[0]) if (mask >> j) & 1]
+    acc = torch.zeros_like(G[0])
+    for j in members:
+      acc = torch.add(acc, G[j])
+    Y[b] = torch.div(acc, torch.tensor(float(len(members)), dtype=G.dtype, device=G.device))
+  return Y
+
+
+def torch_bucketing(G, s, seed, step, return_details=False):
+  """Bucketing of the [n, d] rows G with the torch back-end in G's dtype -> [n', d] bucket means; `return_details` also gives
+  (pi [n] int32, masks [n'] int32), the layout the sm_90a kernel reports."""
+  n = G.shape[0]
+  check_bucketing(n, s)
+  perm = bucketing_permutation(n, seed, step)
+  masks = bucketing_masks(n, s, perm)
+  Y = bucketing_mean(G, masks)
+  if not return_details:
+    return Y
+  return Y, torch.tensor(perm, dtype=torch.int32), torch.tensor([v - (1 << 32) if v >= 1 << 31 else v for v in masks], dtype=torch.int32)
 
 
 def krum_select(dist, f, m):

@@ -29,8 +29,18 @@ def mark_exit(*args, **kwargs):
   exit_pending = True
 
 
+class _Parser(argparse.ArgumentParser):
+  """Bucketing is only complete with its bucket size: '--pre-aggregation bucketing' without '--bucket-size' is a usage error."""
+
+  def parse_args(self, args=None, namespace=None):
+    parsed = super().parse_args(args, namespace)
+    if getattr(parsed, "pre_aggregation", None) == "bucketing" and getattr(parsed, "bucket_size", None) is None:
+      self.error("'--pre-aggregation bucketing' needs '--bucket-size s' (the rows per bucket, e.g. 2)")
+    return parsed
+
+
 def make_parser():
-  parser = argparse.ArgumentParser(description="Start/continue a distributed training session.", formatter_class=argparse.RawTextHelpFormatter)
+  parser = _Parser(description="Start/continue a distributed training session.", formatter_class=argparse.RawTextHelpFormatter)
   add = parser.add_argument
   add("--client", type=str, default="", help="Trusted node URL in the cluster (usually the parameter server) to connect to as a client; one and only one of '--server' and '--client' must be specified")
   add("--server", type=str, default="", help="Full JSON cluster specification, on which to act as the only parameter server, or special value(s): " + tools.cluster_parsers + "; one and only one of '--server' and '--client' must be specified")
@@ -80,7 +90,8 @@ def make_parser():
   add("--authenticate", action="store_true", default=False, help="Sign every published gradient (ed25519) and verify before aggregating; slices failing the check become NaN")
   add("--worker-momentum", type=float, default=0.0, help="Worker momentum beta in [0, 1): every worker submits its momentum m <- beta m + (1 - dampening) g instead of its gradient (0 with a zero dampening: off)")
   add("--worker-momentum-dampening", type=float, default=0.0, help="Dampening of the worker momentum in [0, 1)")
-  add("--pre-aggregation", type=str, default="none", choices=("none", "nnm", "arc", "arc+nnm"), help="Pre-aggregation of the gathered rows before the rule: 'nnm' replaces every row by the mean of its n - f nearest rows (nearest-neighbour mixing), 'arc' clips the floor(2 f (n - f) / n) rows of largest norm to the norm of the largest row left alone (adaptive robust clipping), 'arc+nnm' clips then mixes; all need 0 <= 2 f < n; 'none' by default")
+  add("--pre-aggregation", type=str, default="none", choices=("none", "nnm", "arc", "arc+nnm", "bucketing"), help="Pre-aggregation of the gathered rows before the rule: 'nnm' replaces every row by the mean of its n - f nearest rows (nearest-neighbour mixing), 'arc' clips the floor(2 f (n - f) / n) rows of largest norm to the norm of the largest row left alone (adaptive robust clipping), 'arc+nnm' clips then mixes; all need 0 <= 2 f < n; 'bucketing' shuffles the rows (keyed by '--seed' and the step) and replaces them by the means of buckets of '--bucket-size' rows, so the rule sees ceil(n / s) rows; 'none' by default")
+  add("--bucket-size", type=int, default=None, help="Rows per bucket s of '--pre-aggregation bucketing', 1 <= s <= n (required with it; 2 is the usual choice)")
   return parser
 
 
@@ -119,6 +130,18 @@ def _tee_streams(args):
     tee.write("Duplicating " + label + " to " + repr(str(path.resolve())) + os.linesep)
 
 
+def _instantiate_aggregator(args, nb_instantiated):
+  """The GAR of the run: for the n declared workers, or with bucketing for the n' = ceil(n / s) bucket means of the n instantiated
+  workers' rows; a rule that cannot run on n' rows fails with its own message and the n -> n' context."""
+  if args.pre_aggregation != "bucketing":
+    return aggregators.instantiate(args.aggregator, args.nb_workers, args.nb_decl_byz_workers, args.aggregator_args)
+  rows = -(-nb_instantiated // args.bucket_size)
+  try:
+    return aggregators.instantiate(args.aggregator, rows, args.nb_decl_byz_workers, args.aggregator_args)
+  except tools.UserException as err:
+    raise tools.UserException("%s (bucketing with s = %d turns n = %d workers into n' = %d bucket means)" % (err, args.bucket_size, nb_instantiated, rows)) from err
+
+
 def _validate(args):
   """Fatal problems raise `UserException`, suspicious settings only warn; list arguments left out become empty lists."""
   n, f, real = args.nb_workers, args.nb_decl_byz_workers, args.nb_real_byz_workers
@@ -133,7 +156,8 @@ def _validate(args):
     (n <= 0, "Expected at least one non-Byzantine worker"),
     (n < real, "Got more real Byzantine workers (" + repr(real) + ") than total number of workers (" + repr(n) + ")"),
     (args.pre_aggregation == "nnm" and not 0 <= 2 * f < n, "Nearest-neighbour mixing needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)),
-    (args.pre_aggregation in ("arc", "arc+nnm") and not 0 <= 2 * f < n, "Adaptive robust clipping needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)))
+    (args.pre_aggregation in ("arc", "arc+nnm") and not 0 <= 2 * f < n, "Adaptive robust clipping needs 0 <= 2 f < n (got n = %d, f = %d)" % (n, f)),
+    (args.pre_aggregation == "bucketing" and not 1 <= (args.bucket_size or 0) <= n, "Bucketing needs a bucket size 1 <= s <= n (got n = %d, s = %r)" % (n, args.bucket_size)))
   for failed, message in fatal:
     if failed:
       raise tools.UserException(message)
@@ -198,7 +222,8 @@ def main(argv=None):
       print("Using a total of " + repr(args.nb_workers) + " worker(s):")
       print("· " + repr(nb_nonbyz_workers) + " non-Byzantine worker(s)")
       pre = {"nnm": ", nearest-neighbour mixing (NNM) before the rule", "arc": ", adaptive robust clipping (ARC) before the rule",
-             "arc+nnm": ", adaptive robust clipping (ARC) then nearest-neighbour mixing (NNM) before the rule"}
+             "arc+nnm": ", adaptive robust clipping (ARC) then nearest-neighbour mixing (NNM) before the rule",
+             "bucketing": ", bucketing (means of buckets of %s rows) before the rule" % args.bucket_size}
       print("· " + repr(args.nb_decl_byz_workers) + " declared Byzantine worker(s)" + pre.get(args.pre_aggregation, ""))
       print("  " + repr(args.nb_real_byz_workers) + " real Byzantine worker(s)")
       tools.print_args("experiment", args.experiment, args.experiment_args, head="")
@@ -248,7 +273,7 @@ def main(argv=None):
     tools.success("Graph construction phase...")
   with tools.Context("graph", "info"):
     experiment = experiments.instantiate(args.experiment, args.experiment_args)
-    aggregator = aggregators.instantiate(args.aggregator, args.nb_workers, args.nb_decl_byz_workers, args.aggregator_args)
+    aggregator = _instantiate_aggregator(args, nb_instantiated)
     attack = attacks.instantiate(args.attack, args.nb_workers, args.nb_real_byz_workers, args.attack_args) if attacked else None
     engine = args.engine
     if nb_instantiated != args.nb_workers and engine in ("auto", "fused"):
@@ -258,6 +283,7 @@ def main(argv=None):
                         device=device, engine=engine, backend=args.nn_backend, seed=args.seed, placement=placement, debug_checksum=args.debug_checksum, authenticate=args.authenticate,
                         worker_momentum=args.worker_momentum, worker_momentum_dampening=args.worker_momentum_dampening,
                         pre_aggregation=args.pre_aggregation, nb_decl_byz=args.nb_decl_byz_workers,
+                        bucket_size=args.bucket_size if args.pre_aggregation == "bucketing" else None, bucketing_seed=args.seed,
                         dtype={"bf16": torch.bfloat16, "tf32": torch.float32, "fp32": torch.float32}.get(args.dtype))
   if exit_pending:
     return 0

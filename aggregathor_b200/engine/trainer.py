@@ -17,7 +17,9 @@ One synchronous step on a rank:
      Byzantine rows from the honest ones, a collective call on every rank);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast), after the optional pre-aggregation
      (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing"; "arc": adaptive
-     robust clipping, Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"; "arc+nnm": both);
+     robust clipping, Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"; "arc+nnm": both;
+     "bucketing": means of shuffled buckets of s rows, Karimireddy, He & Jaggi, "Byzantine-Robust Learning on Heterogeneous Datasets
+     via Bucketing");
   5. the bf16 compute copy of the parameters is refreshed (unless the fused kernel already wrote it).
 """
 
@@ -48,12 +50,14 @@ class Manager:
   def __init__(self, experiment, aggregator, nbworkers, optimizer="sgd", optimizer_args=None, learning_rate="fixed", learning_rate_args=None,
                regularizations=(-1., -1.), trace=False, *, attack=None, nb_real_byz=0, device=None, group=None, engine="auto", backend="auto",
                dtype=None, seed=0, placement=None, debug_checksum=False, engine_args=None, use_graphs=None, authenticate=False,
-               worker_momentum=0.0, worker_momentum_dampening=0.0, pre_aggregation="none", nb_decl_byz=None):
+               worker_momentum=0.0, worker_momentum_dampening=0.0, pre_aggregation="none", nb_decl_byz=None, bucket_size=None, bucketing_seed=0):
     """`pre_aggregation`: "none", "nnm" (every row replaced by the mean of its n - f nearest rows before the rule), "arc" (adaptive
     robust clipping: the floor(2 f (n - f) / n) rows of largest norm clipped to the norm of the largest row left alone) or "arc+nnm"
-    (ARC, then NNM), with f = `nb_decl_byz`, the declared Byzantine workers (default: the rule's own f)."""
+    (ARC, then NNM), with f = `nb_decl_byz`, the declared Byzantine workers (default: the rule's own f); or "bucketing" (the rows,
+    shuffled by a permutation keyed by `bucketing_seed` and the update number, replaced by the means of buckets of `bucket_size` rows;
+    `aggregator` is then built for ceil(nbworkers / bucket_size) workers)."""
     from ..aggregators import _ops
-    self.pre_aggregation = _ops.check_pre_aggregation(pre_aggregation)   # None, "nnm", "arc" or "arc+nnm"
+    self.pre_aggregation = _ops.check_pre_aggregation(pre_aggregation, bucket_size)   # None, "nnm", "arc", "arc+nnm" or "bucketing"
     # (beta, c = 1 - dampening) in fp32; beta = dampening = 0 is off: no buffer, no kernel, the step is unchanged
     self.momentum = _ops.check_worker_momentum(worker_momentum, worker_momentum_dampening)
     self.momentum_on = self.momentum[0] != 0.0 or _ops.fp32(worker_momentum_dampening) != 0.0
@@ -103,6 +107,8 @@ class Manager:
         if len(buckets) > 1:
           engine_args["buckets"] = buckets
     mix = dict(pre_aggregation=self.pre_aggregation, nb_decl_byz=nb_decl_byz)
+    if self.pre_aggregation == "bucketing":
+      mix.update(bucket_size=bucket_size, bucketing_seed=bucketing_seed)
     try:
       self.aggregation = make_aggregation(engine, aggregator, self.layout, nbworkers, self.optimizer, group, self.device, **mix, **engine_args)
     except TypeError:   # engines without these options (host, baseline)

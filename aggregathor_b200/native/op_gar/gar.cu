@@ -22,7 +22,9 @@
 // exchange, one selection warp, then every row of the staged tile is replaced by the mean of its n - f nearest rows; the rule then
 // reads the mixed tile (see `nnm_pre_aggregation`). Adaptive robust clipping (ARC, bit kMixArc of `a.mix`) runs before NNM: a norm pass
 // (staging every row), one exchange of the squared norms, one selection warp, then the clipped rows of the tile are rescaled in
-// place (see `arc_pre_aggregation`).
+// place (see `arc_pre_aggregation`). Bucketing (bit kMixBucketing, alone) runs first: the n_rows gathered rows are shuffled by a keyed
+// permutation and replaced by the n = ceil(n_rows / s) means of buckets of s rows, staged as rows [0, n) of the tile; the rule then
+// reads n rows (see `bucketing_pre_aggregation`). Its "buckets" are sets of rows, not the gradient buckets (coordinate segments) above.
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
 // whole-vector sums between the ranks, then the same per-coordinate write.
@@ -72,7 +74,8 @@ constexpr int kDncRegion = kCraftRegion + kMaxRanks * kCraftStats;   // mailbox 
 constexpr int kArcStride = kMaxWorkers + 1;   // ARC post of one rank: the n partial squared norms, then the loss
 constexpr int kArcRegion = kDncRegion + kMaxRanks * kDncStride;   // mailbox region 4: kMaxRanks x kArcStride floats
 constexpr int kMailboxFloats = kArcRegion + kMaxRanks * kArcStride;
-constexpr int kMixNnm = 1, kMixArc = 2;   // GarArgs::mix bits
+constexpr int kMixNnm = 1, kMixArc = 2, kMixBucketing = 4;   // GarArgs::mix bits (bucketing is never combined with the others)
+constexpr unsigned long long kBucketingTag = 0x42554B54ull;   // "BUKT": third input of bucketing's key; >= 8, never a DnC iteration
 constexpr int kJacobiSweeps = 32;         // DnC: sweep budget of the cyclic Jacobi
 constexpr double kJacobiTol = 1e-26;      // DnC: stop once sum_{i != j} B_ij^2 <= kJacobiTol * sum_i B_ii^2
 constexpr int kBlockRows = 8;             // rows held in registers at a time
@@ -84,7 +87,10 @@ enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKr
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
-    int n, f, m, beta, rule;
+    int n, f, m, beta, rule;           // n: the rows the rule sees (with bucketing: the n = ceil(n_rows / bkt_size) bucket means)
+    int n_rows;                        // the gathered rows grad[0, n_rows): n, or the rows bucketing reduces to n
+    int bkt_size;                      // bucketing: rows per bucket s in [1, n_rows]
+    unsigned long long bkt_seed;       // bucketing: seed of the permutation (its step key is DnC's: dnc_step / dnc_step_ptr)
     int R, rank;
     int nseg, first_seg;               // owned segments; segments [0, first_seg) were pre-accumulated by phase A kernels
     long long seg_lo[kMaxSeg], seg_hi[kMaxSeg];   // multiples of 4
@@ -113,7 +119,8 @@ struct GarArgs {
     float* staging;                    // [n][owned length] or null
     float* dist_out;                   // optional [n * n] (geometric median, centered clipping: [iterations][n]); with NNM: of the mixed rows
     float* raw_dist_out;               // optional [n * n]: NNM's distances of the raw rows
-    int* info;                         // optional [128]: selection masks for tests/diagnostics; [64, 64 + n): NNM masks
+    int* info;                         // optional [192]: selection masks for tests/diagnostics; [64, 64 + n): NNM masks;
+                                       // bucketing: [128, 128 + n_rows) the permutation, [160, 160 + n) the bucket masks
     float const* loss_in;              // optional [nloss] local per-worker losses
     int nloss;
     float* loss_out;                   // [1]: total loss over all ranks (summed in rank order)
@@ -128,7 +135,7 @@ struct GarArgs {
     int dnc_r;                         // rows removed per iteration, r = floor(c f)
     long long dnc_b, dnc_domain;       // subsample b and sample domain D: b' = min(b, D) coordinates of [0, D) per iteration
     unsigned long long dnc_seed;
-    long long dnc_step;                // step key, used when dnc_step_ptr is null
+    long long dnc_step;                // step key (DnC, bucketing), used when dnc_step_ptr is null
     long long const* dnc_step_ptr;     // device step key (graph replay), or null
     float* dnc_scratch;                // [grid][kDncIterations][kMaxPairs] CTA partials, then the samples [T][n][b'4]
     double* smea_scratch;              // SMEA: one [m][m] slab per warp of the grid (m = n - f), the double-centred matrix of its set
@@ -167,6 +174,10 @@ struct Shared {
     unsigned nnm_mask[kMaxWorkers];  // NNM: neighbourhood of every row (itself included); outlives the rule's phases
     float arc_c[kMaxWorkers];        // ARC: clipping factor of every row
     unsigned arc_clipped;            // ARC: the rows the clip pass rescales
+    unsigned bkt_mask[kMaxWorkers];  // bucketing: members of every bucket
+    unsigned char bkt_perm[kMaxWorkers];    // bucketing: the permutation pi
+    unsigned char bkt_order[kMaxWorkers];   // bucketing: the rows bucket by bucket, ascending inside a bucket
+    signed char bkt_last[kMaxWorkers];      // bucketing: at the last position of a bucket, its index; -1 elsewhere
     int selcount[kMaxWorkers];
     int theta;
     float hyper[4];
@@ -1286,6 +1297,101 @@ __device__ __forceinline__ long long dnc_permute(unsigned long long key, int h, 
     return static_cast<long long>(y);
 }
 
+// ---- bucketing (Karimireddy, He & Jaggi, "Byzantine-Robust Learning on Heterogeneous Datasets via Bucketing", ICLR 2022) -------- //
+// K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ kBucketingTag); pi starts as the identity and, for i = n_rows - 1 down to 1,
+// pi[i] and pi[j] swap with j = splitmix64(K ^ i) mod (i + 1). Bucket b < n = ceil(n_rows / s) holds pi[b s], ..., pi[min((b + 1) s,
+// n_rows) - 1]; y_b = (((x_a0 + x_a1) + ...) / |M_b|, its members in ascending worker order from +0, every operation rounded once
+// (NNM's mixing arithmetic).
+//   1. warp 0 of every CTA builds pi, the masks and the order in which the mean pass visits the rows (identical everywhere: the key is
+//      the same on every CTA and every rank). No exchange: a bucket mean is per coordinate, and the loss keeps its usual path;
+//   2. mean pass over all owned segments, with the rules' (tid, VEC) mapping (the instance is the rule's, chosen from n): the rows
+//      are visited bucket by bucket, 8 loads in flight, into one running sum that is divided and stored as staging row b at the last member of bucket b. Every raw row
+//      crosses NVLink once; only the n means are staged. A coordinate-wise or iterative rule's thread reads back only what it stored
+//      itself, so no grid barrier follows; the distance rules and DnC's gather add one.
+template<int N, int VEC>
+__device__ __forceinline__ void bucketing_pre_aggregation(GarArgs const& a, Shared& sh, long long tid, long long nthreads) {
+    int const nr = a.n_rows, s = a.bkt_size;
+    if (threadIdx.x < 32) {
+        int const lane = threadIdx.x;
+        unsigned long long const step = static_cast<unsigned long long>(a.dnc_step_ptr ? *a.dnc_step_ptr : a.dnc_step);
+        unsigned long long const key = splitmix64(splitmix64(splitmix64(a.bkt_seed) ^ step) ^ kBucketingTag);
+        // the swap partner of every i, computed in parallel; the swaps themselves are sequential
+        unsigned long long const i = static_cast<unsigned long long>(lane);
+        int const partner = lane >= 1 && lane < nr ? static_cast<int>(splitmix64(key ^ i) % (i + 1ull)) : 0;
+        if (lane < nr)
+            sh.bkt_perm[lane] = static_cast<unsigned char>(lane);
+        __syncwarp();
+        for (int k = nr - 1; k >= 1; --k) {
+            int const j = __shfl_sync(0xffffffffu, partner, k);
+            if (lane == 0) {
+                unsigned char const t = sh.bkt_perm[k];
+                sh.bkt_perm[k] = sh.bkt_perm[j];
+                sh.bkt_perm[j] = t;
+            }
+            __syncwarp();
+        }
+        if (lane < nr)
+            sh.bkt_last[lane] = -1;
+        __syncwarp();
+        int const nb = a.n;
+        if (lane < nb) {
+            int const lo = lane * s, hi = lo + s < nr ? lo + s : nr;
+            unsigned mask = 0u;
+            for (int p = lo; p < hi; ++p)
+                mask |= 1u << sh.bkt_perm[p];
+            sh.bkt_mask[lane] = mask;
+            int p = lo;
+            for (unsigned rest = mask; rest != 0u; rest &= rest - 1u)
+                sh.bkt_order[p++] = static_cast<unsigned char>(__ffs(rest) - 1);
+            sh.bkt_last[hi - 1] = static_cast<signed char>(lane);
+            if (a.info && blockIdx.x == 0)
+                a.info[160 + lane] = static_cast<int>(mask);
+        }
+        if (a.info && blockIdx.x == 0 && lane < nr)
+            a.info[128 + lane] = sh.bkt_perm[lane];
+    }
+    __syncthreads();
+    long long const owned = owned_length(a);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            float* const tile = a.staging + soff + v * VEC;
+            float acc[VEC];
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                acc[c] = 0.f;
+            // 8 rows in flight at a time, in a loop over the n_rows gathered rows: the instance N only bounds the rule's n rows
+            for (int p0 = 0; p0 < nr; p0 += kBlockRows) {
+                float g[kBlockRows][VEC];
+#pragma unroll
+                for (int p = 0; p < kBlockRows; ++p)
+                    if (p0 + p < nr)
+                        V<VEC>::load_stream(a.grad[sh.bkt_order[p0 + p]] + x, g[p]);
+#pragma unroll
+                for (int p = 0; p < kBlockRows; ++p) {
+                    if (p0 + p < nr) {
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            acc[c] = __fadd_rn(acc[c], g[p][c]);
+                        int const b = sh.bkt_last[p0 + p];
+                        if (b >= 0) {
+                            float const count = static_cast<float>(p0 + p + 1 - b * s);
+#pragma unroll
+                            for (int c = 0; c < VEC; ++c)
+                                acc[c] = __fdiv_rn(acc[c], count);
+                            V<VEC>::store(tile + b * owned, acc);
+#pragma unroll
+                            for (int c = 0; c < VEC; ++c)
+                                acc[c] = 0.f;
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
 __device__ __forceinline__ bool before_d(double a, int ia, double b, int ib) {
     bool const fa = isfinite(a), fb = isfinite(b);
     if (fa != fb)
@@ -1873,6 +1979,13 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
             local_loss += a.loss_in[j];
 
     if (a.mix) {
+        if (a.mix & kMixBucketing) {
+            bucketing_pre_aggregation<N, VEC>(a, sh, tid, nthreads);
+            if (distance_rule) {
+                __threadfence();
+                grid.sync();   // the mean pass wrote the tile with the rule's (tid, VEC) mapping; distance passes read it by float4 blocks
+            }
+        }
         if (a.mix & kMixArc) {
             arc_pre_aggregation<N, VEC>(a, sh, grid, epoch, local_loss, tid, nthreads);
             if (distance_rule || (a.mix & kMixNnm)) {
@@ -2011,7 +2124,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fused_kernel(GarArg
             coordinate_rules<N, VEC, false>(a, hyper, tid, nthreads);
     }
 
-    bool const exchanged_loss = distance_rule || a.mix;   // the loss went through an exchange of distances (distance rules, NNM)
+    // the loss went through an exchange (distance rules, NNM, ARC); bucketing exchanges nothing
+    bool const exchanged_loss = distance_rule || (a.mix & (kMixNnm | kMixArc));
     if (multi) { // exit barrier: all slices have landed on all ranks, gradient buffers are free again
         fence_sys();
         grid.sync();
@@ -2072,6 +2186,8 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs 
         for (int j = 0; j < a.nloss; ++j)
             local_loss += a.loss_in[j];
     if (a.mix) {
+        if (a.mix & kMixBucketing)
+            bucketing_pre_aggregation<N, VEC>(a, sh, tid, nthreads);
         if (a.mix & kMixArc) {
             arc_pre_aggregation<N, VEC>(a, sh, grid, epoch, local_loss, tid, nthreads);
             if (a.mix & kMixNnm) {
@@ -2082,7 +2198,7 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs 
         if (a.mix & kMixNnm)
             nnm_pre_aggregation<N, VEC>(a, sh, pair_of, grid, epoch, local_loss, tid, nthreads);
         __threadfence();
-        grid.sync();   // the clip or mix pass wrote the tile with the rule's (tid, VEC) mapping; the gather reads any coordinate of it
+        grid.sync();   // the mean, clip or mix pass wrote the tile with the rule's (tid, VEC) mapping; the gather reads any coordinate of it
     }
     dnc_selection<N>(a, sh, ds, pair_of, grid, epoch, local_loss, tid, nthreads);   // carries the loss
     __syncthreads();
@@ -2659,10 +2775,11 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 //   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
 //   [115] arc_out (ARC: [2n] squared norms, then factors) | [116] SMEA scratch (doubles)
+//   [113] is also bucketing's step key
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-//       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC) | [27] DnC r
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step
-//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles)
+//       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC, 4 bucketing) | [27] DnC r | [28] bucketing: s | [29] gathered rows n_rows (0: n)
+// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step (also bucketing's)
+//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles) | [22] bucketing: seed
 // floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
@@ -2682,7 +2799,12 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.dnc_step_ptr = reinterpret_cast<long long const*>(ptrs[113]);
     a.dnc_scratch = reinterpret_cast<float*>(ptrs[114]);
     a.smea_scratch = reinterpret_cast<double*>(ptrs[116]);
-    if (a.n < 1 || a.n > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
+    a.bkt_size = ints[28];
+    a.n_rows = ints[29] != 0 ? ints[29] : a.n;
+    a.bkt_seed = static_cast<unsigned long long>(longs[22]);
+    if (a.n < 1 || a.n > kMaxWorkers || a.n_rows < 1 || a.n_rows > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
+        return 100;
+    if (!(a.mix & kMixBucketing) && a.n_rows != a.n)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
         return 101;
@@ -2695,8 +2817,11 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     }
     if (a.rule < 0 || a.rule > kSmea)
         return 102;
-    if (a.mix < 0 || a.mix > (kMixNnm | kMixArc))
+    if (a.mix < 0 || a.mix > (kMixNnm | kMixArc | kMixBucketing))
         return 117;
+    if ((a.mix & kMixBucketing) && (a.mix != kMixBucketing || a.bkt_size < 1 || a.bkt_size > a.n_rows ||
+                                    a.n != (a.n_rows + a.bkt_size - 1) / a.bkt_size || !ptrs[38]))   // the means land in the staging tile
+        return 123;
     if ((a.mix & kMixArc) && (a.f < 0 || 2 * a.f >= a.n))
         return 120;
     if ((a.mix & kMixNnm) && (a.f < 0 || 2 * a.f >= a.n))
@@ -2734,7 +2859,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 104;
     if (a.rule == kAveragedMedian && (a.beta < 1 || a.beta > a.n))
         return 105;
-    for (int i = 0; i < a.n; ++i)
+    for (int i = 0; i < a.n_rows; ++i)
         a.grad[i] = reinterpret_cast<float const*>(ptrs[i]);
     a.agg_out = reinterpret_cast<float*>(ptrs[32]);
     a.param = reinterpret_cast<float*>(ptrs[33]);
@@ -2781,7 +2906,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     if (a.mix && (!a.cta_partials || !a.mailbox[0] || !a.staging))
         return 108;   // NNM mixes, ARC clips the staged tile in place
     if (a.mix && a.first_seg > 0)
-        return 111;   // NNM's raw distance pass and ARC's norm pass cover every segment: nothing is pre-accumulated
+        return 111;   // NNM's raw distance pass, ARC's norm pass and bucketing's mean pass cover every segment: nothing is pre-accumulated
     if (a.R > 1 && !a.signal[0])
         return 109;
     if (a.n > kBlockRows && a.R > 1 && (a.rule == kKrum || a.rule == kBulyan || a.rule == kMda || a.rule == kSmea) && !a.staging)
@@ -2830,6 +2955,8 @@ int agb_gar_fused(unsigned long long const* ptrs, int const* ints, long long con
     if (total == 0 && a.R == 1)
         return 0;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    // the instance follows the rule's n rows (with bucketing n <= n_rows; the mean pass loops over the gathered rows), so the rule adds
+    // in the same order as on n plain rows
     if (a.n <= 8)
         return launch<8, 4>(a, max_ctas, longs[21], s);
     if (a.n <= 16)

@@ -35,8 +35,8 @@ ARC_STATS = MAX_WORKERS + 1
 MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS) * 4
 PTRS = 117
 # [0]: theta, [1, 1 + theta): selection masks; [32, 34): SMEA's winning score (float64 bits); [64, 64 + n): NNM masks;
-# [96, 96 + T): DnC's mask of every iteration
-INFO_INTS = 128
+# [96, 96 + T): DnC's mask of every iteration; bucketing: [128, 128 + n_rows) the permutation, [160, 160 + n') the bucket masks
+INFO_INTS = 192
 OPTIMIZERS = {"none": 0, "sgd": 1, "adam": 2, "rmsprop": 3, "adagrad": 4, "adadelta": 5}
 
 _ERRORS = {
@@ -51,7 +51,8 @@ _ERRORS = {
   117: "invalid NNM parameters (0 <= 2 f < n)",
   118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)",
   119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)",
-  120: "invalid ARC parameters (0 <= 2 f < n)", 122: "invalid SMEA parameters (0 <= 2 f < n and C(n, f) <= 2^14)"}
+  120: "invalid ARC parameters (0 <= 2 f < n)", 122: "invalid SMEA parameters (0 <= 2 f < n and C(n, f) <= 2^14)",
+  123: "invalid bucketing parameters (1 <= s <= n_rows, n = ceil(n_rows / s), not combined with NNM or ARC, a staging tile)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
@@ -107,7 +108,7 @@ class FusedLauncher:
     self.craft_stats = torch.zeros(1 + CRAFT_STATS, dtype=torch.float32, device=self.device)
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
-    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 5))()
+    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 6))()
     self._floats = (ctypes.c_float * 6)()
     self._func = _lib().agb_gar_fused
     self._func.restype = ctypes.c_int
@@ -120,11 +121,15 @@ class FusedLauncher:
 
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
-            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None):
+            first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None,
+            bucketing_seed=0):
     ptrs = self._ptrs
     for i in range(PTRS):
       ptrs[i] = 0
-    if len(rows) != spec.n:
+    if not spec.gathered_rows(len(rows)):
+      if spec.mix == FusedSpec.BUCKETING:
+        raise tools.UserException("Bucketing with s = %d reduces %d gradient rows to %d, not the rule's %d" % (
+          spec.bucket_size, len(rows), -(-len(rows) // spec.bucket_size), spec.n))
       raise tools.UserException("Expected %d gradient rows, got %d" % (spec.n, len(rows)))
     if not 1 <= len(segments) <= MAX_SEGMENTS:
       raise tools.UserException("Between 1 and %d coordinate segments per rank (got %d)" % (MAX_SEGMENTS, len(segments)))
@@ -161,9 +166,11 @@ class FusedLauncher:
     self._floats[0], self._floats[1], self._floats[2], self._floats[3], self._floats[4] = lr, hyper[0], hyper[1], hyper[2], spec.nu
     self._floats[5] = spec.tau
     ints[27] = spec.removed if spec.rule == "dnc" else 0
+    ints[28], ints[29] = spec.bucket_size or 0, len(rows)
     longs = self._longs
-    longs[17], longs[18], longs[19], longs[20] = spec.subsample, domain, spec.seed - (1 << 64) if spec.seed >= 1 << 63 else spec.seed, step
-    longs[21] = scratch.numel() if scratch is not None else 0
+    signed = lambda seed: seed - (1 << 64) if seed >= 1 << 63 else seed
+    longs[17], longs[18], longs[19], longs[20] = spec.subsample, domain, signed(spec.seed), step
+    longs[21], longs[22] = scratch.numel() if scratch is not None else 0, signed(int(bucketing_seed))
 
   def dnc_scratch(self, spec, domain):
     """DnC's scratch for rule `spec` over `domain` coordinates: the CTA partials of the sampled distances of the largest grid, then the
@@ -209,7 +216,7 @@ def _torch_rules(spec, step=0):
           "smea": lambda M: _ops.torch_smea(M, spec.f)}[spec.rule]
 
 
-def aggregate(spec, G, return_details=False, center=None, step=0):
+def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed=0):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
   iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
@@ -219,40 +226,46 @@ def aggregate(spec, G, return_details=False, center=None, step=0):
   With `spec.mix == "nnm"` the rule runs on the mixed rows (its distances and masks are those of the mixed rows), and
   `return_details` adds a fourth element: (distances of the raw rows [n, n], NNM masks [n] int32). With "arc" the rule runs on the
   clipped rows and `return_details` adds (squared norms N [n], factors c [n]); with "arc+nnm" NNM mixes the clipped rows (its
-  distances are theirs) and both elements follow, NNM's first."""
+  distances are theirs) and both elements follow, NNM's first.
+  With "bucketing" G holds the n gathered rows and the rule runs on the n' = ceil(n / spec.bucket_size) bucket means, drawn with step
+  key `step` and seed `bucketing_seed` (its distances and masks are those of the means); `return_details` adds (permutation [n] int32,
+  bucket masks [n'] int32)."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
+  from ..aggregators import _ops
   n, d = G.shape
-  if n != spec.n:
-    spec = FusedSpec(spec.rule, n, spec.f, spec.m, spec.beta, iterations=spec.iterations, nu=spec.nu, tau=spec.tau, mix=spec.mix,
-                     subsample=spec.subsample, c=spec.c, seed=spec.seed)
-  if spec.rule == "centered-clipping":
-    return _aggregate_centered_clipping(spec, G, return_details, center)
+  bucketing = spec.mix == FusedSpec.BUCKETING
+  m = _ops.check_bucketing(n, spec.bucket_size) if bucketing else n   # the rows the rule sees
+  if m != spec.n:
+    spec = spec.with_rows(m)
   if spec.rule == "dnc":
-    from ..aggregators import _ops
     step = _ops.check_dnc_step(step)
+  if bucketing:
+    bucketing_seed, step = _ops.check_bucketing_key(bucketing_seed, step)
+  if spec.rule == "centered-clipping":
+    return _aggregate_centered_clipping(spec, G, return_details, center, step, bucketing_seed)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
-    return _torch_rules(spec, step)(_torch_mixed(spec, G))
+    return _torch_rules(spec, step)(_torch_mixed(spec, G, step, bucketing_seed))
   if G.dtype != torch.float32:
-    out = aggregate(spec, G.float(), return_details, step=step)
+    out = aggregate(spec, G.float(), return_details, step=step, bucketing_seed=bucketing_seed)
     return (out[0].to(G.dtype),) + out[1:] if return_details else out.to(G.dtype)
   if n > MAX_WORKERS:  # beyond the kernels' worker limit: torch ops on the same device
-    return _torch_rules(spec, step)(_torch_mixed(spec, G))
+    return _torch_rules(spec, step)(_torch_mixed(spec, G, step, bucketing_seed))
   G, dp = _aligned_rows(G)
-  launcher = _launcher(G.device, n)
+  launcher = _launcher(G.device, n, m)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=_staging(spec, n, dp, G.device), step=step, domain=d)
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=_staging(spec, dp, G.device), step=step, domain=d, bucketing_seed=bucketing_seed)
   out = out[:d]
   if return_details:
     if spec.rule in ITERATIVE_RULES:
-      dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n)
+      dist = launcher.geo_dist_out[:spec.iterations * m].view(spec.iterations, m)
     elif spec.rule == "dnc":
-      dist = launcher.dnc_dist_out[:spec.iterations * n * n].view(spec.iterations, n, n)
+      dist = launcher.dnc_dist_out[:spec.iterations * m * m].view(spec.iterations, m, m)
     else:
-      dist = launcher.dist_out.view(n, n)
+      dist = launcher.dist_out[:m * m].view(m, m)
     info = launcher.info.clone()
     score = (info[32:34].cpu().view(torch.float64)[0],) if spec.rule == "smea" else ()
     return (out, dist.clone(), info) + score + _mix_details(spec, launcher, n)
@@ -271,14 +284,17 @@ def _aligned_rows(G):
   return G, d + pad
 
 
-def _staging(spec, n, dp, device):
-  """NNM mixes and ARC clips the rows in place in a local [n, dp] tile: the stand-alone op has to provide one."""
-  return torch.empty((n, dp), dtype=torch.float32, device=device) if spec.mix is not None else None
+def _staging(spec, dp, device):
+  """NNM mixes and ARC clips the rows in place in a local [n, dp] tile, bucketing stores its n' means there: the stand-alone op has to
+  provide one (of the rule's spec.n rows)."""
+  return torch.empty((spec.n, dp), dtype=torch.float32, device=device) if spec.mix is not None else None
 
 
 def _mix_details(spec, launcher, n):
-  """The `return_details` elements of the pre-aggregation: with NNM (raw distances [n, n], NNM masks [n] int32), then with ARC
-  (squared norms [n], factors [n])."""
+  """The `return_details` elements of the pre-aggregation over n gathered rows: with NNM (raw distances [n, n], NNM masks [n] int32),
+  then with ARC (squared norms [n], factors [n]); with bucketing (permutation [n] int32, bucket masks [n'] int32)."""
+  if spec.mix == FusedSpec.BUCKETING:
+    return ((launcher.info[128:128 + n].clone(), launcher.info[160:160 + spec.n].clone()),)
   details = ()
   if spec.mix_id & FusedSpec.MIX_NNM:
     details += ((launcher.raw_dist_out.view(n, n).clone(), launcher.info[64:64 + n].clone()),)
@@ -288,24 +304,27 @@ def _mix_details(spec, launcher, n):
   return details
 
 
-def _torch_mixed(spec, G):
+def _torch_mixed(spec, G, step=0, bucketing_seed=0):
   """The fall-backs' pre-aggregation: `spec.mix` with the torch reference on G's device."""
   from ..aggregators import _ops
-  return _ops.torch_pre_aggregate(G, spec.mix, spec.f)
+  return _ops.torch_pre_aggregate(G, spec.mix, spec.f, bucket_size=spec.bucket_size, seed=bucketing_seed, step=step)
 
 
-def _launcher(device, n):
-  key = (device.index, n)
+def _launcher(device, n, rule_rows=None):
+  """The cached launcher for n gathered rows; with bucketing one per rule row count too, since the kernels leave the diagonal of the
+  [n', n'] distance view untouched (+0 from the allocation) and a view of another size would see other entries there."""
+  key = (device.index, n) if rule_rows in (None, n) else (device.index, n, rule_rows)
   launcher = _launchers.get(key)
   if launcher is None:
     launcher = _launchers[key] = FusedLauncher(device, n)
   return launcher
 
 
-def _aggregate_centered_clipping(spec, G, return_details, center):
+def _aggregate_centered_clipping(spec, G, return_details, center, step=0, bucketing_seed=0):
   """`aggregate` for centered clipping: the sm_90a kernel for fp32 and n <= 32, the torch reference on the device otherwise."""
   from ..aggregators import _ops
   n, d = G.shape
+  m = spec.n   # the rows the rule sees
   if center is None or center.shape != (d,) or center.device != G.device:
     raise tools.UserException("Centered clipping needs a [%d] center on %s" % (d, G.device))
   if G.dtype == torch.float64 or n > MAX_WORKERS:
@@ -313,7 +332,7 @@ def _aggregate_centered_clipping(spec, G, return_details, center):
       raise tools.UserException("Centered clipping needs a center of type %s (got %s)" % (G.dtype, center.dtype))
     if return_details:
       raise tools.UserException("Centered clipping returns its details from the sm_90a kernel only (fp32, n <= %d)" % MAX_WORKERS)
-    return _ops.torch_centered_clipping(_torch_mixed(spec, G), spec.iterations, spec.tau, center)
+    return _ops.torch_centered_clipping(_torch_mixed(spec, G, step, bucketing_seed), spec.iterations, spec.tau, center)
   if G.dtype != torch.float32 or center.dtype != torch.float32:
     raise tools.UserException("Centered clipping on the device needs fp32 rows and center (got %s, %s)" % (G.dtype, center.dtype))
   G, dp = _aligned_rows(G)
@@ -322,15 +341,15 @@ def _aggregate_centered_clipping(spec, G, return_details, center):
   if pad or not center.is_contiguous() or center.data_ptr() % 16:
     work = torch.zeros(dp, dtype=torch.float32, device=G.device)
     work[:d] = center
-  launcher = _launcher(G.device, n)
+  launcher = _launcher(G.device, n, m)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher.launch(spec, rows, 0, dp, agg_out=out, center=work, staging=_staging(spec, n, dp, G.device))
+  launcher.launch(spec, rows, 0, dp, agg_out=out, center=work, staging=_staging(spec, dp, G.device), step=step, bucketing_seed=bucketing_seed)
   if work is not center:
     center.copy_(work[:d])
   out = out[:d]
   if return_details:
-    dist = launcher.geo_dist_out[:spec.iterations * n].view(spec.iterations, n)
+    dist = launcher.geo_dist_out[:spec.iterations * m].view(spec.iterations, m)
     return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
   return out
 

@@ -25,6 +25,8 @@ nearest rows before the rule runs, on every engine: inside the fused kernel, in 
 the host library's distances on the host engine and with the torch reference for plug-ins without a fused spec. The GAR object
 itself does not mix. `pre_aggregation="arc"` (adaptive robust clipping) clips the k = floor(2 f (n - f) / n) rows of largest norm to
 the norm of the largest row left alone, in the same places (the host engine with the torch reference); "arc+nnm" clips, then mixes.
+`pre_aggregation="bucketing"` with `bucket_size` s shuffles the n gathered rows with a permutation keyed by `bucketing_seed` and the
+update number (DnC's step key), and replaces them by the n' = ceil(n / s) means of buckets of s rows: the GAR is built for n' workers.
 """
 
 import os
@@ -43,20 +45,27 @@ def _world(group=None):
   return 0, 1
 
 
-_MIX_NAMES = {"nnm": "Nearest-neighbour mixing", "arc": "Adaptive robust clipping", "arc+nnm": "Adaptive robust clipping with nearest-neighbour mixing"}
+_MIX_NAMES = {"nnm": "Nearest-neighbour mixing", "arc": "Adaptive robust clipping", "arc+nnm": "Adaptive robust clipping with nearest-neighbour mixing",
+              "bucketing": "Bucketing"}
 
 
-def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz):
+def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz, bucket_size=None):
   """-> (mix, f of the mix, fused spec or None). The pre-aggregation (NNM, ARC or both) runs with the declared f: `nb_decl_byz`, or by
   default the rule's own f. Rules whose spec ignores f (average, average-nan, median, averaged-median) carry the declared f in their
-  spec for the kernel's pre-aggregation."""
+  spec for the kernel's pre-aggregation. Bucketing needs no f; the GAR must have been built for the n' = ceil(n / s) bucket means."""
   from ..aggregators import FusedSpec, _ops
-  mix = _ops.check_pre_aggregation(pre_aggregation)   # None, "nnm", "arc" or "arc+nnm"
+  mix = _ops.check_pre_aggregation(pre_aggregation, bucket_size)   # None, "nnm", "arc", "arc+nnm" or "bucketing"
   spec = gar.fused_spec()
   own = spec.f if spec is not None and spec.rule in FusedSpec.RULES_WITH_F else getattr(gar, "_f", None)
   f = own if nb_decl_byz is None else int(nb_decl_byz)
   if mix is None:
     return None, f, spec
+  if mix == FusedSpec.BUCKETING:
+    rows = _ops.check_bucketing(nbworkers, bucket_size)
+    if spec is not None and spec.n != rows:
+      raise tools.UserException("Bucketing with s = %d turns n = %d workers into n' = %d bucket means: the GAR must be built for %d workers (got %d)" % (
+        bucket_size, nbworkers, rows, rows, spec.n))
+    return mix, f, (spec.with_mix(mix, bucket_size=bucket_size) if spec is not None else None)
   name = _MIX_NAMES[mix]
   if f is None:
     raise tools.UserException(name + " needs the declared number of Byzantine workers f of GAR " + type(gar).__name__)
@@ -70,9 +79,11 @@ def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz):
 class _AggregationBase:
   """Common state: layout, optimizer spec and slots, update counter."""
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, pre_aggregation=None, nb_decl_byz=None):
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, pre_aggregation=None, nb_decl_byz=None, bucket_size=None, bucketing_seed=0):
     self.gar = gar
-    self.mix, self.f, self.spec = _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz)
+    self.mix, self.f, self.spec = _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz, bucket_size)
+    self.bucket_size = bucket_size if self.mix == "bucketing" else None
+    self.bucketing_seed = int(bucketing_seed)
     self.layout = layout
     self.n = nbworkers
     self.optimizer = optimizer
@@ -122,6 +133,11 @@ class _AggregationBase:
       return {"step": self.updates + 1}
     return {}
 
+  def _pre_aggregate(self, rows, host=False):
+    """The torch reference of the pre-aggregation for the step about to be counted (bucketing: step key updates + 1)."""
+    from ..aggregators import _ops
+    return _ops.torch_pre_aggregate(rows, self.mix, self.f, host=host, bucket_size=self.bucket_size, seed=self.bucketing_seed, step=self.updates + 1)
+
   def full_slots(self):
     return self.slots
 
@@ -148,8 +164,8 @@ class HostAggregation(_AggregationBase):
 
   name = "host"
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None):
-    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None, bucket_size=None, bucketing_seed=0):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz, bucket_size, bucketing_seed)
     self.device = torch.device(device)
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
@@ -178,8 +194,7 @@ class HostAggregation(_AggregationBase):
     self._gather()
     rows = self._gathered
     if self.mix is not None:
-      from ..aggregators import _ops
-      rows = _ops.torch_pre_aggregate(rows, self.mix, self.f, host=True)
+      rows = self._pre_aggregate(rows, host=True)
     aggregated = self.gar.aggregate(rows, **self._rule_kwargs())
     self.updates += 1
     self.optimizer.apply_torch(self.params, aggregated, self.slots, rate, self.updates)
@@ -191,8 +206,8 @@ class BaselineAggregation(_AggregationBase):
 
   name = "baseline"
 
-  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", pre_aggregation=None, nb_decl_byz=None):
-    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
+  def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", pre_aggregation=None, nb_decl_byz=None, bucket_size=None, bucketing_seed=0):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz, bucket_size, bucketing_seed)
     self.device = torch.device(device)
     self.params = torch.zeros(self.d, dtype=torch.float32, device=self.device)
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
@@ -221,12 +236,13 @@ class BaselineAggregation(_AggregationBase):
     self._gather()
     state = self._rule_kwargs()
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
+      if self.mix == "bucketing":   # the permutation's step key is DnC's
+        state = dict(state, step=self.updates + 1, bucketing_seed=self.bucketing_seed)
       aggregated = gar_ops.aggregate(self.spec, self._gathered, **state)   # pre-aggregates inside the kernel
     else:
       rows = self._gathered
       if self.mix is not None:
-        from ..aggregators import _ops
-        rows = _ops.torch_pre_aggregate(rows, self.mix, self.f)
+        rows = self._pre_aggregate(rows)
       aggregated = self.gar.aggregate(rows, **state)
     self.updates += 1
     if self.optimizer.name == "sgd":
@@ -250,12 +266,12 @@ class FusedAggregation(_AggregationBase):
   name = "fused"
 
   def __init__(self, gar, layout, nbworkers, optimizer, group=None, device="cuda", keep_aggregate=False, bf16_copy=False, max_ctas=0, buckets=None, device_state=False,
-               pre_aggregation=None, nb_decl_byz=None):
-    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz)
+               pre_aggregation=None, nb_decl_byz=None, bucket_size=None, bucketing_seed=0):
+    super().__init__(gar, layout, nbworkers, optimizer, group, pre_aggregation, nb_decl_byz, bucket_size, bucketing_seed)
     self.device = torch.device(device)
     if self.spec is None:
       raise tools.UserException("GAR " + type(gar).__name__ + " has no fused kernel; use the baseline/host engine")
-    if self.spec.n != nbworkers:
+    if not self.spec.gathered_rows(nbworkers):   # with bucketing `_mixed_spec` already checked n' = ceil(n / s)
       raise tools.UserException("GAR built for %d workers used with %d" % (self.spec.n, nbworkers))
     d, w, R = self.d, self.w, self.world
     self.distance_rule = self.spec.rule in ("krum", "bulyan", "mda", "smea")
@@ -279,10 +295,11 @@ class FusedAggregation(_AggregationBase):
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
     # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; a pre-aggregation (NNM mixes, ARC
-    # clips) rewrites the staged tile in place and every rule then reads it (n * owned * 4 bytes, also with R = 1)
+    # clips) rewrites the staged tile in place and every rule then reads it (n * owned * 4 bytes, also with R = 1); bucketing stores its
+    # n' means there, so the tile has the rule's spec.n rows
     need_staging = ((self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
                     or self.mix is not None)
-    self.staging = torch.empty((self.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
+    self.staging = torch.empty((self.spec.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     if self.spec.rule == "dnc":
       self.launcher.dnc_scratch(self.spec, d)   # allocated before any graph capture
@@ -294,9 +311,9 @@ class FusedAggregation(_AggregationBase):
     self.epoch_dev = torch.zeros(1, dtype=torch.int32, device=self.device) if device_state else None
     self.hyper_dev = torch.zeros(4, dtype=torch.float32, device=self.device) if device_state else None
     self._hyper_host = torch.zeros(4, dtype=torch.float32).pin_memory() if device_state else None
-    dnc = self.spec.rule == "dnc"
-    # DnC: the step key of its samples, refreshed by `prepare` so that graph replays draw new samples
-    self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device) if device_state and dnc else None
+    keyed = self.spec.rule == "dnc" or self.mix == "bucketing"
+    # DnC, bucketing: the step key of the samples and of the permutation, refreshed by `prepare` so that graph replays draw new ones
+    self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device) if device_state and keyed else None
     self.loss_out = torch.zeros(1, dtype=torch.float32, device=self.device)
     self._pre_accumulated = 0
     self._craft_mode = None   # Min-Max / Min-Sum: (mode, H) of the last `craft_byzantine`
@@ -312,7 +329,7 @@ class FusedAggregation(_AggregationBase):
     # in-switch (NVLS) reduction of the gradients for the `average` rule instead of 7 P2P loads (0.241 vs 0.312 ms at 8 GPUs); AGB_NVLS_REDUCE=0 disables
     self._grad_mc = heap.multicast("grads") if (R > 1 and self.spec.rule == "average" and self.mix is None and os.environ.get("AGB_NVLS_REDUCE", "1") not in ("", "0")) else 0
     tools.info("Fused aggregation: rule %r%s, n = %d (%d per rank), d = %d, %d bucket(s), %d owned coordinates, provider %s, NVLS multicast %s" % (
-      self.spec.rule, {"nnm": " after NNM", "arc": " after ARC", "arc+nnm": " after ARC and NNM"}.get(self.mix, ""), self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
+      self.spec.rule, {"nnm": " after NNM", "arc": " after ARC", "arc+nnm": " after ARC and NNM", "bucketing": " after bucketing (s = %s)" % self.bucket_size}.get(self.mix, ""), self.n, w, d, len(self.buckets), owned, heap.provider, "on" if self._param_mc else "off"), context="fused")
 
   @staticmethod
   def _check_buckets(buckets, d):
@@ -338,7 +355,7 @@ class FusedAggregation(_AggregationBase):
   @property
   def overlappable(self):
     """Whether `phase_a` exists for this rule (the distance pass of Krum / Bulyan / MDA / SMEA is additive over coordinates); not with a
-    pre-aggregation, whose first pass (NNM's raw distances, ARC's norms) runs in the finish kernel over every segment."""
+    pre-aggregation, whose first pass (NNM's raw distances, ARC's norms, bucketing's means) runs in the finish kernel over every segment."""
     return self.distance_rule and len(self.buckets) > 1 and self.mix is None
 
   def visible_rows(self):
@@ -413,7 +430,7 @@ class FusedAggregation(_AggregationBase):
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
                          loss_in=loss_in, loss_out=self.loss_out, center=self.center, step=self.updates, step_ptr=self.step_dev, domain=self.d,
-                         **self._common(self._rate_args))
+                         bucketing_seed=self.bucketing_seed, **self._common(self._rate_args))
 
   def _assemble(self, vector):
     """Full copy of a [d] vector maintained on the owned segments only (collective when R > 1)."""
@@ -451,11 +468,12 @@ def _single_host(group=None):
   return len(set(hosts)) == 1
 
 
-def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None, **kwargs):
+def make_aggregation(kind, gar, layout, nbworkers, optimizer, group=None, device="cpu", pre_aggregation=None, nb_decl_byz=None, bucket_size=None,
+                     bucketing_seed=0, **kwargs):
   """`kind` in {"auto", "fused", "baseline", "host"}; "auto" = fused on CUDA when the rule has a kernel and all ranks share one
   machine, the NCCL baseline engine on CUDA otherwise, host on CPU. `pre_aggregation`: None / "none", "nnm", "arc" or "arc+nnm", on every engine, with
-  `nb_decl_byz` declared Byzantine workers (default: the rule's f)."""
-  mix = dict(pre_aggregation=pre_aggregation, nb_decl_byz=nb_decl_byz)
+  `nb_decl_byz` declared Byzantine workers (default: the rule's f), or "bucketing" with `bucket_size` and `bucketing_seed`."""
+  mix = dict(pre_aggregation=pre_aggregation, nb_decl_byz=nb_decl_byz, bucket_size=bucket_size, bucketing_seed=bucketing_seed)
   device = torch.device(device)
   if kind == "auto":
     if device.type != "cuda":

@@ -22,6 +22,9 @@ mixed step), and also times the fused step of each rule without NNM, alternating
 the measured cost of the mix (`nnm_ms`, `plain_ms`, `nnm_overhead_ms`: medians over the alternated rounds).
 `--gar-pre-aggregation arc` (adaptive robust clipping) and `arc+nnm` (ARC, then NNM) do the same, with keys `arc_ms`,
 `arc_overhead_ms` and `arc_nnm_ms`, `arc_nnm_overhead_ms`.
+`--gar-pre-aggregation bucketing --gar-bucket-size s` builds every rule for the n' = ceil(n / s) bucket means and compares it with the
+same rule on the n plain rows (`bucketing_ms`, `plain_ms`, `bucketing_overhead_ms`, `rule_rows`); a rule that refuses the n rows
+(e.g. SMEA at (32, 4)) is timed with bucketing only (`plain_refused`).
 `dnc` (divide-and-conquer) takes `--gar-rule-args iterations:<T> subsample:<b> c:<c> seed:<s>`; both engines draw the same samples (the
 step key is the update count), so the fused-vs-baseline check holds for it as for the other rules; its entry also reports the rows
 each engine kept in the checked step (`fused_mask`, `baseline_mask`, `masks_agree`).
@@ -63,9 +66,11 @@ def main():
                       help="`--aggregator-args` of every rule of --gar-rules (e.g. iterations:1 nu:1e-6 for geometric-median)")
   parser.add_argument("--gar-worker-momentum", dest="worker_momentum", type=float, default=None, metavar="BETA",
                       help="also time the worker-momentum kernel with this beta on the [w, d] rows of a rank")
-  parser.add_argument("--gar-pre-aggregation", dest="pre_aggregation", choices=("none", "nnm", "arc", "arc+nnm"), default="none",
+  parser.add_argument("--gar-pre-aggregation", dest="pre_aggregation", choices=("none", "nnm", "arc", "arc+nnm", "bucketing"), default="none",
                       help="pre-aggregation of both engines, with the rule's f (nnm: nearest-neighbour mixing, arc: adaptive robust clipping, "
-                           "arc+nnm: both); also times each rule without it")
+                           "arc+nnm: both; bucketing: means of buckets of --gar-bucket-size rows, the rule built for ceil(n / s) rows); "
+                           "also times each rule without it")
+  parser.add_argument("--gar-bucket-size", dest="bucket_size", type=int, default=2, help="rows per bucket s of --gar-pre-aggregation bucketing")
   args = parser.parse_args()
   world = int(os.environ.get("WORLD_SIZE", "1"))
   rank = int(os.environ.get("RANK", "0"))
@@ -115,12 +120,16 @@ def main():
   d = layout.padded_size
   w = n // world
   results = {}
+  bucketing = args.pre_aggregation == "bucketing"
+  rows = -(-n // args.bucket_size) if bucketing else n   # the rows every rule sees
   for rule in args.rules.split(","):
-    f = args.byz if args.byz is not None else 1 if rule == "bulyan" and n < 11 else 2
+    f = args.byz if args.byz is not None else 1 if rule == "bulyan" and rows < 11 else 2
     name = {"krum": "krum", "bulyan": "bulyan"}.get(rule, rule)
-    gar = aggregators.instantiate(name, n, f, args.rule_args or [])
+    gar = aggregators.instantiate(name, rows, f, args.rule_args or [])
     sgd = build(optimizers, "optimizer", "sgd", [])
     mix = dict(pre_aggregation=args.pre_aggregation, nb_decl_byz=f)
+    if bucketing:
+      mix.update(bucket_size=args.bucket_size, bucketing_seed=0)
     fused = FusedAggregation(gar, layout, n, sgd, device=device, keep_aggregate=True, **mix)
     base = BaselineAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, **mix)
     gen = torch.Generator(device=device).manual_seed(1234)
@@ -154,7 +163,7 @@ def main():
     mask_entry = {}
     if rule == "dnc":   # the rows each engine kept in the checked step (bit i: row i)
       fused_mask = int(fused.launcher.info[1].item()) & 0xffffffff
-      base_mask = int(gar_ops._launcher(base._gathered.device, n).info[1].item()) & 0xffffffff
+      base_mask = int(gar_ops._launcher(base._gathered.device, n, rows).info[1].item()) & 0xffffffff
       mask_entry = {"fused_mask": fused_mask, "baseline_mask": base_mask, "masks_agree": fused_mask == base_mask}
     gamma_entry = {}
     if attack is not None and attack.deviation is not None:
@@ -208,30 +217,44 @@ def main():
     if fused.mix is not None:
       # the same rule without the pre-aggregation on the same rows, alternated with the pre-aggregating engine round by round (clock and
       # thermal drift hit both); keys are prefixed by the pre-aggregation: nnm_ms, arc_ms, arc_nnm_ms, ...
-      plain = FusedAggregation(gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True)
-      plain.params.copy_(init)
-      plain.grads.copy_(fused.grads)
-      for _ in range(3):
-        craft(plain)
-        plain.step(0.1)
+      # with bucketing the plain arm is the same rule built for the n rows, which it may refuse (e.g. SMEA at (32, 4)): then only
+      # the bucketing arm is timed
+      try:
+        plain_gar = aggregators.instantiate(name, n, f, args.rule_args or []) if bucketing else gar
+        plain = FusedAggregation(plain_gar, layout, n, build(optimizers, "optimizer", "sgd", []), device=device, keep_aggregate=True)
+      except tools.UserException as err:
+        plain, plain_refused = None, str(err)
+      if plain is not None:
+        plain.params.copy_(init)
+        plain.grads.copy_(fused.grads)
+        for _ in range(3):
+          craft(plain)
+          plain.step(0.1)
       rounds = {"pre": [], "plain": []}
       for _ in range(5):
         rounds["pre"].append(time_engine(fused))
-        rounds["plain"].append(time_engine(plain))
-      median = lambda values: sorted(values)[len(values) // 2]
+        if plain is not None:
+          rounds["plain"].append(time_engine(plain))
+      median = lambda values: sorted(values)[len(values) // 2] if values else None
       pre_ms, plain_ms = median(rounds["pre"]), median(rounds["plain"])
       key = fused.mix.replace("+", "_")
-      slice_rows = n * (fused.hi - fused.lo) * 4
+      # bucketing stages only the rule's rows (its n' means), the other pre-aggregations all n rows
+      slice_rows = fused.spec.n * (fused.hi - fused.lo) * 4
       # local HBM bytes of the staged tile: the staging store; ARC's clip pass (read + write of its k rows); NNM's mix pass (read + write)
       # after its distance pass (a read of the tile when ARC staged it); the rule's read of the tile; and one more read for the distance
       # pass of the pre-aggregated rows (Krum / Bulyan / MDA / SMEA)
       k = _ops.arc_clip_count(n, f) if "arc" in fused.mix else 0
       tile_reads = 2 + (1 if rule in ("krum", "bulyan", "mda", "smea") else 0) + (2 if "nnm" in fused.mix else 0) + (1 if fused.mix == "arc+nnm" else 0)
-      mix_entry = {"pre_aggregation": fused.mix, key + "_ms": pre_ms, "plain_ms": plain_ms, key + "_overhead_ms": pre_ms - plain_ms,
+      mix_entry = {"pre_aggregation": fused.mix, key + "_ms": pre_ms, "plain_ms": plain_ms,
+                   key + "_overhead_ms": pre_ms - plain_ms if plain_ms is not None else None,
                    key + "_rounds_ms": rounds["pre"], "plain_rounds_ms": rounds["plain"],
                    key + "_tile_hbm_bytes": tile_reads * slice_rows + 2 * k * (fused.hi - fused.lo) * 4}
       if k:
         mix_entry["arc_clipped_rows"] = k
+      if bucketing:
+        mix_entry.update(bucket_size=args.bucket_size, rule_rows=rows)
+        if plain is None:
+          mix_entry["plain_refused"] = plain_refused
       del plain
     attack_entry = {}
     if attack is not None:
