@@ -1016,11 +1016,12 @@ def host_smea(G, f, return_details=False):
 
 OPTIMIZED_MODES = ("min-max", "min-sum")   # Shejwalkar & Houmansadr, NDSS 2021: gamma solved from whole-vector sums
 DEVIATIONS = ("unit-vec", "sign", "std")
+MIMIC_WARMUP = 100   # default number of warm-up steps T0 of mimic
 
 
 def check_byzantine_slots(n, byz_slots, mode):
   """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("ipm" needs 1 honest row, the others 2)."""
-  if mode not in ("alie", "ipm") + OPTIMIZED_MODES:
+  if mode not in ("alie", "ipm", "mimic") + OPTIMIZED_MODES:
     raise tools.UserException("Unknown omniscient attack mode " + repr(mode))
   slots = sorted({int(i) for i in byz_slots})
   if not slots or slots[0] < 0 or slots[-1] >= n:
@@ -1164,6 +1165,85 @@ def torch_craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return
     row = torch_byzantine_row(G, byz_slots, mode, coef)
   for i in check_byzantine_slots(G.shape[0], byz_slots, mode):
     G[i].copy_(row)
+  return details if return_details else G
+
+
+def check_mimic(n, byz_slots, warmup):
+  """-> (ascending Byzantine slots, T0) of mimic: at least 2 honest rows, an integer warm-up T0 >= 1 (below 2^24, so that the kernel's fp32
+  t is exact)."""
+  slots = check_byzantine_slots(n, byz_slots, "mimic")
+  if isinstance(warmup, bool) or not isinstance(warmup, int) or not 1 <= warmup < 1 << 24:
+    raise tools.UserException("mimic: the warm-up must be an integer in [1, 2^24) (got %r)" % (warmup,))
+  return slots, warmup
+
+
+def mimic_state(d, device="cpu", mask=None, real=None):
+  """The state of mimic before its first step over [d] rows whose real coordinates are `mask` (a [d] bool tensor; None: all of them):
+  t = 0, z = the fp32 of 1 / sqrt(real) on the real coordinates and 0 on the others, i* = -1 (no target yet: the first honest slot).
+  `real` defaults to the number of real coordinates; a state that holds only some of the coordinates passes the total."""
+  if real is None:
+    real = d if mask is None else int(mask.sum())
+  if real < 1:
+    raise tools.UserException("mimic needs at least one real coordinate")
+  z = torch.zeros(d, dtype=torch.float32, device=device)
+  value = fp32(1.0 / math.sqrt(real))
+  if mask is None:
+    z.fill_(value)
+  else:
+    z[mask.to(device)] = value
+  return {"t": 0, "z": z, "istar": torch.full((1,), -1, dtype=torch.int32, device=device)}
+
+
+def mimic_target(istar, honest):
+  """The slot i* designates among the ascending `honest` slots: itself when it is one, the first honest slot otherwise."""
+  return istar if istar in honest else honest[0]
+
+
+def torch_mimic_step_(G, byz_slots, state, warmup, return_details=False):
+  """Mimic (Karimireddy, He & Jaggi, ICLR 2022) on the [n, d] fp32 matrix G, in place: every Byzantine row <- the honest row h_{i*}.
+  While state["t"] < warmup, one update of the online power iteration first, on the honest rows h (ascending slots, H of them):
+  mu = `_honest_mean`, s_i = sum_j (h_i - mu)_j z_j, u = (s_0 (h_0 - mu) + s_1 (h_1 - mu) + ...) / H, y = (t z + u) / (t + 1) (fp32, one
+  rounded operation at a time), then, unless ||y||^2 is 0 or not finite, z <- y * (1 / ||y||) and i* <- argmax_i q_i, q_i = sum_j h_i,j y_j
+  (ties: lower slot; non-finite q never wins; none finite: the first honest slot); t <- t + 1 in every case. The whole-vector sums are
+  float64 sums of the fp32 values; s_i and 1 / ||y|| are rounded once to fp32. `state` (`mimic_state`) is updated in place. With
+  `return_details`, returns (s, q, ||y||^2, 1 / ||y||) of the warm-up update (None after the warm-up) instead of G."""
+  if G.dtype != torch.float32:
+    raise tools.UserException("Omniscient attacks craft fp32 rows (got %s)" % G.dtype)
+  n = G.shape[0]
+  slots, warmup = check_mimic(n, byz_slots, warmup)
+  honest_ids = [i for i in range(n) if i not in set(slots)]
+  details = None
+  t = int(state["t"])
+  if t < warmup:
+    honest = [G[i] for i in honest_ids]
+    scalar = _scalar(G)
+    mu = _honest_mean(honest, scalar)
+    devs = [h - mu for h in honest]
+    z = state["z"]
+    z64 = z.double()
+    s = [fp32(float((dev.double() * z64).sum())) for dev in devs]
+    acc = None
+    for si, dev in zip(s, devs):
+      term = scalar(si) * dev
+      acc = term if acc is None else acc + term
+    y = (scalar(float(t)) * z + acc / scalar(len(honest))) / scalar(float(t + 1))
+    y64 = y.double()
+    norm2 = float((y64 * y64).sum())
+    q = [float((h.double() * y64).sum()) for h in honest]
+    inv = 0.0
+    if norm2 > 0 and math.isfinite(norm2):
+      inv = fp32(1.0 / math.sqrt(norm2))
+      z.copy_(y * scalar(inv))
+      best = None
+      for k, value in enumerate(q):
+        if math.isfinite(value) and (best is None or value > q[best]):
+          best = k
+      state["istar"].fill_(honest_ids[0 if best is None else best])
+    state["t"] = t + 1
+    details = (s, q, norm2, inv)
+  target = mimic_target(int(state["istar"][0]), honest_ids)
+  for i in slots:
+    G[i].copy_(G[target])
   return details if return_details else G
 
 

@@ -10,6 +10,12 @@
           keeps b inside the spread of the honest rows: Min-Max bounds max_i ||b - h_i||^2 by the largest honest distance
           max_jk ||h_j - h_k||^2, Min-Sum bounds sum_i ||b - h_i||^2 by max_i sum_j ||h_i - h_j||^2. gamma is solved in closed form
           (`aggregators._ops.optimized_gamma`) instead of the authors' search, and is not capped (their search stays below 20).
+* `mimic` (Karimireddy, He & Jaggi, "Byzantine-Robust Learning on Heterogeneous Datasets via Bucketing", ICLR 2022): every Byzantine
+          row is a copy of one honest row h_{i*}, which over-weights that worker's data without sending any outlier. During the first
+          `warmup` steps (T0, default 100) i* follows the honest row furthest along the top principal direction of the honest rows,
+          estimated by an online power iteration; then i* is frozen. It does nothing under IID data and is the standard test of the
+          heterogeneity defences (bucketing, NNM) under non-IID data (`dirichlet:<alpha>`). The arithmetic is
+          `aggregators._ops.torch_mimic_step_`; the engine keeps the state (z, t, i*) and checkpoints it.
 
 The rows are crafted by the aggregation engine (`craft_byzantine`), not per worker: on the fused engine every rank computes its owned
 coordinates of every Byzantine row from the honest values it already reads for the rule, and stores them into the Byzantine rows over
@@ -106,7 +112,29 @@ class MinSumAttack(_OptimizedAttack):
   mode = "min-sum"
 
 
+class MimicAttack(_Omniscient):
+  """Mimic: no coefficient, only the warm-up length T0 (`warmup:<T0>`, an integer >= 1)."""
+  mode = "mimic"
+  min_honest = 2
+
+  def __init__(self, nbworkers, nbbyzwrks, args):
+    super().__init__(nbworkers, nbbyzwrks, args)
+    from ..aggregators import _ops
+    unknown = set(self.args) - {"warmup"}
+    if unknown:
+      raise tools.UserException("mimic: unknown argument(s) %s (expected 'warmup:<steps>')" % ", ".join(sorted(unknown)))
+    warmup = _ops.MIMIC_WARMUP
+    if "warmup" in self.args:
+      try:
+        warmup = int(self.args["warmup"])
+      except ValueError:
+        raise tools.UserException("mimic: 'warmup' expects an integer >= 1 (got %r)" % (self.args["warmup"],))
+    self.warmup = _ops.check_mimic(nbworkers, range(nbworkers - nbbyzwrks, nbworkers), warmup)[1]
+    self.coef = None
+
+
 register("alie", AlieAttack)
 register("ipm", IpmAttack)
 register("min-max", MinMaxAttack)
 register("min-sum", MinSumAttack)
+register("mimic", MimicAttack)

@@ -186,6 +186,8 @@ class Manager:
     self.attack = attack
     self.byzantine = set(range(nbworkers - nb_real_byz, nbworkers)) if (attack is not None and nb_real_byz > 0) else set()
     self._attack_state = {i: {} for i in self.byzantine}
+    if self.byzantine and getattr(attack, "mode", None) == "mimic":   # created now, so that a restored checkpoint finds it
+      self.aggregation.mimic_state()
     # rows in the gathered matrix (slots) of the Byzantine workers, as the aggregation engines address them
     self.byzantine_slots = sorted(placement[i][0] * self.w + placement[i][1] for i in self.byzantine)
     # -- gradient authentication (opt-in; reference: signed worker -> PS messages of the hardened transport) -- #
@@ -391,6 +393,8 @@ class Manager:
       if self.byzantine_slots:   # collective: every rank crafts its share, whether or not it hosts a Byzantine worker
         deviation = getattr(self.attack, "deviation", None)   # Min-Max / Min-Sum only: other engines' signatures stay as they were
         extra = {} if deviation is None else {"deviation": deviation}
+        if getattr(self.attack, "warmup", None) is not None:   # mimic only
+          extra["warmup"] = self.attack.warmup
         self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef, **extra)
       return losses
     forging = self.authenticator is not None and getattr(self.attack, "forges", False)

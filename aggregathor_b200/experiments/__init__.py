@@ -40,6 +40,34 @@ class _Experiment:
   def eval_batch(self, device):
     raise NotImplementedError
 
+  def _check_dirichlet(self):
+    """Validates `dirichlet:<alpha>` in `self.args` (absent: the IID streams of every worker are unchanged)."""
+    if "dirichlet" not in self.args:
+      return
+    from ._data import check_dirichlet
+    self.args["dirichlet"] = check_dirichlet(self.args["dirichlet"])
+    if self.args.get("shared-batch"):
+      raise tools.UserException("dirichlet gives every worker its own part of the data: it cannot be combined with shared-batch:1")
+
+  def _dirichlet_indices(self, data, worker, nbworkers, labels=None):
+    """The training samples of `worker` under `dirichlet:<alpha>` (None without it): its part of `_data.dirichlet_partition` of
+    `data.train_labels()` (a streamed dataset's labels are read from its shards), drawn from the experiment's seed with the per-worker
+    batch size as the least part, the same on every rank. Logs its size and the classes of `labels` (default: the training labels), the
+    array the worker's stream serves."""
+    alpha = self.args.get("dirichlet")
+    if alpha is None:
+      return None
+    import numpy as np
+    from ._data import dirichlet_partition
+    parts = self.__dict__.setdefault("_dirichlet_parts", {})
+    if nbworkers not in parts:
+      parts[nbworkers] = dirichlet_partition(data.train_labels(), nbworkers, alpha, self.args["seed"], self.args["batch-size"])
+    part = parts[nbworkers][worker]
+    labels = data.train_labels() if labels is None else labels
+    tools.info("Worker %d: %d training samples of %d classes (Dirichlet alpha = %g)" % (worker, len(part), len(np.unique(labels[part])), alpha),
+               context="dirichlet")
+    return part
+
   def preprocess(self, inputs, ctx, training):
     """Device-side conversion of a raw input batch into the model's activation format."""
     return inputs.to(ctx.dtype)

@@ -163,12 +163,28 @@ class Dataset:
     self.x_test = self._render(self.y_test, rng)
     self.train_count = ntrain
 
-  def train_stream(self, batch_size, device, seed=0, transform=None, readers=1, part=0, parts=1):
+  def train_stream(self, batch_size, device, seed=0, transform=None, readers=1, part=0, parts=1, indices=None):
     """The training input pipeline of one worker: in-memory `BatchStream`, or the native shard reader when the dataset is streamed
-    (`readers` = reader threads, the reference's `nb-fetcher-threads`; `part`/`parts` give each worker a disjoint residue class)."""
+    (`readers` = reader threads, the reference's `nb-fetcher-threads`; `part`/`parts` give each worker a disjoint residue class).
+    `indices`: the worker's own training samples (a `dirichlet_partition` part of `train_labels()`), which replace `part`/`parts`."""
     if self.streaming:
-      return ShardStream(self.train_shards, batch_size, device, seed=seed, transform=transform, readers=readers, part=part, parts=parts)
-    return BatchStream(self.x_train, self.y_train, batch_size, device, seed=seed, transform=transform)
+      return ShardStream(self.train_shards, batch_size, device, seed=seed, transform=transform, readers=readers, part=part, parts=parts, subset=indices)
+    return BatchStream(self.x_train, self.y_train, batch_size, device, seed=seed, transform=transform, indices=indices)
+
+  def train_labels(self):
+    """The labels of the training set by global record index: in memory, or read from the label section of every shard, in the sorted
+    order of the shard files (no image is read)."""
+    if not self.streaming:
+      return self.y_train
+    if getattr(self, "_shard_labels", None) is None:
+      parts = []
+      for path in self.train_shards:
+        header = read_shard_header(path)
+        with open(path, "rb") as fd:
+          fd.seek(64 + header["count"] * header["record_bytes"])
+          parts.append(np.frombuffer(fd.read(header["count"] * 8), dtype=np.int64))
+      self._shard_labels = np.concatenate(parts)
+    return self._shard_labels
 
   def _render(self, labels, rng):
     h, w, c = self.shape
@@ -225,16 +241,59 @@ def _take(self):
   return item
 
 
-class BatchStream:
-  """Infinite shuffled batch iterator with pinned double buffering and asynchronous H2D copies."""
+DIRICHLET_TAG = 0x4449524C   # "DIRL": second word of the partition's generator seed
+DIRICHLET_ATTEMPTS = 100
 
-  def __init__(self, images, labels, batch_size, device, seed=0, shuffle=True, depth=2, transform=None):
+
+def check_dirichlet(alpha):
+  """The concentration of `dirichlet:<alpha>`: a finite float > 0."""
+  try:
+    value = float(alpha)
+  except (TypeError, ValueError):
+    raise tools.UserException("dirichlet: expected a number (got %r)" % (alpha,))
+  if not np.isfinite(value) or value <= 0:
+    raise tools.UserException("dirichlet: alpha must be finite and > 0 (got %r)" % (alpha,))
+  return value
+
+
+def dirichlet_partition(labels, n, alpha, seed, min_size):
+  """Label-skewed split of a training set over n workers (Hsu, Qi & Brown, 2019): n sorted, disjoint int64 index arrays whose union is
+  every sample. With rng = numpy's default_rng([seed, DIRICHLET_TAG]), for each class c in ascending order: the ascending indices of class
+  c are permuted by rng.permutation, p = rng.dirichlet([alpha] * n) is drawn and the permuted indices are cut at floor(cumsum(p)[:-1] *
+  count); worker i gets slice i. While a worker gets fewer than `min_size` samples, the whole partition is drawn again from the same rng,
+  at most DIRICHLET_ATTEMPTS times in all. Small alpha concentrates every class on few workers; large alpha approaches an IID split."""
+  labels = np.asarray(labels).reshape(-1)
+  n, alpha, min_size = int(n), check_dirichlet(alpha), int(min_size)
+  if n < 1:
+    raise tools.UserException("dirichlet: needs at least one worker (got %d)" % n)
+  rng = np.random.default_rng([int(seed), DIRICHLET_TAG])
+  classes = np.unique(labels)
+  for _ in range(DIRICHLET_ATTEMPTS):
+    parts = [[] for _ in range(n)]
+    for c in classes:
+      members = rng.permutation(np.flatnonzero(labels == c))
+      p = rng.dirichlet([alpha] * n)
+      cuts = np.floor(np.cumsum(p)[:-1] * len(members)).astype(np.int64)
+      for i, piece in enumerate(np.split(members, cuts)):
+        parts[i].append(piece)
+    parts = [np.sort(np.concatenate(piece)).astype(np.int64) for piece in parts]
+    if min(len(part) for part in parts) >= min_size:
+      return parts
+  raise tools.UserException("dirichlet: no partition of the %d samples over n = %d workers with alpha = %g gives every worker a batch of %d "
+                            "samples in %d draws" % (len(labels), n, alpha, min_size, DIRICHLET_ATTEMPTS))
+
+
+class BatchStream:
+  """Infinite shuffled batch iterator with pinned double buffering and asynchronous H2D copies. `indices` (optional) restricts the stream
+  to those samples (its order before the first shuffle replaces `arange(len(labels))`); no image is copied."""
+
+  def __init__(self, images, labels, batch_size, device, seed=0, shuffle=True, depth=2, transform=None, indices=None):
     self.images, self.labels, self.batch = images, labels, int(batch_size)
     self.device = _indexed(device)
     self.shuffle, self.transform = shuffle, transform
     self._rng = np.random.default_rng(seed)
-    self._order = np.arange(len(labels))
-    self._cursor = len(labels)  # forces a shuffle at first use
+    self._order = np.arange(len(labels)) if indices is None else np.array(indices, dtype=np.int64)
+    self._cursor = len(self._order)  # forces a shuffle at first use
     self._cuda = self.device.type == "cuda"
     self._depth = depth
     self._queue = None
@@ -405,18 +464,32 @@ class StreamGroup:
 class ShardStream(BatchStream):
   """`BatchStream` fed by the native streaming reader (`native/py_loader`): nothing but the pinned ring lives in host memory."""
 
-  def __init__(self, paths, batch_size, device, seed=0, shuffle=True, depth=2, transform=None, readers=1, part=0, parts=1, pool=0, min_after_dequeue=-1):
+  def __init__(self, paths, batch_size, device, seed=0, shuffle=True, depth=2, transform=None, readers=1, part=0, parts=1, pool=0, min_after_dequeue=-1,
+               subset=None):
+    """`subset`: the global record indices (shards in the order of `paths`, then records) this stream serves instead of `part`/`parts`."""
     from .. import native
     self._lib = native.library("py_loader")
     lib = self._lib
     lib.agb_loader_open.restype = ctypes.c_void_p
+    lib.agb_loader_open_subset.restype = ctypes.c_void_p
     lib.agb_loader_last_error.restype = ctypes.c_char_p
     lib.agb_loader_next.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     lib.agb_loader_info.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     lib.agb_loader_close.argtypes = [ctypes.c_void_p]
     names = (ctypes.c_char_p * len(paths))(*[str(p).encode() for p in paths])
-    self._handle = lib.agb_loader_open(names, ctypes.c_int(len(paths)), ctypes.c_int(int(batch_size)), ctypes.c_int(max(1, int(readers))), ctypes.c_ulonglong(seed & (2 ** 64 - 1)),
-                                       ctypes.c_int(1 if shuffle else 0), ctypes.c_longlong(pool), ctypes.c_longlong(min_after_dequeue), ctypes.c_int(part), ctypes.c_int(parts))
+    common = (names, ctypes.c_int(len(paths)), ctypes.c_int(int(batch_size)), ctypes.c_int(max(1, int(readers))), ctypes.c_ulonglong(seed & (2 ** 64 - 1)),
+              ctypes.c_int(1 if shuffle else 0), ctypes.c_longlong(pool), ctypes.c_longlong(min_after_dequeue))
+    if subset is None:
+      self._handle = lib.agb_loader_open(*common, ctypes.c_int(part), ctypes.c_int(parts))
+    else:
+      records = sum(read_shard_header(p)["count"] for p in paths)
+      subset = np.asarray(subset, dtype=np.int64)
+      if subset.size and (subset.min() < 0 or subset.max() >= records):
+        raise tools.UserException("Shard subset indices must lie in [0, %d)" % records)
+      member = np.zeros(-(-records // 64) * 64, dtype=bool)
+      member[subset] = True
+      bitmap = np.packbits(member.reshape(-1, 64)[:, ::-1], axis=1).view(">u8").astype(np.uint64).reshape(-1)
+      self._handle = lib.agb_loader_open_subset(*common, bitmap.ctypes.data_as(ctypes.c_void_p), ctypes.c_ulonglong(records))
     if not self._handle:
       raise tools.UserException("Cannot open the dataset shards: " + lib.agb_loader_last_error().decode())
     info = (ctypes.c_ulonglong * 6)()

@@ -1,7 +1,8 @@
 """`cnnet`: small CNN on CIFAR-10 (reference: `experiments/cnnet.py:54-196`).
 
 Args: `batch-size:32`, `eval-batch-size:1024`, `nb-fetcher-threads` (reader threads when CIFAR-10 is streamed from shards),
-`nb-batcher-threads` (accepted), `preprocessing:cifarnet`. Each worker dequeues its own batches.
+`nb-batcher-threads` (accepted), `preprocessing:cifarnet`, `dirichlet:<alpha>` (optional: every worker draws from its own label-skewed
+part of the training set, `_data.dirichlet_partition`, also when CIFAR-10 is streamed). Each worker dequeues its own batches.
 slim's `cifarnet` preprocessing runs on the device in one kernel (`ops/preprocess.py`): training = zero-pad 4 + random 32x32 crop +
 mirror + random brightness (63) + random contrast [0.2, 1.8] + per-image standardisation, evaluation = standardisation; its random
 draws come from a device-resident counter, so the training step stays CUDA-graph replayable.
@@ -36,6 +37,7 @@ class CNNetExperiment(_Experiment):
     self.data = Dataset("cifar10", synthetic_limit=8192)
     if self.data.synthetic:
       tools.warning("CIFAR-10 files not found: using the synthetic CIFAR-10-shaped dataset", context="cnnet")
+    self._check_dirichlet()
     self._streams = {}
     from ..ops.preprocess import Preprocessor
     self.preprocessor = Preprocessor("cifarnet", 32, pad=4, seed=self.args["seed"])
@@ -47,7 +49,7 @@ class CNNetExperiment(_Experiment):
   def train_stream(self, worker, nbworkers, device):
     if worker not in self._streams:
       self._streams[worker] = self.data.train_stream(self.args["batch-size"], device, seed=self.args["seed"] + worker, readers=self.args["nb-fetcher-threads"],
-                                                     part=worker, parts=nbworkers)
+                                                     part=worker, parts=nbworkers, indices=self._dirichlet_indices(self.data, worker, nbworkers))
     return self._streams[worker]
 
   def eval_batch(self, device):

@@ -2,7 +2,8 @@
 
 Args: `batch-size:32` (per worker), `shared-batch:0` (1 = every worker gets the *same* batch each step, the
 behaviour of the reference where one iterator's `get_next()` is shared by all replicas, `mnist.py:76-81,124`),
-`eval-batch-size:0` (0 = the whole test set in one batch, as the reference). Pixels are scaled to [0, 1].
+`eval-batch-size:0` (0 = the whole test set in one batch, as the reference), `dirichlet:<alpha>` (optional: every worker draws from its
+own label-skewed part of the training set, `_data.dirichlet_partition`; not with `shared-batch:1`). Pixels are scaled to [0, 1].
 """
 
 import torch
@@ -25,6 +26,7 @@ class MNIST(_Experiment):
       self.data = Dataset(self.dataset_name, synthetic_limit=16384)
       if self.data.synthetic:
         tools.warning("MNIST files not found: using the synthetic MNIST-shaped dataset")
+    self._check_dirichlet()
     self._streams = {}
 
   def model(self):
@@ -39,7 +41,8 @@ class MNIST(_Experiment):
       # `shared-batch:1` (the reference's quirk, `experiments/mnist.py:76-81,124`): every worker draws THE SAME batch each step — one
       # stream object per worker (a shared iterator would hand consecutive, i.e. different, batches to the workers), all seeded alike
       seed = self.args["seed"] + (0 if self.args["shared-batch"] else worker)
-      self._streams[worker] = BatchStream(images, labels, self.args["batch-size"], device, seed=seed)
+      self._streams[worker] = BatchStream(images, labels, self.args["batch-size"], device, seed=seed,
+                                          indices=self._dirichlet_indices(self.data, worker, nbworkers, labels))
     return self._streams[worker]
 
   def eval_batch(self, device):

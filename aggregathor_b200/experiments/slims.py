@@ -4,7 +4,8 @@
 Args: `batch-size:32`, `eval-batch-size:1024`, `weight-decay:4e-5` (accepted; as in the reference the
 regularisation losses are *not* added to the training loss, `slims.py:122-125`), `label-smoothing:0`,
 `labels-offset:0`, `preprocessing:<model default>`, `image-size:<model default>`, `augment:slim|none|flip|crop-flip`,
-`nb-fetcher-threads` (reader threads of a streamed dataset). Loss = softmax cross-entropy on one-hot labels (+ label smoothing).
+`nb-fetcher-threads` (reader threads of a streamed dataset), `dirichlet:<alpha>` (optional: every worker draws from its own label-skewed part
+of the training set, `_data.dirichlet_partition`; a streamed dataset reads only that part's records). Loss = softmax cross-entropy on one-hot labels (+ label smoothing).
 Images are uint8 NHWC on the host at their storage resolution; preprocessing runs on the device in one kernel
 (`ops/preprocess.py`): with `augment:slim` (default for real datasets) the model's slim preprocessing — `vgg`: aspect-preserving
 resize to a random side in [256, 512] + random crop + mirror + mean subtraction, evaluation = resize 256 + central crop;
@@ -51,6 +52,7 @@ class SlimExperiment(_Experiment):
       print("Model name in use:     " + repr(model))
     self.data = Dataset(dataset, image_size=self.args["image-size"], synthetic_limit=self.args["synthetic-samples"])
     self.num_classes = self.data.classes - self.args["labels-offset"]
+    self._check_dirichlet()
     self._streams = {}
     if self.args["augment"] == "auto":
       self.args["augment"] = "none" if self.data.synthetic else "slim"
@@ -82,7 +84,8 @@ class SlimExperiment(_Experiment):
   def train_stream(self, worker, nbworkers, device):
     if worker not in self._streams:
       self._streams[worker] = self.data.train_stream(self.args["batch-size"], device, seed=self.args["seed"] + worker, transform=self._offset,
-                                                     readers=self.args["nb-fetcher-threads"], part=worker, parts=nbworkers)
+                                                     readers=self.args["nb-fetcher-threads"], part=worker, parts=nbworkers,
+                                                     indices=self._dirichlet_indices(self.data, worker, nbworkers))
     return self._streams[worker]
 
   def eval_batch(self, device):

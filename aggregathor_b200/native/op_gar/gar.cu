@@ -27,7 +27,8 @@
 // reads n rows (see `bucketing_pre_aggregation`). Its "buckets" are sets of rows, not the gradient buckets (coordinate segments) above.
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
-// whole-vector sums between the ranks, then the same per-coordinate write.
+// whole-vector sums between the ranks, then the same per-coordinate write. Mimic runs `gar_mimic_warmup_kernel` (two exchanges) during
+// its warm-up and `gar_mimic_copy_kernel` after it.
 // DnC (rule kDnc) has a finish kernel of its own, `gar_dnc_kernel`: a sampled distance pass, one exchange, a float64 Jacobi per CTA,
 // then Krum's phase D (see `dnc_selection`).
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
@@ -61,13 +62,18 @@ constexpr int kSlotMix = kSlotGeoMedian + kMaxIterations;   // NNM: exchange of 
 constexpr int kSlotCraftStats = kSlotMix + 1;   // Min-Max / Min-Sum: exchange of the crafting statistics
 constexpr int kSlotDnc = kSlotCraftStats + 1;   // DnC: exchange of the sampled distances
 constexpr int kSlotArc = kSlotDnc + 1;   // ARC: exchange of the squared row norms
-constexpr int kFlagSlots = kSlotArc + 1;
+constexpr int kSlotMimic = kSlotArc + 1;   // mimic: second exchange of a warm-up step (the first one signals on kSlotCraftStats)
+constexpr int kFlagSlots = kSlotMimic + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 // Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
 // They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
 constexpr int kStatA = kMaxPairs, kStatB = kStatA + kMaxWorkers, kStatC = kStatB + kMaxWorkers;
 constexpr int kCraftStats = kStatC + 1;   // 561
 constexpr int kCraftRegion = 2 * kMailboxRegion;
+// mimic's posts in the same region 2 (one rank's kCraftStats floats): exchange 1 the s_i at [kMimicS, +32), exchange 2 the q_i at
+// [kMimicQ, +32) and ||y||^2 at [kMimicY]; its `stats_out` (float64) adds 1 / ||y|| at [kMimicY + 1]
+constexpr int kMimicS = 0, kMimicQ = kMaxWorkers, kMimicY = 2 * kMaxWorkers;
+constexpr int kMimicStats = kMimicY + 2;
 constexpr int kDncIterations = 8;         // DnC: iterations T in [1, kDncIterations]
 constexpr int kDncStride = kDncIterations * kMaxPairs + 1;   // DnC post of one rank: T x [kMaxPairs] sampled distances, then the loss
 constexpr int kDncRegion = kCraftRegion + kMaxRanks * kCraftStats;   // mailbox region 3: kMaxRanks x kDncStride floats
@@ -2305,6 +2311,13 @@ struct ByzArgs {
     float* mailbox[kMaxRanks];         // every rank's mailbox; region 2 (float offset kCraftRegion) carries the statistics
     float* partials;                   // [grid][kCraftStats] CTA partials of this rank
     float* stats_out;                  // optional [1 + kCraftStats]: gamma, then the statistics summed over the ranks
+    // mimic only (`gar_mimic_warmup_kernel`, `gar_mimic_copy_kernel`)
+    unsigned honest_mask;
+    int t;                             // warm-up updates done before this one
+    float* z;                          // (local) direction estimate of the owned coordinates, segments back to back (as the staged tile)
+    float* y;                          // (local) scratch, same layout: y, kept apart so that z survives a degenerate ||y||
+    int* istar;                        // [1] (local) target slot i*; a value that is no honest slot (-1 before any update) means the first one
+    double* mimic_stats;               // optional [kMimicStats]: s_i, q_i, ||y||^2, 1 / ||y|| of the last warm-up step
 };
 enum ByzMode { kAlie = 0, kIpm = 1, kMinMax = 2, kMinSum = 3 };
 enum Deviation { kUnitVec = 0, kSign = 1, kStd = 2 };
@@ -2665,6 +2678,302 @@ __global__ void __launch_bounds__(256) gar_optimized_kernel(ByzArgs const a) {
     fence_sys();
 }
 
+// ---- mimic (Karimireddy, He & Jaggi, ICLR 2022) ------------------------------------------------ //
+// Every Byzantine row is a bit-for-bit copy of one honest row h_{i*}. During the T0 warm-up steps, i* follows the honest row that reaches
+// furthest along the top principal direction z of the honest rows, estimated by the online power iteration of the paper's appendix:
+//   mu = ((h_0 + h_1) + ...) / H, s_i = sum_j (h_i - mu)_j z_j,
+//   u = (s_0 (h_0 - mu) + s_1 (h_1 - mu) + ...) / H, y = (t z + u) / (t + 1)   (fp32, one rounded operation at a time),
+//   z <- y * (1 / ||y||), i* = argmax_i q_i with q_i = sum_j h_i,j y_j (ties: lower slot; non-finite q never wins; none finite: the first
+//   honest slot); when ||y||^2 is 0 or not finite, z and i* keep their values.
+// The whole-vector sums are fp32 partials per thread (FMA), folded lanes -> warps -> CTA (`fold_pass`) -> CTAs in index order, posted
+// per rank and added over the ranks in rank order in float64; s_i and 1 / ||y|| are rounded once to fp32, every rank gets the same bits.
+//
+// Warm-up: one cooperative launch per rank (`gar_mimic_warmup_kernel`):
+//   1. entry barrier (slot kSlotCraft), as for ALIE / IPM;
+//   2. pass 1 over the owned segments: the s_i partials (H <= 8: the honest values in registers; above, 8-row blocks, mu recomputed);
+//   3. exchange 1: region 2 floats [kMimicS, +32), slot kSlotCraftStats;
+//   4. pass 2: mu and u recomputed, y stored into the y scratch, ||y||^2 and q_i partials;
+//   5. exchange 2: region 2 floats [kMimicQ, kMimicY], slot kSlotMimic;
+//   6. pass 3: z <- y / ||y|| on the owned coordinates, h_{i*} copied into every Byzantine row (P2P stores); block 0 stores i* and the
+//      statistics.
+// After the warm-up, `gar_mimic_copy_kernel` copies h_{i*}, with i* read from device memory: no exchange, no host read-back.
+// Both end with a system-scope fence and no exit barrier, as `gar_byzantine_kernel` (same argument). Within a step the two posts are
+// disjoint floats of region 2, so a fast rank's second post never overwrites a first post a slow rank is still adding; a rank's next
+// post comes after the next entry barrier, i.e. after every rank has finished this kernel (same stream). Region 2 is Min-Max's, and an
+// engine runs one attack.
+
+// the slot i* designates: itself when it is an honest slot, the first honest slot otherwise
+__device__ __forceinline__ int mimic_target(ByzArgs const& a, int istar) {
+    return istar >= 0 && istar < kMaxWorkers && ((a.honest_mask >> istar) & 1u) ? istar : a.honest[0];
+}
+
+// the 4 values of honest row i (ascending honest index) at x: from the registers (N > 0) or from memory
+template<int N>
+__device__ __forceinline__ void honest_value(ByzArgs const& a, long long x, float const (&g)[N > 0 ? N : 1][4], int i, float (&h)[4]) {
+    if constexpr (N > 0) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            h[c] = g[i][c];
+    } else {
+        V<4>::load(a.rows[a.honest[i]] + x, h);
+    }
+}
+
+// pass 1: the s_i partials of the honest rows [i0, i0 + 8) over every owned segment, folded into `out`
+template<int N>
+__device__ void mimic_s_pass(ByzArgs const& a, Shared& sh, int* pair_of, int i0, float* out, long long tid, long long nthreads) {
+    constexpr int B = kBlockRows;
+    static_assert(N == 0 || N == B, "registers hold one block of honest rows");
+    int const H = a.H;
+    if (threadIdx.x < B)
+        pair_of[threadIdx.x] = i0 + static_cast<int>(threadIdx.x) < H ? kMimicS + i0 + static_cast<int>(threadIdx.x) : -1;
+    __syncthreads();
+    float acc[B];
+#pragma unroll
+    for (int k = 0; k < B; ++k)
+        acc[k] = 0.f;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4, soff = staged_offset(a, seg);   // z, y: owned order
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4], z[4];
+            mean_and_deviation<N>(a, x, g, mu, p);
+            V<4>::load(a.z + soff + v * 4, z);
+#pragma unroll
+            for (int i = 0; i < B; ++i) {
+                if (i0 + i < H) {
+                    float h[4];
+                    honest_value<N>(a, x, g, N > 0 ? i : i0 + i, h);   // N > 0: one block, i0 == 0, a static register index
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        acc[i] = __fmaf_rn(__fsub_rn(h[c], mu[c]), z[c], acc[i]);
+                }
+            }
+        }
+    }
+    fold_pass<B>(sh, acc, out, pair_of);
+}
+
+// pass 2: y = (t z + u) / (t + 1) into the y scratch, and the partials of q_i and ||y||^2, folded into `out`
+template<int N>
+__device__ void mimic_y_pass(ByzArgs const& a, Shared& sh, int* pair_of, float const* s, float* out, long long tid, long long nthreads) {
+    constexpr int M = N > 0 ? N : kMaxWorkers, COUNT = M + 1;
+    int const H = a.H;
+    if (threadIdx.x < COUNT) {
+        int const k = threadIdx.x;
+        pair_of[k] = k == M ? kMimicY : k < H ? kMimicQ + k : -1;
+    }
+    __syncthreads();
+    float const tf = static_cast<float>(a.t), t1 = static_cast<float>(a.t + 1), count = static_cast<float>(H);
+    float acc[COUNT];
+#pragma unroll
+    for (int k = 0; k < COUNT; ++k)
+        acc[k] = 0.f;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4, soff = staged_offset(a, seg);   // z, y: owned order
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4], z[4], u[4], y[4];
+            mean_and_deviation<N>(a, x, g, mu, p);
+            V<4>::load(a.z + soff + v * 4, z);
+#pragma unroll
+            for (int i = 0; i < M; ++i) {
+                if (i < H) {
+                    float h[4];
+                    honest_value<N>(a, x, g, i, h);
+                    float const si = s[i];
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        float const term = __fmul_rn(si, __fsub_rn(h[c], mu[c]));
+                        u[c] = i == 0 ? term : __fadd_rn(u[c], term);
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                y[c] = __fdiv_rn(__fadd_rn(__fmul_rn(tf, z[c]), __fdiv_rn(u[c], count)), t1);
+                acc[M] = __fmaf_rn(y[c], y[c], acc[M]);
+            }
+            V<4>::store(a.y + soff + v * 4, y);
+#pragma unroll
+            for (int i = 0; i < M; ++i) {
+                if (i < H) {
+                    float h[4];
+                    honest_value<N>(a, x, g, i, h);
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        acc[i] = __fmaf_rn(h[c], y[c], acc[i]);
+                }
+            }
+        }
+    }
+    fold_pass<COUNT>(sh, acc, out, pair_of);
+}
+
+// block 0 adds the CTA partials [lo, hi) in index order and posts them into region 2 of every rank, then signals `slot`; returns once
+// every rank's post is visible to every CTA
+__device__ void mimic_exchange(ByzArgs const& a, cg::grid_group& grid, int lo, int hi, int slot, uint32_t epoch) {
+    bool const multi = a.R > 1;
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int k = lo + threadIdx.x; k < hi; k += blockDim.x) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.partials + static_cast<long long>(b) * kCraftStats + k);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kCraftRegion + a.rank * kCraftStats + k] = s;
+        }
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, slot, epoch);
+    }
+    if (multi) {
+        wait_all(a, slot, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+}
+
+// the posts of float k of every rank, added in rank order in float64
+__device__ __forceinline__ double mimic_total(ByzArgs const& a, int k) {
+    float const* const box = a.mailbox[a.rank] + kCraftRegion;
+    double s = 0.0;
+    for (int q = 0; q < a.R; ++q)
+        s += static_cast<double>(ld_volatile_f(box + q * kCraftStats + k));
+    return s;
+}
+
+template<int N>
+__global__ void __launch_bounds__(256) gar_mimic_warmup_kernel(ByzArgs const a) {
+    __shared__ Shared sh;
+    __shared__ int pair_of[kBlockRows * kBlockRows];
+    __shared__ float s_sh[kMaxWorkers];
+    __shared__ double q_sh[kMaxWorkers];
+    __shared__ float inv_sh;
+    __shared__ int target_sh, ok_sh;
+    __shared__ double norm_sh;
+    cg::grid_group grid = cg::this_grid();
+    uint32_t const epoch = current_epoch(a);
+    if (a.R > 1) {
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    int const previous = *a.istar;   // read before the first grid barrier; block 0 stores the new i* after the last one
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const H = a.H;
+    float* const mine = a.partials + static_cast<long long>(blockIdx.x) * kCraftStats;
+    for (int k = threadIdx.x; k <= kMimicY; k += blockDim.x)
+        mine[k] = 0.f;
+    __syncthreads();
+    // -------- pass 1 and exchange 1: s_i -------- //
+    for (int i0 = 0; i0 < H; i0 += kBlockRows)
+        mimic_s_pass<N>(a, sh, pair_of, i0, mine, tid, nthreads);
+    mimic_exchange(a, grid, kMimicS, kMimicS + H, kSlotCraftStats, epoch);
+    int const lane = threadIdx.x;
+    if (lane < H)
+        s_sh[lane] = __double2float_rn(mimic_total(a, kMimicS + lane));
+    __syncthreads();
+    // -------- pass 2 and exchange 2: y, q_i, ||y||^2 -------- //
+    mimic_y_pass<N>(a, sh, pair_of, s_sh, mine, tid, nthreads);
+    mimic_exchange(a, grid, kMimicQ, kMimicY + 1, kSlotMimic, epoch);
+    if (lane < H)
+        q_sh[lane] = mimic_total(a, kMimicQ + lane);
+    if (lane == kMaxWorkers)
+        norm_sh = mimic_total(a, kMimicY);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double const norm2 = norm_sh;
+        bool const ok = norm2 > 0.0 && isfinite(norm2);
+        int best = -1;
+        for (int i = 0; i < H; ++i)
+            if (isfinite(q_sh[i]) && (best < 0 || q_sh[i] > q_sh[best]))
+                best = i;
+        ok_sh = ok;
+        inv_sh = ok ? __double2float_rn(__ddiv_rn(1.0, __dsqrt_rn(norm2))) : 0.f;
+        target_sh = ok ? a.honest[best < 0 ? 0 : best] : mimic_target(a, previous);
+    }
+    __syncthreads();
+    float const inv = inv_sh;
+    int const target = target_sh;
+    bool const ok = ok_sh != 0;
+    // -------- pass 3: z <- y / ||y||, h_{i*} into every Byzantine row -------- //
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4, soff = staged_offset(a, seg);   // z, y: owned order
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            if (ok) {
+                float y[4];
+                V<4>::load(a.y + soff + v * 4, y);
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    y[c] = __fmul_rn(y[c], inv);
+                V<4>::store(a.z + soff + v * 4, y);
+            }
+            float h[4];
+            V<4>::load_stream(a.rows[target] + x, h);
+            for (int k = 0; k < a.K; ++k)
+                V<4>::store_stream(a.rows[a.byz[k]] + x, h);
+        }
+    }
+    if (blockIdx.x == 0) {
+        if (threadIdx.x == 0)
+            *a.istar = target;
+        if (a.mimic_stats) {
+            if (lane < H) {
+                a.mimic_stats[kMimicS + lane] = s_sh[lane];
+                a.mimic_stats[kMimicQ + lane] = q_sh[lane];
+            }
+            if (threadIdx.x == 0) {
+                a.mimic_stats[kMimicY] = norm_sh;
+                a.mimic_stats[kMimicY + 1] = inv;
+            }
+        }
+    }
+    fence_sys();
+}
+
+__global__ void __launch_bounds__(256) gar_mimic_copy_kernel(ByzArgs const a) {
+    if (a.R > 1) {
+        uint32_t const epoch = current_epoch(a);
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    float const* const src = a.rows[mimic_target(a, *a.istar)];
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float h[4];
+            V<4>::load_stream(src + x, h);
+            for (int k = 0; k < a.K; ++k)
+                V<4>::store_stream(a.rows[a.byz[k]] + x, h);
+        }
+    }
+    fence_sys();
+}
+
 // ---- small stand-alone kernels (baseline path, attacks, diagnostics) ------------- //
 __global__ void sgd_kernel(float* __restrict__ p, float const* __restrict__ g, float lr, long long d) {
     long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
@@ -2919,7 +3228,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
 extern "C" {
 
 char const* agb_op_list() {
-    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,gar_byzantine_optimized,sgd,worker_momentum,drop_chunks,checksum,cast_bf16";
+    return "gar_fused,gar_phase_a,gar_max_ctas,gar_byzantine,gar_byzantine_optimized,gar_byzantine_mimic,sgd,worker_momentum,drop_chunks,checksum,cast_bf16";
 }
 
 // Wall-clock bound (seconds, 0 = none) of the cross-GPU flag waits of this library's kernels.
@@ -3122,6 +3431,97 @@ int agb_gar_byzantine_optimized(unsigned long long const* rows, int n, long long
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_optimized_kernel<kBlockRows>)
                                                          : reinterpret_cast<void*>(gar_optimized_kernel<0>),
+                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
+    return 0;
+}
+
+// Mimic over this rank's owned segments; see `gar_mimic_warmup_kernel`. Arguments as `agb_gar_byzantine_optimized`, plus: `warmup`: 1 runs
+// the warm-up update number t + 1 (`z`, `y`: local fp32 buffers of the owned coordinates, segments back to back: the direction estimate
+// and its scratch), 0 the copy pass alone;
+// `istar`: [1] local int32, the target slot, read and (warm-up) written; `stats_out`: optional [66] float64, s_i [0, 32), q_i [32, 64),
+// ||y||^2 [64], 1 / ||y|| [65]. The warm-up is a cooperative launch. Collective when R > 1.
+int agb_gar_byzantine_mimic(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                            unsigned byzantine, int warmup, int t, int R, int rank, unsigned long long const* signals,
+                            unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long z,
+                            unsigned long long y, unsigned long long istar, unsigned long long stats_out, unsigned epoch,
+                            unsigned long long epoch_ptr, void* stream) {
+    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
+        return 100;
+    if (nseg < 1 || nseg > kMaxSeg)
+        return 101;
+    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
+    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1)
+        return 114;
+    if (H < 2 || (warmup != 0 && warmup != 1) || t < 0 || t >= (1 << 24) || !istar || (warmup && (!z || !y)))
+        return 124;
+    ByzArgs a{};
+    a.H = H;
+    a.K = K;
+    a.honest_mask = honest;
+    for (int i = 0, h = 0, b = 0; i < n; ++i) {
+        a.rows[i] = reinterpret_cast<float*>(rows[i]);
+        if ((honest >> i) & 1u)
+            a.honest[h++] = i;
+        if ((byzantine >> i) & 1u)
+            a.byz[b++] = i;
+    }
+    a.nseg = nseg;
+    long long work = 0;
+    for (int s = 0; s < nseg; ++s) {
+        a.seg_lo[s] = seg_lo[s];
+        a.seg_hi[s] = seg_hi[s];
+        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
+            return 101;
+        work += (seg_hi[s] - seg_lo[s]) / 4;
+    }
+    a.R = R;
+    a.rank = rank;
+    for (int q = 0; q < R; ++q) {
+        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
+        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
+        if (R > 1 && !a.signal[q])
+            return 109;
+        if (warmup && !a.mailbox[q])
+            return 108;
+    }
+    a.t = t;
+    a.z = reinterpret_cast<float*>(z);
+    a.y = reinterpret_cast<float*>(y);
+    a.istar = reinterpret_cast<int*>(istar);
+    a.mimic_stats = reinterpret_cast<double*>(stats_out);
+    a.partials = reinterpret_cast<float*>(partials);
+    a.epoch = epoch;
+    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
+    int const threads = 256;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (!warmup) {
+        if (work == 0 && R == 1)
+            return 0;
+        long long grid = (work + threads - 1) / threads;
+        long long const cap = static_cast<long long>(agb::sm_count()) * 8;
+        grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
+        gar_mimic_copy_kernel<<<static_cast<int>(grid), threads, 0, s>>>(a);
+        AGB_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+    if (!a.partials || partial_ctas < 1)
+        return 108;
+    // the grid depends only on the owned work (and the device): the fused engine at R = 1 and the stand-alone op on the same rows fold
+    // the same partials in the same order
+    bool const in_registers = H <= kBlockRows;
+    int per_sm = 0;
+    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_mimic_warmup_kernel<kBlockRows> : gar_mimic_warmup_kernel<0>,
+                                                              threads, 0));
+    if (per_sm < 1)
+        return 2;
+    long long grid = (work + threads - 1) / threads;
+    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
+    cap = cap > partial_ctas ? partial_ctas : cap;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
+    void* params[] = {&a};
+    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_mimic_warmup_kernel<kBlockRows>)
+                                                         : reinterpret_cast<void*>(gar_mimic_warmup_kernel<0>),
                                             dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
     return 0;
 }

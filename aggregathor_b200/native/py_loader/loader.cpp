@@ -9,7 +9,11 @@
 // one batch by drawing uniformly from the pool once it holds `min_after_dequeue` records (the RandomShuffleQueue discipline),
 // copying each record straight into the caller's buffer — pinned host memory from which the H2D copy is issued.
 //
-// C ABI (ctypes): agb_loader_open / agb_loader_next / agb_loader_info / agb_loader_close.
+// A reader opened with `agb_loader_open_subset` serves only the records of a membership bitmap over the global record index (the
+// shards in the order given, then the records of each shard), e.g. one worker's part of a label-skewed split; the others are skipped
+// before any read.
+//
+// C ABI (ctypes): agb_loader_open / agb_loader_open_subset / agb_loader_next / agb_loader_info / agb_loader_close.
 
 #include <fcntl.h>
 #include <sys/stat.h>
@@ -45,6 +49,7 @@ struct Shard {
     std::string path;
     int fd = -1;
     uint64_t count = 0;
+    uint64_t first = 0;       // global index of its record 0 (records of the shards before it)
 };
 
 struct Record {
@@ -54,13 +59,20 @@ struct Record {
 
 class Loader {
 public:
-    Loader(std::vector<Shard> shards, ShardHeader const& proto, int batch, int nthreads, uint64_t seed, bool shuffle, size_t pool_capacity, size_t min_after_dequeue, int part, int parts)
-        : shards_(std::move(shards)), proto_(proto), batch_(batch), shuffle_(shuffle), capacity_(pool_capacity), min_after_(min_after_dequeue), part_(part), parts_(parts), draw_rng_(seed ^ 0x9E3779B97F4A7C15ull) {
+    Loader(std::vector<Shard> shards, ShardHeader const& proto, int batch, int nthreads, uint64_t seed, bool shuffle, size_t pool_capacity, size_t min_after_dequeue, int part, int parts,
+           std::vector<uint64_t> members = {})
+        : shards_(std::move(shards)), proto_(proto), batch_(batch), shuffle_(shuffle), capacity_(pool_capacity), min_after_(min_after_dequeue), part_(part), parts_(parts),
+          members_(std::move(members)), draw_rng_(seed ^ 0x9E3779B97F4A7C15ull) {
         if (!shuffle_)
             nthreads = 1;   // sequential order is only defined with one reader
-        total_ = 0;   // records this reader can ever serve per epoch (its residue class of every shard)
-        for (auto const& s : shards_)
-            total_ += parts_ > 1 ? (s.count + parts_ - 1 - part_) / parts_ : s.count;
+        total_ = 0;   // records this reader can ever serve per epoch (its residue class of every shard, or its subset)
+        if (!members_.empty()) {
+            for (uint64_t word : members_)
+                total_ += static_cast<uint64_t>(__builtin_popcountll(word));
+        } else {
+            for (auto const& s : shards_)
+                total_ += parts_ > 1 ? (s.count + parts_ - 1 - part_) / parts_ : s.count;
+        }
         for (int t = 0; t < nthreads; ++t)
             readers_.emplace_back([this, t, nthreads, seed] { read_loop(t, nthreads, seed); });
     }
@@ -152,6 +164,9 @@ private:
                 for (uint32_t index : order) {
                     if (parts_ > 1 && static_cast<int>(index % parts_) != part_)
                         continue;
+                    uint64_t const global = shard.first + index;
+                    if (!members_.empty() && !((members_[global >> 6] >> (global & 63)) & 1ull))
+                        continue;
                     Record record;
                     record.pixels.resize(proto_.record_bytes);
                     off_t const at = static_cast<off_t>(sizeof(ShardHeader) + static_cast<uint64_t>(index) * proto_.record_bytes);
@@ -195,6 +210,7 @@ private:
     bool shuffle_;
     size_t capacity_, min_after_;
     int part_, parts_;
+    std::vector<uint64_t> members_;   // membership bitmap over the global record index (empty: every record)
     uint64_t total_ = 0;
     std::atomic<uint64_t> served_{0};
     std::mutex mutex_;
@@ -208,20 +224,15 @@ private:
 
 thread_local std::string g_last_error;
 
-} // namespace
-
-extern "C" {
-
-// `paths`: nshards NUL-terminated file names. Returns an opaque handle or null (see agb_loader_last_error).
-// `part` / `parts`: this reader only serves records whose index in their shard is congruent to part modulo parts.
-void* agb_loader_open(char const* const* paths, int nshards, int batch, int nthreads, unsigned long long seed, int shuffle, long long pool_capacity, long long min_after_dequeue,
-                      int part, int parts) {
+void* open_loader(char const* const* paths, int nshards, int batch, int nthreads, unsigned long long seed, int shuffle, long long pool_capacity, long long min_after_dequeue,
+                  int part, int parts, unsigned long long const* bitmap, unsigned long long nbits) {
     if (nshards < 1 || batch < 1) {
         g_last_error = "need at least one shard and a positive batch size";
         return nullptr;
     }
     std::vector<Shard> shards;
     ShardHeader proto{};
+    uint64_t total = 0;
     for (int i = 0; i < nshards; ++i) {
         Shard shard;
         shard.path = paths[i];
@@ -254,7 +265,26 @@ void* agb_loader_open(char const* const* paths, int nshards, int batch, int nthr
             return nullptr;
         }
         shard.count = header.count;
+        shard.first = total;
+        total += header.count;
         shards.push_back(shard);
+    }
+    std::vector<uint64_t> members;
+    if (bitmap) {
+        uint64_t set = 0;
+        if (nbits == total) {
+            members.assign(bitmap, bitmap + (total + 63) / 64);
+            if (total % 64)
+                members.back() &= (1ull << (total % 64)) - 1;
+            for (uint64_t word : members)
+                set += static_cast<uint64_t>(__builtin_popcountll(word));
+        }
+        if (nbits != total || set == 0) {
+            g_last_error = "the membership bitmap must cover the " + std::to_string(total) + " records of the shards and select at least one";
+            for (auto& s : shards)
+                ::close(s.fd);
+            return nullptr;
+        }
     }
     if (nthreads < 1)
         nthreads = 1;
@@ -268,9 +298,31 @@ void* agb_loader_open(char const* const* paths, int nshards, int batch, int nthr
         capacity = static_cast<size_t>(batch);
     if (min_after >= capacity)
         min_after = capacity - 1;
-    return new Loader(std::move(shards), proto, batch, nthreads, seed, shuffle != 0, capacity, min_after, part, parts);
+    return new Loader(std::move(shards), proto, batch, nthreads, seed, shuffle != 0, capacity, min_after, part, parts, std::move(members));
 }
 
+} // namespace
+
+extern "C" {
+
+// `paths`: nshards NUL-terminated file names. Returns an opaque handle or null (see agb_loader_last_error).
+// `part` / `parts`: this reader only serves records whose index in their shard is congruent to part modulo parts.
+void* agb_loader_open(char const* const* paths, int nshards, int batch, int nthreads, unsigned long long seed, int shuffle, long long pool_capacity, long long min_after_dequeue,
+                      int part, int parts) {
+    return open_loader(paths, nshards, batch, nthreads, seed, shuffle, pool_capacity, min_after_dequeue, part, parts, nullptr, 0);
+}
+
+// As `agb_loader_open` without part / parts, serving only the records whose bit is set in `bitmap` (64-bit words, bit g % 64 of word
+// g / 64 for global record g: the shards in the order given, then the records of each). `nbits` must be the total number of records,
+// and at least one bit must be set.
+void* agb_loader_open_subset(char const* const* paths, int nshards, int batch, int nthreads, unsigned long long seed, int shuffle, long long pool_capacity,
+                             long long min_after_dequeue, unsigned long long const* bitmap, unsigned long long nbits) {
+    if (!bitmap) {
+        g_last_error = "the subset reader needs a membership bitmap";
+        return nullptr;
+    }
+    return open_loader(paths, nshards, batch, nthreads, seed, shuffle, pool_capacity, min_after_dequeue, 0, 1, bitmap, nbits);
+}
 int agb_loader_next(void* handle, void* images, void* labels) {
     Loader* loader = static_cast<Loader*>(handle);
     int status = loader->next(static_cast<uint8_t*>(images), static_cast<int64_t*>(labels));

@@ -20,12 +20,15 @@ MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
-# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange;
-# DnC's exchange; ARC's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 4
+# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
+# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 5
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
-# Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]
+# Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]; mimic posts into the
+# same region: s_i [0, 32) in its first exchange, q_i [32, 64) and ||y||^2 [64] in its second
 CRAFT_STATS = MAX_PAIRS + 2 * MAX_WORKERS + 1
+# mimic's statistics of a warm-up step (float64): s_i [0, 32), q_i [32, 64), ||y||^2 [64], 1 / ||y|| [65]
+MIMIC_STATS = 2 * MAX_WORKERS + 2
 DNC_MAX_ITERATIONS = 8
 # DnC's post of one rank: the sampled distances of every iteration ([DNC_MAX_ITERATIONS][MAX_PAIRS]), then the loss
 DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
@@ -52,9 +55,10 @@ _ERRORS = {
   118: "unknown Min-Max / Min-Sum mode or deviation (modes: min-max, min-sum; deviations: unit-vec, sign, std)",
   119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)",
   120: "invalid ARC parameters (0 <= 2 f < n)", 122: "invalid SMEA parameters (0 <= 2 f < n and C(n, f) <= 2^14)",
-  123: "invalid bucketing parameters (1 <= s <= n_rows, n = ceil(n_rows / s), not combined with NNM or ARC, a staging tile)"}
+  123: "invalid bucketing parameters (1 <= s <= n_rows, n = ceil(n_rows / s), not combined with NNM or ARC, a staging tile)",
+  124: "invalid mimic parameters (H >= 2, 0 <= t < 2^24, a target buffer, and z and y buffers for a warm-up step)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
-BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3}
+BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3, "mimic": 4}
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
 
 
@@ -106,6 +110,9 @@ class FusedLauncher:
     self.craft_ctas = ctas
     self.craft_partials = torch.zeros(ctas * CRAFT_STATS, dtype=torch.float32, device=self.device)
     self.craft_stats = torch.zeros(1 + CRAFT_STATS, dtype=torch.float32, device=self.device)
+    # mimic: the statistics of the last warm-up step, and the y scratch of the owned coordinates (`mimic_scratch`)
+    self.mimic_stats = torch.zeros(MIMIC_STATS, dtype=torch.float64, device=self.device)
+    self._mimic_y = None
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
     self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 6))()
@@ -188,6 +195,12 @@ class FusedLauncher:
     if self._smea_scratch is None or self._smea_scratch.numel() < need:
       self._smea_scratch = torch.zeros(need, dtype=torch.float64, device=self.device)
     return self._smea_scratch
+
+  def mimic_scratch(self, d):
+    """Mimic's y scratch over d coordinates (grown on demand): y of a warm-up step, kept apart from z until its norm is known."""
+    if self._mimic_y is None or self._mimic_y.numel() < d:
+      self._mimic_y = torch.zeros(d, dtype=torch.float32, device=self.device)
+    return self._mimic_y
 
   def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
@@ -376,13 +389,17 @@ def worker_momentum_(G, M, beta, c):
 
 
 def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, launcher=None, mailboxes=None, R=1, rank=0, signals=None, epoch=1,
-          epoch_ptr=None, stream=None):
+          epoch_ptr=None, stream=None, state=None, warmup=None):
   """Craft the omniscient Byzantine rows (`attacks/omniscient.py`) over the owned `segments` of the n rows at device addresses `rows`
   (raw ints, local or peer-mapped): every slot of `byzantine` receives the ALIE / IPM / Min-Max / Min-Sum value of the `honest` slots.
   Collective when R > 1 (entry barrier through the signal pads, at flag value `epoch`, or `*epoch_ptr + 1` when given).
   Min-Max and Min-Sum (`coef` unused) take the `deviation` (default "unit-vec") and the `FusedLauncher` whose scratch holds the CTA
   partials and receives gamma and the summed statistics (`launcher.craft_stats`); their statistics are exchanged through `mailboxes`
-  (R addresses, every rank's; default: the launcher's local mailbox when R = 1)."""
+  (R addresses, every rank's; default: the launcher's local mailbox when R = 1).
+  Mimic (`coef` unused) takes the caller-owned `state` (`aggregators._ops.mimic_state`: "t", the fp32 "z" of the owned coordinates,
+  `segments` back to back, and the [1] int32 "istar", both on the device) and the warm-up length `warmup`: while state["t"] < warmup it runs one
+  warm-up update (two exchanges through `mailboxes`, the launcher's scratch; `launcher.mimic_stats` receives s_i, q_i, ||y||^2 and
+  1 / ||y||) and counts it in state["t"]; then the copy pass alone, with i* read on the device."""
   n = len(rows)
   if n > MAX_WORKERS:
     raise tools.UserException("The sm_90a crafting kernel supports n <= %d workers (got %d)" % (MAX_WORKERS, n))
@@ -394,6 +411,30 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
   lo = (ctypes.c_longlong * len(segments))(*[int(a) for a, _ in segments])
   hi = (ctypes.c_longlong * len(segments))(*[int(b) for _, b in segments])
   c_signals = (ctypes.c_ulonglong * R)(*[addr(signals[q]) for q in range(R)]) if signals is not None else None
+  if mode == "mimic":
+    if launcher is None or state is None or warmup is None:
+      raise tools.UserException("mimic needs the scratch of a FusedLauncher, its state and its warm-up length")
+    if mailboxes is None:
+      if R != 1:
+        raise tools.UserException("mimic over %d ranks needs every rank's mailbox" % R)
+      mailboxes = [launcher.local_mailbox]
+    c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
+    t = int(state["t"])
+    warm = t < int(warmup)
+    z = state["z"]
+    if z.numel() != sum(int(b) - int(a) for a, b in segments):
+      raise tools.UserException("mimic's z holds the %d owned coordinates (got %d)" % (sum(int(b) - int(a) for a, b in segments), z.numel()))
+    y = launcher.mimic_scratch(z.numel()) if warm else None
+    func = _lib().agb_gar_byzantine_mimic
+    func.restype = ctypes.c_int
+    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
+                ctypes.c_int(1 if warm else 0), ctypes.c_int(t), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+                ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(addr(z)),
+                ctypes.c_ulonglong(addr(y)), ctypes.c_ulonglong(addr(state["istar"])), ctypes.c_ulonglong(launcher.mimic_stats.data_ptr()),
+                ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_mimic")
+    if warm:
+      state["t"] = t + 1
+    return
   if mode in ("min-max", "min-sum"):
     if deviation is None:
       deviation = "unit-vec"
@@ -430,11 +471,56 @@ def craft_details(launcher, mode, H):
   return stats[0], st[a:a + H], st[b:b + H], st[c], T
 
 
-def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False):
+def mimic_details(launcher, H):
+  """(s [H], q [H], ||y||^2, 1 / ||y||) of the last mimic warm-up step run with `launcher`: Python floats, as the kernel summed them (s and
+  1 / ||y|| are fp32 values)."""
+  stats = launcher.mimic_stats.cpu().tolist()
+  return stats[:H], stats[MAX_WORKERS:MAX_WORKERS + H], stats[2 * MAX_WORKERS], stats[2 * MAX_WORKERS + 1]
+
+
+def _craft_mimic_(G, byz_slots, state, warmup, return_details):
+  """`craft_byzantine_` for mimic: the sm_90a kernels on CUDA fp32 rows with n <= 32, the torch reference otherwise."""
+  from ..aggregators import _ops
+  n, d = G.shape
+  slots, warmup = _ops.check_mimic(n, byz_slots, warmup)
+  if state is None or state["z"].shape != (d,) or state["z"].dtype != torch.float32 or state["z"].device != G.device or state["istar"].device != G.device:
+    raise tools.UserException("mimic needs a state with an fp32 [%d] z and its target on %s (`aggregators._ops.mimic_state`)" % (d, G.device))
+  if not G.is_cuda or n > MAX_WORKERS:
+    return _ops.torch_mimic_step_(G, slots, state, warmup, return_details=return_details)
+  if G.dtype != torch.float32:
+    raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
+  work, dp = _aligned_rows(G)
+  z = state["z"]
+  zwork = z
+  if dp != d or not z.is_contiguous() or z.data_ptr() % 16:
+    zwork = torch.zeros(dp, dtype=torch.float32, device=G.device)
+    zwork[:d] = z
+  run = dict(state, z=zwork)
+  warm = run["t"] < warmup
+  launcher = _launcher(G.device, n)
+  rows = [work.data_ptr() + i * dp * 4 for i in range(n)]
+  with torch.cuda.device(G.device):
+    craft(rows, [(0, dp)], [i for i in range(n) if i not in slots], slots, "mimic", None, launcher=launcher, state=run, warmup=warmup)
+  state["t"] = run["t"]
+  if zwork is not z:
+    z.copy_(zwork[:d])
+  if work is not G:
+    index = torch.tensor(slots, dtype=torch.int64, device=G.device)
+    G[index] = work[index, :d]
+  if return_details:
+    return mimic_details(launcher, n - len(slots)) if warm else None
+  return G
+
+
+def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False, state=None, warmup=None):
   """Stand-alone omniscient attack on the [n, d] fp32 matrix `G`, in place: rows `byz_slots` <- the ALIE (`coef` = z), IPM
   (`coef` = epsilon), Min-Max or Min-Sum (`deviation`) row of the other rows. CUDA tensors with n <= 32 run the sm_90a kernel; others
-  the torch reference. Min-Max / Min-Sum with `return_details` return (gamma, A, B, C, T) instead of G (see `craft_details`)."""
+  the torch reference. Min-Max / Min-Sum with `return_details` return (gamma, A, B, C, T) instead of G (see `craft_details`).
+  Mimic takes its `state` (`aggregators._ops.mimic_state(d, G.device)`, updated in place) and `warmup`; with `return_details` it returns
+  (s, q, ||y||^2, 1 / ||y||) of a warm-up step (see `mimic_details`), None after the warm-up."""
   from ..aggregators import _ops
+  if mode == "mimic":
+    return _craft_mimic_(G, byz_slots, state, warmup, return_details)
   n, d = G.shape
   byz_slots = _ops.check_byzantine_slots(n, byz_slots, mode)
   optimized = mode in _ops.OPTIMIZED_MODES

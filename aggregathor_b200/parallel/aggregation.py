@@ -14,9 +14,11 @@ Three interchangeable engines share one interface (`params`, `grads`, `step()`):
   (`mnist` + `average`, 2 workers) and the fallback for user plug-in GARs without a fused spec.
 
 Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always sees n rows.
-Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None)`, the omniscient attacks (`attacks/omniscient.py`): the
-rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM / Min-Max / Min-Sum row of the others, on every rank
-(a collective call); `last_craft` then holds Min-Max / Min-Sum's (gamma, A, B, C, T) of that call.
+Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None, warmup=None)`, the omniscient attacks
+(`attacks/omniscient.py`): the rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM / Min-Max / Min-Sum /
+mimic row of the others, on every rank (a collective call); `last_craft` then holds Min-Max / Min-Sum's (gamma, A, B, C, T) of that
+call, or mimic's (s, q, ||y||^2, 1 / ||y||) of a warm-up step. Mimic's state (t, z, i*; `mimic_state()`) lives in the engine (the fused
+engine holds z for its owned segments only, back to back) and is checkpointed under "attack_state" as the full [d] vector.
 Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
 `dnc` draws its samples with the number of the optimizer update the aggregation feeds as step key (`updates` once it is counted,
 checkpointed with it) over the padded flat size `layout.padded_size`, on every engine.
@@ -96,6 +98,7 @@ class _AggregationBase:
     self.updates = 0  # number of optimizer updates applied so far
     self.slots = []
     self.center = None   # centered clipping: the rule's center v, [d] fp32
+    self.attack_state = None   # mimic: {"t", "z", "istar"} (`mimic_state`)
 
   def _make_center(self):
     """Allocate the center (+0) when the rule is centered clipping; it lives as long as the engine and travels in checkpoints."""
@@ -107,10 +110,23 @@ class _AggregationBase:
   def first_worker(self):
     return self.rank * self.w
 
+  def mimic_state(self):
+    """Mimic's state, created at first use: t = 0, z = 1 / sqrt(d) on the real coordinates of the layout (`_ops.mimic_state`), no target."""
+    if self.attack_state is None:
+      from ..aggregators import _ops
+      mask = self.layout.mask(self.device) if hasattr(self.layout, "mask") else torch.ones(self.d, dtype=torch.bool, device=self.device)
+      packed = self._pack(mask)
+      self.attack_state = _ops.mimic_state(packed.numel(), self.device, packed, real=int(mask.sum()))
+    return self.attack_state
+
   def state_dict(self):
     state = {"updates": self.updates, "slots": [s.detach().to("cpu", copy=True) for s in self.full_slots()]}
     if self.center is not None:
       state["rule_state"] = self.full_center().detach().to("cpu", copy=True)
+    if self.attack_state is not None:
+      mimic = self.attack_state
+      state["attack_state"] = {"mode": "mimic", "t": int(mimic["t"]), "z": self._assemble(self._unpack(mimic["z"])).detach().to("cpu", copy=True),
+                               "istar": int(mimic["istar"][0])}
     return state
 
   def load_state_dict(self, state):
@@ -123,6 +139,28 @@ class _AggregationBase:
       else:
         tools.warning("The checkpoint holds no center for centered clipping: it starts from zero", context="restore")
         self.center.zero_()
+    if self.attack_state is not None:
+      saved = state.get("attack_state")
+      if saved is not None and saved.get("mode") == "mimic":
+        self.attack_state["t"] = int(saved["t"])
+        self.attack_state["z"].copy_(self._pack(saved["z"].to(self.device)))
+        self.attack_state["istar"].fill_(int(saved["istar"]))
+      else:
+        tools.warning("The checkpoint holds no state for mimic: its warm-up starts again", context="restore")
+        self.attack_state = None
+        self.mimic_state()
+
+  def _assemble(self, vector):
+    """Full copy of a [d] vector the engine maintains (the fused engine: on the owned segments only, collective when R > 1)."""
+    return vector
+
+  def _pack(self, vector):
+    """The coordinates of a [d] vector that mimic's z holds: all of them (the fused engine: its owned segments, back to back)."""
+    return vector
+
+  def _unpack(self, owned):
+    """The [d] vector of `_pack`'s output (the fused engine: zero outside the owned segments)."""
+    return owned
 
   def _rule_kwargs(self):
     """Keywords of the rule's `aggregate` (and of `ops.gar.aggregate`) for the step about to be counted: centered clipping's center,
@@ -181,11 +219,13 @@ class HostAggregation(_AggregationBase):
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef, deviation=None):
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None):
     """Gather, then the torch reference on the gathered matrix (every rank computes the same bits)."""
     from ..aggregators import _ops
     self.visible_rows()
-    if mode in _ops.OPTIMIZED_MODES:
+    if mode == "mimic":
+      self.last_craft = _ops.torch_mimic_step_(self._gathered, byz_slots, self.mimic_state(), warmup, return_details=True)
+    elif mode in _ops.OPTIMIZED_MODES:
       self.last_craft = _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
     else:
       _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef)
@@ -223,11 +263,13 @@ class BaselineAggregation(_AggregationBase):
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef, deviation=None):
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None):
     """Gather, then the stand-alone crafting kernel (R = 1) on the gathered matrix (every rank computes the same bits)."""
     from ..aggregators import _ops
     self.visible_rows()
-    if mode in _ops.OPTIMIZED_MODES:
+    if mode == "mimic":
+      self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, state=self.mimic_state(), warmup=warmup, return_details=True)
+    elif mode in _ops.OPTIMIZED_MODES:
       self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
     else:
       gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef)
@@ -394,25 +436,35 @@ class FusedAggregation(_AggregationBase):
       if self.step_dev is not None:   # the value travels as a kernel argument of the fill, fixed when it is enqueued
         self.step_dev.fill_(self.updates)
 
-  def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None):
+  def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None, warmup=None):
     """Collective: this rank crafts its owned segments of every Byzantine row, local or on a peer (`ops.gar.craft`), behind an entry
     barrier at the epoch of the step about to be aggregated. Every rank calls it, including ranks that host no Byzantine worker.
-    Min-Max / Min-Sum exchange their statistics through the mailboxes; `last_craft` reads gamma and the sums back (a synchronisation)."""
+    Min-Max / Min-Sum exchange their statistics through the mailboxes; `last_craft` reads gamma and the sums back (a synchronisation).
+    Mimic's warm-up steps exchange theirs the same way and update z on the owned segments."""
     from ..aggregators import _ops
     byz_slots = _ops.check_byzantine_slots(self.n, byz_slots, mode)
     optimized = mode in _ops.OPTIMIZED_MODES
+    mimic = mode == "mimic"
     if optimized:
       deviation = _ops.check_deviation(mode, deviation)
+    state = None
+    if mimic:
+      warmup = _ops.check_mimic(self.n, byz_slots, warmup)[1]
+      state = self.mimic_state()
+      warm = state["t"] < warmup
     epoch = self.epoch if self._prepared else self.epoch + 1
     gar_ops.craft(self._rows, self.segments, [i for i in range(self.n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation,
-                  launcher=self.launcher if optimized else None, mailboxes=self._mailboxes if optimized else None, R=self.world, rank=self.rank,
-                  signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream)
-    self._craft_mode = (mode, self.n - len(byz_slots)) if optimized else None
+                  launcher=self.launcher if optimized or mimic else None, mailboxes=self._mailboxes if optimized or mimic else None, R=self.world,
+                  rank=self.rank, signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream, state=state, warmup=warmup)
+    self._craft_mode = (mode, self.n - len(byz_slots)) if optimized or (mimic and warm) else None
 
   @property
   def last_craft(self):
-    """Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`, as the kernel solved them (identical on every rank)."""
+    """Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`, as the kernel solved them (identical on every rank); mimic:
+    (s, q, ||y||^2, 1 / ||y||) of the last call when it was a warm-up step."""
     mode = self._craft_mode
+    if mode is not None and mode[0] == "mimic":
+      return gar_ops.mimic_details(self.launcher, mode[1])
     return None if mode is None else gar_ops.craft_details(self.launcher, *mode)
 
   def phase_a(self, seg, stream=None):
@@ -455,6 +507,18 @@ class FusedAggregation(_AggregationBase):
   def full_center(self):
     """The center of centered clipping, assembled from the owned segments of every rank (checkpoints)."""
     return None if self.center is None else self._assemble(self.center)
+
+  def _pack(self, vector):
+    """Mimic's z and y scratch hold the owned segments only, back to back in segment order (as the staged tile): d / R floats each."""
+    return torch.cat([vector[lo:hi] for lo, hi in self.segments])
+
+  def _unpack(self, owned):
+    full = torch.zeros(self.d, dtype=owned.dtype, device=owned.device)
+    at = 0
+    for lo, hi in self.segments:
+      full[lo:hi] = owned[at:at + hi - lo]
+      at += hi - lo
+    return full
 
 
 def _single_host(group=None):

@@ -13,6 +13,8 @@ the crafting kernel is also timed alone, next to the torch reference on the same
 `--gar-dump-rows` then saves, from the last rank, every row the fused engine aggregated (honest and crafted, all d coordinates).
 `--gar-attack min-max|min-sum` (Shejwalkar & Houmansadr, NDSS 2021; `--gar-attack-args deviation:unit-vec|sign|std`) also reports the
 gamma every rank solved, and times the crafting kernel alternated round by round with ALIE's on the same rows.
+`--gar-attack mimic` (Karimireddy, He & Jaggi, ICLR 2022; `--gar-attack-args warmup:<T0>`) reports the target i* every rank chose and
+whether the Byzantine rows equal the baseline engine's, and times the warm-up kernel and the copy pass, each alternated with ALIE.
 `--gar-rule-args key:value ...` passes the same `--aggregator-args` to every rule (rules ignore keys they do not use). The
 `geometric-median` and `centered-clipping` entries also report their T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
 `--gar-worker-momentum beta` also times the worker-momentum kernel alone on the [w, d] rows of a rank (`ops.gar.worker_momentum_`,
@@ -57,7 +59,7 @@ def main():
   parser.add_argument("--gar-rules", dest="rules", type=str, default="average,average-nan,median,averaged-median,krum,bulyan")
   parser.add_argument("--gar-out", dest="out", type=str, default=".")
   parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
-  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm", "min-max", "min-sum"), default=None,
+  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm", "min-max", "min-sum", "mimic"), default=None,
                       help="omniscient attack by the last f workers, crafted every step")
   parser.add_argument("--gar-attack-args", dest="attack_args", nargs="*", default=None, metavar="KEY:VALUE",
                       help="`--attack-args` of --gar-attack (e.g. deviation:std for min-max / min-sum)")
@@ -147,6 +149,9 @@ def main():
     attack = attacks.instantiate(args.attack, n, f, args.attack_args or []) if args.attack else None
     byz_slots = list(range(n - f, n))
     extra = {"deviation": attack.deviation} if attack is not None and attack.deviation is not None else {}
+    mimic = attack is not None and attack.mode == "mimic"
+    if mimic:
+      extra = {"warmup": attack.warmup}
 
     def craft(engine):
       if attack is not None:
@@ -175,6 +180,21 @@ def main():
       else:
         gammas = [gamma]
       gamma_entry = {"deviation": attack.deviation, "gamma_per_rank": [float(x.item()) for x in gammas], "baseline_gamma": base.last_craft[0]}
+    if mimic:
+      # i* as every rank chose it (fused engine) and as the baseline engine's stand-alone kernel chose it on the gathered rows; the
+      # Byzantine rows this rank sees through the peer mapping against the baseline engine's gathered matrix, bit for bit
+      target = fused.attack_state["istar"].to(torch.int64)
+      targets = [torch.zeros_like(target) for _ in range(world)]
+      if world > 1:
+        dist.all_gather(targets, target)
+      else:
+        targets = [target]
+      rows = fused.visible_rows()
+      same = torch.tensor([int(all(torch.equal(rows[b].view(torch.int32), base._gathered[b].view(torch.int32)) for b in byz_slots))], device=device)
+      if world > 1:
+        dist.all_reduce(same, op=dist.ReduceOp.MIN)
+      gamma_entry = {"warmup": attack.warmup, "istar_per_rank": [int(x.item()) for x in targets], "baseline_istar": int(base.attack_state["istar"][0]),
+                     "rows_match_baseline": bool(same.item())}
     if attack is not None and args.dump_rows and rank == world - 1:
       rows = fused.visible_rows()
       os.makedirs(args.out, exist_ok=True)
@@ -275,17 +295,48 @@ def main():
         if world > 1:
           dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
-      craft_ms = time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra))
+      def craft_at(engine, t):
+        """Mimic at warm-up step t (t < T0: the warm-up kernel; t = T0: the copy pass); other attacks: their usual crafting."""
+        if mimic:
+          engine.attack_state["t"] = t
+        engine.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra)
+      craft_ms = time_craft(lambda: craft_at(fused, 1))
       # the torch reference on this device, over the full [n, d] matrix (what a torch attack would run after an all-gather)
-      reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef, **extra))
+      if mimic:
+        ref_state = _ops.mimic_state(base._gathered.shape[1], device)
+
+        def reference():
+          ref_state["t"] = 1
+          _ops.torch_mimic_step_(base._gathered, byz_slots, ref_state, attack.warmup)
+        reference_ms = time_craft(reference)
+      else:
+        reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef, **extra))
       craft_bytes = n * d * 4   # (H + k) * d * 4: every honest value read once, every Byzantine value written once (over all ranks)
       if attack.deviation is not None:
         # Min-Max / Min-Sum read the honest values again in the write pass, and Min-Max once more in its honest-distance pass
         craft_bytes += (2 if attack.mode == "min-max" else 1) * (n - f) * d * 4
+      if mimic:
+        # warm-up: the honest rows read in passes 1 and 2 (twice in pass 2 beyond the registers, counted once), z read twice and written
+        # once, y written and read, then h_{i*} read and the k rows written; the copy pass alone: h_{i*} read, the k rows written
+        craft_bytes = (2 * (n - f) + 5 + 1 + f) * d * 4
+        copy_bytes = (1 + f) * d * 4
       attack_entry = {"attack": attack.mode, "coef": attack.coef, "k": f, "craft_ms": craft_ms, "torch_reference_ms": reference_ms,
                       "craft_bytes": craft_bytes, "craft_gbs": craft_bytes / craft_ms / 1e6,
                       "torch_reference_gbs": craft_bytes / reference_ms / 1e6}
       attack_entry.update(gamma_entry)
+      if mimic:
+        # the warm-up kernel and the copy pass, each alternated round by round with ALIE's kernel on the same rows
+        alie = attacks.instantiate("alie", n, f, [])
+        rounds = {"warmup": [], "copy": [], "alie": []}
+        for _ in range(5):
+          rounds["warmup"].append(time_craft(lambda: craft_at(fused, 1)))
+          rounds["copy"].append(time_craft(lambda: craft_at(fused, attack.warmup)))
+          rounds["alie"].append(time_craft(lambda: fused.craft_byzantine(byz_slots, "alie", alie.coef)))
+        median = lambda values: sorted(values)[len(values) // 2]
+        attack_entry.update({"warmup_rounds_ms": rounds["warmup"], "copy_rounds_ms": rounds["copy"], "alie_craft_rounds_ms": rounds["alie"],
+                             "warmup_median_ms": median(rounds["warmup"]), "copy_median_ms": median(rounds["copy"]),
+                             "alie_craft_median_ms": median(rounds["alie"]), "warmup_bytes": craft_bytes, "copy_bytes": copy_bytes,
+                             "warmup_gbs": craft_bytes / median(rounds["warmup"]) / 1e6, "copy_gbs": copy_bytes / median(rounds["copy"]) / 1e6})
       if attack.deviation is not None:
         # ALIE's crafting kernel on the same rows, alternated with this attack's round by round (clock and thermal drift hit both).
         # Repeated calls at one step's epoch pass the flag barriers at once: with R > 1 they time the kernels, their gamma is not checked.
