@@ -11,6 +11,8 @@ Omniscient attacks (`omniscient = True`, `omniscient.py`) see every honest row i
 ("alie", "ipm", "min-max", "min-sum" or "mimic"), the fp32 coefficient `coef` (None for Min-Max / Min-Sum, which solve theirs every step,
 and for mimic), `deviation` (Min-Max / Min-Sum; None otherwise) and `warmup` (mimic only); the aggregation engine crafts the Byzantine
 rows (`craft_byzantine`) on every rank.
+Label-flipping attacks (`flips_labels = True`, `data.py`) implement no `apply` either: the Byzantine workers' loss trains on flipped
+labels (the trainer sets `Context.flip_from`), so nothing rewrites their rows after the backward pass.
 Construction raises `UserException` for arguments outside an attack's bounds.
 """
 
@@ -24,6 +26,7 @@ __all__ = ["_Attack", "register", "instantiate", "itemize"]
 class _Attack:
   forges = False  # True: the attack tampers with the row *after* it was signed (only meaningful with `--authenticate`)
   omniscient = False  # True: the rows are crafted from the honest rows by the aggregation engine (no `apply`)
+  flips_labels = False  # True: the Byzantine workers compute their gradient on flipped labels (no `apply`)
 
   def __init__(self, nbworkers, nbbyzwrks, args):
     raise NotImplementedError

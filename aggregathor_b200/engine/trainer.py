@@ -14,7 +14,8 @@ One synchronous step on a rank:
      Byzantine-resilient SGD"): every local row becomes its worker's momentum M <- beta M + (1 - delta) G, before anything else
      reads it — a real Byzantine worker keeps its honest momentum, the attack then transforms or replaces what is submitted;
   3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
-     Byzantine rows from the honest ones, a collective call on every rank);
+     Byzantine rows from the honest ones, a collective call on every rank; label flipping: nothing, step 1 already trained the
+     Byzantine workers on flipped labels through `Context.flip_from`);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast), after the optional pre-aggregation
      (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing"; "arc": adaptive
      robust clipping, Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"; "arc+nnm": both;
@@ -91,8 +92,10 @@ class Manager:
     engine_args = dict(engine_args or {})
     self._bucket_layers = {}
     # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum); with
-    # a pre-aggregation the rule's distances are those of the mixed or clipped rows, which exist only once every row is complete
-    plain_step = (attack is None and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
+    # a pre-aggregation the rule's distances are those of the mixed or clipped rows, which exist only once every row is complete.
+    # Label flipping rewrites no row: its Byzantine rows are complete when the backward pass ends, like the honest ones.
+    self._rewrites_rows = attack is not None and not getattr(attack, "flips_labels", False)
+    plain_step = (not self._rewrites_rows and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
                   and self.pre_aggregation is None)
     if cuda and engine in ("auto", "fused") and aggregator.fused_spec() is not None:
       engine_args.setdefault("device_state", True)
@@ -188,6 +191,15 @@ class Manager:
     self._attack_state = {i: {} for i in self.byzantine}
     if self.byzantine and getattr(attack, "mode", None) == "mimic":   # created now, so that a restored checkpoint finds it
       self.aggregation.mimic_state()
+    if self.byzantine and getattr(attack, "flips_labels", False):   # training contexts only: `eval_ctx` never flips
+      for ctx, i in zip(self.contexts, self.local_workers):
+        ctx.flip_from = 0 if i in self.byzantine else None
+      if self.batched_ctx is not None:
+        # group j of the batched pass is local worker j (ascending ids, rows 0..w-1): the Byzantine workers, the last k ids, are
+        # the groups from the number of honest local workers on
+        honest = sum(i not in self.byzantine for i in self.local_workers)
+        assert self.local_workers == sorted(self.local_workers) and all((i in self.byzantine) == (j >= honest) for j, i in enumerate(self.local_workers))
+        self.batched_ctx.flip_from = honest if honest < len(self.local_workers) else None
     # rows in the gathered matrix (slots) of the Byzantine workers, as the aggregation engines address them
     self.byzantine_slots = sorted(placement[i][0] * self.w + placement[i][1] for i in self.byzantine)
     # -- gradient authentication (opt-in; reference: signed worker -> PS messages of the hardened transport) -- #
@@ -235,7 +247,7 @@ class Manager:
   @property
   def _whole_step_graph(self):
     """The captured graph holds the aggregation too (fused engine with device-resident step state, nothing host-driven in between)."""
-    return (getattr(self.aggregation, "device_state", False) and self.attack is None and self.authenticator is None
+    return (getattr(self.aggregation, "device_state", False) and not self._rewrites_rows and self.authenticator is None
             and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and os.environ.get("AGB_GRAPH_AGGREGATION", "1") not in ("", "0"))
 
   def _capture(self, batches):
@@ -396,6 +408,8 @@ class Manager:
         if getattr(self.attack, "warmup", None) is not None:   # mimic only
           extra["warmup"] = self.attack.warmup
         self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef, **extra)
+      return losses
+    if not self._rewrites_rows:   # no attack, or label flipping: the rows are final
       return losses
     forging = self.authenticator is not None and getattr(self.attack, "forges", False)
     for j, i in enumerate(self.local_workers):

@@ -750,14 +750,17 @@ __global__ void avgpool_bwd_kernel(T const* __restrict__ dy, T* __restrict__ dx,
 // ---------------------------------------------------------------------------- //
 // Softmax cross-entropy, one warp per row. logits bf16 [B, ld] (K valid columns), labels int64.
 // loss += mean_b(-sum_k t_k log p_k) ; dlogits = (p - t) / B  (bf16, same leading dimension).
+// Label flipping (Fang et al., USENIX Security 2020): the rows of groups >= flip_from train on K - 1 - y instead of y; a label
+// outside [0, K) matches no class and is left as it is. flip_from == groups flips nothing.
 template<typename T>
 __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long const* __restrict__ labels, T* __restrict__ dlogits, float* __restrict__ loss,
-                                    int B, int K, long long ld, float smoothing, int rows_per_group) {
+                                    int B, int K, long long ld, float smoothing, int rows_per_group, int flip_from) {
     pdl_trigger();
     pdl_wait();
     int const warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= B)
         return;
+    int const group = warp / rows_per_group;
     T const* row = logits + static_cast<long long>(warp) * ld;
     float mx = -INFINITY;
     for (int k = lane; k < K; k += 32)
@@ -769,7 +772,8 @@ __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long cons
         sum += __expf(to_f(row[k]) - mx);
     sum = warp_sum(sum);
     float const lse = mx + __logf(sum);
-    int const label = static_cast<int>(labels[warp]);
+    long long const y = labels[warp];
+    int const label = group >= flip_from && y >= 0 && y < K ? K - 1 - static_cast<int>(y) : static_cast<int>(y);
     float const off_t = smoothing / static_cast<float>(K), on_t = 1.f - smoothing + off_t;
     float const inv_b = 1.f / static_cast<float>(rows_per_group);   // each group (logical worker) averages over its own batch
     float local = 0.f;
@@ -783,7 +787,7 @@ __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long cons
     }
     local = warp_sum(local);
     if (lane == 0)
-        atomicAdd(loss + warp / rows_per_group, local * inv_b);
+        atomicAdd(loss + group, local * inv_b);
 }
 
 // uint8 NHWC image -> bf16 NHWC activations with C padded to `Cpad`: y = (x - mean[c]) * scale
@@ -1614,14 +1618,14 @@ int avgpool_backward_impl(void const* dy, void* dx, int N, int HW, int C, void* 
 }
 
 template<typename T>
-int softmax_xent_impl(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, void* stream) {
-    if (groups < 1 || B % groups)
+int softmax_xent_impl(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
+    if (groups < 1 || B % groups || flip_from < 0 || flip_from > groups)
         return 301;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     AGB_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float) * groups, s));
     int const warps_per_cta = 4;
     AGB_CUDA_OK(launch_pdl(softmax_xent_kernel<T>, dim3((B + warps_per_cta - 1) / warps_per_cta), dim3(warps_per_cta * 32), 0, s, static_cast<T const*>(logits), static_cast<long long const*>(labels),
-        static_cast<T*>(dlogits), static_cast<float*>(loss), B, K, ld, smoothing, B / groups));
+        static_cast<T*>(dlogits), static_cast<float*>(loss), B, K, ld, smoothing, B / groups, flip_from));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1818,10 +1822,17 @@ int agb_avgpool_backward_f32(void const* dy, void* dx, int N, int HW, int C, voi
 
 
 int agb_softmax_xent(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, void* stream) {
-    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, stream);
+    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, stream);
 }
 int agb_softmax_xent_f32(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, void* stream) {
-    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, stream);
+    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, stream);
+}
+// The same, with the labels of the groups >= flip_from (0 <= flip_from <= groups) flipped to K - 1 - y.
+int agb_softmax_xent_flip(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
+    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, stream);
+}
+int agb_softmax_xent_flip_f32(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
+    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, stream);
 }
 
 

@@ -451,21 +451,34 @@ def subsample_backward(backend, dy, shape, stride):
 # ---------------------------------------------------------------------------- #
 # Loss
 
-def softmax_xent(backend, logits, labels, label_smoothing=0.0, groups=1):
+def flip_labels(labels, classes, groups=1, flip_from=0):
+  """Labels of the label-flipping attack: y -> `classes` - 1 - y in the consecutive batch slices (groups) >= `flip_from`; a label outside
+  [0, classes) matches no class and is left as it is."""
+  if not 0 <= flip_from <= groups:
+    raise ValueError("flip_from must lie in [0, groups] (got %r for %d groups)" % (flip_from, groups))
+  lo = labels.shape[0] // groups * flip_from
+  tail = labels[lo:]
+  return torch.cat([labels[:lo], torch.where((tail >= 0) & (tail < classes), classes - 1 - tail, tail)])
+
+
+def softmax_xent(backend, logits, labels, label_smoothing=0.0, groups=1, flip_from=None):
   """Mean softmax cross-entropy -> (loss, dlogits [B, K]). `groups` == 1: 0-d loss over the batch; `groups` > 1: one mean per
-  consecutive batch slice (logical worker), loss of shape [groups], gradients scaled by 1 / (B / groups)."""
+  consecutive batch slice (logical worker), loss of shape [groups], gradients scaled by 1 / (B / groups). `flip_from`: the groups
+  >= flip_from train on `flip_labels` (label-flipping attack; None: no flip). A label outside [0, K) matches no class."""
   if backend == "native" and logits.is_cuda:
-    out = _native().softmax_xent(logits, labels, label_smoothing, groups)
+    out = _native().softmax_xent(logits, labels, label_smoothing, groups, flip_from)
     if out is not None:
       return out
     _fallback("softmax_xent")
+  if flip_from is not None:
+    labels = flip_labels(labels, logits.shape[1], groups, flip_from)
   if groups > 1:
     outs = [softmax_xent(backend, lg, lb, label_smoothing) for lg, lb in zip(_chunks(logits, groups), _chunks(labels, groups))]
     return torch.stack([o[0] for o in outs]), torch.cat([o[1] for o in outs], dim=0)
   z = logits if logits.dtype == torch.float64 else logits.float()
   logp = torch.log_softmax(z, dim=1)
   batch, classes = z.shape
-  target = torch.zeros_like(z).scatter_(1, labels.view(-1, 1).long(), 1.0)
+  target = (torch.arange(classes, device=z.device) == labels.view(-1, 1)).to(z.dtype)
   if label_smoothing > 0.:
     target = target * (1.0 - label_smoothing) + label_smoothing / classes
   loss = -(target * logp).sum(dim=1).mean()

@@ -818,15 +818,20 @@ def global_avgpool_backward(dy, shape):
   return dx
 
 
-def softmax_xent(logits, labels, label_smoothing, groups=1):
+def softmax_xent(logits, labels, label_smoothing, groups=1, flip_from=None):
+  """`flip_from`: the rows of groups >= flip_from train on the flipped labels K - 1 - y (label-flipping attack; None: no flip)."""
   if not enabled("xent") or logits.dtype not in _DTYPES or logits.stride(1) != 1:
     return None
   batch, classes = logits.shape
   dlogits = torch.empty_strided(logits.shape, logits.stride(), dtype=logits.dtype, device=logits.device)
   loss = torch.empty((groups,) if groups > 1 else (), dtype=torch.float32, device=logits.device)
   labels = labels if labels.dtype == torch.int64 else labels.long()
-  _check(_fn("agb_softmax_xent", logits)(_ptr(logits), _ptr(labels), _ptr(dlogits), _ptr(loss), ctypes.c_int(batch), ctypes.c_int(classes), ctypes.c_longlong(logits.stride(0)),
-                                 ctypes.c_float(label_smoothing), ctypes.c_int(groups), _stream()), "softmax_xent")
+  common = (_ptr(logits), _ptr(labels), _ptr(dlogits), _ptr(loss), ctypes.c_int(batch), ctypes.c_int(classes), ctypes.c_longlong(logits.stride(0)),
+            ctypes.c_float(label_smoothing), ctypes.c_int(groups))
+  if flip_from is None:
+    _check(_fn("agb_softmax_xent", logits)(*common, _stream()), "softmax_xent")
+  else:
+    _check(_fn("agb_softmax_xent_flip", logits)(*common, ctypes.c_int(flip_from), _stream()), "softmax_xent")
   return loss, dlogits
 
 
