@@ -1017,16 +1017,22 @@ def host_smea(G, f, return_details=False):
 OPTIMIZED_MODES = ("min-max", "min-sum")   # Shejwalkar & Houmansadr, NDSS 2021: gamma solved from whole-vector sums
 DEVIATIONS = ("unit-vec", "sign", "std")
 MIMIC_WARMUP = 100   # default number of warm-up steps T0 of mimic
+FANG_MODES = ("fang-krum", "fang-trim")   # Fang, Cao, Jia & Gong, USENIX Security 2020: full-knowledge Krum and trimmed-mean attacks
+FANG_THRESHOLD = 1e-5   # fang-krum: smallest candidate gamma tested after the first, in gradient units
+FANG_SCALE = 2.0   # fang-trim: the paper's b, the width of the interval beyond the extreme honest value
+FANG_MAX_CANDIDATES = 64
+FANG_TAG = 0x46414E47   # "FANG": the third splitmix64 input of fang-trim's key; >= 8 and != BUCKETING_TAG, so no DnC or bucketing key
 
 
 def check_byzantine_slots(n, byz_slots, mode):
-  """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("ipm" needs 1 honest row, the others 2)."""
-  if mode not in ("alie", "ipm", "mimic") + OPTIMIZED_MODES:
+  """Validated, ascending list of Byzantine slots of an n-row matrix for attack `mode` ("ipm" and "fang-trim" need 1 honest row, the
+  others 2)."""
+  if mode not in ("alie", "ipm", "mimic") + OPTIMIZED_MODES + FANG_MODES:
     raise tools.UserException("Unknown omniscient attack mode " + repr(mode))
   slots = sorted({int(i) for i in byz_slots})
   if not slots or slots[0] < 0 or slots[-1] >= n:
     raise tools.UserException("Byzantine slots must be a non-empty subset of [0, %d) (got %r)" % (n, list(byz_slots)))
-  need = 1 if mode == "ipm" else 2
+  need = 1 if mode in ("ipm", "fang-trim") else 2
   if n - len(slots) < need:
     raise tools.UserException("%s needs at least %d honest row(s) (n = %d, %d Byzantine)" % (mode.upper(), need, n, len(slots)))
   return slots
@@ -1147,12 +1153,34 @@ def torch_optimized_row(G, byz_slots, mode, deviation, gamma):
   return mu - _scalar(G)(gamma) * p
 
 
-def torch_craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False):
+def torch_craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False, f=None, threshold=None, scale=None, seed=None,
+                           step=None):
   """In place on the [n, d] fp32 matrix G: every Byzantine row <- `torch_byzantine_row` (ALIE, IPM) or, for Min-Max / Min-Sum, the row
   of `torch_optimized_row` with the gamma of `optimized_gamma`; honest rows are not written. Min-Max / Min-Sum with `return_details`
-  return (gamma, A, B, C, T) instead of G."""
+  return (gamma, A, B, C, T) instead of G. fang-krum (declared `f`, `threshold`) writes (-gamma) * sign(mu) with the gamma of
+  `fang_krum_gamma` and with `return_details` returns (gamma, selected, t, gamma_max, A, B, C, T); fang-trim (`scale`, `seed`, `step`)
+  writes every Byzantine row k its own `torch_fang_trim_row`."""
   if G.dtype != torch.float32:
     raise tools.UserException("Omniscient attacks craft fp32 rows (got %s)" % G.dtype)
+  if mode == "fang-krum":
+    slots = check_byzantine_slots(G.shape[0], byz_slots, mode)
+    threshold = check_fang_krum(G.shape[0], len(slots), f, threshold)
+    mu, p, A, B, C, T = fang_krum_statistics(G, slots)
+    gamma, selected, t, gamma_max = fang_krum_gamma(A, B, C, T, G.shape[0], f, slots, threshold)
+    row = torch.neg(_scalar(G)(gamma)) * p
+    for i in slots:
+      G[i].copy_(row)
+    return (gamma, selected, t, gamma_max, A, B, C, T) if return_details else G
+  if mode == "fang-trim":
+    if return_details:
+      raise tools.UserException("return_details is for Min-Max / Min-Sum / fang-krum only")
+    slots = check_byzantine_slots(G.shape[0], byz_slots, mode)
+    key = fang_trim_key(0 if seed is None else seed, step)
+    mu, lo, hi = fang_trim_interval(G, slots, check_fang_scale(scale))
+    rows = [fang_trim_value(mu, lo, hi, fang_trim_uniform(G.shape[1], k, key, G.device)) for k in slots]
+    for k, row in zip(slots, rows):
+      G[k].copy_(row)
+    return G
   details = None
   if mode in OPTIMIZED_MODES:
     mu, p, A, B, C, T = optimized_statistics(G, byz_slots, mode, deviation)
@@ -1166,6 +1194,162 @@ def torch_craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return
   for i in check_byzantine_slots(G.shape[0], byz_slots, mode):
     G[i].copy_(row)
   return details if return_details else G
+
+
+# Fang, Cao, Jia & Gong ("Local Model Poisoning Attacks to Byzantine-Robust Federated Learning", USENIX Security 2020), full knowledge,
+# written on gradient rows: the paper's crafted local model w' = w - lr g' becomes the gradient g'; its lambda becomes gamma = lambda / lr
+
+def check_fang_krum(n, K, f, threshold):
+  """-> the fp32 threshold of fang-krum for n rows, K of them Byzantine, the rule's declared f: n - f - 2 >= 1 (Krum's score has a
+  term), n - 2K - 1 >= 1 (the paper's bound on lambda), H = n - K >= 2, a finite threshold > 0 (default `FANG_THRESHOLD`)."""
+  if isinstance(f, bool) or not isinstance(f, int) or f < 0:
+    raise tools.UserException("fang-krum needs the declared number of Byzantine workers f, an integer >= 0 (got %r)" % (f,))
+  if n - f - 2 < 1 or n - 2 * K - 1 < 1 or n - K < 2:
+    raise tools.UserException("fang-krum needs n - f - 2 >= 1, n - 2 K - 1 >= 1 and at least 2 honest rows (got n = %d, f = %d, K = %d)" % (n, f, K))
+  value = fp32(FANG_THRESHOLD if threshold is None else threshold)
+  if not math.isfinite(value) or value <= 0:
+    raise tools.UserException("fang-krum: the threshold must be finite and > 0 in fp32 (got %r)" % (threshold,))
+  return value
+
+
+def check_fang_scale(scale):
+  """-> the fp32 scale beta of fang-trim (default `FANG_SCALE`): finite and > 1."""
+  value = fp32(FANG_SCALE if scale is None else scale)
+  if not math.isfinite(value) or value <= 1:
+    raise tools.UserException("fang-trim: the scale must be finite and > 1 in fp32 (got %r)" % (scale,))
+  return value
+
+
+def _sign(mu):
+  """+1, -1, +0 for +-0, NaN for NaN (Min-Max's `sign` deviation)."""
+  one = torch.ones_like(mu)
+  return torch.where(mu > 0, one, torch.where(mu < 0, -one, torch.where(mu == 0, torch.zeros_like(mu), mu)))
+
+
+def fang_krum_statistics(G, byz_slots):
+  """(mu, p, A, B, C, T) of fang-krum: ALIE's fp32 mu and p = sign(mu) per coordinate; A_i = sum h_i^2 and B_i = sum h_i p over the honest
+  rows (ascending slots), C = sum p^2, and T the honest pair distances sum (h_j - h_k)^2, pairs (j, k), j < k, in lexicographic order
+  (the kernel's layout). Every sum is taken in float64 from the fp32 values and rounded once to fp32 (Python floats)."""
+  byz = set(check_byzantine_slots(G.shape[0], byz_slots, "fang-krum"))
+  honest = [G[i] for i in range(G.shape[0]) if i not in byz]
+  mu = _honest_mean(honest, _scalar(G))
+  p = _sign(mu)
+  p64 = p.double()
+  X = torch.stack(honest).double()
+  A = [fp32(float((h * h).sum())) for h in X]
+  B = [fp32(float((h * p64).sum())) for h in X]
+  C = fp32(float((p64 * p64).sum()))
+  T = [fp32(float(((X[j] - X[k]) ** 2).sum())) for j in range(len(honest)) for k in range(j + 1, len(honest))]
+  return mu, p, A, B, C, T
+
+
+def _ascending_sum(values, count):
+  """0 + v_0 + v_1 + ... over the `count` smallest of `values`, ascending, in float64 (one rounding per addition)."""
+  total = 0.0
+  for v in sorted(values)[:count]:
+    total += v
+  return total
+
+
+def fang_krum_gamma(A, B, C, T, n, f, slots, threshold):
+  """-> (gamma, selected, t, gamma_max) of fang-krum from the fp32 sums of `fang_krum_statistics` (Python floats; T in pair order), for
+  n rows whose Byzantine slots are `slots`, Krum's declared f and the fp32 `threshold`. float64, one rounding per operation (the sm_90a
+  kernel runs the same operations):
+    gamma_max = min_i R_i / ((n - 2K - 1) sqrt(C)) + max_i sqrt(A_i) / sqrt(C), R_i the ascending sum of the H - 2 smallest sqrt(T_il),
+    l != i honest (the paper's bound on lambda, sqrt(C) in place of sqrt(d));
+    candidates gamma_t = gamma_max 2^-t, t = 0, 1, ... while t == 0 or gamma_t >= threshold, at most 64; the first one for which Krum
+    with f ranks a Byzantine slot first (ascending score, ties to the lower slot) is kept, else the last one tested. Krum sees the n
+    rows with distances 0 between Byzantine rows, max(0, (A_i + (2 gamma) B_i) + (gamma gamma) C) between a Byzantine row and honest
+    row i, T between honest rows; a score is the ascending sum of the row's n - f - 2 smallest distances.
+  gamma is rounded once to fp32. When C == 0 or any sum is not finite: (0.0, False, -1, 0.0), no candidate tested."""
+  slots = sorted(int(i) for i in slots)
+  K, H = len(slots), n - len(slots)
+  threshold = check_fang_krum(n, K, f, threshold)
+  values = list(A) + list(B) + [C] + list(T)
+  if len(A) != H or len(B) != H or len(T) != H * (H - 1) // 2:
+    raise tools.UserException("fang-krum: expected %d A_i, %d B_i and %d pair distances (got %d, %d, %d)" % (H, H, H * (H - 1) // 2, len(A), len(B), len(T)))
+  if C == 0 or not all(math.isfinite(v) for v in values):
+    return 0.0, False, -1, 0.0
+  pair = {}
+  at = 0
+  for j in range(H):
+    for k in range(j + 1, H):
+      pair[j, k] = pair[k, j] = float(T[at])
+      at += 1
+  others = [[pair[i, l] for l in range(H) if l != i] for i in range(H)]
+  R = [_ascending_sum([math.sqrt(v) for v in row], H - 2) for row in others]
+  root = math.sqrt(C)
+  gamma_max = min(R) / (float(n - 2 * K - 1) * root) + max(math.sqrt(a) for a in A) / root
+  honest_slots = [i for i in range(n) if i not in set(slots)]
+  m = n - f - 2
+  tested = None
+  for t in range(FANG_MAX_CANDIDATES):
+    gamma = gamma_max * 2.0 ** -t
+    if t > 0 and not gamma >= threshold:
+      break
+    tested = (gamma, t)
+    D = [(A[i] + (2.0 * gamma) * B[i]) + (gamma * gamma) * C for i in range(H)]
+    D = [v if v > 0.0 else 0.0 for v in D]
+    best = (_ascending_sum([0.0] * (K - 1) + D, m), slots[0])
+    for i, slot in enumerate(honest_slots):
+      best = min(best, (_ascending_sum(others[i] + [D[i]] * K, m), slot))
+    if best[1] in slots:
+      return fp32(gamma), True, t, gamma_max
+  return fp32(tested[0]), False, tested[1], gamma_max
+
+
+def fang_trim_key(seed, step):
+  """fang-trim's key K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ FANG_TAG): seed in [0, 2^64), step (the number of the update
+  the rows feed) in [0, 2^63)."""
+  if not isinstance(seed, (int, np.integer)) or isinstance(seed, bool) or not 0 <= seed <= _MASK64:
+    raise tools.UserException("fang-trim needs a seed in [0, 2^64) (got %r)" % (seed,))
+  if not isinstance(step, (int, np.integer)) or isinstance(step, bool) or not 0 <= step < 1 << 63:
+    raise tools.UserException("fang-trim needs a step key in [0, 2^63) (got %r)" % (step,))
+  return _splitmix64_int(_splitmix64_int(_splitmix64_int(int(seed)) ^ int(step)) ^ FANG_TAG)
+
+
+def fang_trim_uniform(d, slot, key, device="cpu"):
+  """u of Byzantine slot `slot` at the coordinates [0, d): (splitmix64(K ^ (x 32 + slot)) >> 40) 2^-24, an fp32 [d] tensor (exact)."""
+  with np.errstate(over="ignore"):
+    index = np.arange(d, dtype=np.uint64) * np.uint64(32) + np.uint64(slot)
+    z = _splitmix64(np.uint64(key) ^ index)
+  return torch.from_numpy((z >> np.uint64(40)).astype(np.float32) * np.float32(2.0 ** -24)).to(device)
+
+
+def fang_trim_interval(G, byz_slots, scale):
+  """(mu, lo, hi) of fang-trim per coordinate, fp32, one rounded operation at a time: ALIE's mu over the honest rows h (ascending slots);
+  mu > 0: e = min_i h_i, [lo, hi] = [e beta, e] if e <= 0 else [e / beta, e]; mu < 0: e = max_i h_i, [lo, hi] = [e, e beta] if e >= 0
+  else [e, e / beta]. The minimum and maximum are taken in ascending slot order, a later value replacing the running one only when
+  strictly smaller (larger). lo and hi are meaningless where mu is +-0 or NaN."""
+  byz = set(check_byzantine_slots(G.shape[0], byz_slots, "fang-trim"))
+  honest = [G[i] for i in range(G.shape[0]) if i not in byz]
+  scalar = _scalar(G)
+  mu = _honest_mean(honest, scalar)
+  low, high = honest[0], honest[0]
+  for h in honest[1:]:
+    low = torch.where(h < low, h, low)
+    high = torch.where(h > high, h, high)
+  beta = scalar(scale)
+  pos = mu > 0
+  e = torch.where(pos, low, high)
+  scaled, shrunk = e * beta, e / beta
+  lo = torch.where(pos, torch.where(e <= 0, scaled, shrunk), e)
+  hi = torch.where(pos, e, torch.where(e >= 0, scaled, shrunk))
+  return mu, lo, hi
+
+
+def fang_trim_value(mu, lo, hi, u):
+  """b = lo + u (hi - lo), fp32 with one rounding per operation; b = mu where mu is +-0 or NaN."""
+  b = lo + u * (hi - lo)
+  return torch.where((mu > 0) | (mu < 0), b, mu)
+
+
+def torch_fang_trim_row(G, byz_slots, slot, scale, key):
+  """The fang-trim row of Byzantine slot `slot` of the [n, d] fp32 matrix G, with scale beta and key K (`fang_trim_key`): per coordinate
+  x, b = lo + u (hi - lo) over `fang_trim_interval`, u = `fang_trim_uniform`; b = mu where mu is +-0 or NaN. The row is pushed past
+  every honest value, against the sign of the mean."""
+  mu, lo, hi = fang_trim_interval(G, byz_slots, check_fang_scale(scale))
+  return fang_trim_value(mu, lo, hi, fang_trim_uniform(G.shape[1], slot, key, G.device))
 
 
 def check_mimic(n, byz_slots, warmup):

@@ -8,9 +8,10 @@ overwrites their row of the gradient matrix, on the device, before the aggregati
 Contract: `cls(nbworkers, nbbyzwrks, args)`; `apply(row, worker, step, state)` mutates the flat fp32 gradient `row`
 in place (`state` is a per-worker dict that persists across steps). Dropping a `.py` file here auto-registers it.
 Omniscient attacks (`omniscient = True`, `omniscient.py`) see every honest row instead: they implement no `apply`, and expose `mode`
-("alie", "ipm", "min-max", "min-sum" or "mimic"), the fp32 coefficient `coef` (None for Min-Max / Min-Sum, which solve theirs every step,
-and for mimic), `deviation` (Min-Max / Min-Sum; None otherwise) and `warmup` (mimic only); the aggregation engine crafts the Byzantine
-rows (`craft_byzantine`) on every rank.
+("alie", "ipm", "min-max", "min-sum", "mimic", "fang-krum" or "fang-trim"), the fp32 coefficient `coef` (None for Min-Max / Min-Sum and
+fang-krum, which solve theirs every step, and for mimic and fang-trim), `deviation` (Min-Max / Min-Sum; None otherwise), `warmup` (mimic
+only), `threshold` (fang-krum only), `scale` and `seed` (fang-trim only); the aggregation engine crafts the Byzantine rows
+(`craft_byzantine`) on every rank.
 Label-flipping attacks (`flips_labels = True`, `data.py`) implement no `apply` either: the Byzantine workers' loss trains on flipped
 labels (the trainer sets `Context.flip_from`), so nothing rewrites their rows after the backward pass.
 Construction raises `UserException` for arguments outside an attack's bounds.

@@ -16,10 +16,24 @@
           estimated by an online power iteration; then i* is frozen. It does nothing under IID data and is the standard test of the
           heterogeneity defences (bucketing, NNM) under non-IID data (`dirichlet:<alpha>`). The arithmetic is
           `aggregators._ops.torch_mimic_step_`; the engine keeps the state (z, t, i*) and checkpoints it.
+* `fang-krum`, `fang-trim`  the full-knowledge local model poisoning attacks of Fang, Cao, Jia & Gong ("Local Model Poisoning Attacks
+          to Byzantine-Robust Federated Learning", USENIX Security 2020) against Krum and against trimmed mean (also used against median).
+          The paper crafts local models w' = w - lr g'; here, as for every attack, the Byzantine rows are gradients g', so its lambda is
+          gamma = lambda / lr and its direction s = -sign(mu) (mu the honest mean). Under Adam or RMSProp this gradient-space attack is
+          what runs, not a model-space one.
+          fang-krum: every Byzantine row is (-gamma) * sign(mu). gamma_max is the paper's upper bound on lambda in gradient units, with
+          sqrt(sum p^2) in place of sqrt(d); gamma halves from gamma_max until Krum, modelled on the exchanged whole-vector sums with the
+          engine's declared f, ranks a Byzantine row first, or until it falls below `threshold:<x>` (default 1e-5, in gradient units).
+          All K rows are identical (the paper's other c - 1 models sit in an epsilon-ball around the first one): Krum's index-stable
+          ranking then selects one of them exactly when it would select that first one (`aggregators._ops.fang_krum_gamma`).
+          fang-trim: per coordinate, every Byzantine row draws its own value in the interval past the honest extreme against the sign of
+          mu: [e beta, e] or [e / beta, e] below e = min_i h_i when mu > 0, [e, e beta] or [e, e / beta] above e = max_i h_i when mu < 0
+          (`scale:<beta>`, the paper's b, default 2, > 1). The draw is keyed by `seed:<int>` (default 0), the update number, the row's
+          slot and the coordinate, so the rows are the same bits on every engine and rank count (`aggregators._ops.torch_fang_trim_row`).
 
 The rows are crafted by the aggregation engine (`craft_byzantine`), not per worker: on the fused engine every rank computes its owned
 coordinates of every Byzantine row from the honest values it already reads for the rule, and stores them into the Byzantine rows over
-NVLink (Min-Max / Min-Sum first exchange their whole-vector sums between the ranks). The exact arithmetic is
+NVLink (Min-Max / Min-Sum and fang-krum first exchange their whole-vector sums between the ranks). The exact arithmetic is
 `aggregators._ops.torch_byzantine_row` and `torch_optimized_row`. The Byzantine workers are the last k logical workers.
 """
 
@@ -51,6 +65,9 @@ class _Omniscient(_Attack):
   omniscient = True
   mode = None
   deviation = None   # Min-Max / Min-Sum: "unit-vec", "sign" or "std"
+  threshold = None   # fang-krum: smallest candidate gamma tested after the first
+  scale = None   # fang-trim: beta
+  seed = None   # fang-trim: seed of the draw
   min_honest = 1
 
   def __init__(self, nbworkers, nbbyzwrks, args):
@@ -133,8 +150,51 @@ class MimicAttack(_Omniscient):
     self.coef = None
 
 
+class FangKrumAttack(_Omniscient):
+  """fang-krum: no coefficient (gamma is searched every step), only the threshold (`threshold:<x>`, finite, > 0, in gradient units)."""
+  mode = "fang-krum"
+  min_honest = 2
+
+  def __init__(self, nbworkers, nbbyzwrks, args):
+    super().__init__(nbworkers, nbbyzwrks, args)
+    from ..aggregators import _ops
+    unknown = set(self.args) - {"threshold"}
+    if unknown:
+      raise tools.UserException("fang-krum: unknown argument(s) %s (expected 'threshold:<x>')" % ", ".join(sorted(unknown)))
+    if 2 * nbbyzwrks + 1 >= nbworkers:
+      raise tools.UserException("fang-krum needs n - 2 k - 1 >= 1 (got n = %d, k = %d)" % (nbworkers, nbbyzwrks))
+    self.threshold = self._coefficient("threshold", lambda: _ops.fp32(_ops.FANG_THRESHOLD))
+    if not self.threshold > 0:
+      raise tools.UserException("fang-krum: the threshold must be > 0 (got %r)" % (self.args["threshold"],))
+    self.coef = None
+
+
+class FangTrimAttack(_Omniscient):
+  """fang-trim: no coefficient, the scale beta (`scale:<beta>`, finite, > 1) and the seed of the draw (`seed:<int>`, in [0, 2^64))."""
+  mode = "fang-trim"
+
+  def __init__(self, nbworkers, nbbyzwrks, args):
+    super().__init__(nbworkers, nbbyzwrks, args)
+    from ..aggregators import _ops
+    unknown = set(self.args) - {"scale", "seed"}
+    if unknown:
+      raise tools.UserException("fang-trim: unknown argument(s) %s (expected 'scale:<beta>', 'seed:<int>')" % ", ".join(sorted(unknown)))
+    self.scale = _ops.check_fang_scale(self._coefficient("scale", lambda: _ops.FANG_SCALE))
+    seed = 0
+    if "seed" in self.args:
+      try:
+        seed = int(self.args["seed"])
+      except ValueError:
+        raise tools.UserException("fang-trim: 'seed' expects an integer in [0, 2^64) (got %r)" % (self.args["seed"],))
+    _ops.fang_trim_key(seed, 0)
+    self.seed = seed
+    self.coef = None
+
+
 register("alie", AlieAttack)
 register("ipm", IpmAttack)
 register("min-max", MinMaxAttack)
 register("min-sum", MinSumAttack)
 register("mimic", MimicAttack)
+register("fang-krum", FangKrumAttack)
+register("fang-trim", FangTrimAttack)

@@ -407,6 +407,9 @@ class Manager:
         extra = {} if deviation is None else {"deviation": deviation}
         if getattr(self.attack, "warmup", None) is not None:   # mimic only
           extra["warmup"] = self.attack.warmup
+        for key in ("threshold", "scale", "seed"):   # fang-krum: threshold; fang-trim: scale, seed
+          if getattr(self.attack, key, None) is not None:
+            extra[key] = getattr(self.attack, key)
         self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef, **extra)
       return losses
     if not self._rewrites_rows:   # no attack, or label flipping: the rows are final

@@ -28,7 +28,8 @@
 // Attacked steps with an omniscient attack (ALIE / IPM) run `gar_byzantine_kernel` first: each rank crafts its owned coordinates of
 // every Byzantine row from the honest values. Min-Max / Min-Sum run `gar_optimized_kernel` instead: a statistics pass, one exchange of
 // whole-vector sums between the ranks, then the same per-coordinate write. Mimic runs `gar_mimic_warmup_kernel` (two exchanges) during
-// its warm-up and `gar_mimic_copy_kernel` after it.
+// its warm-up and `gar_mimic_copy_kernel` after it. Fang et al.'s Krum attack runs `gar_fang_krum_kernel` (Min-Max's passes and exchange,
+// then a one-warp search over gamma), their trimmed-mean attack `gar_fang_trim_kernel` (one pass, a counter-based draw per row).
 // DnC (rule kDnc) has a finish kernel of its own, `gar_dnc_kernel`: a sampled distance pass, one exchange, a float64 Jacobi per CTA,
 // then Krum's phase D (see `dnc_selection`).
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
@@ -2318,8 +2319,15 @@ struct ByzArgs {
     float* y;                          // (local) scratch, same layout: y, kept apart so that z survives a degenerate ||y||
     int* istar;                        // [1] (local) target slot i*; a value that is no honest slot (-1 before any update) means the first one
     double* mimic_stats;               // optional [kMimicStats]: s_i, q_i, ||y||^2, 1 / ||y|| of the last warm-up step
+    // Fang et al. only (`gar_fang_krum_kernel`: coef is the threshold; `gar_fang_trim_kernel`: coef is the scale beta)
+    int f;                             // fang-krum: the rule's declared f
+    int search;                        // fang-krum: 0 skips the candidate search (gamma = gamma_max), to time the passes alone
+    double* fang_out;                  // fang-krum, optional [kFangOut]: gamma_max, t, selected
+    unsigned long long key;            // fang-trim: K = splitmix64(splitmix64(splitmix64(seed) ^ step) ^ TAG), from the host
 };
 enum ByzMode { kAlie = 0, kIpm = 1, kMinMax = 2, kMinSum = 3 };
+constexpr int kFangCandidates = 64;   // fang-krum: candidates gamma_max 2^-t, t < 64
+constexpr int kFangOut = 3;           // fang-krum's `fang_out`: gamma_max, t (-1: no candidate tested), selected (0 / 1)
 enum Deviation { kUnitVec = 0, kSign = 1, kStd = 2 };
 
 template<int N>
@@ -2825,8 +2833,8 @@ __device__ void mimic_y_pass(ByzArgs const& a, Shared& sh, int* pair_of, float c
 }
 
 // block 0 adds the CTA partials [lo, hi) in index order and posts them into region 2 of every rank, then signals `slot`; returns once
-// every rank's post is visible to every CTA
-__device__ void mimic_exchange(ByzArgs const& a, cg::grid_group& grid, int lo, int hi, int slot, uint32_t epoch) {
+// every rank's post is visible to every CTA (mimic's two exchanges, fang-krum's one)
+__device__ void stats_exchange(ByzArgs const& a, cg::grid_group& grid, int lo, int hi, int slot, uint32_t epoch) {
     bool const multi = a.R > 1;
     __threadfence();
     grid.sync();
@@ -2887,14 +2895,14 @@ __global__ void __launch_bounds__(256) gar_mimic_warmup_kernel(ByzArgs const a) 
     // -------- pass 1 and exchange 1: s_i -------- //
     for (int i0 = 0; i0 < H; i0 += kBlockRows)
         mimic_s_pass<N>(a, sh, pair_of, i0, mine, tid, nthreads);
-    mimic_exchange(a, grid, kMimicS, kMimicS + H, kSlotCraftStats, epoch);
+    stats_exchange(a, grid, kMimicS, kMimicS + H, kSlotCraftStats, epoch);
     int const lane = threadIdx.x;
     if (lane < H)
         s_sh[lane] = __double2float_rn(mimic_total(a, kMimicS + lane));
     __syncthreads();
     // -------- pass 2 and exchange 2: y, q_i, ||y||^2 -------- //
     mimic_y_pass<N>(a, sh, pair_of, s_sh, mine, tid, nthreads);
-    mimic_exchange(a, grid, kMimicQ, kMimicY + 1, kSlotMimic, epoch);
+    stats_exchange(a, grid, kMimicQ, kMimicY + 1, kSlotMimic, epoch);
     if (lane < H)
         q_sh[lane] = mimic_total(a, kMimicQ + lane);
     if (lane == kMaxWorkers)
@@ -2969,6 +2977,342 @@ __global__ void __launch_bounds__(256) gar_mimic_copy_kernel(ByzArgs const a) {
             V<4>::load_stream(src + x, h);
             for (int k = 0; k < a.K; ++k)
                 V<4>::store_stream(a.rows[a.byz[k]] + x, h);
+        }
+    }
+    fence_sys();
+}
+
+// ---- Fang, Cao, Jia & Gong (USENIX Security 2020): full-knowledge Krum and trimmed-mean attacks, on gradient rows ------------- //
+// fang-krum: every Byzantine row is b = (-gamma) * p, p = sign(mu) (Min-Max's `sign` deviation), one fp32 multiply. gamma comes from the
+// fp32 sums A_i = sum h_i^2, B_i = sum h_i p, C = sum p^2 and the honest distances T_jk = sum (h_j - h_k)^2, posted in Min-Max's layout
+// (pairs, A[32], B[32], C). In float64 with explicit roundings, as `_ops.fang_krum_gamma`:
+//   gamma_max = min_i R_i / ((n - 2K - 1) sqrt(C)) + max_i sqrt(A_i) / sqrt(C), R_i the ascending sum of the H - 2 smallest sqrt(T_il);
+//   candidates gamma_max 2^-t, t = 0, 1, ... while t == 0 or gamma_t >= threshold (at most 64): the first one for which Krum with the
+//   declared f ranks a Byzantine slot first (ascending score, ties to the lower slot) is kept, else the last one tested; rounded once.
+//   Krum sees 0 between Byzantine rows, max(0, (A_i + (2 gamma) B_i) + (gamma gamma) C) between a Byzantine row and honest row i, T
+//   between honest rows; a score is the ascending sum of the row's n - f - 2 smallest distances.
+//   gamma = 0 (not selected, t = -1) when C == 0 or any sum is not finite.
+// One cooperative launch per rank on `gar_optimized_kernel`'s scaffolding: entry barrier (slot kSlotCraft); statistics pass and honest
+// distance pass (`phase_a_segment` on the honest rows); one exchange through region 2 and slot kSlotCraftStats; the search on warp 0 of
+// every CTA (a lane per honest row, whose distances are sorted once; per candidate a lane merges them with its K copies of the
+// Byzantine distance, O(n) additions, and one lane scores the Byzantine rows, which all have the same score); write pass. No exit
+// barrier, system-scope fence at the end, as `gar_optimized_kernel` (same argument: region 2 and its slot belong to the crafting kernels
+// and an engine runs one attack).
+//
+// fang-trim: per coordinate x (global index of the padded vector) and Byzantine slot k, b = lo + u (hi - lo) (fp32, one rounding per
+// operation) with, from ALIE's mu and the honest rows h (ascending slots):
+//   mu > 0: e = min_i h_i, [lo, hi] = [e beta, e] if e <= 0, else [e / beta, e];
+//   mu < 0: e = max_i h_i, [lo, hi] = [e, e beta] if e >= 0, else [e, e / beta];
+//   b = mu when mu is +-0 or NaN; u = (splitmix64(K ^ (x 32 + k)) >> 40) 2^-24.
+// The draw depends on (seed, step, slot, x) only: the rows are the same bits on every engine and every rank count. One pass, no
+// exchange, `gar_byzantine_kernel`'s entry barrier and closing fence.
+
+// A_i and B_i of the honest rows [i0, i0 + 8) (and C with the first block) over every owned segment, folded into `out`
+template<int N>
+__device__ void fang_stats_pass(ByzArgs const& a, Shared& sh, int* pair_of, int i0, float* out, long long tid, long long nthreads) {
+    constexpr int B = kBlockRows, COUNT = 2 * B + 1;
+    static_assert(N == 0 || N == B, "registers hold one block of honest rows");
+    int const H = a.H;
+    if (threadIdx.x < COUNT) {
+        int const t = threadIdx.x, i = i0 + t % B;
+        pair_of[t] = t == 2 * B ? (i0 == 0 ? kStatC : -1) : i < H ? (t < B ? kStatA : kStatB) + i : -1;
+    }
+    __syncthreads();
+    float acc[COUNT];
+#pragma unroll
+    for (int k = 0; k < COUNT; ++k)
+        acc[k] = 0.f;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4];
+            mean_and_deviation<N>(a, x, g, mu, p);   // a.deviation == kSign
+#pragma unroll
+            for (int i = 0; i < B; ++i) {
+                if (i0 + i < H) {
+                    float h[4];
+                    honest_value<N>(a, x, g, N > 0 ? i : i0 + i, h);   // N > 0: one block, i0 == 0, a static register index
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        acc[i] = __fmaf_rn(h[c], h[c], acc[i]);
+                        acc[B + i] = __fmaf_rn(h[c], p[c], acc[B + i]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                acc[2 * B] = __fmaf_rn(p[c], p[c], acc[2 * B]);
+        }
+    }
+    fold_pass<COUNT>(sh, acc, out, pair_of);
+}
+
+// the search of fang-krum on warp 0 over the statistics `st` summed over the ranks: lane i < H is honest row i (slot honest[i]), lane H
+// the Byzantine rows. `sorted`: [32][32] float64 scratch (row i: the H - 1 honest distances of row i, ascending), `dist` / `ranked`: [32].
+// Lane 0 stores gamma_max, t, selected and the float64 gamma into `out`.
+__device__ void fang_krum_search(ByzArgs const& a, float const* st, double (*sorted)[kMaxWorkers], double* dist, double* ranked, double* out) {
+    unsigned const all = 0xffffffffu;
+    int const lane = threadIdx.x & 31, H = a.H, K = a.K, n = H + K, m = n - a.f - 2, npairs = H * (H - 1) / 2;
+    bool finite = lane != 0 || (is_finite(st[kStatC]) && st[kStatC] != 0.f);
+    for (int k = lane; k < npairs; k += 32)
+        finite = finite && is_finite(st[k]);
+    if (lane < H)
+        finite = finite && is_finite(st[kStatA + lane]) && is_finite(st[kStatB + lane]);
+    if (!__all_sync(all, finite)) {
+        if (lane == 0) {
+            out[0] = 0.0;
+            out[1] = -1.0;
+            out[2] = 0.0;
+            out[3] = 0.0;
+        }
+        return;
+    }
+    double const C = st[kStatC];
+    double R = __longlong_as_double(0x7ff0000000000000ll), root_a = -R;   // +inf, -inf: neutral for the lanes >= H
+    double A = 0.0, Bi = 0.0;
+    if (lane < H) {
+        A = st[kStatA + lane];
+        Bi = st[kStatB + lane];
+        int count = 0;
+        for (int l = 0; l < H; ++l) {   // insertion sort of the row's honest distances
+            if (l == lane)
+                continue;
+            double const v = st[l < lane ? pair_index(l, lane, H) : pair_index(lane, l, H)];
+            int at = count++;
+            for (; at > 0 && sorted[lane][at - 1] > v; --at)
+                sorted[lane][at] = sorted[lane][at - 1];
+            sorted[lane][at] = v;
+        }
+        R = 0.0;
+        for (int k = 0; k < H - 2; ++k)
+            R = __dadd_rn(R, __dsqrt_rn(sorted[lane][k]));
+        root_a = __dsqrt_rn(A);
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        R = fmin(R, __shfl_xor_sync(all, R, off));
+        root_a = fmax(root_a, __shfl_xor_sync(all, root_a, off));
+    }
+    double const root = __dsqrt_rn(C);
+    double const gamma_max = __dadd_rn(__ddiv_rn(R, __dmul_rn(static_cast<double>(n - 2 * K - 1), root)), __ddiv_rn(root_a, root));
+    double const threshold = a.coef;
+    double gamma = gamma_max;
+    int t = 0, selected = 0;
+    int const candidates = a.search ? kFangCandidates : 1;
+    for (int c = 0; c < candidates; ++c) {
+        double const g = __dmul_rn(gamma_max, ldexp(1.0, -c));
+        if (c > 0 && !(g >= threshold))
+            break;
+        gamma = g;
+        t = c;
+        if (!a.search)
+            break;
+        double D = 0.0;
+        if (lane < H) {
+            D = __dadd_rn(__dadd_rn(A, __dmul_rn(__dmul_rn(2.0, g), Bi)), __dmul_rn(__dmul_rn(g, g), C));
+            D = D > 0.0 ? D : 0.0;
+            dist[lane] = D;
+        }
+        __syncwarp();
+        double score = __longlong_as_double(0x7ff0000000000000ll);
+        int slot = kMaxWorkers;
+        if (lane < H) {   // merge the sorted honest distances with K copies of D, the m smallest added in ascending order
+            int rank = 0;
+            for (int l = 0; l < H; ++l)
+                rank += dist[l] < D || (dist[l] == D && l < lane);
+            ranked[rank] = D;
+            score = 0.0;
+            for (int q = 0, j = 0, copies = 0; q < m; ++q) {
+                double v;
+                if (j < H - 1 && (copies >= K || sorted[lane][j] <= D)) {
+                    v = sorted[lane][j++];
+                } else {
+                    v = D;
+                    ++copies;
+                }
+                score = __dadd_rn(score, v);
+            }
+            slot = a.honest[lane];
+        }
+        __syncwarp();
+        if (lane == H) {   // K - 1 zeros, then the distances to the honest rows in ascending order
+            score = 0.0;
+            for (int q = 0; q < m; ++q)
+                score = __dadd_rn(score, q < K - 1 ? 0.0 : ranked[q - (K - 1)]);
+            slot = a.byz[0];
+        }
+        for (int off = 16; off > 0; off >>= 1) {
+            double const other = __shfl_xor_sync(all, score, off);
+            int const other_slot = __shfl_xor_sync(all, slot, off);
+            if (other < score || (other == score && other_slot < slot)) {
+                score = other;
+                slot = other_slot;
+            }
+        }
+        __syncwarp();
+        if (slot == a.byz[0]) {
+            selected = 1;
+            break;
+        }
+    }
+    if (lane == 0) {
+        out[0] = gamma_max;
+        out[1] = t;
+        out[2] = selected;
+        out[3] = gamma;
+    }
+}
+
+template<int N>
+__global__ void __launch_bounds__(256) gar_fang_krum_kernel(ByzArgs const a) {
+    __shared__ Shared sh;
+    __shared__ int pair_of[kBlockRows * kBlockRows];
+    __shared__ float stats[kCraftStats];
+    __shared__ double sorted[kMaxWorkers][kMaxWorkers];
+    __shared__ double dist[kMaxWorkers], ranked[kMaxWorkers];
+    __shared__ double result[kFangOut + 1];
+    cg::grid_group grid = cg::this_grid();
+    uint32_t const epoch = current_epoch(a);
+    if (a.R > 1) {
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const H = a.H;
+    float* const mine = a.partials + static_cast<long long>(blockIdx.x) * kCraftStats;
+    for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x)
+        mine[k] = 0.f;
+    __syncthreads();
+    // -------- statistics of the owned coordinates, then the honest distances -------- //
+    for (int i0 = 0; i0 < H; i0 += kBlockRows)
+        fang_stats_pass<N>(a, sh, pair_of, i0, mine, tid, nthreads);
+    for (int seg = 0; seg < a.nseg; ++seg)
+        phase_a_segment<(N == 0)>(a, sh, pair_of, seg, mine, tid, nthreads);
+    // -------- exchange: CTAs in index order, then ranks in rank order -------- //
+    stats_exchange(a, grid, 0, kCraftStats, kSlotCraftStats, epoch);
+    float const* const box = a.mailbox[a.rank] + kCraftRegion;
+    for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x) {
+        float s = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            s += ld_volatile_f(box + q * kCraftStats + k);
+        stats[k] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32)
+        fang_krum_search(a, stats, sorted, dist, ranked, result);
+    __syncthreads();
+    float const gamma = __double2float_rn(result[kFangOut]);
+    if (blockIdx.x == 0) {
+        if (a.stats_out) {
+            for (int k = threadIdx.x; k < kCraftStats; k += blockDim.x)
+                a.stats_out[1 + k] = stats[k];
+            if (threadIdx.x == 0)
+                a.stats_out[0] = gamma;
+        }
+        if (a.fang_out && threadIdx.x < kFangOut)
+            a.fang_out[threadIdx.x] = result[threadIdx.x];
+    }
+    // -------- b = (-gamma) * sign(mu) into every Byzantine row -------- //
+    float const neg = -gamma;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float g[N > 0 ? N : 1][4];
+            if constexpr (N > 0) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+            }
+            float mu[4], p[4], out[4];
+            mean_and_deviation<N>(a, x, g, mu, p);
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                out[c] = __fmul_rn(neg, p[c]);
+            for (int k = 0; k < a.K; ++k)
+                V<4>::store_stream(a.rows[a.byz[k]] + x, out);
+        }
+    }
+    fence_sys();
+}
+
+template<int N>
+__global__ void __launch_bounds__(256) gar_fang_trim_kernel(ByzArgs const a) {
+    if (a.R > 1) {
+        uint32_t const epoch = current_epoch(a);
+        signal_all(a, kSlotCraft, epoch);
+        wait_all(a, kSlotCraft, epoch);
+        __syncthreads();
+    }
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const H = a.H;
+    float const count = static_cast<float>(H), beta = a.coef;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / 4;
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * 4;
+            float mu[4], low[4], high[4];
+            auto add = [&](int i, float const (&h)[4]) {   // the sum of ALIE's mean, and the running min / max (strict comparisons)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    mu[c] = i == 0 ? h[c] : __fadd_rn(mu[c], h[c]);
+                    low[c] = i == 0 || h[c] < low[c] ? h[c] : low[c];
+                    high[c] = i == 0 || h[c] > high[c] ? h[c] : high[c];
+                }
+            };
+            if constexpr (N > 0) {   // registers: the H honest values are loaded together
+                float g[N][4];
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        V<4>::load_stream(a.rows[a.honest[i]] + x, g[i]);
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if (i < H)
+                        add(i, g[i]);
+            } else {
+                for (int i = 0; i < H; ++i) {
+                    float h[4];
+                    V<4>::load_stream(a.rows[a.honest[i]] + x, h);
+                    add(i, h);
+                }
+            }
+            float base[4], span[4];
+            bool push[4];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                mu[c] = __fdiv_rn(mu[c], count);
+                bool const pos = mu[c] > 0.f;
+                push[c] = pos || mu[c] < 0.f;
+                float const e = pos ? low[c] : high[c];
+                float const scaled = __fmul_rn(e, beta), shrunk = __fdiv_rn(e, beta);
+                float const l = pos ? (e <= 0.f ? scaled : shrunk) : e;
+                float const h = pos ? e : (e >= 0.f ? scaled : shrunk);
+                base[c] = l;
+                span[c] = __fsub_rn(h, l);
+            }
+            for (int k = 0; k < a.K; ++k) {
+                unsigned long long const slot = static_cast<unsigned long long>(a.byz[k]);
+                float out[4];
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    unsigned long long const z = splitmix64(a.key ^ (static_cast<unsigned long long>(x + c) * 32ull + slot));
+                    float const u = __fmul_rn(static_cast<float>(static_cast<unsigned>(z >> 40)), 5.9604644775390625e-08f);   // 2^-24, exact
+                    out[c] = push[c] ? __fadd_rn(base[c], __fmul_rn(u, span[c])) : mu[c];
+                }
+                V<4>::store_stream(a.rows[a.byz[k]] + x, out);
+            }
         }
     }
     fence_sys();
@@ -3523,6 +3867,131 @@ int agb_gar_byzantine_mimic(unsigned long long const* rows, int n, long long con
     AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_mimic_warmup_kernel<kBlockRows>)
                                                          : reinterpret_cast<void*>(gar_mimic_warmup_kernel<0>),
                                             dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
+    return 0;
+}
+
+// The arguments the Fang kernels share with `agb_gar_byzantine`: the rows (honest ones also as `grad` for `phase_a_segment`), the slot
+// masks, the owned segments (`work`: their float4 count), the ranks and their signal pads. Returns a status.
+static int fang_args(ByzArgs& a, unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg,
+                     unsigned honest, unsigned byzantine, int R, int rank, unsigned long long const* signals, unsigned epoch,
+                     unsigned long long epoch_ptr, long long& work) {
+    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
+        return 100;
+    if (nseg < 1 || nseg > kMaxSeg)
+        return 101;
+    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
+    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < 1)
+        return 114;
+    a.H = H;
+    a.K = K;
+    a.n = H;
+    for (int i = 0, h = 0, b = 0; i < n; ++i) {
+        a.rows[i] = reinterpret_cast<float*>(rows[i]);
+        if ((honest >> i) & 1u) {
+            a.grad[h] = a.rows[i];
+            a.honest[h++] = i;
+        }
+        if ((byzantine >> i) & 1u)
+            a.byz[b++] = i;
+    }
+    a.nseg = nseg;
+    work = 0;
+    for (int s = 0; s < nseg; ++s) {
+        a.seg_lo[s] = seg_lo[s];
+        a.seg_hi[s] = seg_hi[s];
+        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
+            return 101;
+        work += (seg_hi[s] - seg_lo[s]) / 4;
+    }
+    a.R = R;
+    a.rank = rank;
+    for (int q = 0; q < R; ++q) {
+        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
+        if (R > 1 && !a.signal[q])
+            return 109;
+    }
+    a.epoch = epoch;
+    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
+    return 0;
+}
+
+// fang-krum over this rank's owned segments; see `gar_fang_krum_kernel`. Arguments as `agb_gar_byzantine_optimized`, plus: `f`: the rule's
+// declared f; `threshold`: finite, > 0; `search`: 0 skips the candidate search (gamma = gamma_max, for timing the passes alone);
+// `fang_out`: optional [3] float64, gamma_max, t, selected. Every row must be honest or Byzantine, with n - f - 2 >= 1,
+// n - 2K - 1 >= 1 and H >= 2 (status 125 otherwise). Cooperative launch; collective when R > 1.
+int agb_gar_byzantine_fang_krum(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                                unsigned byzantine, int f, float threshold, int search, int R, int rank, unsigned long long const* signals,
+                                unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long stats_out,
+                                unsigned long long fang_out, unsigned epoch, unsigned long long epoch_ptr, void* stream) {
+    ByzArgs a{};
+    long long work = 0;
+    int const status = fang_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, R, rank, signals, epoch, epoch_ptr, work);
+    if (status)
+        return status;
+    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
+    if ((honest | byzantine) != all || f < 0 || n - f - 2 < 1 || n - 2 * a.K - 1 < 1 || a.H < 2 || !(threshold > 0.f) || !std::isfinite(threshold))
+        return 125;
+    a.deviation = kSign;
+    a.f = f;
+    a.coef = threshold;
+    a.search = search ? 1 : 0;
+    for (int q = 0; q < R; ++q) {
+        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
+        if (!a.mailbox[q])
+            return 108;
+    }
+    a.partials = reinterpret_cast<float*>(partials);
+    a.stats_out = reinterpret_cast<float*>(stats_out);
+    a.fang_out = reinterpret_cast<double*>(fang_out);
+    if (!a.partials || partial_ctas < 1)
+        return 108;
+    // the grid depends only on the owned work (and the device), as for `gar_optimized_kernel`
+    int const threads = 256;
+    bool const in_registers = a.H <= kBlockRows;
+    int per_sm = 0;
+    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_fang_krum_kernel<kBlockRows> : gar_fang_krum_kernel<0>,
+                                                              threads, 0));
+    if (per_sm < 1)
+        return 2;
+    long long grid = (work + threads - 1) / threads;
+    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
+    cap = cap > partial_ctas ? partial_ctas : cap;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
+    void* params[] = {&a};
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_fang_krum_kernel<kBlockRows>)
+                                                         : reinterpret_cast<void*>(gar_fang_krum_kernel<0>),
+                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
+    return 0;
+}
+
+// fang-trim over this rank's owned segments; see `gar_fang_trim_kernel`. Arguments as `agb_gar_byzantine`, plus: `scale`: beta, finite and
+// > 1 (status 125 otherwise); `key`: splitmix64(splitmix64(splitmix64(seed) ^ step) ^ TAG) (`_ops.fang_trim_key`). Collective when R > 1.
+int agb_gar_byzantine_fang_trim(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                                unsigned byzantine, float scale, unsigned long long key, int R, int rank, unsigned long long const* signals,
+                                unsigned epoch, unsigned long long epoch_ptr, void* stream) {
+    ByzArgs a{};
+    long long work = 0;
+    int const status = fang_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, R, rank, signals, epoch, epoch_ptr, work);
+    if (status)
+        return status;
+    if (!(scale > 1.f) || !std::isfinite(scale))
+        return 125;
+    a.coef = scale;
+    a.key = key;
+    if (work == 0 && R == 1)
+        return 0;
+    int const threads = 256;
+    long long grid = (work + threads - 1) / threads;
+    long long const cap = static_cast<long long>(agb::sm_count()) * 8;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (a.H <= kBlockRows)
+        gar_fang_trim_kernel<kBlockRows><<<static_cast<int>(grid), threads, 0, s>>>(a);
+    else
+        gar_fang_trim_kernel<0><<<static_cast<int>(grid), threads, 0, s>>>(a);
+    AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
 

@@ -56,9 +56,12 @@ _ERRORS = {
   119: "invalid DnC parameters (0 <= 2 f < n, 1 <= iterations <= 8, n - iterations * r >= 1, 1 <= subsample <= 2^20, 1 <= domain <= 2^48, step >= 0)",
   120: "invalid ARC parameters (0 <= 2 f < n)", 122: "invalid SMEA parameters (0 <= 2 f < n and C(n, f) <= 2^14)",
   123: "invalid bucketing parameters (1 <= s <= n_rows, n = ceil(n_rows / s), not combined with NNM or ARC, a staging tile)",
-  124: "invalid mimic parameters (H >= 2, 0 <= t < 2^24, a target buffer, and z and y buffers for a warm-up step)"}
+  124: "invalid mimic parameters (H >= 2, 0 <= t < 2^24, a target buffer, and z and y buffers for a warm-up step)",
+  125: "invalid Fang attack parameters (fang-krum: every row honest or Byzantine, n - f - 2 >= 1, n - 2 K - 1 >= 1, H >= 2, a finite "
+       "threshold > 0; fang-trim: a finite scale > 1)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
-BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3, "mimic": 4}
+BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3, "mimic": 4, "fang-krum": 5, "fang-trim": 6}
+FANG_OUT = 3   # fang-krum's float64 details of the last run: gamma_max, t, selected
 DEVIATIONS = {"unit-vec": 0, "sign": 1, "std": 2}
 
 
@@ -112,6 +115,7 @@ class FusedLauncher:
     self.craft_stats = torch.zeros(1 + CRAFT_STATS, dtype=torch.float32, device=self.device)
     # mimic: the statistics of the last warm-up step, and the y scratch of the owned coordinates (`mimic_scratch`)
     self.mimic_stats = torch.zeros(MIMIC_STATS, dtype=torch.float64, device=self.device)
+    self.fang_out = torch.zeros(FANG_OUT, dtype=torch.float64, device=self.device)   # fang-krum: gamma_max, t, selected
     self._mimic_y = None
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
@@ -389,7 +393,7 @@ def worker_momentum_(G, M, beta, c):
 
 
 def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, launcher=None, mailboxes=None, R=1, rank=0, signals=None, epoch=1,
-          epoch_ptr=None, stream=None, state=None, warmup=None):
+          epoch_ptr=None, stream=None, state=None, warmup=None, f=None, threshold=None, scale=None, seed=None, step=None, search=True):
   """Craft the omniscient Byzantine rows (`attacks/omniscient.py`) over the owned `segments` of the n rows at device addresses `rows`
   (raw ints, local or peer-mapped): every slot of `byzantine` receives the ALIE / IPM / Min-Max / Min-Sum value of the `honest` slots.
   Collective when R > 1 (entry barrier through the signal pads, at flag value `epoch`, or `*epoch_ptr + 1` when given).
@@ -399,7 +403,12 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
   Mimic (`coef` unused) takes the caller-owned `state` (`aggregators._ops.mimic_state`: "t", the fp32 "z" of the owned coordinates,
   `segments` back to back, and the [1] int32 "istar", both on the device) and the warm-up length `warmup`: while state["t"] < warmup it runs one
   warm-up update (two exchanges through `mailboxes`, the launcher's scratch; `launcher.mimic_stats` receives s_i, q_i, ||y||^2 and
-  1 / ||y||) and counts it in state["t"]; then the copy pass alone, with i* read on the device."""
+  1 / ||y||) and counts it in state["t"]; then the copy pass alone, with i* read on the device.
+  fang-krum (`coef` unused) takes the rule's declared `f` and the `threshold` (default `_ops.FANG_THRESHOLD`), and the launcher and
+  mailboxes as Min-Max; `launcher.craft_stats` receives gamma and the summed statistics, `launcher.fang_out` gamma_max, t and the
+  selected flag. `search=False` skips the candidate search (gamma = gamma_max): the passes alone, for timing. fang-trim (`coef` unused)
+  takes the `scale` beta (default `_ops.FANG_SCALE`), the `seed` and the `step` key; it exchanges nothing."""
+  from ..aggregators import _ops
   n = len(rows)
   if n > MAX_WORKERS:
     raise tools.UserException("The sm_90a crafting kernel supports n <= %d workers (got %d)" % (MAX_WORKERS, n))
@@ -435,6 +444,32 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
     if warm:
       state["t"] = t + 1
     return
+  if mode == "fang-trim":
+    scale = _ops.check_fang_scale(scale)
+    key = _ops.fang_trim_key(0 if seed is None else seed, step)
+    func = _lib().agb_gar_byzantine_fang_trim
+    func.restype = ctypes.c_int
+    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
+                ctypes.c_float(scale), ctypes.c_ulonglong(key), ctypes.c_int(R), ctypes.c_int(rank), c_signals, ctypes.c_uint(epoch & 0x7fffffff),
+                ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_fang_trim")
+    return
+  if mode == "fang-krum":
+    threshold = _ops.check_fang_krum(n, len(set(byzantine)), f, threshold)
+    if launcher is None:
+      raise tools.UserException("fang-krum needs the scratch of a FusedLauncher")
+    if mailboxes is None:
+      if R != 1:
+        raise tools.UserException("fang-krum over %d ranks needs every rank's mailbox" % R)
+      mailboxes = [launcher.local_mailbox]
+    c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
+    func = _lib().agb_gar_byzantine_fang_krum
+    func.restype = ctypes.c_int
+    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
+                ctypes.c_int(f), ctypes.c_float(threshold), ctypes.c_int(1 if search else 0), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+                ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(launcher.craft_stats.data_ptr()),
+                ctypes.c_ulonglong(launcher.fang_out.data_ptr()), ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)),
+                _stream_ptr(stream)), "gar_byzantine_fang_krum")
+    return
   if mode in ("min-max", "min-sum"):
     if deviation is None:
       deviation = "unit-vec"
@@ -469,6 +504,16 @@ def craft_details(launcher, mode, H):
   a, b, c = MAX_PAIRS, MAX_PAIRS + MAX_WORKERS, MAX_PAIRS + 2 * MAX_WORKERS
   T = max(st[:H * (H - 1) // 2]) if mode == "min-max" else None
   return stats[0], st[a:a + H], st[b:b + H], st[c], T
+
+
+def fang_krum_details(launcher, H):
+  """(gamma, selected, t, gamma_max, A [H], B [H], C, T [H (H - 1) / 2]) of the last fang-krum crafting run with `launcher`, as the kernel
+  solved them: the sums are fp32 values, gamma_max a float64 value, T the honest pair distances in pair order."""
+  stats = launcher.craft_stats.cpu().tolist()
+  gamma_max, t, selected = launcher.fang_out.cpu().tolist()
+  st = stats[1:]
+  a, b, c = MAX_PAIRS, MAX_PAIRS + MAX_WORKERS, MAX_PAIRS + 2 * MAX_WORKERS
+  return stats[0], bool(selected), int(t), gamma_max, st[a:a + H], st[b:b + H], st[c], st[:H * (H - 1) // 2]
 
 
 def mimic_details(launcher, H):
@@ -512,24 +557,36 @@ def _craft_mimic_(G, byz_slots, state, warmup, return_details):
   return G
 
 
-def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False, state=None, warmup=None):
+def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_details=False, state=None, warmup=None, f=None, threshold=None,
+                     scale=None, seed=None, step=None):
   """Stand-alone omniscient attack on the [n, d] fp32 matrix `G`, in place: rows `byz_slots` <- the ALIE (`coef` = z), IPM
   (`coef` = epsilon), Min-Max or Min-Sum (`deviation`) row of the other rows. CUDA tensors with n <= 32 run the sm_90a kernel; others
   the torch reference. Min-Max / Min-Sum with `return_details` return (gamma, A, B, C, T) instead of G (see `craft_details`).
   Mimic takes its `state` (`aggregators._ops.mimic_state(d, G.device)`, updated in place) and `warmup`; with `return_details` it returns
-  (s, q, ||y||^2, 1 / ||y||) of a warm-up step (see `mimic_details`), None after the warm-up."""
+  (s, q, ||y||^2, 1 / ||y||) of a warm-up step (see `mimic_details`), None after the warm-up.
+  fang-krum needs the rule's declared `f` and takes `threshold`; with `return_details` it returns (gamma, selected, t, gamma_max, A, B, C,
+  T) (see `fang_krum_details`). fang-trim takes `scale`, `seed` (default 0) and the `step` key (required); the column index of G is the
+  coordinate x of its draw."""
   from ..aggregators import _ops
   if mode == "mimic":
     return _craft_mimic_(G, byz_slots, state, warmup, return_details)
   n, d = G.shape
   byz_slots = _ops.check_byzantine_slots(n, byz_slots, mode)
   optimized = mode in _ops.OPTIMIZED_MODES
+  fang = dict(f=f, threshold=threshold, scale=scale, seed=0 if seed is None else seed, step=step)
   if optimized:
     deviation = _ops.check_deviation(mode, deviation)
+  elif mode == "fang-krum":
+    _ops.check_fang_krum(n, len(byz_slots), f, threshold)
+  elif mode == "fang-trim":
+    _ops.check_fang_scale(scale)
+    _ops.fang_trim_key(fang["seed"], step)
+    if return_details:
+      raise tools.UserException("return_details is for Min-Max / Min-Sum / fang-krum only")
   elif return_details:
-    raise tools.UserException("return_details is for Min-Max / Min-Sum only")
+    raise tools.UserException("return_details is for Min-Max / Min-Sum / fang-krum only")
   if not G.is_cuda or n > MAX_WORKERS:
-    return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef, deviation=deviation, return_details=return_details)
+    return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef, deviation=deviation, return_details=return_details, **fang)
   if G.dtype != torch.float32:
     raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
   pad = (-d) % 4
@@ -539,13 +596,15 @@ def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_detai
     work[:, :d] = G
   dp = d + pad
   rows = [work.data_ptr() + i * dp * 4 for i in range(n)]
-  launcher = _launcher(G.device, n) if optimized else None
+  launcher = _launcher(G.device, n) if optimized or mode == "fang-krum" else None
   with torch.cuda.device(G.device):
-    craft(rows, [(0, dp)], [i for i in range(n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation, launcher=launcher)
+    craft(rows, [(0, dp)], [i for i in range(n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation, launcher=launcher, **fang)
   if work is not G:
     index = torch.tensor(byz_slots, dtype=torch.int64, device=G.device)
     G[index] = work[index, :d]
   if return_details:
+    if mode == "fang-krum":
+      return fang_krum_details(launcher, n - len(byz_slots))
     return craft_details(launcher, mode, n - len(byz_slots))
   return G
 

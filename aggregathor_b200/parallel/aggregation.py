@@ -14,10 +14,12 @@ Three interchangeable engines share one interface (`params`, `grads`, `step()`):
   (`mnist` + `average`, 2 workers) and the fallback for user plug-in GARs without a fused spec.
 
 Logical workers: n = R * w; rank r hosts workers [r*w, (r+1)*w). The GAR always sees n rows.
-Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None, warmup=None)`, the omniscient attacks
-(`attacks/omniscient.py`): the rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM / Min-Max / Min-Sum /
-mimic row of the others, on every rank (a collective call); `last_craft` then holds Min-Max / Min-Sum's (gamma, A, B, C, T) of that
-call, or mimic's (s, q, ||y||^2, 1 / ||y||) of a warm-up step. Mimic's state (t, z, i*; `mimic_state()`) lives in the engine (the fused
+Every engine also has `craft_byzantine(byz_slots, mode, coef, deviation=None, warmup=None, threshold=None, scale=None, seed=None)`, the
+omniscient attacks (`attacks/omniscient.py`): the rows at the given slots of the gathered matrix are overwritten with the ALIE / IPM /
+Min-Max / Min-Sum / mimic / fang-krum / fang-trim row of the others, on every rank (a collective call); `last_craft` then holds Min-Max /
+Min-Sum's (gamma, A, B, C, T) of that call, fang-krum's (gamma, selected, t, gamma_max, A, B, C, T), or mimic's (s, q, ||y||^2, 1 / ||y||)
+of a warm-up step. fang-krum models Krum with the engine's declared f (`f`; the number of Byzantine rows when the engine has none),
+fang-trim draws with the number of the update the rows feed as step key. Mimic's state (t, z, i*; `mimic_state()`) lives in the engine (the fused
 engine holds z for its owned segments only, back to back) and is checkpointed under "attack_state" as the full [d] vector.
 Rules with state (`centered-clipping`: its center, `center`) keep it in the engine, and checkpoint it under "rule_state".
 `dnc` draws its samples with the number of the optimizer update the aggregation feeds as step key (`updates` once it is counted,
@@ -162,6 +164,15 @@ class _AggregationBase:
     """The [d] vector of `_pack`'s output (the fused engine: zero outside the owned segments)."""
     return owned
 
+  def _fang_kwargs(self, mode, byz_slots, threshold, scale, seed, step):
+    """The keywords of a Fang attack for `craft_byzantine_` / `craft`: fang-krum's declared f and threshold, fang-trim's scale, seed and
+    step key (`step`: the number of the update the crafted rows feed); none for the other attacks."""
+    if mode == "fang-krum":
+      return {"f": self.f if self.f is not None else len(byz_slots), "threshold": threshold}
+    if mode == "fang-trim":
+      return {"scale": scale, "seed": 0 if seed is None else seed, "step": step}
+    return {}
+
   def _rule_kwargs(self):
     """Keywords of the rule's `aggregate` (and of `ops.gar.aggregate`) for the step about to be counted: centered clipping's center,
     DnC's step key."""
@@ -212,23 +223,24 @@ class HostAggregation(_AggregationBase):
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
-    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`
+    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`; fang-krum: see the module
 
   def visible_rows(self):
     self._gather()
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None):
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None, threshold=None, scale=None, seed=None):
     """Gather, then the torch reference on the gathered matrix (every rank computes the same bits)."""
     from ..aggregators import _ops
     self.visible_rows()
+    fang = self._fang_kwargs(mode, byz_slots, threshold, scale, seed, self.updates + 1)
     if mode == "mimic":
       self.last_craft = _ops.torch_mimic_step_(self._gathered, byz_slots, self.mimic_state(), warmup, return_details=True)
-    elif mode in _ops.OPTIMIZED_MODES:
-      self.last_craft = _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
+    elif mode in _ops.OPTIMIZED_MODES or mode == "fang-krum":
+      self.last_craft = _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True, **fang)
     else:
-      _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef)
+      _ops.torch_craft_byzantine_(self._gathered, byz_slots, mode, coef, **fang)
 
   def step(self, rate):
     self._gather()
@@ -256,23 +268,24 @@ class BaselineAggregation(_AggregationBase):
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
-    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`
+    self.last_craft = None   # Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`; fang-krum: see the module
 
   def visible_rows(self):
     self._gather()
     self._gathered_ready = True
     return {i: self._gathered[i] for i in range(self.n)}
 
-  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None):
+  def craft_byzantine(self, byz_slots, mode, coef, deviation=None, warmup=None, threshold=None, scale=None, seed=None):
     """Gather, then the stand-alone crafting kernel (R = 1) on the gathered matrix (every rank computes the same bits)."""
     from ..aggregators import _ops
     self.visible_rows()
+    fang = self._fang_kwargs(mode, byz_slots, threshold, scale, seed, self.updates + 1)
     if mode == "mimic":
       self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, state=self.mimic_state(), warmup=warmup, return_details=True)
-    elif mode in _ops.OPTIMIZED_MODES:
-      self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True)
+    elif mode in _ops.OPTIMIZED_MODES or mode == "fang-krum":
+      self.last_craft = gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef, deviation=deviation, return_details=True, **fang)
     else:
-      gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef)
+      gar_ops.craft_byzantine_(self._gathered, byz_slots, mode, coef, **fang)
 
   def step(self, rate):
     self._gather()
@@ -436,16 +449,16 @@ class FusedAggregation(_AggregationBase):
       if self.step_dev is not None:   # the value travels as a kernel argument of the fill, fixed when it is enqueued
         self.step_dev.fill_(self.updates)
 
-  def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None, warmup=None):
+  def craft_byzantine(self, byz_slots, mode, coef, stream=None, deviation=None, warmup=None, threshold=None, scale=None, seed=None):
     """Collective: this rank crafts its owned segments of every Byzantine row, local or on a peer (`ops.gar.craft`), behind an entry
     barrier at the epoch of the step about to be aggregated. Every rank calls it, including ranks that host no Byzantine worker.
-    Min-Max / Min-Sum exchange their statistics through the mailboxes; `last_craft` reads gamma and the sums back (a synchronisation).
-    Mimic's warm-up steps exchange theirs the same way and update z on the owned segments."""
+    Min-Max / Min-Sum and fang-krum exchange their statistics through the mailboxes; `last_craft` reads gamma and the sums back (a
+    synchronisation). Mimic's warm-up steps exchange theirs the same way and update z on the owned segments."""
     from ..aggregators import _ops
     byz_slots = _ops.check_byzantine_slots(self.n, byz_slots, mode)
-    optimized = mode in _ops.OPTIMIZED_MODES
+    optimized = mode in _ops.OPTIMIZED_MODES or mode == "fang-krum"
     mimic = mode == "mimic"
-    if optimized:
+    if mode in _ops.OPTIMIZED_MODES:
       deviation = _ops.check_deviation(mode, deviation)
     state = None
     if mimic:
@@ -453,18 +466,21 @@ class FusedAggregation(_AggregationBase):
       state = self.mimic_state()
       warm = state["t"] < warmup
     epoch = self.epoch if self._prepared else self.epoch + 1
+    fang = self._fang_kwargs(mode, byz_slots, threshold, scale, seed, self.updates if self._prepared else self.updates + 1)
     gar_ops.craft(self._rows, self.segments, [i for i in range(self.n) if i not in byz_slots], byz_slots, mode, coef, deviation=deviation,
                   launcher=self.launcher if optimized or mimic else None, mailboxes=self._mailboxes if optimized or mimic else None, R=self.world,
-                  rank=self.rank, signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream, state=state, warmup=warmup)
+                  rank=self.rank, signals=self._signals, epoch=epoch, epoch_ptr=self.epoch_dev, stream=stream, state=state, warmup=warmup, **fang)
     self._craft_mode = (mode, self.n - len(byz_slots)) if optimized or (mimic and warm) else None
 
   @property
   def last_craft(self):
-    """Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`, as the kernel solved them (identical on every rank); mimic:
-    (s, q, ||y||^2, 1 / ||y||) of the last call when it was a warm-up step."""
+    """Min-Max / Min-Sum: (gamma, A, B, C, T) of the last `craft_byzantine`, as the kernel solved them (identical on every rank); fang-krum:
+    (gamma, selected, t, gamma_max, A, B, C, T); mimic: (s, q, ||y||^2, 1 / ||y||) of the last call when it was a warm-up step."""
     mode = self._craft_mode
     if mode is not None and mode[0] == "mimic":
       return gar_ops.mimic_details(self.launcher, mode[1])
+    if mode is not None and mode[0] == "fang-krum":
+      return gar_ops.fang_krum_details(self.launcher, mode[1])
     return None if mode is None else gar_ops.craft_details(self.launcher, *mode)
 
   def phase_a(self, seg, stream=None):

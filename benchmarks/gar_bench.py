@@ -15,6 +15,10 @@ the crafting kernel is also timed alone, next to the torch reference on the same
 gamma every rank solved, and times the crafting kernel alternated round by round with ALIE's on the same rows.
 `--gar-attack mimic` (Karimireddy, He & Jaggi, ICLR 2022; `--gar-attack-args warmup:<T0>`) reports the target i* every rank chose and
 whether the Byzantine rows equal the baseline engine's, and times the warm-up kernel and the copy pass, each alternated with ALIE.
+`--gar-attack fang-krum|fang-trim` (Fang, Cao, Jia & Gong, USENIX Security 2020; `--gar-attack-args threshold:<x>` or `scale:<beta>
+seed:<int>`) times the crafting kernel alternated round by round with ALIE's on the same rows. fang-krum also reports the gamma, the
+candidate t and the selected flag every rank solved, and times the same kernel without its candidate search (`nosearch_*`: the passes
+alone, so `search_share_ms` is the search's own cost); fang-trim reports whether the Byzantine rows equal the baseline engine's.
 `--gar-rule-args key:value ...` passes the same `--aggregator-args` to every rule (rules ignore keys they do not use). The
 `geometric-median` and `centered-clipping` entries also report their T + 1 passes' (T + 1) * n * slice * 4 bytes and their rate.
 `--gar-worker-momentum beta` also times the worker-momentum kernel alone on the [w, d] rows of a rank (`ops.gar.worker_momentum_`,
@@ -59,7 +63,7 @@ def main():
   parser.add_argument("--gar-rules", dest="rules", type=str, default="average,average-nan,median,averaged-median,krum,bulyan")
   parser.add_argument("--gar-out", dest="out", type=str, default=".")
   parser.add_argument("--gar-byz", dest="byz", type=int, default=None, help="declared Byzantine workers f of every rule (default: 1 for Bulyan below 11 workers, else 2)")
-  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm", "min-max", "min-sum", "mimic"), default=None,
+  parser.add_argument("--gar-attack", dest="attack", choices=("alie", "ipm", "min-max", "min-sum", "mimic", "fang-krum", "fang-trim"), default=None,
                       help="omniscient attack by the last f workers, crafted every step")
   parser.add_argument("--gar-attack-args", dest="attack_args", nargs="*", default=None, metavar="KEY:VALUE",
                       help="`--attack-args` of --gar-attack (e.g. deviation:std for min-max / min-sum)")
@@ -152,6 +156,9 @@ def main():
     mimic = attack is not None and attack.mode == "mimic"
     if mimic:
       extra = {"warmup": attack.warmup}
+    fang = attack.mode if attack is not None and attack.mode in _ops.FANG_MODES else None
+    if fang:
+      extra = {key: getattr(attack, key) for key in ("threshold", "scale", "seed") if getattr(attack, key) is not None}
 
     def craft(engine):
       if attack is not None:
@@ -195,11 +202,30 @@ def main():
         dist.all_reduce(same, op=dist.ReduceOp.MIN)
       gamma_entry = {"warmup": attack.warmup, "istar_per_rank": [int(x.item()) for x in targets], "baseline_istar": int(base.attack_state["istar"][0]),
                      "rows_match_baseline": bool(same.item())}
+    if fang == "fang-krum":
+      # gamma, t and the selected flag as every rank solved them (fused engine), and the baseline engine's on the gathered rows
+      solved = torch.tensor([fused.last_craft[0], fused.last_craft[2], float(fused.last_craft[1])], dtype=torch.float64, device=device)
+      solved_all = [torch.zeros_like(solved) for _ in range(world)]
+      if world > 1:
+        dist.all_gather(solved_all, solved)
+      else:
+        solved_all = [solved]
+      gamma_entry = {"gamma_per_rank": [float(x[0]) for x in solved_all], "t_per_rank": [int(x[1]) for x in solved_all],
+                     "selected_per_rank": [bool(x[2]) for x in solved_all], "gamma_max": fused.last_craft[3], "baseline_gamma": base.last_craft[0],
+                     "baseline_t": base.last_craft[2], "baseline_selected": base.last_craft[1]}
+    if fang == "fang-trim":
+      # the Byzantine rows this rank sees through the peer mapping against the baseline engine's gathered matrix, bit for bit
+      rows = fused.visible_rows()
+      same = torch.tensor([int(all(torch.equal(rows[b].view(torch.int32), base._gathered[b].view(torch.int32)) for b in byz_slots))], device=device)
+      if world > 1:
+        dist.all_reduce(same, op=dist.ReduceOp.MIN)
+      gamma_entry = {"rows_match_baseline": bool(same.item())}
     if attack is not None and args.dump_rows and rank == world - 1:
       rows = fused.visible_rows()
       os.makedirs(args.out, exist_ok=True)
+      gamma = fused.last_craft[0] if attack.deviation is not None or fang == "fang-krum" else None
       torch.save({"rows": torch.stack([rows[i].cpu() for i in range(n)]), "byzantine": byz_slots, "mode": attack.mode, "coef": attack.coef,
-                  "deviation": attack.deviation, "gamma": fused.last_craft[0] if attack.deviation is not None else None},
+                  "deviation": attack.deviation, "gamma": gamma},
                  os.path.join(args.out, "gar_rows_%s_%d.pt" % (rule, world)))
     diff = float((fused.params - base.params).abs().max())
     digest = gar_ops.checksum(fused.params)
@@ -310,11 +336,15 @@ def main():
           _ops.torch_mimic_step_(base._gathered, byz_slots, ref_state, attack.warmup)
         reference_ms = time_craft(reference)
       else:
-        reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef, **extra))
+        ref_extra = dict(extra, f=f) if fang == "fang-krum" else dict(extra, step=1) if fang == "fang-trim" else extra
+        reference_ms = time_craft(lambda: _ops.torch_craft_byzantine_(base._gathered, byz_slots, attack.mode, attack.coef, **ref_extra))
       craft_bytes = n * d * 4   # (H + k) * d * 4: every honest value read once, every Byzantine value written once (over all ranks)
       if attack.deviation is not None:
         # Min-Max / Min-Sum read the honest values again in the write pass, and Min-Max once more in its honest-distance pass
         craft_bytes += (2 if attack.mode == "min-max" else 1) * (n - f) * d * 4
+      if fang == "fang-krum":
+        # the honest values are read by the statistics pass, the honest distance pass and the write pass (Min-Max's bytes)
+        craft_bytes += 2 * (n - f) * d * 4
       if mimic:
         # warm-up: the honest rows read in passes 1 and 2 (twice in pass 2 beyond the registers, counted once), z read twice and written
         # once, y written and read, then h_{i*} read and the k rows written; the copy pass alone: h_{i*} read, the k rows written
@@ -337,17 +367,29 @@ def main():
                              "warmup_median_ms": median(rounds["warmup"]), "copy_median_ms": median(rounds["copy"]),
                              "alie_craft_median_ms": median(rounds["alie"]), "warmup_bytes": craft_bytes, "copy_bytes": copy_bytes,
                              "warmup_gbs": craft_bytes / median(rounds["warmup"]) / 1e6, "copy_gbs": copy_bytes / median(rounds["copy"]) / 1e6})
-      if attack.deviation is not None:
+      if attack.deviation is not None or fang:
         # ALIE's crafting kernel on the same rows, alternated with this attack's round by round (clock and thermal drift hit both).
         # Repeated calls at one step's epoch pass the flag barriers at once: with R > 1 they time the kernels, their gamma is not checked.
         alie = attacks.instantiate("alie", n, f, [])
-        rounds = {"craft": [], "alie": []}
+        rounds = {"craft": [], "alie": [], "nosearch": []}
+        honest = [i for i in range(n) if i not in byz_slots]
+
+        def nosearch():
+          """fang-krum's kernel with the candidate search skipped (gamma = gamma_max): the statistics, exchange and write passes alone."""
+          gar_ops.craft(fused._rows, fused.segments, honest, byz_slots, "fang-krum", None, f=fused.f, threshold=attack.threshold,
+                        launcher=fused.launcher, mailboxes=fused._mailboxes, R=world, rank=rank, signals=fused._signals, epoch=fused.epoch + 1,
+                        epoch_ptr=fused.epoch_dev, search=False)
         for _ in range(5):
           rounds["craft"].append(time_craft(lambda: fused.craft_byzantine(byz_slots, attack.mode, attack.coef, **extra)))
           rounds["alie"].append(time_craft(lambda: fused.craft_byzantine(byz_slots, "alie", alie.coef)))
+          if fang == "fang-krum":
+            rounds["nosearch"].append(time_craft(nosearch))
         median = lambda values: sorted(values)[len(values) // 2]
         attack_entry.update({"craft_rounds_ms": rounds["craft"], "alie_craft_rounds_ms": rounds["alie"], "craft_median_ms": median(rounds["craft"]),
-                             "alie_craft_median_ms": median(rounds["alie"])})
+                             "alie_craft_median_ms": median(rounds["alie"]), "craft_median_gbs": craft_bytes / median(rounds["craft"]) / 1e6})
+        if fang == "fang-krum":
+          attack_entry.update({"nosearch_rounds_ms": rounds["nosearch"], "nosearch_median_ms": median(rounds["nosearch"]),
+                               "search_share_ms": median(rounds["craft"]) - median(rounds["nosearch"])})
     # overlapped variant (Krum / Bulyan): the distance pass of the first three buckets runs as separate small launches (in training:
     # on a side stream under the backward pass); what stays exposed at the end of the step is the finish kernel alone
     exposed_ms = bucketed_ms = None
