@@ -26,7 +26,7 @@ class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
   RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
-           "centered-clipping", "dnc", "smea")
+           "centered-clipping", "dnc", "smea", "fltrust")
 
   RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc", "smea")   # the others ignore f
   MIXES = (None, "nnm", "arc", "arc+nnm")   # the index is the kernel's bit mask: MIX_NNM | MIX_ARC

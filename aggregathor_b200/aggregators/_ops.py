@@ -1012,6 +1012,114 @@ def host_smea(G, f, return_details=False):
 
 
 # ---------------------------------------------------------------------------- #
+# FLTrust (Cao, Fang, Liu & Gong, "FLTrust: Byzantine-robust Federated Learning via Trust Bootstrapping", NDSS 2021): every row is
+# weighted by the ReLU of its cosine with a trusted root gradient r and rescaled to r's norm.
+#
+# The arithmetic every back-end shares:
+#   1. fp32 sums P_i = <x_i, r>, N_i = ||x_i||^2, N0 = ||r||^2 (fold order engine-dependent, as every rule's distances);
+#   2. from those sums, in float64 with every operation rounded once, in this order:
+#        t_i  = P_i / (sqrt(N_i) * sqrt(N0));
+#        TS_i = t_i if t_i is finite and > 0, else 0 (also a non-finite row, N_i = 0, N0 = 0, a non-finite root);
+#        S    = sum TS_i, added in worker order from +0;
+#        a_i  = ((TS_i * sqrt(N0)) / sqrt(N_i)) / S, rounded once to the rows' type (fp32, or float64 for double rows);
+#        every a_i = 0 when S = 0;
+#   3. y = sum a_i * x_i, from +0 in worker order, every product and sum rounded once (no FMA); rows with a_i = 0 are skipped, so a
+#      NaN row contributes nothing and y = +0 when S = 0.
+# Given the sums, every back-end produces the same bits. f is not used (any 0 <= f < n). ||y|| <= ||r|| up to rounding: y is a convex
+# combination of rows of norm ||r||.
+
+FLTRUST_ROOT_SIZE = 100   # the paper's root dataset size
+
+
+def check_fltrust(n, f, root_size=FLTRUST_ROOT_SIZE):
+  """Validate FLTrust's parameters -> the root dataset size (an integer >= 1). f is not used but must satisfy 0 <= f < n."""
+  if not 0 <= f < n:
+    raise tools.UserException("FLTrust needs 0 <= f < n (got n = %d, f = %d)" % (n, f))
+  if isinstance(root_size, bool) or not isinstance(root_size, int) or root_size < 1:
+    raise tools.UserException("FLTrust needs a root dataset of root-size >= 1 samples (got %r)" % (root_size,))
+  return root_size
+
+
+def fltrust_coefficients(P, N, N0, dtype=np.float32):
+  """The fp32 sums P [n], N [n] and N0 -> (TS [n] float64, S, a [n] of `dtype`), as stated above (NumPy float64, one rounding per
+  operation; np.sqrt is correctly rounded)."""
+  P = np.asarray(P, dtype=np.float64).reshape(-1)
+  N = np.asarray(N, dtype=np.float64).reshape(-1)
+  N0 = np.float64(np.asarray(N0, dtype=np.float64).reshape(-1)[0])
+  with np.errstate(all="ignore"):
+    s0 = np.sqrt(N0)
+    sn = np.sqrt(N)
+    t = P / (sn * s0)
+    TS = np.where(np.isfinite(t) & (t > 0), t, 0.0)
+    S = _serial_sum(TS)
+    a = np.zeros(len(P), dtype=dtype)
+    if S != 0.0:
+      keep = TS > 0
+      a[keep] = (((TS[keep] * s0) / sn[keep]) / S).astype(dtype)
+  return TS, S, a
+
+
+def fltrust_weighted_sum(G, a):
+  """y = sum a_i * x_i over the rows with a_i != 0, from +0 in worker order, one `torch.mul` and one `torch.add` per row (G's dtype)."""
+  out = torch.zeros(G.shape[1], dtype=G.dtype, device=G.device)
+  for i, coef in enumerate(np.asarray(a).tolist()):
+    if coef != 0.0:
+      out = torch.add(out, torch.mul(G[i], torch.tensor(coef, dtype=G.dtype, device=G.device)))
+  return out
+
+
+def check_fltrust_root(G, root):
+  """The root gradient of the [n, d] rows G: a [d] tensor, returned in G's dtype on G's device."""
+  if root is None:
+    raise tools.UserException("FLTrust needs the root gradient r (root=)")
+  if root.shape != (G.shape[1],):
+    raise tools.UserException("FLTrust needs a [%d] root gradient (got %s)" % (G.shape[1], tuple(root.shape)))
+  return root.to(device=G.device, dtype=G.dtype)
+
+
+def torch_fltrust(G, root, sums=None, return_details=False):
+  """FLTrust with the torch back-end in G's dtype. `sums`: (P, N, N0) to use instead of the torch sums (e.g. the kernel's).
+  `return_details` also gives (P, N, N0, a)."""
+  r = check_fltrust_root(G, root)
+  if sums is None:
+    P, N, N0 = (G * r).sum(dim=1), (G * G).sum(dim=1), (r * r).sum()
+    sums = tuple(v.detach().cpu().numpy() for v in (P, N, N0))
+  P, N, N0 = sums
+  dtype = np.float64 if G.dtype == torch.float64 else np.float32
+  _, _, a = fltrust_coefficients(P, N, N0, dtype)
+  out = fltrust_weighted_sum(G, a)
+  return (out, P, N, N0, a) if return_details else out
+
+
+def host_fltrust_sums(G, root):
+  """(P [n], N [n], N0) of the [n, d] rows G and the root with the host library (`agb_cpu_fltrust_sums`), as NumPy arrays of G's type."""
+  Gc = G.detach().to("cpu").contiguous()
+  rc = check_fltrust_root(Gc, root).contiguous()
+  n, d = Gc.shape
+  out = torch.zeros(2 * n + 1, dtype=Gc.dtype)
+  if _host("fltrust_sums", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(rc), _ptr(out)) != 0:
+    raise tools.UserException("Host FLTrust sums rejected their arguments (n = %d, d = %d)" % (n, d))
+  out = out.numpy()
+  return out[:n], out[n:2 * n], out[2 * n]
+
+
+def host_fltrust(G, root, sums=None, return_details=False):
+  """FLTrust with the host library: its sums (or `sums`), `fltrust_coefficients`, then `agb_cpu_weighted_sum` (the same skipped rows
+  and order as `fltrust_weighted_sum`). Returns the output on G's device; `return_details` also gives (P, N, N0, a)."""
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  P, N, N0 = host_fltrust_sums(Gc, root) if sums is None else sums
+  dtype = np.float64 if Gc.dtype == torch.float64 else np.float32
+  _, _, a = fltrust_coefficients(P, N, N0, dtype)
+  weights = torch.from_numpy(np.ascontiguousarray(a))
+  out = torch.empty(d, dtype=Gc.dtype)
+  if _host("weighted_sum", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(weights), _ptr(out)) != 0:
+    raise tools.UserException("Host weighted sum rejected its arguments")
+  out = out.to(G.device)
+  return (out, P, N, N0, a) if return_details else out
+
+
+# ---------------------------------------------------------------------------- #
 # Omniscient Byzantine rows (`attacks/omniscient.py`): the literal definition, the CPU back-end and the oracle of the sm_90a kernel
 
 OPTIMIZED_MODES = ("min-max", "min-sum")   # Shejwalkar & Houmansadr, NDSS 2021: gamma solved from whole-vector sums

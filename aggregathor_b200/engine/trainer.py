@@ -22,6 +22,10 @@ One synchronous step on a rank:
      "bucketing": means of shuffled buckets of s rows, Karimireddy, He & Jaggi, "Byzantine-Robust Learning on Heterogeneous Datasets
      via Bucketing");
   5. the bf16 compute copy of the parameters is refreshed (unless the fused kernel already wrote it).
+With a rule that needs a trusted root gradient (`fltrust`), rank 0 alone also runs, in step 1, one unbatched forward/backward on a
+batch of the experiment's root dataset into the engine's root row (never flipped, never poisoned, its loss not reported): the ranks run
+in lock-step, so one root pass costs the same wall time as one on every rank, and one root row owned by rank 0 gives every engine the
+same root gradient at any rank count.
 """
 
 import os
@@ -62,6 +66,9 @@ class Manager:
     # (beta, c = 1 - dampening) in fp32; beta = dampening = 0 is off: no buffer, no kernel, the step is unchanged
     self.momentum = _ops.check_worker_momentum(worker_momentum, worker_momentum_dampening)
     self.momentum_on = self.momentum[0] != 0.0 or _ops.fp32(worker_momentum_dampening) != 0.0
+    self.needs_root = bool(getattr(aggregator, "needs_root", False))
+    if self.needs_root and self.momentum_on:
+      raise tools.UserException("%s compares every row with a raw root gradient: it cannot be combined with --worker-momentum" % type(aggregator).__name__)
     if authenticate and getattr(attack, "omniscient", False):
       raise tools.UserException("Omniscient attacks craft the Byzantine rows on every rank: they cannot be combined with '--authenticate'")
     self.device = torch.device(device) if device is not None else _default_device()
@@ -178,6 +185,21 @@ class Manager:
     self.eval_ctx.weights, self.eval_ctx.master, self.eval_ctx.state = self.weight_views, self.master_views, self.states
     self.eval_ctx.generator = self._dropout_gen
     self.streams = [experiment.train_stream(i, nbworkers, self.device) for i in self.local_workers]
+    # FLTrust: the root pass of rank 0, with its own training context whose gradients are the engine's root row, and its own copy of
+    # the model state (batch-norm moving averages), so that every rank keeps the same state
+    self.root_ctx = self.root_stream = None
+    if self.needs_root:
+      experiment.root_indices(aggregator.root_size)   # the same checks on every rank
+      if self.rank == 0:
+        ctx = Context(self.backend, True, self.dtype, self.device)
+        ctx.weights, ctx.master = self.weight_views, self.master_views
+        ctx.state = {name: value.clone() for name, value in self.states.items()}
+        ctx.grads = self.layout.views(self.aggregation.root)
+        ctx.generator = self._dropout_gen
+        ctx.worker_id, ctx.nbworkers = nbworkers, nbworkers   # one past the workers: its own augmentation stream
+        ctx.flip_from = None
+        self.root_ctx = ctx
+        self.root_stream = experiment.root_stream(aggregator.root_size, self.device)
     self._stream_group = None
     if cuda and os.environ.get("AGB_GROUP_STREAMS", "1") not in ("", "0"):
       from ..experiments._data import StreamGroup
@@ -250,7 +272,7 @@ class Manager:
     return (getattr(self.aggregation, "device_state", False) and not self._rewrites_rows and self.authenticator is None
             and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and os.environ.get("AGB_GRAPH_AGGREGATION", "1") not in ("", "0"))
 
-  def _capture(self, batches):
+  def _capture(self, batches, root_batch=None):
     """Record every local worker's forward + backward — and, with the fused engine, the aggregation kernels and the refresh of the
     compute copy of the parameters — into one CUDA graph (static shapes, static buffers)."""
     from ..ops import counters
@@ -261,6 +283,8 @@ class Manager:
       self._static_batches, self._static_slabs = [(slab_x[j], slab_y[j]) for j in range(len(batches))], (slab_x, slab_y)
     else:
       self._static_batches, self._static_slabs = [(x.clone(), y.clone()) for x, y in batches], (None, None)
+    # FLTrust: the static root batch, refreshed before every replay as the workers' slabs
+    self._static_root = (root_batch[0].clone(), root_batch[1].clone()) if root_batch is not None else None
     torch.cuda.synchronize(self.device)
     if self.world > 1:
       dist.barrier(group=self.group)   # capture is slow and its kernels do not run: keep the ranks aligned around it
@@ -269,7 +293,7 @@ class Manager:
     whole = self._whole_step_graph
     try:
       with torch.cuda.graph(graph):
-        self._static_losses = self._run_workers(self._static_batches, None)
+        self._static_losses = self._run_workers(self._static_batches, None, self._static_root)
         if whole:
           self._apply_momentum()
           self.aggregation.step(stream=None, loss_in=self._static_losses, prepared=True)
@@ -286,15 +310,28 @@ class Manager:
       " + aggregation" if whole else "", self._graph_launches), context="graph")
     return True
 
-  def _run_workers(self, batches, trace):
-    """Forward + backward of every local worker -> fp32 tensor of per-worker losses."""
+  def _run_workers(self, batches, trace, root_batch=None):
+    """Forward + backward of every local worker -> fp32 tensor of per-worker losses; then the root pass on `root_batch` (rank 0 of a
+    rule with a root gradient), whose loss is not returned."""
     if self.backend == "native" and self.device.type == "cuda" and not os.environ.get("AGB_NO_PREZERO"):
-      # one fill of the whole gradient matrix instead of one per split-K weight gradient
+      # one fill of the whole gradient matrix instead of one per split-K weight gradient; the root row obeys the same contract
       from ..ops import nn_native
       self.grads.zero_()
+      if root_batch is not None:
+        self.aggregation.root.zero_()
       with nn_native.prezeroed_gradients():
-        return self._run_workers_inner(batches, trace)
-    return self._run_workers_inner(batches, trace)
+        losses = self._run_workers_inner(batches, trace)
+        self._root_pass(root_batch)
+        return losses
+    losses = self._run_workers_inner(batches, trace)
+    self._root_pass(root_batch)
+    return losses
+
+  def _root_pass(self, root_batch):
+    """One unbatched forward/backward on a root batch into the root row (never poisoned: the model's loss, not the experiment's)."""
+    if root_batch is not None:
+      inputs, labels = root_batch
+      self.model.loss_and_backward(self.experiment.preprocess(inputs, self.root_ctx, True), labels, self.root_ctx)
 
   def _run_workers_inner(self, batches, trace):
     hooked = self.batched_ctx if (self.batched and trace is None) else (self.contexts[-1] if self.contexts else None)
@@ -358,8 +395,11 @@ class Manager:
     buckets = [(lo, hi) for _, lo, hi in cuts] + [(0, upper)]
     return buckets, {id(layer): index for index, (layer, _, _) in enumerate(cuts)}
 
-  def _replay(self, batches):
+  def _replay(self, batches, root_batch=None):
     from ..ops import counters
+    if self._static_root is not None:
+      self._static_root[0].copy_(root_batch[0], non_blocking=True)
+      self._static_root[1].copy_(root_batch[1], non_blocking=True)
     slab_x, slab_y = self._static_slabs
     grouped_x = slab_x is not None and getattr(batches, "x_all", None) is not None and batches.x_all.shape == slab_x.shape
     grouped_y = slab_y is not None and getattr(batches, "y_all", None) is not None and batches.y_all.shape == slab_y.shape
@@ -386,19 +426,22 @@ class Manager:
     """Phase 1-3 of a step: local workers' losses and gradients (+ regularisation, + attacks). Returns the list of losses."""
     group = self._stream_group
     batches = next(group) if (group is not None and self.streams is self._grouped_source) else [next(stream) for stream in self.streams]
+    root_batch = next(self.root_stream) if self.root_stream is not None else None
     trace = self.tracer if self.tracer.enabled else None
     if self.use_graphs and trace is None and self._graph is None and self.step >= self._graph_warmup:
-      self._capture(batches)
+      self._capture(batches, root_batch)
     self._last_step_replayed = self._graph is not None and trace is None
     if self._last_step_replayed:
-      losses = self._replay(batches)
+      losses = self._replay(batches, root_batch)
     else:
-      losses = list(self._run_workers(batches, trace).unbind(0))
+      losses = list(self._run_workers(batches, trace, root_batch).unbind(0))
     if (self.l1 is not None and self.l1 > 0.) or (self.l2 is not None and self.l2 > 0.):
       reg_loss, reg_grad = regularization(self.params, self.l1, self.l2)
       for j in range(len(self.local_workers)):
         self.grads[self.placement[self.local_workers[j]][1]].add_(reg_grad)
         losses[j] = losses[j] + reg_loss
+      if self.root_ctx is not None:
+        self.aggregation.root.add_(reg_grad)
     if not (self._last_step_replayed and self._graph_whole):   # the whole-step graph holds the momentum step
       self._apply_momentum()
     if getattr(self.attack, "omniscient", False):
@@ -552,6 +595,8 @@ class Manager:
   def close(self):
     if self._stream_group is not None:
       self._stream_group.close()
+    if self.root_stream is not None and getattr(self.root_stream, "close", None) is not None:
+      self.root_stream.close()
     for stream in self.streams:
       close = getattr(stream, "close", None)
       if close is not None:

@@ -11,6 +11,7 @@ built TF graph nodes; here an experiment provides
                                       stream per logical worker; `shared-batch:1` reproduces the reference's
                                       mnist quirk where every worker sees the same batch),
   * `eval_batch(device)`           -> one evaluation batch,
+  * `root_stream(size, device)`    -> the batches of the trusted root dataset of FLTrust (`aggregators/fltrust.py`),
 and the base class implements `losses(...)` / `accuracy(...)` on top of them: `losses` runs forward + backward for
 each of this rank's logical workers (writing gradients into their rows) and returns the per-worker loss tensors,
 `accuracy` returns `{"top1-X-acc": tensor}` — the same metric name as the reference.
@@ -23,6 +24,8 @@ import torch
 from .. import tools
 
 __all__ = ["_Experiment", "register", "instantiate", "itemize"]
+
+ROOT_TAG = 0x524F4F54   # "ROOT": second word of the root dataset's generator seed
 
 
 class _Experiment:
@@ -39,6 +42,27 @@ class _Experiment:
 
   def eval_batch(self, device):
     raise NotImplementedError
+
+  def root_stream(self, size, device):
+    """The batches of FLTrust's root dataset of `size` training samples (`root_indices`), never poisoned, in batches of the experiment's
+    batch size."""
+    raise tools.UserException("Experiment %s has no root dataset for FLTrust" % type(self).__name__)
+
+  def root_indices(self, size):
+    """FLTrust's root dataset: `size` training samples drawn uniformly without replacement with numpy's default_rng([seed, ROOT_TAG]),
+    ascending. The same on every rank and for any worker count, and independent of `dirichlet:` (the root set is unbiased even when the
+    workers' data is not). At least one batch of the experiment's batch size."""
+    import numpy as np
+    size, batch, count = int(size), int(self.args["batch-size"]), int(self.data.train_count)
+    if size < batch:
+      raise tools.UserException("FLTrust's root dataset (root-size:%d) must hold at least one batch of batch-size:%d samples" % (size, batch))
+    if size > count:
+      raise tools.UserException("FLTrust's root dataset (root-size:%d) is larger than the training set (%d samples)" % (size, count))
+    return np.sort(np.random.default_rng([int(self.args["seed"]), ROOT_TAG]).choice(count, size, replace=False))
+
+  def _root_stream(self, size, device, **kwargs):
+    """`root_stream` through the dataset's subset paths (`BatchStream(indices=)` in memory, the shard reader's subset when streamed)."""
+    return self.data.train_stream(self.args["batch-size"], device, seed=int(self.args["seed"]) + ROOT_TAG, indices=self.root_indices(size), **kwargs)
 
   def _check_dirichlet(self):
     """Validates `dirichlet:<alpha>` in `self.args` (absent: the IID streams of every worker are unchanged)."""

@@ -45,6 +45,9 @@ class MNIST(_Experiment):
                                           indices=self._dirichlet_indices(self.data, worker, nbworkers, labels))
     return self._streams[worker]
 
+  def root_stream(self, size, device):
+    return self._root_stream(size, device)   # the clean training set: `mnistAttack` poisons only its workers' streams and losses
+
   def eval_batch(self, device):
     count = self.args["eval-batch-size"] or len(self.data.y_test)
     x = torch.from_numpy(self.data.x_test[:count]).to(device)

@@ -88,6 +88,9 @@ class SlimExperiment(_Experiment):
                                                      indices=self._dirichlet_indices(self.data, worker, nbworkers))
     return self._streams[worker]
 
+  def root_stream(self, size, device):
+    return self._root_stream(size, device, transform=self._offset, readers=self.args["nb-fetcher-threads"])
+
   def eval_batch(self, device):
     if not hasattr(self, "_eval_stream"):
       self._eval_stream = BatchStream(self.data.x_test, self.data.y_test, min(self.args["eval-batch-size"], len(self.data.y_test)), device, shuffle=False, transform=self._offset)

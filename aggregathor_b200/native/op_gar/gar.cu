@@ -31,7 +31,8 @@
 // its warm-up and `gar_mimic_copy_kernel` after it. Fang et al.'s Krum attack runs `gar_fang_krum_kernel` (Min-Max's passes and exchange,
 // then a one-warp search over gamma), their trimmed-mean attack `gar_fang_trim_kernel` (one pass, a counter-based draw per row).
 // DnC (rule kDnc) has a finish kernel of its own, `gar_dnc_kernel`: a sampled distance pass, one exchange, a float64 Jacobi per CTA,
-// then Krum's phase D (see `dnc_selection`).
+// then Krum's phase D (see `dnc_selection`). FLTrust (rule kFltrust) too, `gar_fltrust_kernel`: a pass for the sums against the root
+// gradient, one exchange, float64 coefficients, then the weighted sum.
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
 // registers at a time; more rows are processed in 8-row blocks (diagonal + cross passes over the staged copy).
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
@@ -64,7 +65,8 @@ constexpr int kSlotCraftStats = kSlotMix + 1;   // Min-Max / Min-Sum: exchange o
 constexpr int kSlotDnc = kSlotCraftStats + 1;   // DnC: exchange of the sampled distances
 constexpr int kSlotArc = kSlotDnc + 1;   // ARC: exchange of the squared row norms
 constexpr int kSlotMimic = kSlotArc + 1;   // mimic: second exchange of a warm-up step (the first one signals on kSlotCraftStats)
-constexpr int kFlagSlots = kSlotMimic + 1;
+constexpr int kSlotFltrust = kSlotMimic + 1;   // FLTrust: exchange of the sums
+constexpr int kFlagSlots = kSlotFltrust + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 // Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
 // They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
@@ -80,7 +82,10 @@ constexpr int kDncStride = kDncIterations * kMaxPairs + 1;   // DnC post of one 
 constexpr int kDncRegion = kCraftRegion + kMaxRanks * kCraftStats;   // mailbox region 3: kMaxRanks x kDncStride floats
 constexpr int kArcStride = kMaxWorkers + 1;   // ARC post of one rank: the n partial squared norms, then the loss
 constexpr int kArcRegion = kDncRegion + kMaxRanks * kDncStride;   // mailbox region 4: kMaxRanks x kArcStride floats
-constexpr int kMailboxFloats = kArcRegion + kMaxRanks * kArcStride;
+constexpr int kFltrustStride = 2 * kMaxWorkers + 2;   // FLTrust post of one rank: P_i [0, 32), N_i [32, 64), N0 [64], then the loss
+constexpr int kFltrustRegion = kArcRegion + kMaxRanks * kArcStride;   // mailbox region 5: kMaxRanks x kFltrustStride floats
+constexpr int kMailboxFloats = kFltrustRegion + kMaxRanks * kFltrustStride;
+constexpr int kFltrustOut = 3 * kMaxWorkers + 1;   // FLTrust's `fltrust_out`: P [0, 32), N [32, 64), N0 [64], a [65, 97)
 constexpr int kMixNnm = 1, kMixArc = 2, kMixBucketing = 4;   // GarArgs::mix bits (bucketing is never combined with the others)
 constexpr unsigned long long kBucketingTag = 0x42554B54ull;   // "BUKT": third input of bucketing's key; >= 8, never a DnC iteration
 constexpr int kJacobiSweeps = 32;         // DnC: sweep budget of the cyclic Jacobi
@@ -90,7 +95,7 @@ constexpr int kBlockRows = 8;             // rows held in registers at a time
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
 constexpr long long kSmeaMaxSets = 1 << 14;   // SMEA runs one float64 Jacobi per removal set (`_ops.SMEA_MAX_SETS`)
 enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8,
-           kCenteredClipping = 9, kDnc = 10, kSmea = 11 };
+           kCenteredClipping = 9, kDnc = 10, kSmea = 11, kFltrust = 12 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -146,6 +151,8 @@ struct GarArgs {
     long long const* dnc_step_ptr;     // device step key (graph replay), or null
     float* dnc_scratch;                // [grid][kDncIterations][kMaxPairs] CTA partials, then the samples [T][n][b'4]
     double* smea_scratch;              // SMEA: one [m][m] slab per warp of the grid (m = n - f), the double-centred matrix of its set
+    float const* root;                 // FLTrust: the root gradient r [d] (rank 0's, peer-mapped), read on the owned coordinates
+    float* fltrust_out;                // FLTrust: optional [kFltrustOut] sums and coefficients, for tests
 };
 
 // the rows `phase_a_segment` reads in DnC's sampled pass: one segment [0, b'4) of the gathered samples of one iteration, no staging
@@ -2275,6 +2282,243 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs 
         *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
 }
 
+// ---- the FLTrust finish kernel (Cao, Fang, Liu & Gong, NDSS 2021) ---------------------------------------------------- //
+// Rows x_i, root gradient r (rank 0's row, read over P2P on the owned coordinates). The arithmetic is `_ops.fltrust_coefficients`:
+//   1. sums pass over the owned segments, with the rules' (tid, VEC) mapping: the n rows and r are loaded (8 rows in flight at a time,
+//      as ARC's norm pass), P_i = <x_i, r>, N_i = ||x_i||^2 and N0 = ||r||^2 accumulate with one FMA per value; the rows are staged
+//      when the staging tile is given (R > 1 or n > 8), so that the second pass never crosses NVLink again;
+//   2. one exchange of the 2n + 1 partial sums and the loss: lanes -> warps -> CTA -> `cta_partials` -> grid barrier; block 0 folds
+//      the CTAs in order and posts the rank's sums into mailbox region 5 of every rank, then signals slot kSlotFltrust. Every CTA of
+//      every rank adds the R posts in rank order, so the sums are bit-identical everywhere. Region 5 and slot kSlotFltrust belong to
+//      this exchange alone (FLTrust runs no pre-aggregation and no other exchange); every CTA reads region 5 before the exit barrier,
+//      and the next write into it comes from the next step's exchange, which a rank reaches only after every rank's exit barrier;
+//   3. the coefficients on warp 0 of every CTA (one lane per row), in float64 with explicit _rn intrinsics:
+//        t_i = P_i / (sqrt(N_i) sqrt(N0)); TS_i = t_i if finite and > 0, else 0; S = sum TS_i in worker order;
+//        a_i = fp32(((TS_i sqrt(N0)) / sqrt(N_i)) / S), every a_i = 0 when S = 0;
+//   4. phase D: y = sum a_i x_i from +0 in worker order (__fmul_rn / __fadd_rn: no FMA), the rows with a_i = 0 skipped, then the
+//      optimizer and the parameter broadcast; from the staged tile, or the local rows when R = 1 and n <= 8. Exit barrier as for DnC.
+// A kernel of its own keeps the 2n + 1 accumulators out of the register allocation of `gar_fused_kernel`.
+struct FltrustShared {
+    float partials[16][2 * kMaxWorkers + 1];   // per-warp sums: P_i [0, n), N_i [n, 2n), N0 [2n]
+    float coef[kMaxWorkers];                    // a_i
+    unsigned mask;                              // rows with a_i != 0
+    float hyper[4];
+    uint32_t epoch;
+};
+
+template<int N, int VEC>
+__global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fltrust_kernel(GarArgs const a) {
+    __shared__ FltrustShared sh;
+    cg::grid_group grid = cg::this_grid();
+    int const n = a.n, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    bool const multi = a.R > 1;
+    if (threadIdx.x == 0) {
+        sh.epoch = current_epoch(a);
+        for (int i = 0; i < 4; ++i)
+            sh.hyper[i] = a.hyper_ptr ? a.hyper_ptr[i] : (i == 0 ? a.lr : i == 1 ? a.h0 : i == 2 ? a.h1 : a.h2);
+    }
+    __syncthreads();
+    uint32_t const epoch = sh.epoch;
+    float const hyper[4] = {sh.hyper[0], sh.hyper[1], sh.hyper[2], sh.hyper[3]};
+    long long const owned = owned_length(a);
+    if (multi) {   // entry barrier: every rank's gradients, and rank 0's root, are published (nothing is pre-accumulated)
+        if (blockIdx.x == 0)
+            signal_all(a, 0, epoch);
+        wait_all(a, 0, epoch);
+        __syncthreads();
+    }
+    float local_loss = 0.f;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_in)
+        for (int j = 0; j < a.nloss; ++j)
+            local_loss += a.loss_in[j];
+    // -------- 1. sums pass -------- //
+    float P[N], Q[N], R0 = 0.f;   // P_i, N_i, N0
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        P[i] = 0.f;
+        Q[i] = 0.f;
+    }
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            float r[VEC];
+            V<VEC>::load_stream(a.root + x, r);
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                R0 = __fmaf_rn(r[c], r[c], R0);
+#pragma unroll
+            for (int i0 = 0; i0 < N; i0 += kBlockRows) {
+                float g[kBlockRows][VEC];
+#pragma unroll
+                for (int i = 0; i < kBlockRows; ++i)
+                    if (i0 + i < n)
+                        V<VEC>::load_stream(a.grad[i0 + i] + x, g[i]);
+#pragma unroll
+                for (int i = 0; i < kBlockRows; ++i) {
+                    if (i0 + i < n) {
+                        if (a.staging)
+                            V<VEC>::store(a.staging + (i0 + i) * owned + soff + v * VEC, g[i]);
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c) {
+                            P[i0 + i] = __fmaf_rn(g[i][c], r[c], P[i0 + i]);
+                            Q[i0 + i] = __fmaf_rn(g[i][c], g[i][c], Q[i0 + i]);
+                        }
+                    }
+                }
+            }
+        }
+    }
+    // -------- 2. exchange of the 2n + 1 sums (and the loss) -------- //
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        if (i < n) {
+            float const p = warp_sum(P[i]), q = warp_sum(Q[i]);
+            if (lane == 0) {
+                sh.partials[warp][i] = p;
+                sh.partials[warp][n + i] = q;
+            }
+        }
+    }
+    {
+        float const r0 = warp_sum(R0);
+        if (lane == 0)
+            sh.partials[warp][2 * n] = r0;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < 2 * n + 1; k += blockDim.x) {
+        float s = 0.f;
+        for (int w = 0; w < nwarps; ++w)
+            s += sh.partials[w][k];
+        a.cta_partials[static_cast<long long>(blockIdx.x) * kMaxPairs + k] = s;
+    }
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int k = threadIdx.x; k < 2 * n + 1; k += blockDim.x) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kMaxPairs + k);
+            int const at = k < n ? k : k < 2 * n ? kMaxWorkers + (k - n) : 2 * kMaxWorkers;
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kFltrustRegion + a.rank * kFltrustStride + at] = s;
+        }
+        if (threadIdx.x == 0)
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kFltrustRegion + a.rank * kFltrustStride + 2 * kMaxWorkers + 1] = local_loss;
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, kSlotFltrust, epoch);
+    }
+    if (multi) {
+        wait_all(a, kSlotFltrust, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    // -------- 3. coefficients: warp 0 of every CTA -------- //
+    if (warp == 0) {
+        float const* const box = a.mailbox[a.rank] + kFltrustRegion;
+        float Pi = 0.f, Ni = 0.f, N0 = 0.f;
+        for (int q = 0; q < a.R; ++q) {
+            if (lane < n) {
+                Pi += ld_volatile_f(box + q * kFltrustStride + lane);
+                Ni += ld_volatile_f(box + q * kFltrustStride + kMaxWorkers + lane);
+            }
+            N0 += ld_volatile_f(box + q * kFltrustStride + 2 * kMaxWorkers);
+        }
+        double const s0 = __dsqrt_rn(static_cast<double>(N0)), si = __dsqrt_rn(static_cast<double>(Ni));
+        double const t = __ddiv_rn(static_cast<double>(Pi), __dmul_rn(si, s0));
+        double const ts = (lane < n && isfinite(t) && t > 0.0) ? t : 0.0;
+        double S = 0.0;
+        for (int j = 0; j < n; ++j)
+            S = __dadd_rn(S, __shfl_sync(0xffffffffu, ts, j));
+        float const c = (S != 0.0 && ts > 0.0) ? __double2float_rn(__ddiv_rn(__ddiv_rn(__dmul_rn(ts, s0), si), S)) : 0.f;
+        sh.coef[lane] = c;
+        unsigned const mask = __ballot_sync(0xffffffffu, c != 0.f);
+        if (lane == 0)
+            sh.mask = mask;
+        if (blockIdx.x == 0) {
+            if (a.fltrust_out) {
+                if (lane < n) {
+                    a.fltrust_out[lane] = Pi;
+                    a.fltrust_out[kMaxWorkers + lane] = Ni;
+                    a.fltrust_out[2 * kMaxWorkers + 1 + lane] = c;
+                }
+                if (lane == 0)
+                    a.fltrust_out[2 * kMaxWorkers] = N0;
+            }
+            if (lane == 0 && a.loss_out) {
+                float total = 0.f;
+                for (int q = 0; q < a.R; ++q)
+                    total += ld_volatile_f(box + q * kFltrustStride + 2 * kMaxWorkers + 1);
+                *a.loss_out = total;
+            }
+        }
+    }
+    __syncthreads();
+    // -------- 4. phase D: weighted sum, update, broadcast -------- //
+    unsigned const mask = sh.mask;
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            auto load_row = [&](int i, float (&dst)[VEC]) {
+                if (a.staging)
+                    V<VEC>::load(a.staging + i * owned + soff + v * VEC, dst);
+                else
+                    V<VEC>::load_stream(a.grad[i] + x, dst);
+            };
+            float y[VEC];
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                y[c] = 0.f;
+            if (N <= 16) {   // every weighted row in flight at once, added in ascending worker order
+                float g[N][VEC];
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u)
+                        load_row(i, g[i]);
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u) {
+                        float const ai = sh.coef[i];
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[i][c]));
+                    }
+            } else {
+                for (int i = 0; i < n; ++i) {
+                    if ((mask >> i) & 1u) {
+                        float g[VEC];
+                        load_row(i, g);
+                        float const ai = sh.coef[i];
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[c]));
+                    }
+                }
+            }
+            apply_update<VEC>(a, hyper, x, y);
+        }
+    }
+    if (multi) {   // exit barrier, as in `gar_dnc_kernel` (the loss went through the exchange)
+        fence_sys();
+        grid.sync();
+        if (blockIdx.x == 0) {
+            __syncthreads();
+            signal_all(a, kSlotExit, epoch);
+            wait_all(a, kSlotExit, epoch);
+            __syncthreads();
+        }
+    }
+    if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
+        *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
+}
+
 // ---- omniscient Byzantine rows (ALIE / IPM) ------------------------------------------ //
 // Every Byzantine row receives, at each owned coordinate, a value computed from the honest values of that coordinate only:
 //   mu = ((h[Hs0] + h[Hs1]) + ...) / H           honest slots ascending, one division
@@ -3395,7 +3639,7 @@ __global__ void cast_bf16_kernel(float const* __restrict__ src, __nv_bfloat16* _
 template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_floats, cudaStream_t stream) {
     int const threads = N <= 8 ? 512 : 256;
     int device = 0, sms = 0, per_sm = 0;
-    auto const kernel = a.rule == kDnc ? gar_dnc_kernel<N, VEC> : gar_fused_kernel<N, VEC>;
+    auto const kernel = a.rule == kDnc ? gar_dnc_kernel<N, VEC> : a.rule == kFltrust ? gar_fltrust_kernel<N, VEC> : gar_fused_kernel<N, VEC>;
     AGB_CUDA_OK(cudaGetDevice(&device));
     AGB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0));
@@ -3428,7 +3672,7 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
 //   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
 //   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
 //   [115] arc_out (ARC: [2n] squared norms, then factors) | [116] SMEA scratch (doubles)
-//   [113] is also bucketing's step key
+//   [113] is also bucketing's step key | [117] FLTrust root r (rank 0's) | [118] FLTrust's fltrust_out
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
 //       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC, 4 bucketing) | [27] DnC r | [28] bucketing: s | [29] gathered rows n_rows (0: n)
 // longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step (also bucketing's)
@@ -3468,8 +3712,12 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kSmea)
+    if (a.rule < 0 || a.rule > kFltrust)
         return 102;
+    // FLTrust: any 0 <= f < n, a root, no pre-aggregation (it would change the rows whose direction and norm FLTrust scores), nothing
+    // pre-accumulated
+    if (a.rule == kFltrust && (a.f < 0 || a.f >= a.n || !ptrs[117] || a.mix != 0 || a.first_seg != 0))
+        return 126;
     if (a.mix < 0 || a.mix > (kMixNnm | kMixArc | kMixBucketing))
         return 117;
     if ((a.mix & kMixBucketing) && (a.mix != kMixBucketing || a.bkt_size < 1 || a.bkt_size > a.n_rows ||
@@ -3531,6 +3779,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.loss_out = reinterpret_cast<float*>(ptrs[46]);
     a.raw_dist_out = reinterpret_cast<float*>(ptrs[112]);
     a.arc_out = reinterpret_cast<float*>(ptrs[115]);
+    a.root = reinterpret_cast<float const*>(ptrs[117]);
+    a.fltrust_out = reinterpret_cast<float*>(ptrs[118]);
     for (int q = 0; q < a.R; ++q) {
         a.param_dst[q] = reinterpret_cast<float*>(ptrs[48 + q]);
         a.signal[q] = reinterpret_cast<uint32_t*>(ptrs[64 + q]);
@@ -3548,6 +3798,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 108;
     if (a.rule == kSmea && !a.smea_scratch)
         return 108;
+    if (a.rule == kFltrust && (!a.cta_partials || !a.mailbox[0] || ((a.R > 1 || a.n > kBlockRows) && !a.staging)))
+        return 108;   // FLTrust's second pass reads the staged rows over several ranks or beyond the 8 rows of one block
     if ((a.rule == kGeoMedian || a.rule == kCenteredClipping) && a.R > 1 && !a.staging)
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)

@@ -789,6 +789,49 @@ template<class T> int selection_mean_of(T const* g, size_t n, size_t d, int64_t 
     return 0;
 }
 
+// sum_{k in [b, e)} x[k] * y[k], with `squared_difference`'s 16 interleaved partial sums and fixed fold
+template<class T> inline T dot(T const* x, T const* y, size_t b, size_t e) {
+    constexpr size_t kLanes = 16;
+    T acc[kLanes];
+    for (size_t u = 0; u < kLanes; ++u)
+        acc[u] = T(0);
+    size_t k = b;
+    for (; k + kLanes <= e; k += kLanes)
+        for (size_t u = 0; u < kLanes; ++u)
+            acc[u] += x[k + u] * y[k + u];
+    for (size_t u = 0; k < e; ++k, ++u)
+        acc[u] += x[k] * y[k];
+    for (size_t width = kLanes / 2; width > 0; width /= 2)
+        for (size_t u = 0; u < width; ++u)
+            acc[u] += acc[u + width];
+    return acc[0];
+}
+
+// FLTrust's sums (`aggregators/_ops.py`): out = [P_0 .. P_{n-1}, N_0 .. N_{n-1}, N0] with P_i = <x_i, r>, N_i = ||x_i||^2, N0 = ||r||^2,
+// per-chunk partials folded in chunk order. The coefficients and the weighted sum are computed by the callers (one copy of that arithmetic).
+template<class T> int fltrust_sums(T const* g, size_t n, size_t d, T const* root, T* out) {
+    if (n == 0 || n > kMaxWorkers)
+        return 1;
+    size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
+    size_t const width = 2 * n + 1;
+    std::vector<T> partial(chunks * width, T(0));
+    global_pool().run(0, d, kGrainCoord, [&](size_t chunk, size_t b, size_t e) {
+        T* part = partial.data() + chunk * width;
+        for (size_t i = 0; i < n; ++i) {
+            part[i] = dot(g + i * d, root, b, e);
+            part[n + i] = dot(g + i * d, g + i * d, b, e);
+        }
+        part[2 * n] = dot(root, root, b, e);
+    });
+    for (size_t k = 0; k < width; ++k) {
+        T sum = 0;
+        for (size_t c = 0; c < chunks; ++c)
+            sum += partial[c * width + k];
+        out[k] = sum;
+    }
+    return 0;
+}
+
 template<class T> T squared_distance(T const* a, T const* b, size_t d) {
     size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
     std::vector<T> partial(chunks, T(0));
@@ -846,6 +889,7 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_weighted_sum_##S(T const* g, size_t n, size_t d, T const* w, T* out) { weighted_sum<T>(g, n, d, w, out); return 0; } \
     extern "C" int agb_cpu_dnc_sample_distances_##S(T const* g, size_t n, size_t d, size_t iterations, size_t b, uint64_t seed, uint64_t step, size_t domain, T* dist) { return dnc_sample_distances<T>(g, n, d, iterations, b, seed, step, domain, dist); } \
     extern "C" int agb_cpu_selection_mean_##S(T const* g, size_t n, size_t d, int64_t const* selected, size_t count, T* out) { return selection_mean_of<T>(g, n, d, selected, count, out); } \
+    extern "C" int agb_cpu_fltrust_sums_##S(T const* g, size_t n, size_t d, T const* root, T* out) { return fltrust_sums<T>(g, n, d, root, out); } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }
 
 AGB_EXPORT(float, float)

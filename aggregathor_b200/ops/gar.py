@@ -21,8 +21,8 @@ MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
 # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
-# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 5
+# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange; FLTrust's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 6
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 # Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]; mimic posts into the
 # same region: s_i [0, 32) in its first exchange, q_i [32, 64) and ||y||^2 [64] in its second
@@ -34,9 +34,15 @@ DNC_MAX_ITERATIONS = 8
 DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
 # ARC's post of one rank: the partial squared norms of the rows ([MAX_WORKERS]), then the loss
 ARC_STATS = MAX_WORKERS + 1
-# five regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms
-MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS) * 4
-PTRS = 117
+# FLTrust's post of one rank: P_i [0, 32), N_i [32, 64), N0 [64], then the loss
+FLTRUST_STATS = 2 * MAX_WORKERS + 2
+# six regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms,
+# FLTrust's sums
+MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS
+                 + MAX_RANKS * FLTRUST_STATS) * 4
+# FLTrust's sums and coefficients of the last launch: P [0, 32), N [32, 64), N0 [64], a [65, 97)
+FLTRUST_OUT = 3 * MAX_WORKERS + 1
+PTRS = 119
 # [0]: theta, [1, 1 + theta): selection masks; [32, 34): SMEA's winning score (float64 bits); [64, 64 + n): NNM masks;
 # [96, 96 + T): DnC's mask of every iteration; bucketing: [128, 128 + n_rows) the permutation, [160, 160 + n') the bucket masks
 INFO_INTS = 192
@@ -58,7 +64,8 @@ _ERRORS = {
   123: "invalid bucketing parameters (1 <= s <= n_rows, n = ceil(n_rows / s), not combined with NNM or ARC, a staging tile)",
   124: "invalid mimic parameters (H >= 2, 0 <= t < 2^24, a target buffer, and z and y buffers for a warm-up step)",
   125: "invalid Fang attack parameters (fang-krum: every row honest or Byzantine, n - f - 2 >= 1, n - 2 K - 1 >= 1, H >= 2, a finite "
-       "threshold > 0; fang-trim: a finite scale > 1)"}
+       "threshold > 0; fang-trim: a finite scale > 1)",
+  126: "invalid FLTrust parameters (0 <= f < n, a root gradient, no pre-aggregation, nothing pre-accumulated)"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3, "mimic": 4, "fang-krum": 5, "fang-trim": 6}
 FANG_OUT = 3   # fang-krum's float64 details of the last run: gamma_max, t, selected
@@ -116,6 +123,7 @@ class FusedLauncher:
     # mimic: the statistics of the last warm-up step, and the y scratch of the owned coordinates (`mimic_scratch`)
     self.mimic_stats = torch.zeros(MIMIC_STATS, dtype=torch.float64, device=self.device)
     self.fang_out = torch.zeros(FANG_OUT, dtype=torch.float64, device=self.device)   # fang-krum: gamma_max, t, selected
+    self.fltrust_out = torch.zeros(FLTRUST_OUT, dtype=torch.float32, device=self.device)   # FLTrust: P, N, N0, a
     self._mimic_y = None
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
@@ -133,7 +141,7 @@ class FusedLauncher:
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
             first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None,
-            bucketing_seed=0):
+            bucketing_seed=0, root=None):
     ptrs = self._ptrs
     for i in range(PTRS):
       ptrs[i] = 0
@@ -159,6 +167,7 @@ class FusedLauncher:
       scratch = self.smea_scratch(spec)
     ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch) if spec.rule == "dnc" else 0, self.arc_out.data_ptr()
     ptrs[116] = addr(scratch) if spec.rule == "smea" else 0
+    ptrs[117], ptrs[118] = addr(root), self.fltrust_out.data_ptr()   # FLTrust: the root row (rank 0's, raw address or tensor)
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -233,7 +242,7 @@ def _torch_rules(spec, step=0):
           "smea": lambda M: _ops.torch_smea(M, spec.f)}[spec.rule]
 
 
-def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed=0):
+def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed=0, root=None):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
   iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
@@ -246,7 +255,8 @@ def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed
   distances are theirs) and both elements follow, NNM's first.
   With "bucketing" G holds the n gathered rows and the rule runs on the n' = ceil(n / spec.bucket_size) bucket means, drawn with step
   key `step` and seed `bucketing_seed` (its distances and masks are those of the means); `return_details` adds (permutation [n] int32,
-  bucket masks [n'] int32)."""
+  bucket masks [n'] int32).
+  FLTrust needs `root`, the [d] root gradient; its details are (P [n], N [n], N0, a [n]), CPU tensors: the kernel's sums and coefficients."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   from ..aggregators import _ops
@@ -261,6 +271,8 @@ def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed
     bucketing_seed, step = _ops.check_bucketing_key(bucketing_seed, step)
   if spec.rule == "centered-clipping":
     return _aggregate_centered_clipping(spec, G, return_details, center, step, bucketing_seed)
+  if spec.rule == "fltrust":
+    return _aggregate_fltrust(spec, G, return_details, root)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
@@ -368,6 +380,38 @@ def _aggregate_centered_clipping(spec, G, return_details, center, step=0, bucket
   if return_details:
     dist = launcher.geo_dist_out[:spec.iterations * m].view(spec.iterations, m)
     return (out, dist.clone(), launcher.info.clone()) + _mix_details(spec, launcher, n)
+  return out
+
+
+def _aggregate_fltrust(spec, G, return_details, root):
+  """`aggregate` for FLTrust: the sm_90a kernel for fp32 and n <= 32, the torch reference on the device otherwise (double rows in
+  double)."""
+  from ..aggregators import _ops
+  n, d = G.shape
+  if spec.mix is not None:
+    raise tools.UserException("FLTrust takes no pre-aggregation (got %r)" % (spec.mix,))
+  root = _ops.check_fltrust_root(G, root)
+  if G.dtype == torch.float64 or n > MAX_WORKERS:
+    if return_details:
+      raise tools.UserException("FLTrust returns its details from the sm_90a kernel only (fp32, n <= %d)" % MAX_WORKERS)
+    return _ops.torch_fltrust(G, root)
+  if G.dtype != torch.float32:
+    out = _aggregate_fltrust(spec, G.float(), return_details, root.float())
+    return (out[0].to(G.dtype),) + out[1:] if return_details else out.to(G.dtype)
+  G, dp = _aligned_rows(G)
+  work = root
+  if dp != d or not root.is_contiguous() or root.data_ptr() % 16:
+    work = torch.zeros(dp, dtype=torch.float32, device=G.device)
+    work[:d] = root
+  launcher = _launcher(G.device, n)
+  out = torch.empty(dp, dtype=torch.float32, device=G.device)
+  rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
+  staging = torch.empty((n, dp), dtype=torch.float32, device=G.device) if n > 8 else None   # beyond one 8-row block: the staged rows
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=staging, root=work)
+  out = out[:d]
+  if return_details:
+    fo = launcher.fltrust_out.cpu()
+    return out, fo[:n].clone(), fo[MAX_WORKERS:MAX_WORKERS + n].clone(), fo[2 * MAX_WORKERS].clone(), fo[2 * MAX_WORKERS + 1:2 * MAX_WORKERS + 1 + n].clone()
   return out
 
 

@@ -31,6 +31,9 @@ itself does not mix. `pre_aggregation="arc"` (adaptive robust clipping) clips th
 the norm of the largest row left alone, in the same places (the host engine with the torch reference); "arc+nnm" clips, then mixes.
 `pre_aggregation="bucketing"` with `bucket_size` s shuffles the n gathered rows with a permutation keyed by `bucketing_seed` and the
 update number (DnC's step key), and replaces them by the n' = ceil(n / s) means of buckets of s rows: the GAR is built for n' workers.
+Rules that score the rows against a trusted root gradient (`fltrust`, `needs_root`) take it from `root`, a [d] fp32 row that rank 0's
+trainer fills every step: the fused engine keeps it in symmetric memory and its kernel reads rank 0's copy over P2P; the baseline and
+host engines broadcast it from rank 0 before the aggregation. Such rules take no pre-aggregation.
 """
 
 import os
@@ -59,6 +62,9 @@ def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz, bucket_size=None):
   spec for the kernel's pre-aggregation. Bucketing needs no f; the GAR must have been built for the n' = ceil(n / s) bucket means."""
   from ..aggregators import FusedSpec, _ops
   mix = _ops.check_pre_aggregation(pre_aggregation, bucket_size)   # None, "nnm", "arc", "arc+nnm" or "bucketing"
+  if mix is not None and getattr(gar, "needs_root", False):
+    raise tools.UserException("%s scores the direction and norm of the submitted rows against the root gradient: it cannot be combined "
+                              "with a pre-aggregation (got %r)" % (type(gar).__name__, mix))
   spec = gar.fused_spec()
   own = spec.f if spec is not None and spec.rule in FusedSpec.RULES_WITH_F else getattr(gar, "_f", None)
   f = own if nb_decl_byz is None else int(nb_decl_byz)
@@ -101,12 +107,19 @@ class _AggregationBase:
     self.slots = []
     self.center = None   # centered clipping: the rule's center v, [d] fp32
     self.attack_state = None   # mimic: {"t", "z", "istar"} (`mimic_state`)
+    self.root = None   # FLTrust: the root gradient, [d] fp32, written by rank 0's trainer
+    self.needs_root = bool(getattr(gar, "needs_root", False))
 
   def _make_center(self):
     """Allocate the center (+0) when the rule is centered clipping; it lives as long as the engine and travels in checkpoints."""
     spec = self.spec
     if spec is not None and spec.rule == "centered-clipping":
       self.center = torch.zeros(self.d, dtype=torch.float32, device=self.device)
+
+  def _broadcast_root(self):
+    """The baseline and host engines: every rank takes rank 0's root row before the aggregation (collective when R > 1)."""
+    if self.root is not None and self.world > 1:
+      dist.broadcast(self.root, src=dist.get_global_rank(self.group, 0) if self.group is not None else 0, group=self.group)
 
   @property
   def first_worker(self):
@@ -178,6 +191,8 @@ class _AggregationBase:
     DnC's step key."""
     if self.center is not None:
       return {"center": self.center}
+    if self.root is not None:
+      return {"root": self.root}
     if self.spec is not None and self.spec.rule == "dnc":
       return {"step": self.updates + 1}
     return {}
@@ -220,6 +235,7 @@ class HostAggregation(_AggregationBase):
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
     self.slots = optimizer.make_slots(self.params)
     self._make_center()
+    self.root = torch.zeros(self.d, dtype=torch.float32, device=self.device) if self.needs_root else None
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -244,6 +260,7 @@ class HostAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
+    self._broadcast_root()
     rows = self._gathered
     if self.mix is not None:
       rows = self._pre_aggregate(rows, host=True)
@@ -265,6 +282,7 @@ class BaselineAggregation(_AggregationBase):
     self.grads = torch.zeros((self.w, self.d), dtype=torch.float32, device=self.device)
     self.slots = optimizer.make_slots(self.params)
     self._make_center()
+    self.root = torch.zeros(self.d, dtype=torch.float32, device=self.device) if self.needs_root else None
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -289,6 +307,7 @@ class BaselineAggregation(_AggregationBase):
 
   def step(self, rate):
     self._gather()
+    self._broadcast_root()
     state = self._rule_kwargs()
     if self.spec is not None and self.n <= gar_ops.MAX_WORKERS:
       if self.mix == "bucketing":   # the permutation's step key is DnC's
@@ -338,12 +357,15 @@ class FusedAggregation(_AggregationBase):
     sizes = {"grads": w * d * 4, "params": d * 4, "signals": gar_ops.SIGNAL_BYTES, "mailbox": gar_ops.MAILBOX_BYTES}
     if bf16_copy:
       sizes["params_bf16"] = d * 2
+    if self.needs_root:
+      sizes["root"] = d * 4
     self.heap = SymmetricHeap(SymmetricHeap.required(*sizes.values()), self.device, group)
     for name, nbytes in sizes.items():
       self.heap.region(name, nbytes)
     self.grads = self.heap.local("grads", torch.float32, (w, d))
     self.params = self.heap.local("params", torch.float32)
     self.params_bf16 = self.heap.local("params_bf16", torch.bfloat16) if bf16_copy else None
+    self.root = self.heap.local("root", torch.float32) if self.needs_root else None   # only rank 0's copy is read
     self.slots = optimizer.make_slots(self.params)
     self._make_center()   # centered clipping: maintained on the owned segments only, like the optimizer slots
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
@@ -352,8 +374,9 @@ class FusedAggregation(_AggregationBase):
     # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; a pre-aggregation (NNM mixes, ARC
     # clips) rewrites the staged tile in place and every rule then reads it (n * owned * 4 bytes, also with R = 1); bucketing stores its
     # n' means there, so the tile has the rule's spec.n rows
+    # FLTrust's second pass reads the staged rows over several ranks, and beyond one 8-row block
     need_staging = ((self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
-                    or self.mix is not None)
+                    or self.mix is not None or (self.spec.rule == "fltrust" and (R > 1 or self.n > 8)))
     self.staging = torch.empty((self.spec.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     if self.spec.rule == "dnc":
@@ -380,6 +403,7 @@ class FusedAggregation(_AggregationBase):
     self._param_bf16_dst = [heap.peer(q, "params_bf16") for q in range(R)] if bf16_copy else None
     self._signals = [heap.peer(q, "signals") for q in range(R)]
     self._mailboxes = [heap.peer(q, "mailbox") for q in range(R)]
+    self._root_src = heap.peer(0, "root") if self.needs_root else None
     self._param_mc = heap.multicast("params") if R > 1 else 0
     # in-switch (NVLS) reduction of the gradients for the `average` rule instead of 7 P2P loads (0.241 vs 0.312 ms at 8 GPUs); AGB_NVLS_REDUCE=0 disables
     self._grad_mc = heap.multicast("grads") if (R > 1 and self.spec.rule == "average" and self.mix is None and os.environ.get("AGB_NVLS_REDUCE", "1") not in ("", "0")) else 0
@@ -498,7 +522,7 @@ class FusedAggregation(_AggregationBase):
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
                          loss_in=loss_in, loss_out=self.loss_out, center=self.center, step=self.updates, step_ptr=self.step_dev, domain=self.d,
-                         bucketing_seed=self.bucketing_seed, **self._common(self._rate_args))
+                         bucketing_seed=self.bucketing_seed, root=self._root_src, **self._common(self._rate_args))
 
   def _assemble(self, vector):
     """Full copy of a [d] vector maintained on the owned segments only (collective when R > 1)."""

@@ -34,6 +34,8 @@ same rule on the n plain rows (`bucketing_ms`, `plain_ms`, `bucketing_overhead_m
 `dnc` (divide-and-conquer) takes `--gar-rule-args iterations:<T> subsample:<b> c:<c> seed:<s>`; both engines draw the same samples (the
 step key is the update count), so the fused-vs-baseline check holds for it as for the other rules; its entry also reports the rows
 each engine kept in the checked step (`fused_mask`, `baseline_mask`, `masks_agree`).
+`fltrust` seeds a synthetic root gradient on rank 0, which the fused kernel reads over P2P and the baseline engine broadcasts; the
+fused-vs-baseline check holds for it as for the other rules.
 """
 
 import argparse
@@ -150,6 +152,10 @@ def main():
         grads[j].mul_(20.0).add_(3.0)  # the last f workers are outliers
     fused.grads.copy_(grads)
     base.grads.copy_(grads)
+    if fused.root is not None and rank == 0:   # FLTrust: a synthetic root gradient, on rank 0 only (the engines take it from there)
+      root = torch.empty(d, device=device).normal_(0.0, 1.0, generator=torch.Generator(device=device).manual_seed(99))
+      fused.root.copy_(root)
+      base.root.copy_(root)
     attack = attacks.instantiate(args.attack, n, f, args.attack_args or []) if args.attack else None
     byz_slots = list(range(n - f, n))
     extra = {"deviation": attack.deviation} if attack is not None and attack.deviation is not None else {}
@@ -177,6 +183,9 @@ def main():
       fused_mask = int(fused.launcher.info[1].item()) & 0xffffffff
       base_mask = int(gar_ops._launcher(base._gathered.device, n, rows).info[1].item()) & 0xffffffff
       mask_entry = {"fused_mask": fused_mask, "baseline_mask": base_mask, "masks_agree": fused_mask == base_mask}
+    if rule == "fltrust":   # the rows of non-zero weight, the only ones the weighted sum reads
+      coefs = fused.launcher.fltrust_out[2 * gar_ops.MAX_WORKERS + 1:2 * gar_ops.MAX_WORKERS + 1 + n].cpu()
+      mask_entry = {"weighted_rows": int((coefs != 0).sum())}
     gamma_entry = {}
     if attack is not None and attack.deviation is not None:
       # gamma as every rank solved it (fused engine), and as the baseline engine's stand-alone kernel solved it on the gathered rows
