@@ -12,8 +12,10 @@ Omniscient attacks (`omniscient = True`, `omniscient.py`) see every honest row i
 fang-krum, which solve theirs every step, and for mimic and fang-trim), `deviation` (Min-Max / Min-Sum; None otherwise), `warmup` (mimic
 only), `threshold` (fang-krum only), `scale` and `seed` (fang-trim only); the aggregation engine crafts the Byzantine rows
 (`craft_byzantine`) on every rank.
-Label-flipping attacks (`flips_labels = True`, `data.py`) implement no `apply` either: the Byzantine workers' loss trains on flipped
-labels (the trainer sets `Context.flip_from`), so nothing rewrites their rows after the backward pass.
+Data-poisoning attacks (`poisons_data = True`, `data.py`) implement no `apply` either: the Byzantine workers train on poisoned data, so
+nothing rewrites their rows after the backward pass. Label flipping (`flips_labels = True`) has their loss train on flipped labels (the
+trainer sets `Context.flip_from`); the backdoor exposes `target`, `fraction`, `scale`, `poisoned_rows(batch_size)` and
+`check_target(classes)`, and the trainer sets `Context.backdoor` from them.
 Construction raises `UserException` for arguments outside an attack's bounds.
 """
 
@@ -27,7 +29,8 @@ __all__ = ["_Attack", "register", "instantiate", "itemize"]
 class _Attack:
   forges = False  # True: the attack tampers with the row *after* it was signed (only meaningful with `--authenticate`)
   omniscient = False  # True: the rows are crafted from the honest rows by the aggregation engine (no `apply`)
-  flips_labels = False  # True: the Byzantine workers compute their gradient on flipped labels (no `apply`)
+  poisons_data = False  # True: the Byzantine workers compute their gradient on poisoned data (no `apply`)
+  flips_labels = False  # True: the data poisoning is label flipping
 
   def __init__(self, nbworkers, nbbyzwrks, args):
     raise NotImplementedError

@@ -14,8 +14,9 @@ One synchronous step on a rank:
      Byzantine-resilient SGD"): every local row becomes its worker's momentum M <- beta M + (1 - delta) G, before anything else
      reads it — a real Byzantine worker keeps its honest momentum, the attack then transforms or replaces what is submitted;
   3. real Byzantine workers overwrite their row with the selected attack (omniscient attacks: the aggregation engine crafts the
-     Byzantine rows from the honest ones, a collective call on every rank; label flipping: nothing, step 1 already trained the
-     Byzantine workers on flipped labels through `Context.flip_from`);
+     Byzantine rows from the honest ones, a collective call on every rank; data poisoning: nothing, step 1 already trained the
+     Byzantine workers on flipped labels through `Context.flip_from`, or on triggered and relabelled samples with scaled loss
+     gradients through `Context.backdoor`);
   4. the aggregation engine runs (fused kernel: gather + GAR + optimizer + parameter broadcast), after the optional pre-aggregation
      (`pre_aggregation="nnm"`: nearest-neighbour mixing of the gathered rows, Allouah et al., "Fixing by Mixing"; "arc": adaptive
      robust clipping, Allouah et al., "Boosting Robustness by Clipping Gradients in Distributed Learning"; "arc+nnm": both;
@@ -100,8 +101,8 @@ class Manager:
     self._bucket_layers = {}
     # phase A reads the rows during the backward pass: nothing may rewrite them afterwards (attacks, signing, worker momentum); with
     # a pre-aggregation the rule's distances are those of the mixed or clipped rows, which exist only once every row is complete.
-    # Label flipping rewrites no row: its Byzantine rows are complete when the backward pass ends, like the honest ones.
-    self._rewrites_rows = attack is not None and not getattr(attack, "flips_labels", False)
+    # Data poisoning rewrites no row: its Byzantine rows are complete when the backward pass ends, like the honest ones.
+    self._rewrites_rows = attack is not None and not getattr(attack, "poisons_data", False)
     plain_step = (not self._rewrites_rows and not authenticate and not ((self.l1 or -1.) > 0. or (self.l2 or -1.) > 0.) and not self.momentum_on
                   and self.pre_aggregation is None)
     if cuda and engine in ("auto", "fused") and aggregator.fused_spec() is not None:
@@ -197,7 +198,7 @@ class Manager:
         ctx.grads = self.layout.views(self.aggregation.root)
         ctx.generator = self._dropout_gen
         ctx.worker_id, ctx.nbworkers = nbworkers, nbworkers   # one past the workers: its own augmentation stream
-        ctx.flip_from = None
+        ctx.flip_from = ctx.backdoor = None
         self.root_ctx = ctx
         self.root_stream = experiment.root_stream(aggregator.root_size, self.device)
     self._stream_group = None
@@ -213,15 +214,31 @@ class Manager:
     self._attack_state = {i: {} for i in self.byzantine}
     if self.byzantine and getattr(attack, "mode", None) == "mimic":   # created now, so that a restored checkpoint finds it
       self.aggregation.mimic_state()
-    if self.byzantine and getattr(attack, "flips_labels", False):   # training contexts only: `eval_ctx` never flips
+    # the backdoor: its evaluation set and the context that stamps the trigger on all of it, checked on every rank
+    self.backdoor_ctx = self._backdoor_batch = None
+    if self.byzantine and getattr(attack, "poisons_data", False) and not attack.flips_labels:
+      attack.check_target(experiment.num_classes)
+      q = attack.poisoned_rows(int(experiment.args["batch-size"]))
+      self._backdoor_batch = experiment.backdoor_batch(attack.target)
+      ctx = Context(self.backend, False, self.dtype, self.device)
+      ctx.weights, ctx.master, ctx.state = self.weight_views, self.master_views, self.states
+      ctx.generator = self._dropout_gen
+      ctx.backdoor = (0, len(self._backdoor_batch[1]), attack.target, 1.0)
+      self.backdoor_ctx = ctx
+    if self.byzantine and getattr(attack, "poisons_data", False):   # training contexts only: `eval_ctx` is never poisoned
+      def poison(ctx, first):   # the groups >= first of the context's batch are poisoned (None: none)
+        if attack.flips_labels:
+          ctx.flip_from = first
+        else:
+          ctx.backdoor = None if first is None else (first, q, attack.target, attack.scale)
       for ctx, i in zip(self.contexts, self.local_workers):
-        ctx.flip_from = 0 if i in self.byzantine else None
+        poison(ctx, 0 if i in self.byzantine else None)
       if self.batched_ctx is not None:
         # group j of the batched pass is local worker j (ascending ids, rows 0..w-1): the Byzantine workers, the last k ids, are
         # the groups from the number of honest local workers on
         honest = sum(i not in self.byzantine for i in self.local_workers)
         assert self.local_workers == sorted(self.local_workers) and all((i in self.byzantine) == (j >= honest) for j, i in enumerate(self.local_workers))
-        self.batched_ctx.flip_from = honest if honest < len(self.local_workers) else None
+        poison(self.batched_ctx, honest if honest < len(self.local_workers) else None)
     # rows in the gathered matrix (slots) of the Byzantine workers, as the aggregation engines address them
     self.byzantine_slots = sorted(placement[i][0] * self.w + placement[i][1] for i in self.byzantine)
     # -- gradient authentication (opt-in; reference: signed worker -> PS messages of the hardened transport) -- #
@@ -455,7 +472,7 @@ class Manager:
             extra[key] = getattr(self.attack, key)
         self.aggregation.craft_byzantine(self.byzantine_slots, self.attack.mode, self.attack.coef, **extra)
       return losses
-    if not self._rewrites_rows:   # no attack, or label flipping: the rows are final
+    if not self._rewrites_rows:   # no attack, or data poisoning: the rows are final
       return losses
     forging = self.authenticator is not None and getattr(self.attack, "forges", False)
     for j, i in enumerate(self.local_workers):
@@ -516,9 +533,14 @@ class Manager:
     return total
 
   def evaluate(self):
-    """`{"top1-X-acc": float}` on one evaluation batch, with the live parameters."""
+    """`{"top1-X-acc": float}` on one evaluation batch, with the live parameters; under the backdoor attack, also
+    `"backdoor-X-acc"`: the share of the triggered backdoor evaluation set classified as the target."""
     batch = self.experiment.eval_batch(self.device)
     metrics = self.experiment.accuracy(self.model, batch, self.eval_ctx)
+    if self.backdoor_ctx is not None:
+      inputs, labels = self._backdoor_batch
+      metrics.update(self.experiment.backdoor_accuracy(self.model, (inputs.to(self.device), labels.to(self.device)), self.backdoor_ctx,
+                                                       self.attack.target))
     return {key: float(val) for key, val in metrics.items()}
 
   def check_replicas(self):

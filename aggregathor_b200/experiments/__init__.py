@@ -12,9 +12,12 @@ built TF graph nodes; here an experiment provides
                                       mnist quirk where every worker sees the same batch),
   * `eval_batch(device)`           -> one evaluation batch,
   * `root_stream(size, device)`    -> the batches of the trusted root dataset of FLTrust (`aggregators/fltrust.py`),
+  * `num_classes`                  -> the model's class count K (after `labels-offset`),
 and the base class implements `losses(...)` / `accuracy(...)` on top of them: `losses` runs forward + backward for
 each of this rank's logical workers (writing gradients into their rows) and returns the per-worker loss tensors,
-`accuracy` returns `{"top1-X-acc": tensor}` — the same metric name as the reference.
+`accuracy` returns `{"top1-X-acc": tensor}` — the same metric name as the reference. Under the backdoor attack
+(`attacks/data.py`), `preprocess` stamps the trigger on the images `ctx.backdoor` poisons (`trigger`), and
+`backdoor_accuracy` on `backdoor_batch` returns `{"backdoor-X-acc": tensor}`.
 """
 
 import pathlib
@@ -95,6 +98,31 @@ class _Experiment:
   def preprocess(self, inputs, ctx, training):
     """Device-side conversion of a raw input batch into the model's activation format."""
     return inputs.to(ctx.dtype)
+
+  @staticmethod
+  def trigger(ctx):
+    """(groups, first group, q) of the images of a batch of `ctx` that carry the backdoor trigger (`ops.nn.stamp_trigger`), or None."""
+    backdoor = getattr(ctx, "backdoor", None)
+    return None if backdoor is None else (ctx.groups, backdoor[0], backdoor[1])
+
+  def backdoor_batch(self, target):
+    """The backdoor evaluation set, on the host: the first `eval-batch-size` test samples (0: every one) whose label, after
+    `labels-offset`, is not `target`, without the trigger (evaluation preprocessing stamps it). A test set with no such sample is
+    refused."""
+    import numpy as np
+    labels = np.asarray(self.data.y_test).astype(np.int64).reshape(-1) - int(self.args.get("labels-offset", 0))
+    keep = np.flatnonzero(labels != target)[:int(self.args.get("eval-batch-size", 0)) or None]
+    if len(keep) == 0:
+      raise tools.UserException("No test sample has a label other than the backdoor's target %d: the attack's success cannot be measured" % target)
+    return torch.from_numpy(np.ascontiguousarray(self.data.x_test[keep])), torch.from_numpy(labels[keep])
+
+  def backdoor_accuracy(self, model, batch, ctx, target):
+    """`{"backdoor-X-acc": tensor}`: the fraction of `batch` that the model classifies as `target`, each image with the trigger
+    (`ctx.backdoor` poisons the whole batch) and the evaluation preprocessing."""
+    inputs, _ = batch
+    with torch.no_grad():
+      logits = model.logits(self.preprocess(inputs, ctx, False), ctx)
+      return {"backdoor-X-acc": (logits.float().argmax(dim=1) == target).float().mean()}
 
   # -- reference-named entry points ------------------------------------------- #
   def losses(self, model, batches, contexts, trace=None):

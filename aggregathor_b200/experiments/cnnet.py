@@ -16,12 +16,16 @@ from . import _Experiment, register
 from ._data import BatchStream, Dataset
 
 
-def cifarnet_preprocess(images, dtype, training, generator=None):
-  """uint8 NHWC batch -> standardised channels_last activations of `dtype`."""
+def cifarnet_preprocess(images, dtype, training, generator=None, trigger=None):
+  """uint8 NHWC batch -> standardised channels_last activations of `dtype`. `trigger` = (groups, first, q): the backdoor trigger
+  (`ops.nn.stamp_trigger`) on the poisoned images, after the mirror and before the standardisation."""
   x = images.permute(0, 3, 1, 2).to(torch.float32)
   if training:
     flip = torch.rand(x.shape[0], device=x.device, generator=generator) < 0.5
     x = torch.where(flip.view(-1, 1, 1, 1), x.flip(3), x)
+  if trigger is not None:
+    from ..ops.nn import stamp_trigger
+    x = stamp_trigger(x.permute(0, 2, 3, 1), *trigger).permute(0, 3, 1, 2)
   mean = x.mean(dim=(1, 2, 3), keepdim=True)
   std = x.std(dim=(1, 2, 3), keepdim=True, unbiased=False)
   x = (x - mean) / torch.clamp(std, min=1.0 / (x[0].numel() ** 0.5))
@@ -29,6 +33,8 @@ def cifarnet_preprocess(images, dtype, training, generator=None):
 
 
 class CNNetExperiment(_Experiment):
+  num_classes = 10
+
   def __init__(self, args):
     self.args = tools.parse_keyval(args if args is not None else [], defaults={
       "batch-size": 32, "eval-batch-size": 1024, "nb-fetcher-threads": 1, "nb-batcher-threads": 1, "preprocessing": "cifarnet", "seed": 0})
@@ -61,7 +67,8 @@ class CNNetExperiment(_Experiment):
     return next(self._eval_stream)
 
   def preprocess(self, inputs, ctx, training):
-    return self.preprocessor(inputs, ctx.dtype, training, backend=ctx.backend, stream_id=getattr(ctx, "worker_id", 0) or 0).contiguous(memory_format=torch.channels_last)
+    return self.preprocessor(inputs, ctx.dtype, training, backend=ctx.backend, stream_id=getattr(ctx, "worker_id", 0) or 0,
+                             trigger=self.trigger(ctx)).contiguous(memory_format=torch.channels_last)
 
 
 register("cnnet", CNNetExperiment)

@@ -16,6 +16,7 @@ from ._data import BatchStream, Dataset
 
 class MNIST(_Experiment):
   dataset_name = "mnist"
+  num_classes = 10
 
   def __init__(self, args):
     self.args = tools.parse_keyval(args if args is not None else [], defaults={"batch-size": 32, "shared-batch": 0, "eval-batch-size": 0, "seed": 0})
@@ -55,6 +56,10 @@ class MNIST(_Experiment):
     return x, y
 
   def preprocess(self, inputs, ctx, training):
+    trigger = self.trigger(ctx)
+    if trigger is not None:
+      from ..ops.nn import stamp_trigger
+      inputs = stamp_trigger(inputs, *trigger)
     return (inputs.reshape(inputs.shape[0], -1).to(torch.float32) / 255.).to(ctx.dtype)
 
 

@@ -113,14 +113,16 @@ class SlimExperiment(_Experiment):
     return torch.where(flip.view(-1, 1, 1, 1), images.flip(2), images)
 
   def preprocess(self, inputs, ctx, training):
+    trigger = self.trigger(ctx)   # the backdoor trigger, after the geometric augmentation and before the normalisation
     if self.args["augment"] == "slim" or tuple(inputs.shape[1:3]) != (self.args["image-size"], self.args["image-size"]):
-      return self.slim_preprocessor(inputs, ctx.dtype, training, backend=ctx.backend, stream_id=getattr(ctx, "worker_id", 0) or 0).contiguous(memory_format=self._channels_last())
+      return self.slim_preprocessor(inputs, ctx.dtype, training, backend=ctx.backend, stream_id=getattr(ctx, "worker_id", 0) or 0,
+                                    trigger=trigger).contiguous(memory_format=self._channels_last())
     if training and self.stochastic_preprocess:
       inputs = self._augment(inputs, ctx.generator)
     if self.preprocessing == "cifarnet":
-      return cifarnet_preprocess(inputs, ctx.dtype, training, ctx.generator)
+      return cifarnet_preprocess(inputs, ctx.dtype, training, ctx.generator, trigger)
     from ..ops import nn as nn_ops
-    return nn_ops.image_normalize(ctx.backend, inputs, self.preprocessing, ctx.dtype)
+    return nn_ops.image_normalize(ctx.backend, inputs, self.preprocessing, ctx.dtype, trigger)
 
 
 for _model in nets_factory.networks_map:

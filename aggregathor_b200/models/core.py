@@ -46,6 +46,8 @@ class Context:
     self.groups = 1             # logical workers batched in one pass (their batches are consecutive along dim 0)
     self.group_stride = 0       # elements between two workers' gradient rows (`grads` are worker 0's views)
     self.flip_from = None       # label-flipping attack: the groups >= flip_from train on the labels K - 1 - y (None: no flip)
+    self.backdoor = None        # backdoor attack: (first group, q, target, scale): the first q images of every group >= first carry the
+                                # trigger and train on `target`, the groups' loss gradients scaled by `scale` (None: no poisoning)
 
 
 class Module:
@@ -809,12 +811,12 @@ class Model:
   def loss_and_backward(self, x, labels, ctx):
     """Forward, mean softmax cross-entropy, backward. Returns the loss (0-d fp32 tensor; shape [ctx.groups] when several logical
     workers are batched: each worker's loss is the mean over its own slice of the batch). The groups >= `ctx.flip_from` train on
-    flipped labels, in the main and the auxiliary heads alike."""
+    flipped labels, and the groups `ctx.backdoor` poisons on the backdoor's target, in the main and the auxiliary heads alike."""
     logits = self.logits(x, ctx)
-    loss, dlogits = nn_ops.softmax_xent(ctx.backend, logits, labels, self.label_smoothing, ctx.groups, ctx.flip_from)
+    loss, dlogits = nn_ops.softmax_xent(ctx.backend, logits, labels, self.label_smoothing, ctx.groups, ctx.flip_from, ctx.backdoor)
     dlogits = self._shaped(dlogits, self._raw_shape, ctx)
     for aux in ctx.aux_heads:
-      aux_loss, aux_dlogits = nn_ops.softmax_xent(ctx.backend, aux._saved_logits, labels, self.label_smoothing, ctx.groups, ctx.flip_from)
+      aux_loss, aux_dlogits = nn_ops.softmax_xent(ctx.backend, aux._saved_logits, labels, self.label_smoothing, ctx.groups, ctx.flip_from, ctx.backdoor)
       loss = loss + aux.weight * aux_loss
       aux._saved_dlogits = self._shaped(aux_dlogits * aux.weight, aux._saved_shape, ctx)
     ctx.aux_heads = []

@@ -179,4 +179,24 @@ __device__ __forceinline__ bool before(float a, int ia, float b, int ib) {
     return ia < ib;
 }
 
+// ---- backdoor trigger (`attacks/data.py`, `ops.nn.stamp_trigger`) ----------- //
+// A batch of consecutive per-worker batches of `rows` images: image b is poisoned iff b / rows >= first and b % rows < q. A poisoned
+// H x W network input carries an s x s checkerboard, 255 where i + j is even and 0 elsewhere on every channel, at the bottom right one
+// pixel from the edges (top-left corner (H - 1 - s, W - 1 - s)), in the raw [0, 255] domain. s = 0 stamps nothing.
+struct Trigger {
+    int rows, first, q, s;
+};
+__device__ __forceinline__ bool trigger_poisoned(Trigger const& t, long long image) {
+    return t.s > 0 && image / t.rows >= t.first && image % t.rows < t.q;
+}
+// The trigger's value at pixel (y, x) of a poisoned H x W image, or -1 outside the trigger.
+__device__ __forceinline__ float trigger_value(Trigger const& t, int H, int W, int y, int x) {
+    int const i = y - (H - 1 - t.s), j = x - (W - 1 - t.s);
+    return i >= 0 && i < t.s && j >= 0 && j < t.s ? ((i + j) & 1 ? 0.f : 255.f) : -1.f;
+}
+// Host-side check of a descriptor for a batch of N images of H x W (s = 0: nothing to check).
+inline bool trigger_valid(Trigger const& t, long long N, int H, int W) {
+    return t.s == 0 || (t.rows >= 1 && N % t.rows == 0 && t.first >= 0 && t.q >= 0 && t.q <= t.rows && t.s + 1 <= H && t.s + 1 <= W);
+}
+
 } // namespace agb

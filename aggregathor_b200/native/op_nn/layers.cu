@@ -9,6 +9,8 @@
 // `groups` splits the rows into equal consecutive groups with independent statistics: one group per logical worker, so that
 // several workers' batches can share one launch while keeping per-worker BatchNorm semantics.
 
+#include <cmath>
+
 #include <cuda_bf16.h>
 
 #include <agb_device.cuh>
@@ -750,11 +752,14 @@ __global__ void avgpool_bwd_kernel(T const* __restrict__ dy, T* __restrict__ dx,
 // ---------------------------------------------------------------------------- //
 // Softmax cross-entropy, one warp per row. logits bf16 [B, ld] (K valid columns), labels int64.
 // loss += mean_b(-sum_k t_k log p_k) ; dlogits = (p - t) / B  (bf16, same leading dimension).
-// Label flipping (Fang et al., USENIX Security 2020): the rows of groups >= flip_from train on K - 1 - y instead of y; a label
-// outside [0, K) matches no class and is left as it is. flip_from == groups flips nothing.
+// Data poisoning of the groups >= poison_from (poison_from == groups poisons nothing):
+//   label flipping (Fang et al., USENIX Security 2020; target < 0, q = rows_per_group, scale = 1): every row trains on K - 1 - y
+//     instead of y; a label outside [0, K) matches no class and is left as it is;
+//   backdoor (Gu et al., BadNets; Bagdasaryan et al., AISTATS 2020; 0 <= target < K): the rows with row % rows_per_group < q train on
+//     `target`, and every row's dlogits is multiplied by `scale` (the loss is not). scale = 1 gives the unscaled bits exactly.
 template<typename T>
 __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long const* __restrict__ labels, T* __restrict__ dlogits, float* __restrict__ loss,
-                                    int B, int K, long long ld, float smoothing, int rows_per_group, int flip_from) {
+                                    int B, int K, long long ld, float smoothing, int rows_per_group, int poison_from, int q, int target, float scale) {
     pdl_trigger();
     pdl_wait();
     int const warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -773,7 +778,11 @@ __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long cons
     sum = warp_sum(sum);
     float const lse = mx + __logf(sum);
     long long const y = labels[warp];
-    int const label = group >= flip_from && y >= 0 && y < K ? K - 1 - static_cast<int>(y) : static_cast<int>(y);
+    bool const poisoned = group >= poison_from;
+    int label = static_cast<int>(y);
+    if (poisoned && warp % rows_per_group < q)
+        label = target >= 0 ? target : y >= 0 && y < K ? K - 1 - label : label;
+    float const gscale = poisoned ? scale : 1.f;
     float const off_t = smoothing / static_cast<float>(K), on_t = 1.f - smoothing + off_t;
     float const inv_b = 1.f / static_cast<float>(rows_per_group);   // each group (logical worker) averages over its own batch
     float local = 0.f;
@@ -783,26 +792,35 @@ __global__ void softmax_xent_kernel(T const* __restrict__ logits, long long cons
         float const logp = z - lse;
         float const t = k == label ? on_t : off_t;
         local -= t * logp;
-        drow[k] = from_f<T>((__expf(logp) - t) * inv_b);
+        drow[k] = from_f<T>(((__expf(logp) - t) * inv_b) * gscale);
     }
     local = warp_sum(local);
     if (lane == 0)
         atomicAdd(loss + group, local * inv_b);
 }
 
-// uint8 NHWC image -> bf16 NHWC activations with C padded to `Cpad`: y = (x - mean[c]) * scale
+// uint8 NHWC image [.., H, W, C] -> bf16 NHWC activations with C padded to `Cpad`: y = (x - mean[c]) * scale, with the backdoor
+// trigger (agb_device.cuh) in place of x on the poisoned images.
 template<typename T>
-__global__ void image_normalize_kernel(unsigned char const* __restrict__ x, T* __restrict__ y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale) {
+__global__ void image_normalize_kernel(unsigned char const* __restrict__ x, T* __restrict__ y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale,
+                                       int H, int W, Trigger trigger) {
     pdl_trigger();
     pdl_wait();
     long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     long long const stride = static_cast<long long>(gridDim.x) * blockDim.x;
     for (; i < pixels; i += stride) {
+        float stamp = -1.f;
+        if (trigger.s > 0) {
+            long long const hw = static_cast<long long>(H) * W, image = i / hw;
+            int const pixel = static_cast<int>(i - image * hw);
+            if (trigger_poisoned(trigger, image))
+                stamp = trigger_value(trigger, H, W, pixel / W, pixel % W);
+        }
         for (int c = 0; c < Cpad; ++c) {
             float v = 0.f;
             if (c < C) {
                 float const m = c == 0 ? m0 : c == 1 ? m1 : m2;
-                v = (static_cast<float>(x[i * C + c]) - m) * scale;
+                v = ((stamp >= 0.f ? stamp : static_cast<float>(x[i * C + c])) - m) * scale;
             }
             y[i * Cpad + c] = from_f<T>(v);
         }
@@ -1618,21 +1636,23 @@ int avgpool_backward_impl(void const* dy, void* dx, int N, int HW, int C, void* 
 }
 
 template<typename T>
-int softmax_xent_impl(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
-    if (groups < 1 || B % groups || flip_from < 0 || flip_from > groups)
+int softmax_xent_impl(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups,
+                      int poison_from, int q, int target, float scale, void* stream) {
+    if (groups < 1 || B % groups || poison_from < 0 || poison_from > groups)
         return 301;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     AGB_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float) * groups, s));
     int const warps_per_cta = 4;
     AGB_CUDA_OK(launch_pdl(softmax_xent_kernel<T>, dim3((B + warps_per_cta - 1) / warps_per_cta), dim3(warps_per_cta * 32), 0, s, static_cast<T const*>(logits), static_cast<long long const*>(labels),
-        static_cast<T*>(dlogits), static_cast<float*>(loss), B, K, ld, smoothing, B / groups, flip_from));
+        static_cast<T*>(dlogits), static_cast<float*>(loss), B, K, ld, smoothing, B / groups, poison_from, q, target, scale));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 template<typename T>
-int image_normalize_impl(void const* x, void* y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale, void* stream) {
-    AGB_CUDA_OK(launch_pdl(image_normalize_kernel<T>, dim3(grid_for(pixels)), dim3(kThreads), 0, static_cast<cudaStream_t>(stream), static_cast<unsigned char const*>(x), static_cast<T*>(y), pixels, C, Cpad, m0, m1, m2, scale));
+int image_normalize_impl(void const* x, void* y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale, int H, int W, Trigger trigger, void* stream) {
+    AGB_CUDA_OK(launch_pdl(image_normalize_kernel<T>, dim3(grid_for(pixels)), dim3(kThreads), 0, static_cast<cudaStream_t>(stream), static_cast<unsigned char const*>(x), static_cast<T*>(y), pixels, C, Cpad, m0, m1, m2, scale,
+        H, W, trigger));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1822,25 +1842,59 @@ int agb_avgpool_backward_f32(void const* dy, void* dx, int N, int HW, int C, voi
 
 
 int agb_softmax_xent(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, void* stream) {
-    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, stream);
+    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, 0, -1, 1.f, stream);
 }
 int agb_softmax_xent_f32(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, void* stream) {
-    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, stream);
+    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, groups, 0, -1, 1.f, stream);
 }
 // The same, with the labels of the groups >= flip_from (0 <= flip_from <= groups) flipped to K - 1 - y.
 int agb_softmax_xent_flip(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
-    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, stream);
+    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, groups >= 1 ? B / groups : 0, -1, 1.f, stream);
 }
 int agb_softmax_xent_flip_f32(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups, int flip_from, void* stream) {
-    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, stream);
+    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, flip_from, groups >= 1 ? B / groups : 0, -1, 1.f, stream);
+}
+// The backdoor: in the groups >= poison_from (0 <= poison_from <= groups), the rows with row % (B / groups) < q (0 <= q <= B / groups)
+// train on `target` (0 <= target < K), and every row's dlogits is multiplied by `scale` (finite, > 0). Invalid parameters: status 303.
+static bool backdoor_checked(int B, int K, int groups, int poison_from, int q, int target, float scale) {
+    return groups >= 1 && B % groups == 0 && poison_from >= 0 && poison_from <= groups && q >= 0 && q <= B / groups && target >= 0 && target < K
+        && std::isfinite(scale) && scale > 0.f;
+}
+int agb_softmax_xent_backdoor(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups,
+                              int poison_from, int q, int target, float scale, void* stream) {
+    if (!backdoor_checked(B, K, groups, poison_from, q, target, scale))
+        return 303;
+    return softmax_xent_impl<bf16>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, poison_from, q, target, scale, stream);
+}
+int agb_softmax_xent_backdoor_f32(void const* logits, void const* labels, void* dlogits, void* loss, int B, int K, long long ld, float smoothing, int groups,
+                                  int poison_from, int q, int target, float scale, void* stream) {
+    if (!backdoor_checked(B, K, groups, poison_from, q, target, scale))
+        return 303;
+    return softmax_xent_impl<float>(logits, labels, dlogits, loss, B, K, ld, smoothing, groups, poison_from, q, target, scale, stream);
 }
 
 
 int agb_image_normalize(void const* x, void* y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale, void* stream) {
-    return image_normalize_impl<bf16>(x, y, pixels, C, Cpad, m0, m1, m2, scale, stream);
+    return image_normalize_impl<bf16>(x, y, pixels, C, Cpad, m0, m1, m2, scale, 1, 1, Trigger{1, 0, 0, 0}, stream);
 }
 int agb_image_normalize_f32(void const* x, void* y, long long pixels, int C, int Cpad, float m0, float m1, float m2, float scale, void* stream) {
-    return image_normalize_impl<float>(x, y, pixels, C, Cpad, m0, m1, m2, scale, stream);
+    return image_normalize_impl<float>(x, y, pixels, C, Cpad, m0, m1, m2, scale, 1, 1, Trigger{1, 0, 0, 0}, stream);
+}
+// The same on N images of H x W, with the backdoor trigger (side s >= 1) stamped on image b iff b / rows >= first and b % rows < q.
+// Invalid descriptor: status 503.
+int agb_image_normalize_backdoor(void const* x, void* y, int N, int H, int W, int C, int Cpad, float m0, float m1, float m2, float scale,
+                                 int rows, int first, int q, int s, void* stream) {
+    Trigger const t{rows, first, q, s};
+    if (N < 1 || H < 1 || W < 1 || s < 1 || !trigger_valid(t, N, H, W))
+        return 503;
+    return image_normalize_impl<bf16>(x, y, static_cast<long long>(N) * H * W, C, Cpad, m0, m1, m2, scale, H, W, t, stream);
+}
+int agb_image_normalize_backdoor_f32(void const* x, void* y, int N, int H, int W, int C, int Cpad, float m0, float m1, float m2, float scale,
+                                     int rows, int first, int q, int s, void* stream) {
+    Trigger const t{rows, first, q, s};
+    if (N < 1 || H < 1 || W < 1 || s < 1 || !trigger_valid(t, N, H, W))
+        return 503;
+    return image_normalize_impl<float>(x, y, static_cast<long long>(N) * H * W, C, Cpad, m0, m1, m2, scale, H, W, t, stream);
 }
 
 

@@ -12,6 +12,10 @@
 //              standardisation;  eval: central crop / pad + standardisation
 //   plain      (x - mean) * scale after a bilinear resize of the whole image (lenet-style and user-defined preprocessing)
 //
+// The backdoor attack's trigger (`Trigger` in agb_device.cuh) is written into the sampled pixel, after the geometric operations
+// (crop, resize, mirror) and before every photometric one, so that it sits at the same place of the network input and the per-image
+// statistics include it.
+//
 // "Resize then crop" never materialises the resized image: every output pixel samples the source box directly (bilinear,
 // TF1 `resize_bilinear` coordinates: src = origin + index * box / out). One CTA per image; operations that need a per-image
 // statistic (contrast, standardisation) run a first pass that reduces it in the CTA. All randomness is counter based —
@@ -39,6 +43,7 @@ struct PreprocParams {
     float mean[3], scale;       // plain / vgg: (v - mean[c]) * scale
     unsigned long long seed;
     unsigned long long const* counter;   // device step counter (null = 0)
+    Trigger trigger;                     // backdoor trigger of the poisoned images (s = 0: none)
 };
 
 __device__ __forceinline__ float uniform01(unsigned long long seed, unsigned long long step, unsigned image, unsigned slot) {
@@ -198,10 +203,20 @@ __global__ void __launch_bounds__(512) preprocess_kernel(PreprocParams const p) 
     bool const inception_train = p.mode == kInception && p.training;
     bool const cifar = p.mode == kCifarnet;
     bool const need_stats = inception_train || cifar;
+    bool const poisoned = trigger_poisoned(p.trigger, image);
 
     // value of one output pixel up to (not including) the statistic-dependent operation
     auto stage1 = [&](int idx, float (&v)[3]) {
         sample_pixel(p, s, img, idx / p.OW, idx % p.OW, v);
+        if (poisoned) {
+            float const t = trigger_value(p.trigger, p.OH, p.OW, idx / p.OW, idx % p.OW);
+            if (t >= 0.f) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    if (c < p.C)
+                        v[c] = t;
+            }
+        }
         if (p.mode == kInception) {
 #pragma unroll
             for (int c = 0; c < 3; ++c)
@@ -314,12 +329,7 @@ __global__ void __launch_bounds__(512) preprocess_kernel(PreprocParams const p) 
     }
 }
 
-} // namespace
-
-extern "C" {
-
-// ints: N SH SW C OH OW mode training out_fp32 resize_min resize_max pad ; floats: area_min area_max mean0 mean1 mean2 scale
-int agb_image_preprocess(void const* src, void* dst, int const* ints, float const* floats, unsigned long long seed, void const* counter, void* stream) {
+int image_preprocess(void const* src, void* dst, int const* ints, float const* floats, unsigned long long seed, void const* counter, Trigger trigger, void* stream) {
     PreprocParams p{};
     p.src = static_cast<unsigned char const*>(src);
     p.dst = dst;
@@ -330,10 +340,13 @@ int agb_image_preprocess(void const* src, void* dst, int const* ints, float cons
     p.mean[0] = floats[2]; p.mean[1] = floats[3]; p.mean[2] = floats[4]; p.scale = floats[5];
     p.seed = seed;
     p.counter = static_cast<unsigned long long const*>(counter);
+    p.trigger = trigger;
     if (p.N < 1 || p.C < 1 || p.C > 3 || p.SH < 1 || p.SW < 1 || p.OH < 1 || p.OW < 1 || p.mode < 0 || p.mode > kCifarnet)
         return 501;
     if (p.mode == kVgg && (p.resize_min < 1 || p.resize_max < p.resize_min))
         return 502;
+    if (!trigger_valid(p.trigger, p.N, p.OH, p.OW))
+        return 503;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (p.out_fp32)
         preprocess_kernel<float><<<p.N, 512, 0, s>>>(p);
@@ -341,6 +354,22 @@ int agb_image_preprocess(void const* src, void* dst, int const* ints, float cons
         preprocess_kernel<__nv_bfloat16><<<p.N, 512, 0, s>>>(p);
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+// ints: N SH SW C OH OW mode training out_fp32 resize_min resize_max pad ; floats: area_min area_max mean0 mean1 mean2 scale
+int agb_image_preprocess(void const* src, void* dst, int const* ints, float const* floats, unsigned long long seed, void const* counter, void* stream) {
+    return image_preprocess(src, dst, ints, floats, seed, counter, Trigger{1, 0, 0, 0}, stream);
+}
+// The same, with the backdoor trigger (side s >= 1) stamped on image b iff b / rows >= first and b % rows < q; 503: invalid descriptor.
+int agb_image_preprocess_backdoor(void const* src, void* dst, int const* ints, float const* floats, unsigned long long seed, void const* counter,
+                                  int rows, int first, int q, int s, void* stream) {
+    if (s < 1)
+        return 503;
+    return image_preprocess(src, dst, ints, floats, seed, counter, Trigger{rows, first, q, s}, stream);
 }
 
 } // extern "C"

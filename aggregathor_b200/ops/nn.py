@@ -11,6 +11,7 @@ Tensor conventions: activations (N, C, H, W) with channels_last strides (NHWC me
 are tensors of shape [Cout, kh, kw, Cin] (OHWI memory); linear weights [out, in].
 """
 
+import math
 import os
 
 import torch
@@ -461,17 +462,46 @@ def flip_labels(labels, classes, groups=1, flip_from=0):
   return torch.cat([labels[:lo], torch.where((tail >= 0) & (tail < classes), classes - 1 - tail, tail)])
 
 
-def softmax_xent(backend, logits, labels, label_smoothing=0.0, groups=1, flip_from=None):
+def check_backdoor(backdoor, classes, groups, rows):
+  """Validates a backdoor descriptor (first group, q, target, scale) for `groups` groups of `rows` rows and `classes` classes."""
+  first, q, target, scale = backdoor
+  if not (0 <= first <= groups and 0 <= q <= rows and 0 <= target < classes and math.isfinite(scale) and scale > 0.):
+    raise ValueError("invalid backdoor descriptor %r for %d groups of %d rows and %d classes" % (tuple(backdoor), groups, rows, classes))
+
+
+def backdoor_labels(labels, groups, first, q, target):
+  """Labels of the backdoor attack: the first `q` rows of every consecutive batch slice (group) >= `first` become `target`."""
+  rows = labels.shape[0] // groups
+  out = labels.clone()
+  for g in range(first, groups):
+    out[g * rows:g * rows + q] = target
+  return out
+
+
+def softmax_xent(backend, logits, labels, label_smoothing=0.0, groups=1, flip_from=None, backdoor=None):
   """Mean softmax cross-entropy -> (loss, dlogits [B, K]). `groups` == 1: 0-d loss over the batch; `groups` > 1: one mean per
   consecutive batch slice (logical worker), loss of shape [groups], gradients scaled by 1 / (B / groups). `flip_from`: the groups
-  >= flip_from train on `flip_labels` (label-flipping attack; None: no flip). A label outside [0, K) matches no class."""
+  >= flip_from train on `flip_labels` (label-flipping attack; None: no flip). A label outside [0, K) matches no class.
+  `backdoor` = (first, q, target, scale): the groups >= first train on `backdoor_labels` and their dlogits are multiplied by `scale`;
+  the loss is not (backdoor attack; None: no poisoning)."""
+  if flip_from is not None and backdoor is not None:
+    raise ValueError("label flipping and the backdoor are two attacks: give flip_from or backdoor, not both")
+  if backdoor is not None:
+    check_backdoor(backdoor, logits.shape[1], groups, logits.shape[0] // groups)
   if backend == "native" and logits.is_cuda:
-    out = _native().softmax_xent(logits, labels, label_smoothing, groups, flip_from)
+    out = _native().softmax_xent(logits, labels, label_smoothing, groups, flip_from, backdoor)
     if out is not None:
       return out
     _fallback("softmax_xent")
   if flip_from is not None:
     labels = flip_labels(labels, logits.shape[1], groups, flip_from)
+  if backdoor is not None:
+    first, q, target, scale = backdoor
+    loss, dlogits = softmax_xent(backend, logits, backdoor_labels(labels, groups, first, q, target), label_smoothing, groups)
+    if scale != 1.0 and first < groups:
+      rows = logits.shape[0] // groups
+      dlogits = torch.cat([dlogits[:first * rows], dlogits[first * rows:] * scale])
+    return loss, dlogits
   if groups > 1:
     outs = [softmax_xent(backend, lg, lb, label_smoothing) for lg, lb in zip(_chunks(logits, groups), _chunks(labels, groups))]
     return torch.stack([o[0] for o in outs]), torch.cat([o[1] for o in outs], dim=0)
@@ -491,14 +521,50 @@ def softmax_xent(backend, logits, labels, label_smoothing=0.0, groups=1, flip_fr
 _VGG_MEANS = (123.68, 116.78, 103.94)
 
 
-def image_normalize(backend, images, mode, dtype):
+def trigger_size(height, width):
+  """Side s = ceil(min(H, W) / 10) of the backdoor trigger of an H x W network input (MNIST 3, CIFAR 4, 224-pixel ImageNet 23)."""
+  s = -(-min(height, width) // 10)
+  if s + 1 > min(height, width):
+    raise ValueError("a %d x %d input has no room for the backdoor trigger" % (height, width))
+  return s
+
+
+def trigger_descriptor(images, trigger):
+  """The kernels' descriptor (rows, first, q, s) of `trigger` = (groups, first, q) on the NHW[C] batch `images`."""
+  groups, first, q = trigger
+  n, h, w = images.shape[:3]
+  if groups < 1 or n % groups or not (0 <= first and 0 <= q <= n // groups):
+    raise ValueError("invalid backdoor trigger %r for a batch of %d images" % (tuple(trigger), n))
+  return n // groups, first, q, trigger_size(h, w)
+
+
+def stamp_trigger(images, groups, first, q):
+  """The backdoor trigger on a raw NHW[C] batch in the [0, 255] domain (any dtype), as a new tensor: an s x s checkerboard
+  (`trigger_size`), 255 where i + j is even and 0 elsewhere on every channel, at the bottom right one pixel from the edges (rows and
+  columns H - 1 - s .. H - 2 and W - 1 - s .. W - 2), on the first `q` images of every consecutive slice of n / `groups` images from slice
+  `first` on. The one definition of the pattern and its placement: the kernels (`Trigger` in `agb_device.cuh`) are tested against it."""
+  rows, first, q, s = trigger_descriptor(images, (groups, first, q))
+  h, w = images.shape[1:3]
+  out = images.clone()
+  for g in range(first, groups):
+    patch = out[g * rows:g * rows + q, h - 1 - s:h - 1, w - 1 - s:w - 1]
+    patch.fill_(0)
+    patch[:, 0::2, 0::2] = 255
+    patch[:, 1::2, 1::2] = 255
+  return out
+
+
+def image_normalize(backend, images, mode, dtype, trigger=None):
   """uint8 NHWC host-format batch (already on the device) -> normalised (N, C, H, W) channels_last activations.
-  `vgg`: subtract the per-channel ImageNet means; `inception`: x/127.5 - 1; `lenet`: (x - 128)/128."""
+  `vgg`: subtract the per-channel ImageNet means; `inception`: x/127.5 - 1; `lenet`: (x - 128)/128. `trigger` = (groups, first, q):
+  the backdoor trigger on the images `stamp_trigger` poisons (None: none)."""
   if backend == "native" and images.is_cuda:
-    out = _native().image_normalize(images, mode, dtype)
+    out = _native().image_normalize(images, mode, dtype, trigger)
     if out is not None:
       return out
     _fallback("image_normalize")
+  if trigger is not None:
+    images = stamp_trigger(images, *trigger)
   x = images.to(torch.float32)
   if mode == "vgg" and x.shape[-1] == 3:
     x = x - torch.tensor(_VGG_MEANS, device=x.device)

@@ -818,8 +818,10 @@ def global_avgpool_backward(dy, shape):
   return dx
 
 
-def softmax_xent(logits, labels, label_smoothing, groups=1, flip_from=None):
-  """`flip_from`: the rows of groups >= flip_from train on the flipped labels K - 1 - y (label-flipping attack; None: no flip)."""
+def softmax_xent(logits, labels, label_smoothing, groups=1, flip_from=None, backdoor=None):
+  """`flip_from`: the rows of groups >= flip_from train on the flipped labels K - 1 - y (label-flipping attack; None: no flip).
+  `backdoor` = (first, q, target, scale): in the groups >= first, the first q rows of the group train on `target`, and every row's
+  dlogits is multiplied by `scale` (backdoor attack; None: none)."""
   if not enabled("xent") or logits.dtype not in _DTYPES or logits.stride(1) != 1:
     return None
   batch, classes = logits.shape
@@ -828,7 +830,11 @@ def softmax_xent(logits, labels, label_smoothing, groups=1, flip_from=None):
   labels = labels if labels.dtype == torch.int64 else labels.long()
   common = (_ptr(logits), _ptr(labels), _ptr(dlogits), _ptr(loss), ctypes.c_int(batch), ctypes.c_int(classes), ctypes.c_longlong(logits.stride(0)),
             ctypes.c_float(label_smoothing), ctypes.c_int(groups))
-  if flip_from is None:
+  if backdoor is not None:
+    first, q, target, scale = backdoor
+    _check(_fn("agb_softmax_xent_backdoor", logits)(*common, ctypes.c_int(first), ctypes.c_int(q), ctypes.c_int(target), ctypes.c_float(scale), _stream()),
+           "softmax_xent")
+  elif flip_from is None:
     _check(_fn("agb_softmax_xent", logits)(*common, _stream()), "softmax_xent")
   else:
     _check(_fn("agb_softmax_xent_flip", logits)(*common, ctypes.c_int(flip_from), _stream()), "softmax_xent")
@@ -838,8 +844,9 @@ def softmax_xent(logits, labels, label_smoothing, groups=1, flip_from=None):
 _MEANS = {"vgg": (123.68, 116.78, 103.94, 1.0), "inception": (127.5, 127.5, 127.5, 1.0 / 127.5), "lenet": (128.0, 128.0, 128.0, 1.0 / 128.0)}
 
 
-def image_normalize(images, mode, dtype):
-  """uint8 NHWC -> bf16 channels_last (N, Cpad, H, W) with the channel dimension zero-padded to 8 (TMA/im2col friendly)."""
+def image_normalize(images, mode, dtype, trigger=None):
+  """uint8 NHWC -> bf16 channels_last (N, Cpad, H, W) with the channel dimension zero-padded to 8 (TMA/im2col friendly). `trigger` =
+  (groups, first, q): the backdoor trigger on the images `ops.nn.stamp_trigger` poisons (None: none)."""
   if not enabled("image") or images.dtype != torch.uint8 or dtype not in _DTYPES or images.dim() != 4 or not images.is_contiguous():
     return None
   n, h, w, c = images.shape
@@ -849,6 +856,13 @@ def image_normalize(images, mode, dtype):
   if mode == "vgg" and c != 3:
     m0, m1, m2, scale = _MEANS["lenet"]
   out = torch.empty((n, h, w, c), dtype=dtype, device=images.device)
+  if trigger is not None:
+    from .nn import trigger_descriptor
+    rows, first, q, side = trigger_descriptor(images, trigger)
+    _check(_fn("agb_image_normalize_backdoor", out)(_ptr(images), _ptr(out), ctypes.c_int(n), ctypes.c_int(h), ctypes.c_int(w), ctypes.c_int(c), ctypes.c_int(c),
+                                                ctypes.c_float(m0), ctypes.c_float(m1), ctypes.c_float(m2), ctypes.c_float(scale), ctypes.c_int(rows),
+                                                ctypes.c_int(first), ctypes.c_int(q), ctypes.c_int(side), _stream()), "image_normalize")
+    return out.permute(0, 3, 1, 2)
   _check(_fn("agb_image_normalize", out)(_ptr(images), _ptr(out), ctypes.c_longlong(n * h * w), ctypes.c_int(c), ctypes.c_int(c), ctypes.c_float(m0), ctypes.c_float(m1),
                                     ctypes.c_float(m2), ctypes.c_float(scale), _stream()), "image_normalize")
   return out.permute(0, 3, 1, 2)

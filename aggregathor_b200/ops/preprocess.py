@@ -13,6 +13,9 @@ Modes (training / evaluation):
   inception  distorted bbox crop (area 5-100 %, aspect 3/4-4/3), resize, mirror, colour distortion, [-1, 1]  /  central 87.5 % + resize
   cifarnet   pad 4, random crop, mirror, brightness 63, contrast [0.2, 1.8], per-image standardisation  /  central crop + standardisation
   plain      (x - mean) * scale after a resize of the whole image (`lenet`: (x - 128) / 128)
+
+`trigger` = (groups, first, q) writes the backdoor trigger (`ops.nn.stamp_trigger`) on the poisoned images, in the sampled pixels: after
+the geometric operations and before every photometric one.
 """
 
 import ctypes
@@ -70,23 +73,24 @@ class Preprocessor:
     self.host_step += 1
 
   # ------------------------------------------------------------------------------------------------ #
-  def __call__(self, images, dtype, training, backend="torch", advance=True, stream_id=0):
-    """`stream_id` decorrelates callers sharing this object (logical workers): it is folded into the seed."""
+  def __call__(self, images, dtype, training, backend="torch", advance=True, stream_id=0, trigger=None):
+    """`stream_id` decorrelates callers sharing this object (logical workers): it is folded into the seed. `trigger` = (groups, first,
+    q): the backdoor trigger on the images `ops.nn.stamp_trigger` poisons (None: none)."""
     if images.dim() == 3:
       images = images[..., None]
     n, sh, sw, c = images.shape
     seed = (self.seed + 0x9E3779B1 * int(stream_id)) & _M64
     out = None
     if backend == "native" and images.is_cuda and images.dtype == torch.uint8 and c <= 3 and dtype in (torch.bfloat16, torch.float32):
-      out = self._native(images.contiguous(), dtype, training, seed)
+      out = self._native(images.contiguous(), dtype, training, seed, trigger)
     if out is None:
       step = int(self.counter(images.device).item()) if training and self.stochastic else 0
-      out = self._torch(images, dtype, training, step, seed)
+      out = self._torch(images, dtype, training, step, seed, trigger)
     if training and self.stochastic and advance:
       self.advance(images.device)
     return out
 
-  def _native(self, images, dtype, training, seed):
+  def _native(self, images, dtype, training, seed, trigger=None):
     from . import nn_native
     n, sh, sw, c = images.shape
     oh, ow = self.out_size
@@ -94,6 +98,13 @@ class Preprocessor:
     ints = (ctypes.c_int * 12)(n, sh, sw, c, oh, ow, MODES[self.mode], 1 if training else 0, 1 if dtype == torch.float32 else 0, self.resize_min, self.resize_max, self.pad)
     floats = (ctypes.c_float * 6)(self.area[0], self.area[1], self.mean[0], self.mean[1], self.mean[2], self.scale)
     counter = self.counter(images.device)
+    if trigger is not None:
+      from .nn import trigger_descriptor
+      rows, first, q, side = trigger_descriptor(out, trigger)
+      nn_native._check(nn_native._lib().agb_image_preprocess_backdoor(nn_native._ptr(images), nn_native._ptr(out), ints, floats, ctypes.c_ulonglong(seed),
+                                                                      nn_native._ptr(counter), ctypes.c_int(rows), ctypes.c_int(first), ctypes.c_int(q),
+                                                                      ctypes.c_int(side), nn_native._stream()), "image_preprocess")
+      return out.permute(0, 3, 1, 2)
     nn_native._check(nn_native._lib().agb_image_preprocess(nn_native._ptr(images), nn_native._ptr(out), ints, floats, ctypes.c_ulonglong(seed),
                                                            nn_native._ptr(counter), nn_native._stream()), "image_preprocess")
     return out.permute(0, 3, 1, 2)
@@ -146,7 +157,7 @@ class Preprocessor:
       p.update(y0=np.zeros(n, f32), x0=np.zeros(n, f32), sy=np.full(n, sh / oh, f32), sx=np.full(n, sw / ow, f32))
     return p
 
-  def _torch(self, images, dtype, training, step, seed=None):
+  def _torch(self, images, dtype, training, step, seed=None, trigger=None):
     n, sh, sw, c = images.shape
     oh, ow = self.out_size
     dev = images.device
@@ -171,6 +182,9 @@ class Preprocessor:
       return src[batch, yi.clamp(0, sh - 1)[:, :, None], xi.clamp(0, sw - 1)[:, None, :]]
 
     v = ((1 - wy) * (1 - wx)) * gather(y0, x0) + ((1 - wy) * wx) * gather(y0, x0 + 1) + (wy * (1 - wx)) * gather(y0 + 1, x0) + (wy * wx) * gather(y0 + 1, x0 + 1)  # [n, oh, ow, c]
+    if trigger is not None:
+      from .nn import stamp_trigger
+      v = stamp_trigger(v, *trigger)
     per = lambda a: t(a)[:, None, None, None]
     if self.mode == "inception":
       v = v / 255.0
