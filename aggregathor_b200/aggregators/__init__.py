@@ -26,7 +26,7 @@ class FusedSpec:
   """What the fused sm_90a aggregation kernel needs to know about a rule."""
 
   RULES = ("average", "average-nan", "median", "averaged-median", "krum", "bulyan", "trimmed-mean", "mda", "geometric-median",
-           "centered-clipping", "dnc", "smea", "fltrust")
+           "centered-clipping", "dnc", "smea", "fltrust", "foolsgold")
 
   RULES_WITH_F = ("krum", "bulyan", "trimmed-mean", "mda", "geometric-median", "centered-clipping", "dnc", "smea")   # the others ignore f
   MIXES = (None, "nnm", "arc", "arc+nnm")   # the index is the kernel's bit mask: MIX_NNM | MIX_ARC
@@ -34,10 +34,11 @@ class FusedSpec:
   # bucketing is a mix of its own (bit MIX_BUCKETING alone, never combined with NNM or ARC), complete only with its bucket size
   BUCKETING, MIX_BUCKETING = "bucketing", 4
 
-  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None, subsample=10000, c=1.0, seed=0, bucket_size=None):
+  def __init__(self, rule, n, f=0, m=0, beta=0, *, iterations=3, nu=1e-6, tau=10.0, mix=None, subsample=10000, c=1.0, seed=0, bucket_size=None,
+               confidence=1.0):
     """`iterations` and `nu` are the geometric median's Weiszfeld iterations and smoothing, `iterations` and `tau` centered
     clipping's iterations and clipping radius, `iterations`, `subsample`, `c` and `seed` DnC's iterations, sampled coordinates,
-    filtering fraction and sampling seed; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
+    filtering fraction and sampling seed, `confidence` FoolsGold's kappa; the other rules ignore them. `mix` is the pre-aggregation run on the rows before the
     rule, with the same f: None, "nnm" (nearest-neighbour mixing), "arc" (adaptive robust clipping) or "arc+nnm" (ARC, then NNM on
     the clipped rows), or "bucketing" with `bucket_size` s: then `n` is the rule's row count n' = ceil(n_rows / s), the number of
     bucket means, and the kernel gathers the n_rows rows it is given."""
@@ -52,6 +53,7 @@ class FusedSpec:
     self.mix = mix
     self.bucket_size = bucket_size if mix == self.BUCKETING else None
     self.subsample, self.c, self.seed = int(subsample), float(c), int(seed)
+    self.confidence = float(confidence)
 
   @property
   def rule_id(self):
@@ -70,7 +72,7 @@ class FusedSpec:
     """The same rule for `n` rows (every other parameter unchanged unless given)."""
     mix, bucket_size = (self.mix, self.bucket_size) if mix == () else (mix, bucket_size)
     return FusedSpec(self.rule, n, self.f if f is None else f, self.m, self.beta, iterations=self.iterations, nu=self.nu, tau=self.tau,
-                     mix=mix, subsample=self.subsample, c=self.c, seed=self.seed, bucket_size=bucket_size)
+                     mix=mix, subsample=self.subsample, c=self.c, seed=self.seed, bucket_size=bucket_size, confidence=self.confidence)
 
   def gathered_rows(self, n_rows):
     """Whether the rule's n rows are what `n_rows` gathered rows give: n_rows itself, or ceil(n_rows / s) with bucketing."""
@@ -84,7 +86,8 @@ class FusedSpec:
   def __repr__(self):
     extra = {"geometric-median": ", iterations=%d, nu=%r" % (self.iterations, self.nu),
              "centered-clipping": ", iterations=%d, tau=%r" % (self.iterations, self.tau),
-             "dnc": ", iterations=%d, subsample=%d, c=%r, seed=%d" % (self.iterations, self.subsample, self.c, self.seed)}.get(self.rule, "")
+             "dnc": ", iterations=%d, subsample=%d, c=%r, seed=%d" % (self.iterations, self.subsample, self.c, self.seed),
+             "foolsgold": ", confidence=%r" % self.confidence}.get(self.rule, "")
     if self.mix is not None:
       extra += ", mix=%r" % self.mix
     if self.bucket_size is not None:

@@ -1111,12 +1111,147 @@ def host_fltrust(G, root, sums=None, return_details=False):
   P, N, N0 = host_fltrust_sums(Gc, root) if sums is None else sums
   dtype = np.float64 if Gc.dtype == torch.float64 else np.float32
   _, _, a = fltrust_coefficients(P, N, N0, dtype)
+  out = _host_weighted_sum(Gc, a).to(G.device)
+  return (out, P, N, N0, a) if return_details else out
+
+
+def _host_weighted_sum(Gc, a):
+  """`agb_cpu_weighted_sum` of the contiguous CPU rows Gc with the weights a (Gc's type): the rows and order of `fltrust_weighted_sum`."""
+  n, d = Gc.shape
   weights = torch.from_numpy(np.ascontiguousarray(a))
   out = torch.empty(d, dtype=Gc.dtype)
   if _host("weighted_sum", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(weights), _ptr(out)) != 0:
     raise tools.UserException("Host weighted sum rejected its arguments")
-  out = out.to(G.device)
-  return (out, P, N, N0, a) if return_details else out
+  return out
+
+
+# ---------------------------------------------------------------------------- #
+# FoolsGold (Fung, Yoon & Beschastnikh, "The Limitations of Federated Learning in Sybil Settings", RAID 2020): every worker i keeps a
+# history H_i, the sum of the rows it has submitted; workers whose histories point the same way as another worker's get low weight.
+#
+# The arithmetic every back-end shares (rows g_i in worker order, histories H_i fp32 from +0):
+#   1. H_ik <- H_ik + g_ik (one fp32 add) where g_ik is finite; H_ik is unchanged where it is not, and row i is *bad* this step;
+#   2. fp32 sums P_ij = <H_i, H_j> for i <= j of the updated histories, N_i = P_ii (fold order engine-dependent);
+#   3. from those sums, in float64 with every operation rounded once (`foolsgold_coefficients`):
+#        cs_ij = P_ij / (sqrt(N_i) * sqrt(N_j)) for i != j; 0 when N_i or N_j is 0 or non-finite, or the quotient is non-finite; cs_ii = 0;
+#        v_i = max_j cs_ij (>= 0: the diagonal counts);
+#        pardoning: cs_ij <- (cs_ij * v_i) / v_j for i != j with v_j > v_i;
+#        alpha_i = clip(1 - max_j cs_ij, 0, 1);
+#        every c_i = 0 when max alpha = 0; otherwise alpha <- alpha / max alpha, 1 becomes 0.99, alpha <- kappa (ln(alpha / (1 - alpha))
+#        + 0.5) (-inf -> 0), clipped to [0, 1];
+#        alpha_i = 0 for the bad rows and the rows of non-finite N_i; S = sum alpha_i in worker order from +0;
+#        c_i = alpha_i / S rounded once to the rows' type, every c_i = 0 when S = 0;
+#   4. y = sum c_i g_i, FLTrust's weighted sum (`fltrust_weighted_sum`): from +0 in worker order, no FMA, the rows of c_i = 0 skipped.
+# Given the sums, every back-end produces the same bits (the logarithm is the platform's: CUDA's and the C library's double `log` are
+# within 1 ulp of each other, which changes an fp32 c_i only when alpha_i / S lies within that distance of an fp32 rounding boundary).
+# f is not used (any 0 <= f < n). kappa is the paper's confidence parameter.
+
+FOOLSGOLD_CONFIDENCE = 1.0   # kappa, as in the authors' code
+
+
+def check_foolsgold(n, f, confidence=FOOLSGOLD_CONFIDENCE):
+  """Validate FoolsGold's parameters -> the confidence kappa (a finite float > 0). f is not used but must satisfy 0 <= f < n."""
+  if not 0 <= f < n:
+    raise tools.UserException("FoolsGold needs 0 <= f < n (got n = %d, f = %d)" % (n, f))
+  try:
+    kappa = float(confidence) if not isinstance(confidence, bool) else float("nan")
+  except (TypeError, ValueError):
+    kappa = float("nan")
+  if not (math.isfinite(kappa) and kappa > 0):
+    raise tools.UserException("FoolsGold needs a finite confidence > 0 (got %r)" % (confidence,))
+  return kappa
+
+
+def _unit_clip(x):
+  """clip(x, 0, 1) with +0 below (x float64 array, no NaN)."""
+  return np.where(x > 0.0, np.where(x < 1.0, x, 1.0), 0.0)
+
+
+def foolsgold_coefficients(P, N, bad, kappa, dtype=np.float32):
+  """The fp32 sums P [n, n] (symmetric; N_i = P_ii is taken from N [n]) and the bad-row flags [n] -> (alpha [n] float64, S, c [n] of
+  `dtype`), as stated above (NumPy float64, one rounding per operation)."""
+  N = np.asarray(N, dtype=np.float64).reshape(-1)
+  n = len(N)
+  P = np.asarray(P, dtype=np.float64).reshape(n, n)
+  bad = np.asarray(bad).reshape(-1).astype(bool)
+  kappa = np.float64(kappa)
+  with np.errstate(all="ignore"):
+    sn = np.sqrt(N)
+    ok = np.isfinite(N) & (N != 0.0)
+    cs = P / (sn[:, None] * sn[None, :])
+    cs = np.where(ok[:, None] & ok[None, :] & np.isfinite(cs), cs, 0.0)
+    np.fill_diagonal(cs, 0.0)
+    v = cs.max(axis=1)
+    cs = np.where(v[None, :] > v[:, None], (cs * v[:, None]) / v[None, :], cs)
+    alpha = _unit_clip(1.0 - cs.max(axis=1))
+    top = alpha.max()
+    c = np.zeros(n, dtype=dtype)
+    if top == 0.0:
+      return np.zeros(n), 0.0, c
+    alpha = alpha / top
+    alpha = np.where(alpha == 1.0, 0.99, alpha)
+    alpha = _unit_clip(kappa * (np.log(alpha / (1.0 - alpha)) + 0.5))
+    alpha = np.where(bad | ~np.isfinite(N), 0.0, alpha)
+    S = _serial_sum(alpha)
+    if S != 0.0:
+      c = (alpha / S).astype(dtype)
+  return alpha, S, c
+
+
+def check_foolsgold_history(G, history):
+  """The [n, d] history of the [n, d] rows G: of G's dtype, on G's device (it is updated in place)."""
+  if history is None:
+    raise tools.UserException("FoolsGold needs the per-worker history H (history=)")
+  if tuple(history.shape) != tuple(G.shape) or history.dtype != G.dtype or history.device != G.device:
+    raise tools.UserException("FoolsGold needs a %s history of type %s on %s (got %s, %s on %s)" % (
+      tuple(G.shape), G.dtype, G.device, tuple(history.shape), history.dtype, history.device))
+  return history
+
+
+def torch_foolsgold(G, history, confidence=FOOLSGOLD_CONFIDENCE, sums=None, return_details=False):
+  """FoolsGold with the torch back-end in G's dtype: updates `history` in place, then the sums of the updated histories (or `sums`:
+  (P [n, n], N [n], bad [n]), e.g. the kernel's). `return_details` also gives (P, N, bad, c)."""
+  H = check_foolsgold_history(G, history)
+  finite = torch.isfinite(G)
+  H.copy_(torch.where(finite, H + G, H))
+  if sums is None:
+    P = torch.stack([(H * H[i]).sum(dim=1) for i in range(H.shape[0])]).detach().cpu().numpy()
+    sums = P, np.diagonal(P).copy(), (~finite.all(dim=1)).cpu().numpy()
+  P, N, bad = sums
+  dtype = np.float64 if G.dtype == torch.float64 else np.float32
+  _, _, c = foolsgold_coefficients(P, N, bad, confidence, dtype)
+  out = fltrust_weighted_sum(G, c)
+  return (out, P, N, bad, c) if return_details else out
+
+
+def host_foolsgold_sums(G, history):
+  """The history step and (P [n, n], N [n], bad [n] bool) of the [n, d] rows G with the host library (`agb_cpu_foolsgold_sums`), as
+  NumPy arrays of G's type. `history` ([n, d], G's dtype) is updated in place."""
+  Gc = G.detach().to("cpu").contiguous()
+  n, d = Gc.shape
+  H = history if (history.device.type == "cpu" and history.is_contiguous()) else history.detach().to("cpu").contiguous()
+  if tuple(H.shape) != (n, d) or H.dtype != Gc.dtype:
+    raise tools.UserException("FoolsGold needs a %s history of type %s (got %s, %s)" % ((n, d), Gc.dtype, tuple(H.shape), H.dtype))
+  out = torch.zeros(n * n + n, dtype=Gc.dtype)
+  if _host("foolsgold_sums", Gc.dtype)(_ptr(Gc), ctypes.c_size_t(n), ctypes.c_size_t(d), _ptr(H), _ptr(out)) != 0:
+    raise tools.UserException("Host FoolsGold sums rejected their arguments (n = %d, d = %d)" % (n, d))
+  if H is not history:
+    history.copy_(H)
+  out = out.numpy()
+  P = out[:n * n].reshape(n, n)
+  return P, np.diagonal(P).copy(), out[n * n:] != 0
+
+
+def host_foolsgold(G, history, confidence=FOOLSGOLD_CONFIDENCE, sums=None, return_details=False):
+  """FoolsGold with the host library: its history step and sums (`sums`, when given, replace the latter), `foolsgold_coefficients`,
+  then `agb_cpu_weighted_sum`. Returns the output on G's device; `return_details` also gives (P, N, bad, c)."""
+  Gc = G.detach().to("cpu").contiguous()
+  own = host_foolsgold_sums(Gc, history)
+  P, N, bad = own if sums is None else sums
+  dtype = np.float64 if Gc.dtype == torch.float64 else np.float32
+  _, _, c = foolsgold_coefficients(P, N, bad, confidence, dtype)
+  out = _host_weighted_sum(Gc, c).to(G.device)
+  return (out, P, N, bad, c) if return_details else out
 
 
 # ---------------------------------------------------------------------------- #

@@ -32,7 +32,8 @@
 // then a one-warp search over gamma), their trimmed-mean attack `gar_fang_trim_kernel` (one pass, a counter-based draw per row).
 // DnC (rule kDnc) has a finish kernel of its own, `gar_dnc_kernel`: a sampled distance pass, one exchange, a float64 Jacobi per CTA,
 // then Krum's phase D (see `dnc_selection`). FLTrust (rule kFltrust) too, `gar_fltrust_kernel`: a pass for the sums against the root
-// gradient, one exchange, float64 coefficients, then the weighted sum.
+// gradient, one exchange, float64 coefficients, then the weighted sum. FoolsGold (rule kFoolsgold) too, `gar_foolsgold_kernel`: a pass
+// that updates the per-worker histories and sums their products, one exchange, float64 coefficients, then FLTrust's weighted sum.
 // With R = 1 the finish kernel alone is the stand-alone `[n, d] -> [d]` aggregation op. n <= 32 workers: up to 8 rows are held in
 // registers at a time; more rows are processed in 8-row blocks (diagonal + cross passes over the staged copy).
 // Step-varying scalars (flag epoch, learning rate, optimizer hyper-parameters) may be read from device memory so that the
@@ -40,6 +41,7 @@
 // Ordering convention: finite ascending, non-finite last, ties -> lower worker index.
 
 #include <cmath>
+#include <cstring>
 
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
@@ -66,7 +68,8 @@ constexpr int kSlotDnc = kSlotCraftStats + 1;   // DnC: exchange of the sampled 
 constexpr int kSlotArc = kSlotDnc + 1;   // ARC: exchange of the squared row norms
 constexpr int kSlotMimic = kSlotArc + 1;   // mimic: second exchange of a warm-up step (the first one signals on kSlotCraftStats)
 constexpr int kSlotFltrust = kSlotMimic + 1;   // FLTrust: exchange of the sums
-constexpr int kFlagSlots = kSlotFltrust + 1;
+constexpr int kSlotFoolsgold = kSlotFltrust + 1;   // FoolsGold: exchange of the sums and bad-row flags
+constexpr int kFlagSlots = kSlotFoolsgold + 1;
 constexpr int kMailboxRegion = kMaxRanks * (kMaxPairs + 1);  // floats of one mailbox region: [0] the rule's exchanges, [1] NNM's
 // Min-Max / Min-Sum statistics of one rank: [0, kMaxPairs) honest pair distances D_jk | [kStatA, +32) A_i | [kStatB, +32) B_i | [kStatC] C.
 // They travel through mailbox region 2 (float offset kCraftRegion, kMaxRanks x kCraftStats floats), after the two regions above.
@@ -84,8 +87,14 @@ constexpr int kArcStride = kMaxWorkers + 1;   // ARC post of one rank: the n par
 constexpr int kArcRegion = kDncRegion + kMaxRanks * kDncStride;   // mailbox region 4: kMaxRanks x kArcStride floats
 constexpr int kFltrustStride = 2 * kMaxWorkers + 2;   // FLTrust post of one rank: P_i [0, 32), N_i [32, 64), N0 [64], then the loss
 constexpr int kFltrustRegion = kArcRegion + kMaxRanks * kArcStride;   // mailbox region 5: kMaxRanks x kFltrustStride floats
-constexpr int kMailboxFloats = kFltrustRegion + kMaxRanks * kFltrustStride;
+constexpr int kFoolsgoldSums = kMaxWorkers * (kMaxWorkers + 1) / 2;   // 528: FoolsGold's P_ij, i <= j (`sum_index`)
+// FoolsGold post of one rank (and CTA partials): the sums [0, n (n + 1) / 2), the bad-row flags [kFoolsgoldSums, +32), then the loss
+constexpr int kFoolsgoldStride = kFoolsgoldSums + kMaxWorkers + 1;
+constexpr int kFoolsgoldRegion = kFltrustRegion + kMaxRanks * kFltrustStride;   // mailbox region 6: kMaxRanks x kFoolsgoldStride floats
+constexpr int kMailboxFloats = kFoolsgoldRegion + kMaxRanks * kFoolsgoldStride;
 constexpr int kFltrustOut = 3 * kMaxWorkers + 1;   // FLTrust's `fltrust_out`: P [0, 32), N [32, 64), N0 [64], a [65, 97)
+// FoolsGold's `foolsgold_out`: the sums [0, n (n + 1) / 2), the bad flags [kFoolsgoldSums, +32), c [kFoolsgoldSums + 32, +32)
+constexpr int kFoolsgoldOut = kFoolsgoldSums + 2 * kMaxWorkers;
 constexpr int kMixNnm = 1, kMixArc = 2, kMixBucketing = 4;   // GarArgs::mix bits (bucketing is never combined with the others)
 constexpr unsigned long long kBucketingTag = 0x42554B54ull;   // "BUKT": third input of bucketing's key; >= 8, never a DnC iteration
 constexpr int kJacobiSweeps = 32;         // DnC: sweep budget of the cyclic Jacobi
@@ -95,7 +104,7 @@ constexpr int kBlockRows = 8;             // rows held in registers at a time
 constexpr long long kMdaMaxSets = 1 << 20; // MDA enumerates the C(n, f) removal sets
 constexpr long long kSmeaMaxSets = 1 << 14;   // SMEA runs one float64 Jacobi per removal set (`_ops.SMEA_MAX_SETS`)
 enum Rule { kAverage = 0, kAverageNan = 1, kMedian = 2, kAveragedMedian = 3, kKrum = 4, kBulyan = 5, kTrimmedMean = 6, kMda = 7, kGeoMedian = 8,
-           kCenteredClipping = 9, kDnc = 10, kSmea = 11, kFltrust = 12 };
+           kCenteredClipping = 9, kDnc = 10, kSmea = 11, kFltrust = 12, kFoolsgold = 13 };
 enum Opt { kNone = 0, kSgd = 1, kAdam = 2, kRmsprop = 3, kAdagrad = 4, kAdadelta = 5 };
 
 struct GarArgs {
@@ -153,6 +162,9 @@ struct GarArgs {
     double* smea_scratch;              // SMEA: one [m][m] slab per warp of the grid (m = n - f), the double-centred matrix of its set
     float const* root;                 // FLTrust: the root gradient r [d] (rank 0's, peer-mapped), read on the owned coordinates
     float* fltrust_out;                // FLTrust: optional [kFltrustOut] sums and coefficients, for tests
+    float* history;                    // FoolsGold: the histories H [n][owned] (local, the staged tile's layout), updated in place
+    float* foolsgold_out;              // FoolsGold: optional [kFoolsgoldOut] sums, flags and coefficients, for tests
+    double confidence;                 // FoolsGold: kappa, finite and > 0
 };
 
 // the rows `phase_a_segment` reads in DnC's sampled pass: one segment [0, b'4) of the gathered samples of one iteration, no staging
@@ -658,11 +670,50 @@ __device__ __forceinline__ float sq_dist(float4 const& u, float4 const& v) {
     return (dx * dx + dy * dy) + (dz * dz + dw * dw);
 }
 
+__device__ __forceinline__ float dot4(float4 const& u, float4 const& v) {
+    return (u.x * v.x + u.y * v.y) + (u.z * v.z + u.w * v.w);
+}
+
+// FoolsGold's history row `row` at owned float4 `v` of a segment at staged offset `soff` (the history has the staged tile's layout)
+template<class Args> __device__ __forceinline__ float4* history_at(Args const& a, int row, long long owned, long long soff, long long v) {
+    return reinterpret_cast<float4*>(a.history + row * owned + soff + (v << 2));
+}
+
+// FoolsGold's first touch of row `row` at coordinate x: load g (P2P), stage it when a tile is given, add its finite values to the
+// history (one fp32 add each), store the history back and return it; a non-finite value sets bit `row` of `bad`
+template<class Args>
+__device__ __forceinline__ float4 update_history(Args const& a, int row, long long x, long long owned, long long soff, long long v, unsigned& bad) {
+    float4 const g = ld_stream_f4(a.grad[row] + x);
+    if (a.staging)
+        *reinterpret_cast<float4*>(a.staging + row * owned + soff + (v << 2)) = g;
+    float4* const hp = history_at(a, row, owned, soff, v);
+    float4 h = *hp;
+    bool const fx = is_finite(g.x), fy = is_finite(g.y), fz = is_finite(g.z), fw = is_finite(g.w);
+    h.x = fx ? __fadd_rn(h.x, g.x) : h.x;
+    h.y = fy ? __fadd_rn(h.y, g.y) : h.y;
+    h.z = fz ? __fadd_rn(h.z, g.z) : h.z;
+    h.w = fw ? __fadd_rn(h.w, g.w) : h.w;
+    *hp = h;
+    if (!(fx && fy && fz && fw))
+        bad |= 1u << row;
+    return h;
+}
+
+// index of the sum (i <= j) in the row-major upper triangle of an n x n matrix, diagonal included
+__device__ __forceinline__ int sum_index(int i, int j, int n) {
+    return i * n - (i * (i - 1)) / 2 + (j - i);
+}
+
 // STAGED_ONLY (NNM's distances of the mixed rows): every pass, block 0's diagonal included, reads the staged tile and stores nothing.
+// PRODUCTS (FoolsGold's sums, `gar_foolsgold_kernel`): the same blocks and folds over the histories H_i (`a.history`, [n][owned] in the
+// staged tile's layout), with the products <H_i, H_j> for i <= j in place of the squared differences: a diagonal pass also has the
+// pairs i == j, indexed by `sum_index`. The first touch of a row (block 0's diagonal pass, the cross passes (0, b)) is
+// `update_history`; every later pass re-reads the updated history, which the same thread wrote (every pass maps (tid, 4) alike).
 // `Args`: GarArgs, or ByzArgs for the honest distances of Min-Max (n, grad, staging and the segments, as GarArgs names them).
-template<bool CROSS, bool STAGED_ONLY = false, class Args>
-__device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg, float* out, long long tid, long long nthreads) {
-    constexpr int B = kBlockRows, NPB = B * (B - 1) / 2;
+template<bool CROSS, bool STAGED_ONLY = false, bool PRODUCTS = false, class Args>
+__device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg, float* out, long long tid, long long nthreads,
+                                unsigned* bad = nullptr) {
+    constexpr int B = kBlockRows, NPB = PRODUCTS ? B * (B + 1) / 2 : B * (B - 1) / 2;
     int const n = a.n, nb = CROSS ? (n + B - 1) / B : 1;
     long long const lo = a.seg_lo[seg], len4 = (a.seg_hi[seg] - lo) >> 2;
     long long const owned = owned_length(a), soff = staged_offset(a, seg);
@@ -672,12 +723,12 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
         bool const from_copy = STAGED_ONLY || (a.staging != nullptr && bi > 0);   // blocks >= 1 were staged by the cross passes (0, b)
         if (threadIdx.x < NPB) {   // local pair index -> (i, j) -> global pair index
             int i = 0, rest = threadIdx.x;
-            while (rest >= B - 1 - i) {
-                rest -= B - 1 - i;
+            while (rest >= B - (PRODUCTS ? 0 : 1) - i) {
+                rest -= B - (PRODUCTS ? 0 : 1) - i;
                 ++i;
             }
-            int const j = i + 1 + rest;
-            pair_of[threadIdx.x] = i0 + j < n ? pair_index(i0 + i, i0 + j, n) : -1;
+            int const j = i + (PRODUCTS ? 0 : 1) + rest;
+            pair_of[threadIdx.x] = i0 + j < n ? (PRODUCTS ? sum_index(i0 + i, i0 + j, n) : pair_index(i0 + i, i0 + j, n)) : -1;
         }
         __syncthreads();
         {
@@ -690,12 +741,16 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
                 float4 g[B];
 #pragma unroll
                 for (int i = 0; i < B; ++i) {
-                    if (i0 + i < n)
-                        g[i] = from_copy ? *reinterpret_cast<float4 const*>(staged(i0 + i, v)) : ld_stream_f4(a.grad[i0 + i] + x);
-                    else
+                    if (i0 + i < n) {
+                        if constexpr (PRODUCTS)
+                            g[i] = bi > 0 ? *history_at(a, i0 + i, owned, soff, v) : update_history(a, i0 + i, x, owned, soff, v, *bad);
+                        else
+                            g[i] = from_copy ? *reinterpret_cast<float4 const*>(staged(i0 + i, v)) : ld_stream_f4(a.grad[i0 + i] + x);
+                    } else {
                         g[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
                 }
-                if (a.staging && !from_copy) {
+                if (!PRODUCTS && a.staging && !from_copy) {
 #pragma unroll
                     for (int i = 0; i < B; ++i)
                         if (i0 + i < n)
@@ -703,11 +758,11 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
                 }
                 int p = 0;
 #pragma unroll
-                for (int i = 0; i < B - 1; ++i) {
+                for (int i = 0; i < B - (PRODUCTS ? 0 : 1); ++i) {
 #pragma unroll
-                    for (int j = i + 1; j < B; ++j, ++p)
+                    for (int j = i + (PRODUCTS ? 0 : 1); j < B; ++j, ++p)
                         if (i0 + j < n)
-                            acc[p] += sq_dist(g[i], g[j]);
+                            acc[p] += PRODUCTS ? dot4(g[i], g[j]) : sq_dist(g[i], g[j]);
                 }
             }
             fold_pass<NPB>(sh, acc, out, pair_of);
@@ -718,7 +773,7 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
                 bool const j_from_copy = STAGED_ONLY || (a.staging != nullptr && bi > 0);   // first touch of block bj is the pass (0, bj)
                 if (threadIdx.x < B * B) {
                     int const i = threadIdx.x / B, j = threadIdx.x % B;
-                    pair_of[threadIdx.x] = (i0 + i < n && j0 + j < n) ? pair_index(i0 + i, j0 + j, n) : -1;
+                    pair_of[threadIdx.x] = (i0 + i < n && j0 + j < n) ? (PRODUCTS ? sum_index(i0 + i, j0 + j, n) : pair_index(i0 + i, j0 + j, n)) : -1;
                 }
                 __syncthreads();
                 float acc[B * B];
@@ -730,15 +785,21 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
                     float4 gi[B], gj[B];
 #pragma unroll
                     for (int i = 0; i < B; ++i) {
-                        if (i0 + i < n)
-                            gi[i] = a.staging ? *reinterpret_cast<float4 const*>(staged(i0 + i, v)) : ld_stream_f4(a.grad[i0 + i] + x);
-                        else
+                        if (i0 + i < n) {
+                            if constexpr (PRODUCTS)
+                                gi[i] = *history_at(a, i0 + i, owned, soff, v);
+                            else
+                                gi[i] = a.staging ? *reinterpret_cast<float4 const*>(staged(i0 + i, v)) : ld_stream_f4(a.grad[i0 + i] + x);
+                        } else {
                             gi[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        }
                     }
 #pragma unroll
                     for (int j = 0; j < B; ++j) {
                         if (j0 + j < n) {
-                            if (j_from_copy) {
+                            if constexpr (PRODUCTS) {
+                                gj[j] = bi > 0 ? *history_at(a, j0 + j, owned, soff, v) : update_history(a, j0 + j, x, owned, soff, v, *bad);
+                            } else if (j_from_copy) {
                                 gj[j] = *reinterpret_cast<float4 const*>(staged(j0 + j, v));
                             } else {
                                 gj[j] = ld_stream_f4(a.grad[j0 + j] + x);
@@ -753,7 +814,7 @@ __device__ void phase_a_segment(Args const& a, Shared& sh, int* pair_of, int seg
                     for (int i = 0; i < B; ++i) {
 #pragma unroll
                         for (int j = 0; j < B; ++j)
-                            acc[i * B + j] += sq_dist(gi[i], gj[j]);
+                            acc[i * B + j] += PRODUCTS ? dot4(gi[i], gj[j]) : sq_dist(gi[i], gj[j]);
                     }
                 }
                 fold_pass<B * B>(sh, acc, out, pair_of);
@@ -2282,6 +2343,72 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_dnc_kernel(GarArgs 
         *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
 }
 
+// Phase D of FLTrust and FoolsGold: y = sum coef_i x_i from +0 in worker order (__fmul_rn / __fadd_rn: no FMA), the rows outside
+// `mask` (coef_i = 0) skipped, then the optimizer and the parameter broadcast; the rows come from the staged tile, or from the rows
+// themselves when R = 1 and n <= 8. Exit barrier as for DnC (the loss went through the kernel's exchange). `coef`: shared memory.
+template<int N, int VEC>
+__device__ __forceinline__ void weighted_phase_d(GarArgs const& a, cg::grid_group& grid, float const (&hyper)[4], float const* coef,
+                                                 unsigned const mask, uint32_t const epoch, long long const tid, long long const nthreads) {
+    int const n = a.n;
+    bool const multi = a.R > 1;
+    long long const owned = owned_length(a);
+    for (int seg = 0; seg < a.nseg; ++seg) {
+        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
+        for (long long v = tid; v < lenv; v += nthreads) {
+            long long const x = lo + v * VEC;
+            auto load_row = [&](int i, float (&dst)[VEC]) {
+                if (a.staging)
+                    V<VEC>::load(a.staging + i * owned + soff + v * VEC, dst);
+                else
+                    V<VEC>::load_stream(a.grad[i] + x, dst);
+            };
+            float y[VEC];
+#pragma unroll
+            for (int c = 0; c < VEC; ++c)
+                y[c] = 0.f;
+            if (N <= 16) {   // every weighted row in flight at once, added in ascending worker order
+                float g[N][VEC];
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u)
+                        load_row(i, g[i]);
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    if ((mask >> i) & 1u) {
+                        float const ai = coef[i];
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[i][c]));
+                    }
+            } else {
+                for (int i = 0; i < n; ++i) {
+                    if ((mask >> i) & 1u) {
+                        float g[VEC];
+                        load_row(i, g);
+                        float const ai = coef[i];
+#pragma unroll
+                        for (int c = 0; c < VEC; ++c)
+                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[c]));
+                    }
+                }
+            }
+            apply_update<VEC>(a, hyper, x, y);
+        }
+    }
+    if (multi) {   // exit barrier, as in `gar_dnc_kernel` (the loss went through the exchange)
+        fence_sys();
+        grid.sync();
+        if (blockIdx.x == 0) {
+            __syncthreads();
+            signal_all(a, kSlotExit, epoch);
+            wait_all(a, kSlotExit, epoch);
+            __syncthreads();
+        }
+    }
+    if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
+        *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
+}
+
 // ---- the FLTrust finish kernel (Cao, Fang, Liu & Gong, NDSS 2021) ---------------------------------------------------- //
 // Rows x_i, root gradient r (rank 0's row, read over P2P on the owned coordinates). The arithmetic is `_ops.fltrust_coefficients`:
 //   1. sums pass over the owned segments, with the rules' (tid, VEC) mapping: the n rows and r are loaded (8 rows in flight at a time,
@@ -2461,62 +2588,196 @@ __global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_fltrust_kernel(GarA
     }
     __syncthreads();
     // -------- 4. phase D: weighted sum, update, broadcast -------- //
-    unsigned const mask = sh.mask;
-    for (int seg = 0; seg < a.nseg; ++seg) {
-        long long const lo = a.seg_lo[seg], lenv = (a.seg_hi[seg] - lo) / VEC, soff = staged_offset(a, seg);
-        for (long long v = tid; v < lenv; v += nthreads) {
-            long long const x = lo + v * VEC;
-            auto load_row = [&](int i, float (&dst)[VEC]) {
-                if (a.staging)
-                    V<VEC>::load(a.staging + i * owned + soff + v * VEC, dst);
-                else
-                    V<VEC>::load_stream(a.grad[i] + x, dst);
-            };
-            float y[VEC];
-#pragma unroll
-            for (int c = 0; c < VEC; ++c)
-                y[c] = 0.f;
-            if (N <= 16) {   // every weighted row in flight at once, added in ascending worker order
-                float g[N][VEC];
-#pragma unroll
-                for (int i = 0; i < N; ++i)
-                    if ((mask >> i) & 1u)
-                        load_row(i, g[i]);
-#pragma unroll
-                for (int i = 0; i < N; ++i)
-                    if ((mask >> i) & 1u) {
-                        float const ai = sh.coef[i];
-#pragma unroll
-                        for (int c = 0; c < VEC; ++c)
-                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[i][c]));
-                    }
-            } else {
-                for (int i = 0; i < n; ++i) {
-                    if ((mask >> i) & 1u) {
-                        float g[VEC];
-                        load_row(i, g);
-                        float const ai = sh.coef[i];
-#pragma unroll
-                        for (int c = 0; c < VEC; ++c)
-                            y[c] = __fadd_rn(y[c], __fmul_rn(ai, g[c]));
-                    }
+    weighted_phase_d<N, VEC>(a, grid, hyper, sh.coef, sh.mask, epoch, tid, nthreads);
+}
+
+// ---- the FoolsGold finish kernel (Fung, Yoon & Beschastnikh, RAID 2020) ------------------------------------------------- //
+// Rows g_i, histories H_i (`a.history`: [n][owned], local, the staged tile's layout; they persist across steps and graph replays).
+// The arithmetic is `_ops.foolsgold_coefficients`:
+//   1. history pass over the owned segments: `phase_a_segment<.., PRODUCTS>`, Krum's 8-row blocks and folds with products in place of
+//      squared differences. The first touch of a row loads g_i (P2P), stages it when the tile is given (R > 1 or n > 8, so that phase D
+//      never crosses NVLink again), adds its finite values to H_i and stores H_i back; the n (n + 1) / 2 sums P_ij = <H_i, H_j>, i <= j,
+//      of the updated histories land in the CTA's slot of `cta_partials` (kFoolsgoldStride floats), then the CTA's bad-row flags;
+//   2. one exchange of the sums, the flags and the loss: grid barrier; block 0 folds the CTAs in order and posts the rank's values into
+//      mailbox region 6 of every rank, then signals slot kSlotFoolsgold. Every CTA of every rank adds the R posts in rank order, so the
+//      sums are bit-identical everywhere. Region 6 and slot kSlotFoolsgold belong to this exchange alone (FoolsGold runs no
+//      pre-aggregation and no other exchange); every CTA reads region 6 before the exit barrier, and the next write into it comes from
+//      the next step's exchange, which a rank reaches only after every rank's exit barrier;
+//   3. the coefficients on warp 0 of every CTA (one lane per row, cs_ij recomputed from the sums where needed), in float64 with
+//      explicit _rn intrinsics (the logarithm is CUDA's `log`, within 1 ulp):
+//        cs_ij = P_ij / (sqrt(N_i) sqrt(N_j)), 0 for i == j, N_i or N_j zero or non-finite, or a non-finite quotient; v_i = max_j cs_ij;
+//        pardoned (cs_ij v_i) / v_j when v_j > v_i; alpha_i = clip(1 - max_j cs_ij, 0, 1); all zero when max alpha = 0, otherwise
+//        alpha / max alpha, 1 -> 0.99, clip(kappa (ln(alpha / (1 - alpha)) + 0.5), 0, 1); 0 for bad rows and non-finite N_i;
+//        S = sum alpha_i in worker order; c_i = fp32(alpha_i / S), every c_i = 0 when S = 0;
+//   4. FLTrust's phase D (`weighted_phase_d`): y = sum c_i g_i, the optimizer, the parameter broadcast, the exit barrier.
+struct FoolsgoldShared {
+    float coef[kMaxWorkers];   // c_i
+    unsigned mask;             // rows with c_i != 0
+    unsigned bad;              // the CTA's bad rows, then the step's
+};
+
+// cs_ij from the exchanged sums (float64, one rounding per operation)
+__device__ __forceinline__ double foolsgold_cos(float pij, float ni, float nj) {
+    if (!(is_finite(ni) && ni != 0.f && is_finite(nj) && nj != 0.f))
+        return 0.0;
+    double const q = __ddiv_rn(static_cast<double>(pij), __dmul_rn(__dsqrt_rn(static_cast<double>(ni)), __dsqrt_rn(static_cast<double>(nj))));
+    return isfinite(q) ? q : 0.0;
+}
+
+// clip(x, 0, 1), +0 below
+__device__ __forceinline__ double unit_clip(double x) {
+    return x > 0.0 ? (x < 1.0 ? x : 1.0) : 0.0;
+}
+
+template<int N, int VEC>
+__global__ void __launch_bounds__(N <= 8 ? 512 : 256, 1) gar_foolsgold_kernel(GarArgs const a) {
+    __shared__ Shared sh;
+    __shared__ int pair_of[kBlockRows * kBlockRows];
+    __shared__ FoolsgoldShared fs;
+    cg::grid_group grid = cg::this_grid();
+    int const n = a.n, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nsums = n * (n + 1) / 2;
+    long long const tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    bool const multi = a.R > 1;
+    if (threadIdx.x == 0) {
+        sh.epoch = current_epoch(a);
+        for (int i = 0; i < 4; ++i)
+            sh.hyper[i] = a.hyper_ptr ? a.hyper_ptr[i] : (i == 0 ? a.lr : i == 1 ? a.h0 : i == 2 ? a.h1 : a.h2);
+        fs.bad = 0u;
+    }
+    float* const mine = a.cta_partials + static_cast<long long>(blockIdx.x) * kFoolsgoldStride;
+    for (int p = threadIdx.x; p < nsums; p += blockDim.x)
+        mine[p] = 0.f;
+    __syncthreads();
+    uint32_t const epoch = sh.epoch;
+    float const hyper[4] = {sh.hyper[0], sh.hyper[1], sh.hyper[2], sh.hyper[3]};
+    if (multi) {   // entry barrier: every rank's gradients are published (nothing is pre-accumulated)
+        if (blockIdx.x == 0)
+            signal_all(a, 0, epoch);
+        wait_all(a, 0, epoch);
+        __syncthreads();
+    }
+    float local_loss = 0.f;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.loss_in)
+        for (int j = 0; j < a.nloss; ++j)
+            local_loss += a.loss_in[j];
+    // -------- 1. history pass: H_i += g_i, the sums of the updated histories, the bad rows -------- //
+    unsigned bad = 0u;
+    for (int seg = 0; seg < a.nseg; ++seg)
+        phase_a_segment<(N > kBlockRows), false, true>(a, sh, pair_of, seg, mine, tid, nthreads, &bad);
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    if (lane == 0 && bad)
+        atomicOr(&fs.bad, bad);
+    __syncthreads();
+    if (threadIdx.x < n)
+        mine[kFoolsgoldSums + threadIdx.x] = ((fs.bad >> threadIdx.x) & 1u) ? 1.f : 0.f;
+    // -------- 2. exchange of the sums, the flags and the loss -------- //
+    __threadfence();
+    grid.sync();
+    if (blockIdx.x == 0) {
+        for (int k = threadIdx.x; k < nsums + n; k += blockDim.x) {
+            int const at = k < nsums ? k : kFoolsgoldSums + (k - nsums);
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b)
+                s += ld_volatile_f(a.cta_partials + static_cast<long long>(b) * kFoolsgoldStride + at);
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kFoolsgoldRegion + a.rank * kFoolsgoldStride + at] = s;
+        }
+        if (threadIdx.x == 0)
+            for (int q = 0; q < a.R; ++q)
+                a.mailbox[q][kFoolsgoldRegion + a.rank * kFoolsgoldStride + kFoolsgoldStride - 1] = local_loss;
+        fence_sys();
+        __syncthreads();
+        if (multi)
+            signal_all(a, kSlotFoolsgold, epoch);
+    }
+    if (multi) {
+        wait_all(a, kSlotFoolsgold, epoch);
+        __syncthreads();
+    } else {
+        grid.sync();
+    }
+    // -------- 3. the sums of every rank in rank order -> sh.dist (P, symmetric); coefficients on warp 0 -------- //
+    float const* const box = a.mailbox[a.rank] + kFoolsgoldRegion;
+    for (int p = threadIdx.x; p < nsums; p += blockDim.x) {
+        int i = 0, rest = p;
+        while (rest >= n - i) {   // sum index -> (i, j), i <= j
+            rest -= n - i;
+            ++i;
+        }
+        int const j = i + rest;
+        float s = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            s += ld_volatile_f(box + q * kFoolsgoldStride + p);
+        sh.dist[i][j] = s;
+        sh.dist[j][i] = s;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        bool const row = lane < n;
+        float flags = 0.f;
+        for (int q = 0; q < a.R; ++q)
+            flags += row ? ld_volatile_f(box + q * kFoolsgoldStride + kFoolsgoldSums + lane) : 0.f;
+        float const ni = row ? sh.dist[lane][lane] : 0.f;
+        double v = 0.0;   // v_i = max_j cs_ij, the diagonal's 0 included
+        for (int j = 0; j < n; ++j)
+            if (row && j != lane)
+                v = fmax(v, foolsgold_cos(sh.dist[lane][j], ni, sh.dist[j][j]));
+        double top_cs = 0.0;   // max_j of the pardoned cs_ij
+        for (int j = 0; j < n; ++j) {
+            double const vj = __shfl_sync(0xffffffffu, v, j);
+            if (row && j != lane) {
+                double cs = foolsgold_cos(sh.dist[lane][j], ni, sh.dist[j][j]);
+                if (vj > v)
+                    cs = __ddiv_rn(__dmul_rn(cs, v), vj);
+                top_cs = fmax(top_cs, cs);
+            }
+        }
+        double alpha = row ? unit_clip(__dsub_rn(1.0, top_cs)) : 0.0;
+        double top = alpha;
+        for (int o = 16; o > 0; o >>= 1)
+            top = fmax(top, __shfl_xor_sync(0xffffffffu, top, o));
+        float c = 0.f;
+        if (top != 0.0) {
+            alpha = __ddiv_rn(alpha, top);
+            if (alpha == 1.0)
+                alpha = 0.99;
+            alpha = unit_clip(__dmul_rn(a.confidence, __dadd_rn(log(__ddiv_rn(alpha, __dsub_rn(1.0, alpha))), 0.5)));
+            if (!row || flags != 0.f || !is_finite(ni))
+                alpha = 0.0;
+            double S = 0.0;
+            for (int j = 0; j < n; ++j)
+                S = __dadd_rn(S, __shfl_sync(0xffffffffu, alpha, j));
+            c = S != 0.0 ? __double2float_rn(__ddiv_rn(alpha, S)) : 0.f;
+        }
+        fs.coef[lane] = c;
+        unsigned const mask = __ballot_sync(0xffffffffu, c != 0.f);
+        if (lane == 0)
+            fs.mask = mask;
+        if (blockIdx.x == 0) {
+            if (a.foolsgold_out) {
+                for (int p = lane; p < nsums; p += 32) {
+                    float s = 0.f;
+                    for (int q = 0; q < a.R; ++q)
+                        s += ld_volatile_f(box + q * kFoolsgoldStride + p);
+                    a.foolsgold_out[p] = s;
+                }
+                if (row) {
+                    a.foolsgold_out[kFoolsgoldSums + lane] = flags != 0.f ? 1.f : 0.f;
+                    a.foolsgold_out[kFoolsgoldSums + kMaxWorkers + lane] = c;
                 }
             }
-            apply_update<VEC>(a, hyper, x, y);
+            if (lane == 0 && a.loss_out) {
+                float total = 0.f;
+                for (int q = 0; q < a.R; ++q)
+                    total += ld_volatile_f(box + q * kFoolsgoldStride + kFoolsgoldStride - 1);
+                *a.loss_out = total;
+            }
         }
     }
-    if (multi) {   // exit barrier, as in `gar_dnc_kernel` (the loss went through the exchange)
-        fence_sys();
-        grid.sync();
-        if (blockIdx.x == 0) {
-            __syncthreads();
-            signal_all(a, kSlotExit, epoch);
-            wait_all(a, kSlotExit, epoch);
-            __syncthreads();
-        }
-    }
-    if (a.epoch_ptr && blockIdx.x == 0 && threadIdx.x == 0)
-        *a.epoch_ptr = epoch;   // this step is complete (every CTA read the counter before the barriers above)
+    __syncthreads();
+    // -------- 4. phase D: weighted sum, update, broadcast -------- //
+    weighted_phase_d<N, VEC>(a, grid, hyper, fs.coef, fs.mask, epoch, tid, nthreads);
 }
 
 // ---- omniscient Byzantine rows (ALIE / IPM) ------------------------------------------ //
@@ -3639,7 +3900,8 @@ __global__ void cast_bf16_kernel(float const* __restrict__ src, __nv_bfloat16* _
 template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_floats, cudaStream_t stream) {
     int const threads = N <= 8 ? 512 : 256;
     int device = 0, sms = 0, per_sm = 0;
-    auto const kernel = a.rule == kDnc ? gar_dnc_kernel<N, VEC> : a.rule == kFltrust ? gar_fltrust_kernel<N, VEC> : gar_fused_kernel<N, VEC>;
+    auto const kernel = a.rule == kDnc ? gar_dnc_kernel<N, VEC> : a.rule == kFltrust ? gar_fltrust_kernel<N, VEC>
+                      : a.rule == kFoolsgold ? gar_foolsgold_kernel<N, VEC> : gar_fused_kernel<N, VEC>;
     AGB_CUDA_OK(cudaGetDevice(&device));
     AGB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0));
@@ -3654,6 +3916,10 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
         grid = max_ctas;
     if (want < grid)
         grid = want < 1 ? 1 : static_cast<int>(want);
+    if (a.rule == kFoolsgold) {   // CTA slots of kFoolsgoldStride floats in `cta_partials` ([agb_gar_max_ctas()][kMaxPairs] floats)
+        int const slots = static_cast<int>(static_cast<long long>(sms) * 4 * kMaxPairs / kFoolsgoldStride);
+        grid = grid < slots ? grid : slots;
+    }
     if (a.rule == kDnc) {   // CTA partials of this grid, then the samples
         long long const b = a.dnc_b < a.dnc_domain ? a.dnc_b : a.dnc_domain;
         if (static_cast<long long>(grid) * kDncIterations * kMaxPairs + a.iterations * a.n * ((b + 3) & ~3ll) > scratch_floats)
@@ -3673,10 +3939,11 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
 //   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
 //   [115] arc_out (ARC: [2n] squared norms, then factors) | [116] SMEA scratch (doubles)
 //   [113] is also bucketing's step key | [117] FLTrust root r (rank 0's) | [118] FLTrust's fltrust_out
+//   [119] FoolsGold's history [n][owned] | [120] FoolsGold's foolsgold_out
 // ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
 //       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC, 4 bucketing) | [27] DnC r | [28] bucketing: s | [29] gathered rows n_rows (0: n)
 // longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step (also bucketing's)
-//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles) | [22] bucketing: seed
+//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles) | [22] bucketing: seed | [23] FoolsGold: kappa (float64 bits)
 // floats: lr h0 h1 h2 nu tau
 int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
     a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
@@ -3712,12 +3979,22 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
     }
-    if (a.rule < 0 || a.rule > kFltrust)
+    if (a.rule < 0 || a.rule > kFoolsgold)
         return 102;
     // FLTrust: any 0 <= f < n, a root, no pre-aggregation (it would change the rows whose direction and norm FLTrust scores), nothing
     // pre-accumulated
     if (a.rule == kFltrust && (a.f < 0 || a.f >= a.n || !ptrs[117] || a.mix != 0 || a.first_seg != 0))
         return 126;
+    // FoolsGold: any 0 <= f < n, a finite kappa > 0, a history (127); no pre-aggregation (128: NNM mixes, ARC rescales and bucketing
+    // reshuffles the rows every step, so a row would no longer be one worker's); nothing pre-accumulated (129: the history pass runs
+    // in the finish kernel)
+    std::memcpy(&a.confidence, &longs[23], sizeof(double));
+    if (a.rule == kFoolsgold && (a.f < 0 || a.f >= a.n || !ptrs[119] || !std::isfinite(a.confidence) || !(a.confidence > 0.0)))
+        return 127;
+    if (a.rule == kFoolsgold && a.mix != 0)
+        return 128;
+    if (a.rule == kFoolsgold && a.first_seg != 0)
+        return 129;
     if (a.mix < 0 || a.mix > (kMixNnm | kMixArc | kMixBucketing))
         return 117;
     if ((a.mix & kMixBucketing) && (a.mix != kMixBucketing || a.bkt_size < 1 || a.bkt_size > a.n_rows ||
@@ -3781,6 +4058,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     a.arc_out = reinterpret_cast<float*>(ptrs[115]);
     a.root = reinterpret_cast<float const*>(ptrs[117]);
     a.fltrust_out = reinterpret_cast<float*>(ptrs[118]);
+    a.history = reinterpret_cast<float*>(ptrs[119]);
+    a.foolsgold_out = reinterpret_cast<float*>(ptrs[120]);
     for (int q = 0; q < a.R; ++q) {
         a.param_dst[q] = reinterpret_cast<float*>(ptrs[48 + q]);
         a.signal[q] = reinterpret_cast<uint32_t*>(ptrs[64 + q]);
@@ -3800,6 +4079,8 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 108;
     if (a.rule == kFltrust && (!a.cta_partials || !a.mailbox[0] || ((a.R > 1 || a.n > kBlockRows) && !a.staging)))
         return 108;   // FLTrust's second pass reads the staged rows over several ranks or beyond the 8 rows of one block
+    if (a.rule == kFoolsgold && (!a.cta_partials || !a.mailbox[0] || ((a.R > 1 || a.n > kBlockRows) && !a.staging)))
+        return 108;   // as FLTrust's: phase D reads the staged rows
     if ((a.rule == kGeoMedian || a.rule == kCenteredClipping) && a.R > 1 && !a.staging)
         return 108;   // the passes after the first re-read the staged copy instead of the peers' rows
     if (a.first_seg > 0 && !a.seg_partials)
@@ -3877,6 +4158,8 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     if (status)
         return status;
     int const ctas = ints[15];
+    if (a.rule == kFoolsgold)
+        return 129;
     if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda && a.rule != kSmea) ||
         a.mix)
         return 111;

@@ -832,6 +832,51 @@ template<class T> int fltrust_sums(T const* g, size_t n, size_t d, T const* root
     return 0;
 }
 
+// FoolsGold's history step and sums (`aggregators/_ops.py`), one pass over the coordinates: every chunk first adds the finite values of
+// the rows g_i to the histories H_i (in place), then accumulates the partial products <H_i, H_j>, i <= j, of its updated coordinates.
+// out = [P (n x n, computed for i <= j and mirrored), the n bad flags (1: g_i holds a non-finite value)], the per-chunk partials folded
+// in chunk order. The coefficients and the weighted sum are computed by the callers.
+template<class T> int foolsgold_sums(T const* g, size_t n, size_t d, T* H, T* out) {
+    if (n == 0 || n > kMaxWorkers)
+        return 1;
+    size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
+    size_t const pairs = n * (n + 1) / 2, width = pairs + n;
+    std::vector<T> partial(chunks * width, T(0));
+    global_pool().run(0, d, kGrainCoord, [&](size_t chunk, size_t b, size_t e) {
+        T* part = partial.data() + chunk * width;
+        for (size_t i = 0; i < n; ++i) {
+            T const* gi = g + i * d;
+            T* hi = H + i * d;
+            bool bad = false;
+            for (size_t k = b; k < e; ++k) {
+                if (std::isfinite(gi[k]))
+                    hi[k] += gi[k];
+                else
+                    bad = true;
+            }
+            part[pairs + i] = bad ? T(1) : T(0);
+        }
+        for (size_t i = 0, p = 0; i < n; ++i)
+            for (size_t j = i; j < n; ++j, ++p)
+                part[p] = dot(H + i * d, H + j * d, b, e);
+    });
+    for (size_t i = 0, p = 0; i < n; ++i)
+        for (size_t j = i; j < n; ++j, ++p) {
+            T sum = 0;
+            for (size_t c = 0; c < chunks; ++c)
+                sum += partial[c * width + p];
+            out[i * n + j] = sum;
+            out[j * n + i] = sum;
+        }
+    for (size_t i = 0; i < n; ++i) {
+        T flag = 0;
+        for (size_t c = 0; c < chunks; ++c)
+            flag = partial[c * width + pairs + i] != T(0) ? T(1) : flag;
+        out[n * n + i] = flag;
+    }
+    return 0;
+}
+
 template<class T> T squared_distance(T const* a, T const* b, size_t d) {
     size_t const chunks = ThreadPool::chunk_count(0, d, kGrainCoord);
     std::vector<T> partial(chunks, T(0));
@@ -890,6 +935,7 @@ extern "C" uint32_t agb_crc32c(uint8_t const* data, size_t size, uint32_t crc) {
     extern "C" int agb_cpu_dnc_sample_distances_##S(T const* g, size_t n, size_t d, size_t iterations, size_t b, uint64_t seed, uint64_t step, size_t domain, T* dist) { return dnc_sample_distances<T>(g, n, d, iterations, b, seed, step, domain, dist); } \
     extern "C" int agb_cpu_selection_mean_##S(T const* g, size_t n, size_t d, int64_t const* selected, size_t count, T* out) { return selection_mean_of<T>(g, n, d, selected, count, out); } \
     extern "C" int agb_cpu_fltrust_sums_##S(T const* g, size_t n, size_t d, T const* root, T* out) { return fltrust_sums<T>(g, n, d, root, out); } \
+    extern "C" int agb_cpu_foolsgold_sums_##S(T const* g, size_t n, size_t d, T* history, T* out) { return foolsgold_sums<T>(g, n, d, history, out); } \
     extern "C" T agb_cpu_squared_distance_##S(T const* a, T const* b, size_t d) { return squared_distance<T>(a, b, d); }
 
 AGB_EXPORT(float, float)

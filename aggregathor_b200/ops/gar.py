@@ -8,6 +8,7 @@ the reference, which only ever had a CPU kernel: `native/op_krum/op.cpp:98-107`)
 
 import ctypes
 import os
+import struct
 
 import torch
 
@@ -21,8 +22,8 @@ MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
 # per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
-# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange; FLTrust's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 6
+# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange; FLTrust's exchange; FoolsGold's exchange
+FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 7
 SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 # Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]; mimic posts into the
 # same region: s_i [0, 32) in its first exchange, q_i [32, 64) and ||y||^2 [64] in its second
@@ -36,13 +37,18 @@ DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
 ARC_STATS = MAX_WORKERS + 1
 # FLTrust's post of one rank: P_i [0, 32), N_i [32, 64), N0 [64], then the loss
 FLTRUST_STATS = 2 * MAX_WORKERS + 2
-# six regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms,
-# FLTrust's sums
+# FoolsGold's post of one rank: the sums P_ij, i <= j, row-major upper triangle [0, n (n + 1) / 2), the bad-row flags [528, 560), the loss
+FOOLSGOLD_SUMS = MAX_WORKERS * (MAX_WORKERS + 1) // 2
+FOOLSGOLD_STATS = FOOLSGOLD_SUMS + MAX_WORKERS + 1
+# seven regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms,
+# FLTrust's sums, FoolsGold's sums
 MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS
-                 + MAX_RANKS * FLTRUST_STATS) * 4
+                 + MAX_RANKS * FLTRUST_STATS + MAX_RANKS * FOOLSGOLD_STATS) * 4
 # FLTrust's sums and coefficients of the last launch: P [0, 32), N [32, 64), N0 [64], a [65, 97)
 FLTRUST_OUT = 3 * MAX_WORKERS + 1
-PTRS = 119
+# FoolsGold's of the last launch: the sums [0, n (n + 1) / 2), the bad-row flags [528, 560), c [560, 592)
+FOOLSGOLD_OUT = FOOLSGOLD_SUMS + 2 * MAX_WORKERS
+PTRS = 121
 # [0]: theta, [1, 1 + theta): selection masks; [32, 34): SMEA's winning score (float64 bits); [64, 64 + n): NNM masks;
 # [96, 96 + T): DnC's mask of every iteration; bucketing: [128, 128 + n_rows) the permutation, [160, 160 + n') the bucket masks
 INFO_INTS = 192
@@ -65,7 +71,10 @@ _ERRORS = {
   124: "invalid mimic parameters (H >= 2, 0 <= t < 2^24, a target buffer, and z and y buffers for a warm-up step)",
   125: "invalid Fang attack parameters (fang-krum: every row honest or Byzantine, n - f - 2 >= 1, n - 2 K - 1 >= 1, H >= 2, a finite "
        "threshold > 0; fang-trim: a finite scale > 1)",
-  126: "invalid FLTrust parameters (0 <= f < n, a root gradient, no pre-aggregation, nothing pre-accumulated)"}
+  126: "invalid FLTrust parameters (0 <= f < n, a root gradient, no pre-aggregation, nothing pre-accumulated)",
+  127: "invalid FoolsGold parameters (0 <= f < n, a finite confidence > 0, a history buffer)",
+  128: "FoolsGold takes no pre-aggregation (NNM, ARC and bucketing do not keep one row per worker)",
+  129: "FoolsGold runs its history pass in the finish kernel: no bucketed phase A, nothing pre-accumulated"}
 ITERATIVE_RULES = ("geometric-median", "centered-clipping")   # [iterations, n] row distances in `geo_dist_out`
 BYZANTINE_MODES = {"alie": 0, "ipm": 1, "min-max": 2, "min-sum": 3, "mimic": 4, "fang-krum": 5, "fang-trim": 6}
 FANG_OUT = 3   # fang-krum's float64 details of the last run: gamma_max, t, selected
@@ -124,10 +133,11 @@ class FusedLauncher:
     self.mimic_stats = torch.zeros(MIMIC_STATS, dtype=torch.float64, device=self.device)
     self.fang_out = torch.zeros(FANG_OUT, dtype=torch.float64, device=self.device)   # fang-krum: gamma_max, t, selected
     self.fltrust_out = torch.zeros(FLTRUST_OUT, dtype=torch.float32, device=self.device)   # FLTrust: P, N, N0, a
+    self.foolsgold_out = torch.zeros(FOOLSGOLD_OUT, dtype=torch.float32, device=self.device)   # FoolsGold: P, bad, c
     self._mimic_y = None
     self._ptrs = (ctypes.c_ulonglong * PTRS)()
     self._ints = (ctypes.c_int * 32)()
-    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 6))()
+    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 7))()
     self._floats = (ctypes.c_float * 6)()
     self._func = _lib().agb_gar_fused
     self._func.restype = ctypes.c_int
@@ -141,7 +151,7 @@ class FusedLauncher:
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
             param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
             first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None,
-            bucketing_seed=0, root=None):
+            bucketing_seed=0, root=None, history=None):
     ptrs = self._ptrs
     for i in range(PTRS):
       ptrs[i] = 0
@@ -168,6 +178,7 @@ class FusedLauncher:
     ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch) if spec.rule == "dnc" else 0, self.arc_out.data_ptr()
     ptrs[116] = addr(scratch) if spec.rule == "smea" else 0
     ptrs[117], ptrs[118] = addr(root), self.fltrust_out.data_ptr()   # FLTrust: the root row (rank 0's, raw address or tensor)
+    ptrs[119], ptrs[120] = addr(history), self.foolsgold_out.data_ptr()   # FoolsGold: the [n, owned] histories (local)
     for q in range(R):
       ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
       ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
@@ -191,6 +202,7 @@ class FusedLauncher:
     signed = lambda seed: seed - (1 << 64) if seed >= 1 << 63 else seed
     longs[17], longs[18], longs[19], longs[20] = spec.subsample, domain, signed(spec.seed), step
     longs[21], longs[22] = scratch.numel() if scratch is not None else 0, signed(int(bucketing_seed))
+    longs[23] = struct.unpack("<q", struct.pack("<d", spec.confidence))[0]   # FoolsGold's kappa, float64 bits
 
   def dnc_scratch(self, spec, domain):
     """DnC's scratch for rule `spec` over `domain` coordinates: the CTA partials of the sampled distances of the largest grid, then the
@@ -242,7 +254,7 @@ def _torch_rules(spec, step=0):
           "smea": lambda M: _ops.torch_smea(M, spec.f)}[spec.rule]
 
 
-def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed=0, root=None):
+def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed=0, root=None, history=None):
   """Stand-alone aggregation of the CUDA matrix `G` ([n, d], fp32) with rule `spec` -> [d] tensor. `return_details` also returns the
   distances (Krum / Bulyan / MDA: the [n, n] matrix; geometric median, centered clipping: the [iterations, n] row distances of every
   iteration) and the selection masks. Centered clipping needs `center`, a [d] tensor of G's dtype on G's device, updated in place.
@@ -256,7 +268,9 @@ def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed
   With "bucketing" G holds the n gathered rows and the rule runs on the n' = ceil(n / spec.bucket_size) bucket means, drawn with step
   key `step` and seed `bucketing_seed` (its distances and masks are those of the means); `return_details` adds (permutation [n] int32,
   bucket masks [n'] int32).
-  FLTrust needs `root`, the [d] root gradient; its details are (P [n], N [n], N0, a [n]), CPU tensors: the kernel's sums and coefficients."""
+  FLTrust needs `root`, the [d] root gradient; its details are (P [n], N [n], N0, a [n]), CPU tensors: the kernel's sums and coefficients.
+  FoolsGold needs `history`, the [n, d] per-worker histories of G's dtype on G's device, updated in place; its details are (P [n, n],
+  N [n], bad [n] bool, c [n]), NumPy arrays: the kernel's sums of the updated histories, bad-row flags and coefficients."""
   if not G.is_cuda:
     raise tools.UserException("ops.gar.aggregate expects a CUDA tensor")
   from ..aggregators import _ops
@@ -273,6 +287,8 @@ def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed
     return _aggregate_centered_clipping(spec, G, return_details, center, step, bucketing_seed)
   if spec.rule == "fltrust":
     return _aggregate_fltrust(spec, G, return_details, root)
+  if spec.rule == "foolsgold":
+    return _aggregate_foolsgold(spec, G, return_details, history)
   if G.dtype == torch.float64 and not return_details:
     # the reference's ops are registered for double too (`native/op_krum/op.cpp:47`): the sm_90a kernels are fp32, so double inputs are
     # aggregated in double by the device-side torch implementations of the same rules (same ordering convention) instead of being rounded
@@ -413,6 +429,49 @@ def _aggregate_fltrust(spec, G, return_details, root):
     fo = launcher.fltrust_out.cpu()
     return out, fo[:n].clone(), fo[MAX_WORKERS:MAX_WORKERS + n].clone(), fo[2 * MAX_WORKERS].clone(), fo[2 * MAX_WORKERS + 1:2 * MAX_WORKERS + 1 + n].clone()
   return out
+
+
+def _aggregate_foolsgold(spec, G, return_details, history):
+  """`aggregate` for FoolsGold: the sm_90a kernel for fp32 and n <= 32, the torch reference on the device otherwise (double rows in
+  double)."""
+  from ..aggregators import _ops
+  n, d = G.shape
+  if spec.mix is not None:
+    raise tools.UserException("FoolsGold takes no pre-aggregation (got %r)" % (spec.mix,))
+  history = _ops.check_foolsgold_history(G, history)
+  if G.dtype == torch.float64 or n > MAX_WORKERS:
+    if return_details:
+      raise tools.UserException("FoolsGold returns its details from the sm_90a kernel only (fp32, n <= %d)" % MAX_WORKERS)
+    return _ops.torch_foolsgold(G, history, spec.confidence)
+  if G.dtype != torch.float32:
+    raise tools.UserException("FoolsGold on the device needs fp32 or float64 rows (got %s)" % (G.dtype,))
+  G, dp = _aligned_rows(G)
+  work = history
+  if dp != d or not history.is_contiguous() or history.data_ptr() % 16:
+    work = torch.zeros((n, dp), dtype=torch.float32, device=G.device)
+    work[:, :d] = history
+  launcher = _launcher(G.device, n)
+  out = torch.empty(dp, dtype=torch.float32, device=G.device)
+  rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
+  staging = torch.empty((n, dp), dtype=torch.float32, device=G.device) if n > 8 else None   # beyond one 8-row block: the staged rows
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=staging, history=work)
+  if work is not history:
+    history.copy_(work[:, :d])
+  out = out[:d]
+  if return_details:
+    return (out,) + foolsgold_details(launcher, n)
+  return out
+
+
+def foolsgold_details(launcher, n):
+  """FoolsGold's (P [n, n], N [n], bad [n] bool, c [n] float32) of the launcher's last launch, as NumPy arrays (a synchronisation)."""
+  import numpy as np
+  fo = launcher.foolsgold_out.cpu().numpy()
+  P = np.zeros((n, n), dtype=np.float32)
+  iu = np.triu_indices(n)
+  P[iu] = fo[:n * (n + 1) // 2]
+  P.T[iu] = fo[:n * (n + 1) // 2]
+  return P, np.diagonal(P).copy(), fo[FOOLSGOLD_SUMS:FOOLSGOLD_SUMS + n] != 0, fo[FOOLSGOLD_SUMS + MAX_WORKERS:FOOLSGOLD_SUMS + MAX_WORKERS + n].copy()
 
 
 def worker_momentum_(G, M, beta, c):

@@ -34,6 +34,13 @@ update number (DnC's step key), and replaces them by the n' = ceil(n / s) means 
 Rules that score the rows against a trusted root gradient (`fltrust`, `needs_root`) take it from `root`, a [d] fp32 row that rank 0's
 trainer fills every step: the fused engine keeps it in symmetric memory and its kernel reads rank 0's copy over P2P; the baseline and
 host engines broadcast it from rank 0 before the aggregation. Such rules take no pre-aggregation.
+Rules with per-worker state (`foolsgold`, `needs_history`: every worker's history, the sum of the rows it submitted) keep it in the
+engine as `history`, allocated with the engine (before any CUDA-graph capture) and updated by every aggregation: the baseline and host
+engines hold the [n, d] fp32 matrix (every rank the whole of it), the fused engine the [n, owned] tile of its owned segments, back to
+back in segment order like the staged tile, which its kernel reads and writes in place. That tile takes n * owned * 4 bytes: 0.82 GB
+for ResNet-50 (d = 25 558 016) with n = 8 on one GPU, 1/R of it per rank on R ranks. The history is checkpointed under "rule_state"
+as the full [n, d] CPU tensor; a checkpoint without one restores zero histories, with a warning. Such rules take no pre-aggregation:
+NNM, ARC and bucketing mix, rescale or reshuffle the rows, so a row would no longer be one worker's.
 """
 
 import os
@@ -65,6 +72,9 @@ def _mixed_spec(gar, nbworkers, pre_aggregation, nb_decl_byz, bucket_size=None):
   if mix is not None and getattr(gar, "needs_root", False):
     raise tools.UserException("%s scores the direction and norm of the submitted rows against the root gradient: it cannot be combined "
                               "with a pre-aggregation (got %r)" % (type(gar).__name__, mix))
+  if mix is not None and getattr(gar, "needs_history", False):
+    raise tools.UserException("%s keeps a history per worker: it cannot be combined with a pre-aggregation, which does not keep one row "
+                              "per worker (got %r)" % (type(gar).__name__, mix))
   spec = gar.fused_spec()
   own = spec.f if spec is not None and spec.rule in FusedSpec.RULES_WITH_F else getattr(gar, "_f", None)
   f = own if nb_decl_byz is None else int(nb_decl_byz)
@@ -109,12 +119,20 @@ class _AggregationBase:
     self.attack_state = None   # mimic: {"t", "z", "istar"} (`mimic_state`)
     self.root = None   # FLTrust: the root gradient, [d] fp32, written by rank 0's trainer
     self.needs_root = bool(getattr(gar, "needs_root", False))
+    self.history = None   # FoolsGold: every worker's history, [n, d] fp32 (the fused engine: [n, owned])
+    self.needs_history = bool(getattr(gar, "needs_history", False))
 
   def _make_center(self):
     """Allocate the center (+0) when the rule is centered clipping; it lives as long as the engine and travels in checkpoints."""
     spec = self.spec
     if spec is not None and spec.rule == "centered-clipping":
       self.center = torch.zeros(self.d, dtype=torch.float32, device=self.device)
+
+  def _make_history(self, columns):
+    """Allocate the [n, columns] histories (+0) when the rule keeps one per worker; they live as long as the engine and travel in
+    checkpoints."""
+    if self.needs_history:
+      self.history = torch.zeros((self.n, columns), dtype=torch.float32, device=self.device)
 
   def _broadcast_root(self):
     """The baseline and host engines: every rank takes rank 0's root row before the aggregation (collective when R > 1)."""
@@ -138,6 +156,8 @@ class _AggregationBase:
     state = {"updates": self.updates, "slots": [s.detach().to("cpu", copy=True) for s in self.full_slots()]}
     if self.center is not None:
       state["rule_state"] = self.full_center().detach().to("cpu", copy=True)
+    if self.history is not None:
+      state["rule_state"] = self.full_history().detach().to("cpu", copy=True)
     if self.attack_state is not None:
       mimic = self.attack_state
       state["attack_state"] = {"mode": "mimic", "t": int(mimic["t"]), "z": self._assemble(self._unpack(mimic["z"])).detach().to("cpu", copy=True),
@@ -154,6 +174,13 @@ class _AggregationBase:
       else:
         tools.warning("The checkpoint holds no center for centered clipping: it starts from zero", context="restore")
         self.center.zero_()
+    if self.history is not None:
+      saved = state.get("rule_state")
+      if saved is not None and tuple(saved.shape) == (self.n, self.d):
+        self.history.copy_(self._pack_rows(saved.to(self.device)))
+      else:
+        tools.warning("The checkpoint holds no [%d, %d] per-worker history: the histories start from zero" % (self.n, self.d), context="restore")
+        self.history.zero_()
     if self.attack_state is not None:
       saved = state.get("attack_state")
       if saved is not None and saved.get("mode") == "mimic":
@@ -177,6 +204,10 @@ class _AggregationBase:
     """The [d] vector of `_pack`'s output (the fused engine: zero outside the owned segments)."""
     return owned
 
+  def _pack_rows(self, matrix):
+    """The columns of an [n, d] matrix that the engine's history holds: all of them (the fused engine: its owned segments)."""
+    return matrix
+
   def _fang_kwargs(self, mode, byz_slots, threshold, scale, seed, step):
     """The keywords of a Fang attack for `craft_byzantine_` / `craft`: fang-krum's declared f and threshold, fang-trim's scale, seed and
     step key (`step`: the number of the update the crafted rows feed); none for the other attacks."""
@@ -193,6 +224,8 @@ class _AggregationBase:
       return {"center": self.center}
     if self.root is not None:
       return {"root": self.root}
+    if self.history is not None:
+      return {"history": self.history}
     if self.spec is not None and self.spec.rule == "dnc":
       return {"step": self.updates + 1}
     return {}
@@ -207,6 +240,9 @@ class _AggregationBase:
 
   def full_center(self):
     return self.center
+
+  def full_history(self):
+    return self.history
 
   # -- authentication hooks (`parallel/signing.py`) --------------------------------- #
   def visible_rows(self):
@@ -236,6 +272,7 @@ class HostAggregation(_AggregationBase):
     self.slots = optimizer.make_slots(self.params)
     self._make_center()
     self.root = torch.zeros(self.d, dtype=torch.float32, device=self.device) if self.needs_root else None
+    self._make_history(self.d)
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -283,6 +320,7 @@ class BaselineAggregation(_AggregationBase):
     self.slots = optimizer.make_slots(self.params)
     self._make_center()
     self.root = torch.zeros(self.d, dtype=torch.float32, device=self.device) if self.needs_root else None
+    self._make_history(self.d)
     self._gathered = torch.zeros((self.n, self.d), dtype=torch.float32, device=self.device) if self.world > 1 else self.grads
     self._gathered_ready = False
     self.last_aggregate = None
@@ -368,15 +406,16 @@ class FusedAggregation(_AggregationBase):
     self.root = self.heap.local("root", torch.float32) if self.needs_root else None   # only rank 0's copy is read
     self.slots = optimizer.make_slots(self.params)
     self._make_center()   # centered clipping: maintained on the owned segments only, like the optimizer slots
+    self._make_history(owned)   # FoolsGold: the owned segments of every worker's history, back to back
     self.aggregate_out = torch.zeros(d, dtype=torch.float32, device=self.device) if keep_aggregate else None
     # staging keeps the P2P-loaded tiles local so that later passes never cross NVLink again (and rows beyond the 8 held in registers
     # can be re-read); needed whenever the distance pass and the aggregation pass are different launches too
     # the iterative rules' passes after the first re-read the staged copy rather than the peers' rows; a pre-aggregation (NNM mixes, ARC
     # clips) rewrites the staged tile in place and every rule then reads it (n * owned * 4 bytes, also with R = 1); bucketing stores its
     # n' means there, so the tile has the rule's spec.n rows
-    # FLTrust's second pass reads the staged rows over several ranks, and beyond one 8-row block
+    # FLTrust's and FoolsGold's second pass reads the staged rows over several ranks, and beyond one 8-row block
     need_staging = ((self.distance_rule and (R > 1 or len(self.buckets) > 1 or self.n > 8)) or (self.spec.rule in gar_ops.ITERATIVE_RULES and R > 1)
-                    or self.mix is not None or (self.spec.rule == "fltrust" and (R > 1 or self.n > 8)))
+                    or self.mix is not None or (self.spec.rule in ("fltrust", "foolsgold") and (R > 1 or self.n > 8)))
     self.staging = torch.empty((self.spec.n, owned), dtype=torch.float32, device=self.device) if need_staging else None
     self.launcher = gar_ops.FusedLauncher(self.device, self.n)
     if self.spec.rule == "dnc":
@@ -522,7 +561,7 @@ class FusedAggregation(_AggregationBase):
     first_seg, self._pre_accumulated = self._pre_accumulated, 0
     self.launcher.launch(self.spec, self._rows, segments=self.segments, agg_out=self.aggregate_out, epoch=self.epoch, stream=stream, first_seg=first_seg,
                          loss_in=loss_in, loss_out=self.loss_out, center=self.center, step=self.updates, step_ptr=self.step_dev, domain=self.d,
-                         bucketing_seed=self.bucketing_seed, root=self._root_src, **self._common(self._rate_args))
+                         bucketing_seed=self.bucketing_seed, root=self._root_src, history=self.history, **self._common(self._rate_args))
 
   def _assemble(self, vector):
     """Full copy of a [d] vector maintained on the owned segments only (collective when R > 1)."""
@@ -547,6 +586,15 @@ class FusedAggregation(_AggregationBase):
   def full_center(self):
     """The center of centered clipping, assembled from the owned segments of every rank (checkpoints)."""
     return None if self.center is None else self._assemble(self.center)
+
+  def full_history(self):
+    """FoolsGold's [n, d] histories, assembled from the owned segments of every rank (checkpoints; collective when R > 1)."""
+    if self.history is None:
+      return None
+    return torch.stack([self._assemble(self._unpack(row)) for row in self.history])
+
+  def _pack_rows(self, matrix):
+    return torch.cat([matrix[:, lo:hi] for lo, hi in self.segments], dim=1)
 
   def _pack(self, vector):
     """Mimic's z and y scratch hold the owned segments only, back to back in segment order (as the staged tile): d / R floats each."""

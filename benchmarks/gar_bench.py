@@ -36,6 +36,11 @@ step key is the update count), so the fused-vs-baseline check holds for it as fo
 each engine kept in the checked step (`fused_mask`, `baseline_mask`, `masks_agree`).
 `fltrust` seeds a synthetic root gradient on rank 0, which the fused kernel reads over P2P and the baseline engine broadcasts; the
 fused-vs-baseline check holds for it as for the other rules.
+`foolsgold` updates the per-worker histories at every step (both engines start from zero histories and take the same steps); its
+entry reports the rows of non-zero weight (`weighted_rows`), the largest difference between the two engines' histories after the
+checked step, and the local HBM bytes of one fused step counted from the shapes (`foolsgold_hbm_bytes`: the history pass reads g and H
+and writes H, re-reads the histories of the 8-row blocks it pairs when n > 8 and stores the staged rows when there is a tile; phase D
+reads the weighted rows; the SGD update reads and writes the parameters and stores the kept aggregate) with the rate they imply.
 """
 
 import argparse
@@ -55,6 +60,13 @@ from aggregathor_b200.engine.optimizers import optimizers  # noqa: E402
 from aggregathor_b200.engine.schedules import build  # noqa: E402
 from aggregathor_b200.ops import gar as gar_ops  # noqa: E402
 from aggregathor_b200.parallel.aggregation import BaselineAggregation, FusedAggregation  # noqa: E402
+
+
+def foolsgold_hbm_bytes(n, slice_bytes, weighted, staged):
+  """Local HBM bytes of one fused FoolsGold step over `slice_bytes` owned bytes per row (see the module docstring)."""
+  size = [min(8, n - 8 * b) for b in range(-(-n // 8))]   # the rows of every 8-row block
+  rereads = sum(size[1:]) + sum(size[bi] + (size[bj] if bi > 0 else 0) for bi in range(len(size)) for bj in range(bi + 1, len(size)))
+  return (3 * n + rereads + (n if staged else 0) + weighted + 3) * slice_bytes
 
 
 def main():
@@ -186,6 +198,10 @@ def main():
     if rule == "fltrust":   # the rows of non-zero weight, the only ones the weighted sum reads
       coefs = fused.launcher.fltrust_out[2 * gar_ops.MAX_WORKERS + 1:2 * gar_ops.MAX_WORKERS + 1 + n].cpu()
       mask_entry = {"weighted_rows": int((coefs != 0).sum())}
+    if rule == "foolsgold":   # the rows phase D reads, and the histories after the checked step against the baseline engine's
+      at = gar_ops.FOOLSGOLD_SUMS + gar_ops.MAX_WORKERS
+      coefs = fused.launcher.foolsgold_out[at:at + n].cpu()
+      mask_entry = {"weighted_rows": int((coefs != 0).sum()), "history_max_abs_diff_vs_baseline": float((fused.full_history() - base.history).abs().max())}
     gamma_entry = {}
     if attack is not None and attack.deviation is not None:
       # gamma as every rank solved it (fused engine), and as the baseline engine's stand-alone kernel solved it on the gathered rows
@@ -455,6 +471,9 @@ def main():
     results[rule].update(attack_entry)
     results[rule].update(mix_entry)
     results[rule].update(mask_entry)
+    if rule == "foolsgold":
+      counted = foolsgold_hbm_bytes(n, slice_bytes, mask_entry["weighted_rows"], fused.staging is not None)
+      results[rule].update(foolsgold_hbm_bytes=counted, foolsgold_hbm_gbs=counted / fused_ms / 1e6)
     if args.rule_args is not None:
       results[rule]["rule_args"] = args.rule_args
     if rule in ("geometric-median", "centered-clipping"):
