@@ -309,7 +309,10 @@ class Manager:
     before = counters.launches
     whole = self._whole_step_graph
     try:
-      with torch.cuda.graph(graph):
+      # thread-local capture: the input pipelines' producer threads keep allocating, copying and synchronising on their own streams
+      # while this thread captures. Under the default global mode any such call in another thread fails and invalidates the
+      # capture, and a capture that ends that way leaves torch's default CUDA generator in capture mode for the rest of the process.
+      with torch.cuda.graph(graph, capture_error_mode="thread_local"):
         self._static_losses = self._run_workers(self._static_batches, None, self._static_root)
         if whole:
           self._apply_momentum()

@@ -77,12 +77,13 @@ constexpr int kThreads = 256;
 // Per-channel (and per-group) sums: out[g][c] += sum_r f(...). MODE 0: (x - p, (x - p)^2) with the pivot p = the group's first row,
 // so that E[x^2] - E[x]^2 stays well conditioned in fp32 even when |mean| >> std; MODE 1: (dy', dy' * xhat) with
 // dy' = dy masked by (y > 0) when y != null, or by the mask recomputed from x with the forward's coefficients `msc` / `msh`
-// (relu_kept) when those are given; MODE 2: (dy') only (bias gradient). C % 8 == 0.
+// (relu_kept) when those are given; MODE 2: (dy') only (bias gradient). C % 8 == 0. MODE 1 with y and `dmasked` also stores dy' to
+// `dmasked` (dy or +0, the gradient of the residual input of a fused add + ReLU), so that the apply kernel reads it instead of dy and y.
 // 2-D decomposition: blockIdx.x = row chunk, blockIdx.y = strip of STRIP octets (8 * STRIP channels), blockIdx.z = group.
 // Inside a CTA, STRIP lanes cover the strip's octets (up to 512 contiguous bytes per row: whole DRAM bursts instead of
 // 128-byte columns) and 256 / STRIP lanes cover rows, several rows in flight per thread; one fp64 atomic per channel and
 // CTA, so an address only sees (#row chunks) atomics.
-constexpr int kRowUnroll = 4;   // MODE 0 / 2; MODE 1 (three tensors) uses 2 to stay under 64 registers per thread
+constexpr int kRowUnroll = 4;   // rows in flight per thread: MODE 0 / 2, and MODE 1 (three tensors) in bf16; MODE 1 in fp32 uses 2
 
 // Finalisation performed by the LAST CTA of the statistics kernel (atomic ticket): no separate launch.
 struct SumsFinalize {
@@ -146,8 +147,8 @@ __device__ void finalize_sums(double* sums, SumsFinalize const& f, int C, long l
 }
 
 template<typename T, int MODE, int STRIP>
-__global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restrict__ a, T const* __restrict__ b, T const* __restrict__ y, float const* __restrict__ mean,
-                                    float const* __restrict__ rstd, float const* __restrict__ msc, float const* __restrict__ msh, double* __restrict__ out,
+__global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restrict__ a, T const* __restrict__ b, T const* __restrict__ y, T* __restrict__ dmasked,
+                                    float const* __restrict__ mean, float const* __restrict__ rstd, float const* __restrict__ msc, float const* __restrict__ msh, double* __restrict__ out,
                                     long long rows_per_group, int C, int rows_per_cta, SumsFinalize const fin) {
     pdl_trigger();
     pdl_wait();
@@ -184,7 +185,7 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
     if (MODE == 0 && active)
         unpack8(load_oct(a + base * C + o * 8), mu);
     if (active) {
-        constexpr int U = MODE == 1 ? 2 : kRowUnroll;
+        constexpr int U = MODE == 1 && sizeof(T) == 4 ? 2 : kRowUnroll;   // fp32 MODE 1 at 4 would need 175 registers: 1 CTA per SM
         for (long long r0 = row_begin + tr; r0 < row_end; r0 += kRowLanes * U) {
             Oct<T> ra[U], rb[U], ry[U];
 #pragma unroll
@@ -219,6 +220,8 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
 #pragma unroll
                             for (int j = 0; j < 8; ++j)
                                 va[j] = vy[j] > 0.f ? va[j] : 0.f;
+                            if (MODE == 1 && dmasked)
+                                store_oct(dmasked + (base + r) * C + o * 8, pack_oct<T>(va));
                         }
                         if (MODE == 1) {
                             float vx[8];
@@ -279,32 +282,37 @@ __global__ void __launch_bounds__(kThreads) channel_sums_kernel(T const* __restr
     }
 }
 
-// y = relu?(x * scale[g][c] + shift[g][c]). Each thread keeps a fixed channel octet (stride is a multiple of `octets`
-// whenever possible) so the coefficients stay in registers and no division happens in the loop.
+// The apply kernels run `ctas` CTAs per group: CTA k serves group k / ctas, whose octets are a contiguous range. A thread keeps one
+// channel octet for its whole loop (the stride is a multiple of `octets`; the host gives each group at least one CTA per 256
+// octets), so the group's coefficients stay in registers and no division happens in the loop, and it keeps U independent
+// 16-byte loads of each tensor in flight.
+
+// y = relu?(x * scale[g][c] + shift[g][c] (+ residual)).
 template<typename T>
 __global__ void __launch_bounds__(kThreads) bn_apply_kernel(T const* __restrict__ x, T const* __restrict__ residual, T* __restrict__ y, float const* __restrict__ scale,
-                                float const* __restrict__ shift, long long total_octets, int C, long long rows_per_group, int relu) {
+                                float const* __restrict__ shift, long long rows_per_group, int C, int ctas, int relu) {
     pdl_trigger();
     pdl_wait();
     unsigned const octets = static_cast<unsigned>(C >> 3);
-    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const g = blockIdx.x / ctas;
+    long long const nthreads = static_cast<long long>(ctas) * blockDim.x;
     long long const stride = nthreads - nthreads % octets;   // multiple of `octets`: the octet of a thread never changes
-    long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long i = static_cast<long long>(blockIdx.x - g * ctas) * blockDim.x + threadIdx.x;
     if (i >= stride)
         return;
     unsigned const o = static_cast<unsigned>(i % octets);
-    long long const octets_per_group = rows_per_group * octets;
-    bool const single_group = octets_per_group >= total_octets;
-    int cached_group = -1;
+    long long const n = rows_per_group * octets;             // octets of the group
+    long long const base = static_cast<long long>(g) * n * 8;
+    x += base;
+    y += base;
+    if (residual)
+        residual += base;
     float sc[8], sh[8];
-    auto load_coefficients = [&](int g) {
-        cached_group = g;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            sc[j] = scale[g * C + o * 8 + j];
-            sh[j] = shift[g * C + o * 8 + j];
-        }
-    };
+    for (int j = 0; j < 8; ++j) {
+        sc[j] = scale[g * C + o * 8 + j];
+        sh[j] = shift[g * C + o * 8 + j];
+    }
     auto transform = [&](Oct<T> raw, long long index) {   // y = relu?(x * scale + shift (+ residual))
         float v[8], r[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         unpack8(raw, v);
@@ -318,60 +326,56 @@ __global__ void __launch_bounds__(kThreads) bn_apply_kernel(T const* __restrict_
         }
         return pack_oct<T>(v);
     };
-    if (single_group) {
-        load_coefficients(0);
-        constexpr int U = 4;   // four independent 16-byte loads in flight per thread
-        for (; i + (U - 1) * stride < total_octets; i += U * stride) {
-            Oct<T> raw[U];
+    constexpr int U = 4;   // four independent 16-byte loads in flight per thread
+    for (; i + (U - 1) * stride < n; i += U * stride) {
+        Oct<T> raw[U];
 #pragma unroll
-            for (int u = 0; u < U; ++u)
-                raw[u] = load_oct(x + (i + u * stride) * 8);
+        for (int u = 0; u < U; ++u)
+            raw[u] = load_oct(x + (i + u * stride) * 8);
 #pragma unroll
-            for (int u = 0; u < U; ++u)
-                store_oct(y + (i + u * stride) * 8, transform(raw[u], i + u * stride));
-        }
+        for (int u = 0; u < U; ++u)
+            store_oct(y + (i + u * stride) * 8, transform(raw[u], i + u * stride));
     }
-    for (; i < total_octets; i += stride) {
-        int const g = single_group ? 0 : static_cast<int>(i / octets_per_group);
-        if (g != cached_group)
-            load_coefficients(g);
+    for (; i < n; i += stride)
         store_oct(y + i * 8, transform(load_oct(x + i * 8), i));
-    }
 }
 
 // dx = a * dy' + b * x + c0 with per-(group, channel) coefficients prepared by the statistics kernel's last CTA; dy' = dy masked by
-// y > 0, or by the mask recomputed from x (`msc` / `msh`: the forward's coefficients, relu_kept), or dy when neither is given.
+// y > 0, or by the mask recomputed from x (`msc` / `msh`: the forward's coefficients, relu_kept), or dy when neither is given (also
+// when dy is the masked gradient the statistics kernel stored).
 template<typename T>
-__global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restrict__ dy, T const* __restrict__ x, T const* __restrict__ y, T* __restrict__ dx, T* __restrict__ dmasked,
-                                    float const* __restrict__ coef, float const* __restrict__ msc, float const* __restrict__ msh, long long total_octets, int C,
-                                    long long rows_per_group) {
+__global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restrict__ dy, T const* __restrict__ x, T const* __restrict__ y, T* __restrict__ dx,
+                                    float const* __restrict__ coef, float const* __restrict__ msc, float const* __restrict__ msh, long long rows_per_group, int C,
+                                    int ctas) {
     pdl_trigger();
     pdl_wait();
     unsigned const octets = static_cast<unsigned>(C >> 3);
-    long long const nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+    int const g = blockIdx.x / ctas;
+    long long const nthreads = static_cast<long long>(ctas) * blockDim.x;
     long long const stride = nthreads - nthreads % octets;
-    long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    long long i = static_cast<long long>(blockIdx.x - g * ctas) * blockDim.x + threadIdx.x;
     if (i >= stride)
         return;
     unsigned const o = static_cast<unsigned>(i % octets);
-    long long const octets_per_group = rows_per_group * octets;
-    bool const single_group = octets_per_group >= total_octets;
-    int cached_group = -1;
+    long long const n = rows_per_group * octets;
+    long long const base = static_cast<long long>(g) * n * 8;
+    bool const masked = y != nullptr, recompute = msc != nullptr;
+    dy += base;
+    x += base;
+    dx += base;
+    if (masked)
+        y += base;
     float ca[8], cb[8], cc[8], sc[8], sh[8];
-    bool const recompute = msc != nullptr;
-    auto load_coefficients = [&](int g) {
-        cached_group = g;
-        float const* cf = coef + (static_cast<long long>(g) * C + o * 8) * 3;
+    float const* cf = coef + (static_cast<long long>(g) * C + o * 8) * 3;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            ca[j] = cf[3 * j];
-            cb[j] = cf[3 * j + 1];
-            cc[j] = cf[3 * j + 2];
-            sc[j] = recompute ? msc[g * C + o * 8 + j] : 0.f;
-            sh[j] = recompute ? msh[g * C + o * 8 + j] : 0.f;
-        }
-    };
-    auto transform = [&](Oct<T> rd, Oct<T> rx, Oct<T> ry, bool masked, long long index) {
+    for (int j = 0; j < 8; ++j) {
+        ca[j] = cf[3 * j];
+        cb[j] = cf[3 * j + 1];
+        cc[j] = cf[3 * j + 2];
+        sc[j] = recompute ? msc[g * C + o * 8 + j] : 0.f;
+        sh[j] = recompute ? msh[g * C + o * 8 + j] : 0.f;
+    }
+    auto transform = [&](Oct<T> rd, Oct<T> rx, Oct<T> ry) {
         float vd[8], vx[8];
         unpack8(rd, vd);
         unpack8(rx, vx);
@@ -385,38 +389,29 @@ __global__ void __launch_bounds__(kThreads) bn_bwd_apply_kernel(T const* __restr
 #pragma unroll
             for (int j = 0; j < 8; ++j)
                 vd[j] = vy[j] > 0.f ? vd[j] : 0.f;
-            if (dmasked)   // the gradient of the residual input of a fused add + ReLU
-                store_oct(dmasked + index * 8, pack_oct<T>(vd));
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j)
             vd[j] = ca[j] * vd[j] + cb[j] * vx[j] + cc[j];
         return pack_oct<T>(vd);
     };
-    bool const masked = y != nullptr;
-    if (single_group) {
-        load_coefficients(0);
-        constexpr int U = 2;   // 2 x 3 independent 16-byte loads in flight per thread
-        for (; i + (U - 1) * stride < total_octets; i += U * stride) {
-            Oct<T> rd[U], rx[U], ry[U];
+    constexpr int U = sizeof(T) == 2 ? 4 : 2;   // bf16: 4 x 3 loads in flight at the occupancy of 2 (no spill); fp32 stays at 2
+    for (; i + (U - 1) * stride < n; i += U * stride) {
+        Oct<T> rd[U], rx[U], ry[U];
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                long long const e = (i + u * stride) * 8;
-                rd[u] = load_oct(dy + e);
-                rx[u] = load_oct(x + e);
-                ry[u] = masked ? load_oct(y + e) : zero_oct<T>();
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u)
-                store_oct(dx + (i + u * stride) * 8, transform(rd[u], rx[u], ry[u], masked, i + u * stride));
+        for (int u = 0; u < U; ++u) {
+            long long const e = (i + u * stride) * 8;
+            rd[u] = load_oct(dy + e);
+            rx[u] = load_oct(x + e);
+            ry[u] = masked ? load_oct(y + e) : zero_oct<T>();
         }
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            store_oct(dx + (i + u * stride) * 8, transform(rd[u], rx[u], ry[u]));
     }
-    for (; i < total_octets; i += stride) {
-        int const g = single_group ? 0 : static_cast<int>(i / octets_per_group);
-        if (g != cached_group)
-            load_coefficients(g);
+    for (; i < n; i += stride) {
         Oct<T> const ry = masked ? load_oct(y + i * 8) : zero_oct<T>();
-        store_oct(dx + i * 8, transform(load_oct(dy + i * 8), load_oct(x + i * 8), ry, masked, i));
+        store_oct(dx + i * 8, transform(load_oct(dy + i * 8), load_oct(x + i * 8), ry));
     }
 }
 
@@ -1000,6 +995,16 @@ inline int grid_for(long long work, int threads = kThreads, int cap = agb::sm_co
     return blocks < 1 ? 1 : static_cast<int>(blocks);
 }
 
+// CTAs per group of the apply kernels: the grid `grid_for` gives one group's octets, within an equal share of the usual cap (so one
+// group gets the same grid as before the split), and at least one CTA per 256 octets of a row so that every octet has a thread.
+inline int apply_ctas(long long rows_per_group, int C, int groups) {
+    int const octets = C >> 3;
+    int const share = agb::sm_count() * 8 / groups;
+    int const ctas = grid_for(rows_per_group * octets, kThreads, share < 1 ? 1 : share);
+    int const least = (octets + kThreads - 1) / kThreads;
+    return ctas > least ? ctas : least;
+}
+
 struct SumsPlan {
     int rows_per_cta, strip;
     dim3 grid;
@@ -1435,14 +1440,14 @@ int launch_bn_fused(BnFused p, long long rows, cudaStream_t s) {
 }
 
 template<int MODE, typename T>
-int launch_sums(SumsPlan const& plan, cudaStream_t s, T const* a, T const* b, T const* y, float const* mean, float const* rstd, float const* msc, float const* msh,
+int launch_sums(SumsPlan const& plan, cudaStream_t s, T const* a, T const* b, T const* y, T* dmasked, float const* mean, float const* rstd, float const* msc, float const* msh,
                  double* out, long long rows_per_group, int C, SumsFinalize const& fin) {
     if (plan.strip == 32)
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 32>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 32>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, dmasked, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     else if (plan.strip == 16)
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 16>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 16>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, dmasked, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     else
-        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 8>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
+        AGB_CUDA_OK(launch_pdl(channel_sums_kernel<T, MODE, 8>, dim3(plan.grid), dim3(kThreads), 0, s, a, b, y, dmasked, mean, rstd, msc, msh, out, rows_per_group, C, plan.rows_per_cta, fin));
     return 0;
 }
 
@@ -1462,10 +1467,11 @@ int bn_forward_impl(void const* x, void const* residual, void* y, void const* ga
     fin.moving_mean = static_cast<float*>(moving_mean); fin.moving_var = static_cast<float*>(moving_var);
     fin.groups = groups; fin.eps = eps; fin.decay = decay;
     SumsPlan plan = plan_sums(rpg, C, groups);
-    if (int status = launch_sums<0, T>(plan, s, static_cast<T const*>(x), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rpg, C, fin))
+    if (int status = launch_sums<0, T>(plan, s, static_cast<T const*>(x), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rpg, C, fin))
         return status;
-    long long const octets = rows * (C >> 3);
-    AGB_CUDA_OK(launch_pdl(bn_apply_kernel<T>, dim3(grid_for(octets)), dim3(kThreads), 0, s, static_cast<T const*>(x), static_cast<T const*>(residual), static_cast<T*>(y), static_cast<float const*>(scale), static_cast<float const*>(shift), octets, C, rpg, relu));
+    int const ctas = apply_ctas(rpg, C, groups);
+    AGB_CUDA_OK(launch_pdl(bn_apply_kernel<T>, dim3(groups * ctas), dim3(kThreads), 0, s, static_cast<T const*>(x), static_cast<T const*>(residual), static_cast<T*>(y),
+        static_cast<float const*>(scale), static_cast<float const*>(shift), rpg, C, ctas, relu));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1489,12 +1495,16 @@ int bn_backward_impl(void const* dy, void const* x, void const* y, void const* m
     fin.dgamma = static_cast<float*>(dgamma); fin.dbeta = static_cast<float*>(dbeta);
     fin.groups = groups; fin.group_stride = group_stride;
     SumsPlan plan = plan_sums(rpg, C, groups);
-    if (int status = launch_sums<1, T>(plan, s, static_cast<T const*>(dy), static_cast<T const*>(x), static_cast<T const*>(y), static_cast<float const*>(save_mean),
-                   static_cast<float const*>(save_rstd), msc, msh, static_cast<double*>(sums), rpg, C, fin))
+    // with y and `dmasked`, the statistics kernel stores the masked gradient and the apply kernel reads it in place of dy and y
+    T* const masked_out = y ? static_cast<T*>(dmasked) : nullptr;
+    if (int status = launch_sums<1, T>(plan, s, static_cast<T const*>(dy), static_cast<T const*>(x), static_cast<T const*>(y), masked_out,
+                   static_cast<float const*>(save_mean), static_cast<float const*>(save_rstd), msc, msh, static_cast<double*>(sums), rpg, C, fin))
         return status;
-    long long const octets = rows * (C >> 3);
-    AGB_CUDA_OK(launch_pdl(bn_bwd_apply_kernel<T>, dim3(grid_for(octets)), dim3(kThreads), 0, s, static_cast<T const*>(dy), static_cast<T const*>(x), static_cast<T const*>(y), static_cast<T*>(dx),
-        static_cast<T*>(dmasked), static_cast<float const*>(coef), msc, msh, octets, C, rpg));
+    int const ctas = apply_ctas(rpg, C, groups);
+    T const* const grad = masked_out ? masked_out : static_cast<T const*>(dy);
+    T const* const mask = masked_out ? nullptr : static_cast<T const*>(y);
+    AGB_CUDA_OK(launch_pdl(bn_bwd_apply_kernel<T>, dim3(groups * ctas), dim3(kThreads), 0, s, grad, static_cast<T const*>(x), mask, static_cast<T*>(dx),
+        static_cast<float const*>(coef), msc, msh, rpg, C, ctas));
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -1509,7 +1519,7 @@ int colsum_impl(void const* dy, void const* y, void* out, void* sums, long long 
     fin.dbeta = static_cast<float*>(out);
     fin.groups = groups; fin.group_stride = group_stride;
     SumsPlan plan = plan_sums(rows / groups, C, groups);
-    if (int status = launch_sums<2, T>(plan, s, static_cast<T const*>(dy), nullptr, static_cast<T const*>(y), nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rows / groups, C, fin))
+    if (int status = launch_sums<2, T>(plan, s, static_cast<T const*>(dy), nullptr, static_cast<T const*>(y), nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<double*>(sums), rows / groups, C, fin))
         return status;
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
@@ -1692,7 +1702,8 @@ extern "C" {
 //   sums  double [groups*C*2] | coef float [groups*C*3]                              (backward)
 // Backward: the ReLU mask is y > 0 when `y` is given, or is recomputed from x with the forward's `scale` / `shift` ([groups*C]
 // each, what agb_bn_forward(_fused) stored) when `mask_scale` / `mask_shift` are given instead: one activation fewer to read in
-// each of the two passes, same result bit for bit. Neither: no ReLU. `dmasked` needs `y`.
+// each of the two passes, same result bit for bit. Neither: no ReLU. `dmasked` needs `y`: the statistics kernel stores dy * (y > 0)
+// there and the apply kernel reads it in place of dy and y.
 int agb_bn_forward(void const* x, void const* residual, void* y, void const* gamma, void const* beta, void* moving_mean, void* moving_var, void* save_mean, void* save_rstd,
                    void* sums, void* scale, void* shift, long long rows, int C, int groups, float eps, float decay, int relu, void* stream) {
     return bn_forward_impl<bf16>(x, residual, y, gamma, beta, moving_mean, moving_var, save_mean, save_rstd, sums, scale, shift, rows, C, groups, eps, decay, relu, stream);

@@ -187,11 +187,9 @@ def describe(p):
 FUSED_MB = (72, 40)   # single-launch batch norm envelope, forward / backward (`nn_native.set_bn_fused_limits` defaults; no ResNet-50 tensor is under its row minimum at these sizes)
 
 
-def traffic(workers, batch, image_size):
-  """HBM bytes per step of the batch-norm passes (single launch or statistics + apply pair, as the envelope picks) and of the
-  residual-gradient passes, before and after summing the shortcut gradient in the data-gradient epilogue and recomputing the ReLU
-  mask of the pair's backward from x. A pass counts every activation it reads or writes once (bf16); per-channel vectors, and
-  the single-launch kernel's L2 re-reads of rows past its on-chip stash, are left out. Returns {category: [tensors, before, after]}."""
+def norm_layers(image_size):
+  """[((C, H, W), relu, closes)] of every batch norm of ResNet-50 in forward order (closes: the closing norm of a residual unit,
+  fused with the shortcut add and ReLU), and [(numel, shortcut kind)] of every residual unit."""
   from aggregathor_b200.engine.flat import FlatLayout
   from aggregathor_b200.models import Context, get_network
   from aggregathor_b200.models import core
@@ -209,11 +207,11 @@ def traffic(workers, batch, image_size):
   bn_forward, bn_closing, unit_forward = core.BatchNorm.forward, core.BatchNorm.forward_add_relu, core.Residual.forward
 
   def norm(self, x, c):
-    norms.append((x[0].numel(), self.relu, False))
+    norms.append((tuple(x.shape[1:]), self.relu, False))
     return bn_forward(self, x, c)
 
   def closing(self, x, shortcut, c):
-    norms.append((x[0].numel(), True, True))
+    norms.append((tuple(x.shape[1:]), True, True))
     return bn_closing(self, x, shortcut, c)
 
   def unit(self, x, c):
@@ -229,6 +227,34 @@ def traffic(workers, batch, image_size):
       model.root.forward(x, ctx)
   finally:
     core.BatchNorm.forward, core.BatchNorm.forward_add_relu, core.Residual.forward = bn_forward, bn_closing, unit_forward
+  return norms, units
+
+
+def bn_pass(S, relu, closes, backward):
+  """(pass name, activation bytes before, after) of one batch norm moving S-byte tensors, in one direction. A pass counts every
+  activation it reads or writes once; per-channel vectors, and the single-launch kernel's L2 re-reads of rows past its on-chip
+  stash, are left out."""
+  extra = S if closes else 0     # forward: the shortcut read; backward: the masked gradient written for the shortcut
+  if not backward:
+    if S <= FUSED_MB[0] << 20:   # reads x (+ shortcut) once, writes y
+      return "bn forward, single launch", 2 * S + extra, 2 * S + extra
+    return "bn forward, pair", 3 * S + extra, 3 * S + extra   # statistics read x, apply reads x (+ shortcut) and writes y
+  reads = 3 if relu else 2       # dy, x (, y for the mask)
+  if S <= FUSED_MB[1] << 20:
+    return "bn backward, single launch", (reads + 1) * S + extra, (reads + 1) * S + extra
+  if relu and not closes:        # both passes recompute the mask from x: y is no longer read
+    return "bn backward, pair, ReLU", (2 * reads + 1) * S, (2 * reads - 1) * S
+  if closes:                     # the statistics pass stores the masked gradient; the apply reads it and x instead of dy, x and y
+    return "bn backward, pair, closing", (2 * reads + 1) * S + extra, 2 * reads * S + extra
+  return "bn backward, pair, no ReLU", (2 * reads + 1) * S, (2 * reads + 1) * S
+
+
+def traffic(workers, batch, image_size):
+  """HBM bytes per step of the batch-norm passes (single launch or statistics + apply pair, as the envelope picks) and of the
+  residual-gradient passes, before and after summing the shortcut gradient in the data-gradient epilogue, recomputing the ReLU
+  mask of the pair's backward from x and masking the closing norm's gradient once in the pair's backward (`bn_pass`).
+  Returns {category: [tensors, before, after]}."""
+  norms, units = norm_layers(image_size)
   B = workers * batch
   sums = collections.OrderedDict()
 
@@ -238,20 +264,10 @@ def traffic(workers, batch, image_size):
     entry[1] += before
     entry[2] += after
 
-  for numel, relu, closes in norms:
-    S = 2 * B * numel
-    extra = S if closes else 0   # forward: the shortcut read; backward: the masked gradient written for the shortcut
-    if S <= FUSED_MB[0] << 20:   # reads x (+ shortcut) once, writes y
-      add("bn forward, single launch", 2 * S + extra, 2 * S + extra)
-    else:                        # statistics read x, apply reads x (+ shortcut) and writes y
-      add("bn forward, pair", 3 * S + extra, 3 * S + extra)
-    reads = 3 if relu else 2     # dy, x (, y for the mask)
-    if S <= FUSED_MB[1] << 20:
-      add("bn backward, single launch", (reads + 1) * S + extra, (reads + 1) * S + extra)
-    elif relu and not closes:    # both passes recompute the mask from x: y is no longer read
-      add("bn backward, pair, ReLU", (2 * reads + 1) * S, (2 * reads - 1) * S)
-    else:
-      add("bn backward, pair, %s" % ("closing (keeps y)" if closes else "no ReLU"), (2 * reads + 1) * S + extra, (2 * reads + 1) * S + extra)
+  for shape, relu, closes in norms:
+    S = 2 * B * math.prod(shape)
+    for backward in (False, True):
+      add(*bn_pass(S, relu, closes, backward))
   for numel, kind in units:
     X = 2 * B * numel
     if kind == "subsample":   # scatter into a full-size tensor (read X/4, write X) + add (2 reads, 1 write) -> in-place add of a quarter
