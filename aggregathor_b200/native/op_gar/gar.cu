@@ -3932,64 +3932,27 @@ template<int N, int VEC> int launch(GarArgs& a, int max_ctas, long long scratch_
     return 0;
 }
 
-// ptrs layout (all device addresses, 0 = absent):
-//   [0..32) gradient rows | [32] agg_out | [33] param | [34] slot0 | [35] slot1 | [36] param_mc | [37] cta_partials | [38] staging
-//   [39] dist_out | [40] info | [41] grad_mc | [42] epoch_ptr | [43] hyper_ptr | [44] seg_partials | [45] loss_in | [46] loss_out
-//   [48..64) param_dst | [64..80) signal | [80..96) mailbox | [96..112) param_bf16_dst
-//   [47] center (centered clipping) | [112] raw_dist_out (NNM) | [113] DnC step key (device int64) | [114] DnC scratch
-//   [115] arc_out (ARC: [2n] squared norms, then factors) | [116] SMEA scratch (doubles)
-//   [113] is also bucketing's step key | [117] FLTrust root r (rank 0's) | [118] FLTrust's fltrust_out
-//   [119] FoolsGold's history [n][owned] | [120] FoolsGold's foolsgold_out
-// ints: n f m beta rule R rank opt epoch max_ctas workers_per_rank nseg first_seg nloss seg_max_ctas phase_a_ctas | [16..24) seg_ctas | [24] phase_a_threads
-//       [25] iterations | [26] mix (bits: 1 NNM, 2 ARC, 4 bucketing) | [27] DnC r | [28] bucketing: s | [29] gathered rows n_rows (0: n)
-// longs: row_stride | [1..9) seg_lo | [9..17) seg_hi | DnC: [17] subsample b [18] domain D [19] seed [20] step (also bucketing's)
-//        [21] elements of the rule's scratch (DnC: floats, SMEA: doubles) | [22] bucketing: seed | [23] FoolsGold: kappa (float64 bits)
-// floats: lr h0 h1 h2 nu tau
-int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats) {
-    a.n = ints[0]; a.f = ints[1]; a.m = ints[2]; a.beta = ints[3]; a.rule = ints[4];
-    a.R = ints[5]; a.rank = ints[6]; a.opt = ints[7]; a.epoch = static_cast<uint32_t>(ints[8]);
-    a.workers_per_rank = ints[10];
-    a.nseg = ints[11]; a.first_seg = ints[12]; a.nloss = ints[13]; a.seg_max_ctas = ints[14];
-    a.iterations = ints[25];
-    a.mix = ints[26];
-    a.row_stride = longs[0];
-    a.lr = floats[0]; a.h0 = floats[1]; a.h1 = floats[2]; a.h2 = floats[3]; a.nu = floats[4]; a.tau = floats[5];
-    a.center = reinterpret_cast<float*>(ptrs[47]);
-    a.dnc_r = ints[27];
-    a.dnc_b = longs[17];
-    a.dnc_domain = longs[18];
-    a.dnc_seed = static_cast<unsigned long long>(longs[19]);
-    a.dnc_step = longs[20];
-    a.dnc_step_ptr = reinterpret_cast<long long const*>(ptrs[113]);
-    a.dnc_scratch = reinterpret_cast<float*>(ptrs[114]);
-    a.smea_scratch = reinterpret_cast<double*>(ptrs[116]);
-    a.bkt_size = ints[28];
-    a.n_rows = ints[29] != 0 ? ints[29] : a.n;
-    a.bkt_seed = static_cast<unsigned long long>(longs[22]);
+// The host checks of the fused entry points' arguments; returns a status (0: valid).
+int check_args(GarArgs const& a) {
     if (a.n < 1 || a.n > kMaxWorkers || a.n_rows < 1 || a.n_rows > kMaxWorkers || a.R < 1 || a.R > kMaxRanks || a.rank < 0 || a.rank >= a.R)
         return 100;
     if (!(a.mix & kMixBucketing) && a.n_rows != a.n)
         return 100;
     if (a.nseg < 1 || a.nseg > kMaxSeg || a.first_seg < 0 || a.first_seg > a.nseg)
         return 101;
-    for (int s = 0; s < a.nseg; ++s) {
-        a.seg_lo[s] = longs[1 + s];
-        a.seg_hi[s] = longs[1 + kMaxSeg + s];
-        a.seg_ctas[s] = ints[16 + s];
+    for (int s = 0; s < a.nseg; ++s)
         if ((a.seg_lo[s] & 3) || (a.seg_hi[s] & 3) || a.seg_hi[s] < a.seg_lo[s])
             return 101;
-    }
     if (a.rule < 0 || a.rule > kFoolsgold)
         return 102;
     // FLTrust: any 0 <= f < n, a root, no pre-aggregation (it would change the rows whose direction and norm FLTrust scores), nothing
     // pre-accumulated
-    if (a.rule == kFltrust && (a.f < 0 || a.f >= a.n || !ptrs[117] || a.mix != 0 || a.first_seg != 0))
+    if (a.rule == kFltrust && (a.f < 0 || a.f >= a.n || !a.root || a.mix != 0 || a.first_seg != 0))
         return 126;
     // FoolsGold: any 0 <= f < n, a finite kappa > 0, a history (127); no pre-aggregation (128: NNM mixes, ARC rescales and bucketing
     // reshuffles the rows every step, so a row would no longer be one worker's); nothing pre-accumulated (129: the history pass runs
     // in the finish kernel)
-    std::memcpy(&a.confidence, &longs[23], sizeof(double));
-    if (a.rule == kFoolsgold && (a.f < 0 || a.f >= a.n || !ptrs[119] || !std::isfinite(a.confidence) || !(a.confidence > 0.0)))
+    if (a.rule == kFoolsgold && (a.f < 0 || a.f >= a.n || !a.history || !std::isfinite(a.confidence) || !(a.confidence > 0.0)))
         return 127;
     if (a.rule == kFoolsgold && a.mix != 0)
         return 128;
@@ -3998,7 +3961,7 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
     if (a.mix < 0 || a.mix > (kMixNnm | kMixArc | kMixBucketing))
         return 117;
     if ((a.mix & kMixBucketing) && (a.mix != kMixBucketing || a.bkt_size < 1 || a.bkt_size > a.n_rows ||
-                                    a.n != (a.n_rows + a.bkt_size - 1) / a.bkt_size || !ptrs[38]))   // the means land in the staging tile
+                                    a.n != (a.n_rows + a.bkt_size - 1) / a.bkt_size || !a.staging))   // the means land in the staging tile
         return 123;
     if ((a.mix & kMixArc) && (a.f < 0 || 2 * a.f >= a.n))
         return 120;
@@ -4037,35 +4000,6 @@ int fill_args(GarArgs& a, unsigned long long const* ptrs, int const* ints, long 
         return 104;
     if (a.rule == kAveragedMedian && (a.beta < 1 || a.beta > a.n))
         return 105;
-    for (int i = 0; i < a.n_rows; ++i)
-        a.grad[i] = reinterpret_cast<float const*>(ptrs[i]);
-    a.agg_out = reinterpret_cast<float*>(ptrs[32]);
-    a.param = reinterpret_cast<float*>(ptrs[33]);
-    a.slot0 = reinterpret_cast<float*>(ptrs[34]);
-    a.slot1 = reinterpret_cast<float*>(ptrs[35]);
-    a.param_mc = reinterpret_cast<float*>(ptrs[36]);
-    a.cta_partials = reinterpret_cast<float*>(ptrs[37]);
-    a.staging = reinterpret_cast<float*>(ptrs[38]);
-    a.dist_out = reinterpret_cast<float*>(ptrs[39]);
-    a.info = reinterpret_cast<int*>(ptrs[40]);
-    a.grad_mc = reinterpret_cast<float const*>(ptrs[41]);
-    a.epoch_ptr = reinterpret_cast<uint32_t*>(ptrs[42]);
-    a.hyper_ptr = reinterpret_cast<float const*>(ptrs[43]);
-    a.seg_partials = reinterpret_cast<float*>(ptrs[44]);
-    a.loss_in = reinterpret_cast<float const*>(ptrs[45]);
-    a.loss_out = reinterpret_cast<float*>(ptrs[46]);
-    a.raw_dist_out = reinterpret_cast<float*>(ptrs[112]);
-    a.arc_out = reinterpret_cast<float*>(ptrs[115]);
-    a.root = reinterpret_cast<float const*>(ptrs[117]);
-    a.fltrust_out = reinterpret_cast<float*>(ptrs[118]);
-    a.history = reinterpret_cast<float*>(ptrs[119]);
-    a.foolsgold_out = reinterpret_cast<float*>(ptrs[120]);
-    for (int q = 0; q < a.R; ++q) {
-        a.param_dst[q] = reinterpret_cast<float*>(ptrs[48 + q]);
-        a.signal[q] = reinterpret_cast<uint32_t*>(ptrs[64 + q]);
-        a.mailbox[q] = reinterpret_cast<float*>(ptrs[80 + q]);
-        a.param_bf16_dst[q] = reinterpret_cast<__nv_bfloat16*>(ptrs[96 + q]);
-    }
     if (a.opt != kNone && (!a.param || (!a.param_mc && !a.param_dst[0])))
         return 106;
     if ((a.opt == kAdam || a.opt == kRmsprop || a.opt == kAdadelta) && (!a.slot0 || !a.slot1))
@@ -4128,13 +4062,15 @@ int agb_gar_region_bytes(long long* out) {
     return 0;
 }
 
-// The finish kernel (whole aggregation when nothing was pre-accumulated). See `fill_args` for the argument layout.
-int agb_gar_fused(unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats, void* stream) {
-    GarArgs a{};
-    int const status = fill_args(a, ptrs, ints, longs, floats);
+// The finish kernel (whole aggregation when nothing was pre-accumulated), on at most `max_ctas` CTAs (0: no bound); the DnC and SMEA
+// scratch holds `scratch_elems` elements (DnC: floats, SMEA: doubles). `args` points to a `GarArgs` (typed `void const*` since a
+// parameter of a type of this file's anonymous namespace would hide the export); its entries past the n_rows rows, the R ranks and the
+// nseg segments are null or zero.
+int agb_gar_fused(void const* args, int max_ctas, long long scratch_elems, void* stream) {
+    GarArgs a = *static_cast<GarArgs const*>(args);
+    int const status = check_args(a);
     if (status)
         return status;
-    int const max_ctas = ints[9];
     long long total = 0;
     for (int s = 0; s < a.nseg; ++s)
         total += a.seg_hi[s] - a.seg_lo[s];
@@ -4144,20 +4080,19 @@ int agb_gar_fused(unsigned long long const* ptrs, int const* ints, long long con
     // the instance follows the rule's n rows (with bucketing n <= n_rows; the mean pass loops over the gathered rows), so the rule adds
     // in the same order as on n plain rows
     if (a.n <= 8)
-        return launch<8, 4>(a, max_ctas, longs[21], s);
+        return launch<8, 4>(a, max_ctas, scratch_elems, s);
     if (a.n <= 16)
-        return launch<16, 4>(a, max_ctas, longs[21], s);
-    return launch<32, 1>(a, max_ctas, longs[21], s);
+        return launch<16, 4>(a, max_ctas, scratch_elems, s);
+    return launch<32, 1>(a, max_ctas, scratch_elems, s);
 }
 
 // Phase A (partial pairwise distances + local staging) of owned segment `seg` alone, on `ctas` CTAs: launched on a side stream as soon as
 // the backward pass has produced that bucket of gradients; the finish kernel is then called with first_seg > seg.
-int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long const* longs, float const* floats, int seg, void* stream) {
-    GarArgs a{};
-    int const status = fill_args(a, ptrs, ints, longs, floats);
+int agb_gar_phase_a(void const* args, int seg, int ctas, int threads, void* stream) {
+    GarArgs const& a = *static_cast<GarArgs const*>(args);
+    int const status = check_args(a);
     if (status)
         return status;
-    int const ctas = ints[15];
     if (a.rule == kFoolsgold)
         return 129;
     if (seg < 0 || seg >= a.nseg || ctas < 1 || ctas > a.seg_max_ctas || !a.seg_partials || (a.rule != kKrum && a.rule != kBulyan && a.rule != kMda && a.rule != kSmea) ||
@@ -4166,7 +4101,7 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // small CTAs: a 64-thread CTA (8 K registers, 13 KB of static shared memory) fits beside a persistent GEMM CTA of the backward pass
     // (320 threads x 168 registers, ~198 KB), so the distance pass shares SMs with it instead of taking them away
-    int threads = ints[24] >= 32 && ints[24] <= 256 ? (ints[24] / 32) * 32 : 64;
+    threads = threads >= 32 && threads <= 256 ? (threads / 32) * 32 : 64;
     if (a.n <= kBlockRows)
         gar_phase_a_kernel<false><<<ctas, threads, 0, s>>>(a, seg);
     else
@@ -4175,252 +4110,31 @@ int agb_gar_phase_a(unsigned long long const* ptrs, int const* ints, long long c
     return 0;
 }
 
-// Omniscient Byzantine rows (ALIE: mode 0, coef = z; IPM: mode 1, coef = epsilon) over this rank's owned segments; see
-// `gar_byzantine_kernel`. `rows`: n row addresses; `honest` / `byzantine`: disjoint slot masks; `signals`: R signal pads (R > 1);
-// flags use *epoch_ptr + 1 when `epoch_ptr` is set, `epoch` otherwise. Collective when R > 1: every rank calls it.
-int agb_gar_byzantine(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
-                      unsigned byzantine, int mode, float coef, int R, int rank, unsigned long long const* signals, unsigned epoch,
-                      unsigned long long epoch_ptr, void* stream) {
+// The host prologue of the five crafting entry points: checks the workers, ranks and rank (100), the segment count (101), then returns
+// `before_masks` if nonzero (an export's own check of its mode), checks the slot masks (114: disjoint, inside [0, n), at least one
+// Byzantine slot), returns `after_masks` if nonzero, checks the segment bounds (101) and, rank by rank, the signal pads (109, R > 1) and,
+// with `need_mailboxes`, the mailboxes (108). It fills the rows (the honest ones also as `grad` [0, H) with n = H, for
+// `phase_a_segment`), the slot masks, the owned segments (`work`: their float4 count), the ranks, their signal pads and mailboxes and the
+// epoch. Returns a status.
+static int craft_args(ByzArgs& a, unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg,
+                      unsigned honest, unsigned byzantine, int before_masks, int after_masks, int R, int rank,
+                      unsigned long long const* signals, unsigned long long const* mailboxes, bool need_mailboxes, unsigned epoch,
+                      unsigned long long epoch_ptr, long long& work) {
     if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
         return 100;
     if (nseg < 1 || nseg > kMaxSeg)
         return 101;
+    if (before_masks)
+        return before_masks;
     unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
-    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
-    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < (mode == kAlie ? 2 : 1) || (mode != kAlie && mode != kIpm))
+    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || !byzantine)
         return 114;
-    ByzArgs a{};
-    a.H = H;
-    a.K = K;
-    for (int i = 0, h = 0, b = 0; i < n; ++i) {
-        a.rows[i] = reinterpret_cast<float*>(rows[i]);
-        if ((honest >> i) & 1u)
-            a.honest[h++] = i;
-        if ((byzantine >> i) & 1u)
-            a.byz[b++] = i;
-    }
-    a.mode = mode;
-    a.coef = coef;
-    a.nseg = nseg;
-    long long work = 0;
-    for (int s = 0; s < nseg; ++s) {
-        a.seg_lo[s] = seg_lo[s];
-        a.seg_hi[s] = seg_hi[s];
-        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
-            return 101;
-        work += (seg_hi[s] - seg_lo[s]) / 4;
-    }
-    a.R = R;
-    a.rank = rank;
-    for (int q = 0; q < R; ++q) {
-        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
-        if (R > 1 && !a.signal[q])
-            return 109;
-    }
-    a.epoch = epoch;
-    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
-    if (work == 0 && R == 1)
-        return 0;
-    int const threads = 256;
-    long long grid = (work + threads - 1) / threads;
-    long long const cap = static_cast<long long>(agb::sm_count()) * 8;
-    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (H <= kBlockRows)
-        gar_byzantine_kernel<kBlockRows><<<static_cast<int>(grid), threads, 0, s>>>(a);
-    else
-        gar_byzantine_kernel<0><<<static_cast<int>(grid), threads, 0, s>>>(a);
-    AGB_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
-// Min-Max (mode 2) / Min-Sum (mode 3) with deviation 0 unit-vec, 1 sign, 2 std, over this rank's owned segments; see
-// `gar_optimized_kernel`. Arguments as `agb_gar_byzantine`, plus: `mailboxes`: R mailbox addresses (every rank's, its own at `rank`);
-// `partials`: [partial_ctas][561] floats of scratch (the grid never exceeds partial_ctas CTAs); `stats_out`: optional [562] floats,
-// gamma then the statistics summed over the ranks ([0, 496) honest pair distances, [496, 528) A_i, [528, 560) B_i, [560] C).
-// Cooperative launch; collective when R > 1.
-int agb_gar_byzantine_optimized(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
-                                unsigned byzantine, int mode, int deviation, int R, int rank, unsigned long long const* signals,
-                                unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long stats_out,
-                                unsigned epoch, unsigned long long epoch_ptr, void* stream) {
-    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
-        return 100;
-    if (nseg < 1 || nseg > kMaxSeg)
-        return 101;
-    if ((mode != kMinMax && mode != kMinSum) || deviation < kUnitVec || deviation > kStd)
-        return 118;
-    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
-    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
-    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < 2)
-        return 114;
-    ByzArgs a{};
-    a.H = H;
-    a.K = K;
-    a.n = H;
-    for (int i = 0, h = 0, b = 0; i < n; ++i) {
-        a.rows[i] = reinterpret_cast<float*>(rows[i]);
-        if ((honest >> i) & 1u) {
-            a.grad[h] = a.rows[i];
-            a.honest[h++] = i;
-        }
-        if ((byzantine >> i) & 1u)
-            a.byz[b++] = i;
-    }
-    a.mode = mode;
-    a.deviation = deviation;
-    a.nseg = nseg;
-    long long work = 0;
-    for (int s = 0; s < nseg; ++s) {
-        a.seg_lo[s] = seg_lo[s];
-        a.seg_hi[s] = seg_hi[s];
-        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
-            return 101;
-        work += (seg_hi[s] - seg_lo[s]) / 4;
-    }
-    a.R = R;
-    a.rank = rank;
-    for (int q = 0; q < R; ++q) {
-        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
-        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
-        if (R > 1 && !a.signal[q])
-            return 109;
-        if (!a.mailbox[q])
-            return 108;
-    }
-    a.partials = reinterpret_cast<float*>(partials);
-    a.stats_out = reinterpret_cast<float*>(stats_out);
-    if (!a.partials || partial_ctas < 1)
-        return 108;
-    a.epoch = epoch;
-    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
-    // the grid depends only on the owned work (and the device): the fused engine at R = 1 and the stand-alone op on the same rows fold
-    // the same partials in the same order
-    int const threads = 256;
-    bool const in_registers = H <= kBlockRows;
-    int per_sm = 0;
-    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_optimized_kernel<kBlockRows> : gar_optimized_kernel<0>,
-                                                              threads, 0));
-    if (per_sm < 1)
-        return 2;
-    long long grid = (work + threads - 1) / threads;
-    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
-    cap = cap > partial_ctas ? partial_ctas : cap;
-    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
-    void* params[] = {&a};
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_optimized_kernel<kBlockRows>)
-                                                         : reinterpret_cast<void*>(gar_optimized_kernel<0>),
-                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
-    return 0;
-}
-
-// Mimic over this rank's owned segments; see `gar_mimic_warmup_kernel`. Arguments as `agb_gar_byzantine_optimized`, plus: `warmup`: 1 runs
-// the warm-up update number t + 1 (`z`, `y`: local fp32 buffers of the owned coordinates, segments back to back: the direction estimate
-// and its scratch), 0 the copy pass alone;
-// `istar`: [1] local int32, the target slot, read and (warm-up) written; `stats_out`: optional [66] float64, s_i [0, 32), q_i [32, 64),
-// ||y||^2 [64], 1 / ||y|| [65]. The warm-up is a cooperative launch. Collective when R > 1.
-int agb_gar_byzantine_mimic(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
-                            unsigned byzantine, int warmup, int t, int R, int rank, unsigned long long const* signals,
-                            unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long z,
-                            unsigned long long y, unsigned long long istar, unsigned long long stats_out, unsigned epoch,
-                            unsigned long long epoch_ptr, void* stream) {
-    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
-        return 100;
-    if (nseg < 1 || nseg > kMaxSeg)
-        return 101;
-    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
-    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
-    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1)
-        return 114;
-    if (H < 2 || (warmup != 0 && warmup != 1) || t < 0 || t >= (1 << 24) || !istar || (warmup && (!z || !y)))
-        return 124;
-    ByzArgs a{};
-    a.H = H;
-    a.K = K;
+    if (after_masks)
+        return after_masks;
+    a.H = __builtin_popcount(honest);
+    a.K = __builtin_popcount(byzantine);
+    a.n = a.H;
     a.honest_mask = honest;
-    for (int i = 0, h = 0, b = 0; i < n; ++i) {
-        a.rows[i] = reinterpret_cast<float*>(rows[i]);
-        if ((honest >> i) & 1u)
-            a.honest[h++] = i;
-        if ((byzantine >> i) & 1u)
-            a.byz[b++] = i;
-    }
-    a.nseg = nseg;
-    long long work = 0;
-    for (int s = 0; s < nseg; ++s) {
-        a.seg_lo[s] = seg_lo[s];
-        a.seg_hi[s] = seg_hi[s];
-        if ((seg_lo[s] & 3) || (seg_hi[s] & 3) || seg_hi[s] < seg_lo[s])
-            return 101;
-        work += (seg_hi[s] - seg_lo[s]) / 4;
-    }
-    a.R = R;
-    a.rank = rank;
-    for (int q = 0; q < R; ++q) {
-        a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
-        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
-        if (R > 1 && !a.signal[q])
-            return 109;
-        if (warmup && !a.mailbox[q])
-            return 108;
-    }
-    a.t = t;
-    a.z = reinterpret_cast<float*>(z);
-    a.y = reinterpret_cast<float*>(y);
-    a.istar = reinterpret_cast<int*>(istar);
-    a.mimic_stats = reinterpret_cast<double*>(stats_out);
-    a.partials = reinterpret_cast<float*>(partials);
-    a.epoch = epoch;
-    a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
-    int const threads = 256;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (!warmup) {
-        if (work == 0 && R == 1)
-            return 0;
-        long long grid = (work + threads - 1) / threads;
-        long long const cap = static_cast<long long>(agb::sm_count()) * 8;
-        grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
-        gar_mimic_copy_kernel<<<static_cast<int>(grid), threads, 0, s>>>(a);
-        AGB_CUDA_OK(cudaGetLastError());
-        return 0;
-    }
-    if (!a.partials || partial_ctas < 1)
-        return 108;
-    // the grid depends only on the owned work (and the device): the fused engine at R = 1 and the stand-alone op on the same rows fold
-    // the same partials in the same order
-    bool const in_registers = H <= kBlockRows;
-    int per_sm = 0;
-    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_mimic_warmup_kernel<kBlockRows> : gar_mimic_warmup_kernel<0>,
-                                                              threads, 0));
-    if (per_sm < 1)
-        return 2;
-    long long grid = (work + threads - 1) / threads;
-    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
-    cap = cap > partial_ctas ? partial_ctas : cap;
-    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
-    void* params[] = {&a};
-    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_mimic_warmup_kernel<kBlockRows>)
-                                                         : reinterpret_cast<void*>(gar_mimic_warmup_kernel<0>),
-                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
-    return 0;
-}
-
-// The arguments the Fang kernels share with `agb_gar_byzantine`: the rows (honest ones also as `grad` for `phase_a_segment`), the slot
-// masks, the owned segments (`work`: their float4 count), the ranks and their signal pads. Returns a status.
-static int fang_args(ByzArgs& a, unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg,
-                     unsigned honest, unsigned byzantine, int R, int rank, unsigned long long const* signals, unsigned epoch,
-                     unsigned long long epoch_ptr, long long& work) {
-    if (n < 1 || n > kMaxWorkers || R < 1 || R > kMaxRanks || rank < 0 || rank >= R)
-        return 100;
-    if (nseg < 1 || nseg > kMaxSeg)
-        return 101;
-    unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
-    int const H = __builtin_popcount(honest), K = __builtin_popcount(byzantine);
-    if ((honest & byzantine) || (honest & ~all) || (byzantine & ~all) || K < 1 || H < 1)
-        return 114;
-    a.H = H;
-    a.K = K;
-    a.n = H;
     for (int i = 0, h = 0, b = 0; i < n; ++i) {
         a.rows[i] = reinterpret_cast<float*>(rows[i]);
         if ((honest >> i) & 1u) {
@@ -4443,12 +4157,134 @@ static int fang_args(ByzArgs& a, unsigned long long const* rows, int n, long lon
     a.rank = rank;
     for (int q = 0; q < R; ++q) {
         a.signal[q] = reinterpret_cast<uint32_t*>(signals ? signals[q] : 0ull);
+        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
         if (R > 1 && !a.signal[q])
             return 109;
+        if (need_mailboxes && !a.mailbox[q])
+            return 108;
     }
     a.epoch = epoch;
     a.epoch_ptr = reinterpret_cast<uint32_t*>(epoch_ptr);
     return 0;
+}
+
+constexpr int kCraftThreads = 256;
+
+// Grid of a plain crafting launch: one thread per float4 of the owned work, at most 8 CTAs per SM, and at least one CTA: a rank without
+// owned coordinates still signals its peers.
+static int plain_grid(long long work) {
+    long long const grid = (work + kCraftThreads - 1) / kCraftThreads;
+    long long const cap = static_cast<long long>(agb::sm_count()) * 8;
+    return static_cast<int>(grid < 1 ? 1 : grid > cap ? cap : grid);
+}
+
+// Cooperative launch of a crafting kernel over `work` float4s: at most the CTAs that fit on the device at once and `partial_ctas` (the
+// CTA slots of the scratch), and at least one CTA: a rank without owned coordinates still posts and signals. The grid depends only on the
+// owned work (and the device): the fused engine at R = 1 and the stand-alone op on the same rows fold the same partials in the same order.
+static int launch_cooperative(void const* kernel, ByzArgs& a, long long work, int partial_ctas, cudaStream_t stream) {
+    int per_sm = 0;
+    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kCraftThreads, 0));
+    if (per_sm < 1)
+        return 2;
+    long long grid = (work + kCraftThreads - 1) / kCraftThreads;
+    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
+    cap = cap > partial_ctas ? partial_ctas : cap;
+    grid = grid < 1 ? 1 : grid > cap ? cap : grid;
+    void* params[] = {&a};
+    AGB_CUDA_OK(cudaLaunchCooperativeKernel(kernel, dim3(static_cast<unsigned>(grid)), dim3(kCraftThreads), params, 0, stream));
+    return 0;
+}
+
+// Omniscient Byzantine rows (ALIE: mode 0, coef = z; IPM: mode 1, coef = epsilon) over this rank's owned segments; see
+// `gar_byzantine_kernel`. `rows`: n row addresses; `honest` / `byzantine`: disjoint slot masks; `signals`: R signal pads (R > 1);
+// flags use *epoch_ptr + 1 when `epoch_ptr` is set, `epoch` otherwise. Collective when R > 1: every rank calls it.
+int agb_gar_byzantine(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                      unsigned byzantine, int mode, float coef, int R, int rank, unsigned long long const* signals, unsigned epoch,
+                      unsigned long long epoch_ptr, void* stream) {
+    bool const bad_rows = __builtin_popcount(honest) < (mode == kAlie ? 2 : 1) || (mode != kAlie && mode != kIpm);
+    ByzArgs a{};
+    long long work = 0;
+    int const status = craft_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, 0, bad_rows ? 114 : 0, R, rank, signals, nullptr,
+                                  false, epoch, epoch_ptr, work);
+    if (status)
+        return status;
+    a.mode = mode;
+    a.coef = coef;
+    if (work == 0 && R == 1)
+        return 0;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (a.H <= kBlockRows)
+        gar_byzantine_kernel<kBlockRows><<<plain_grid(work), kCraftThreads, 0, s>>>(a);
+    else
+        gar_byzantine_kernel<0><<<plain_grid(work), kCraftThreads, 0, s>>>(a);
+    AGB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// Min-Max (mode 2) / Min-Sum (mode 3) with deviation 0 unit-vec, 1 sign, 2 std, over this rank's owned segments; see
+// `gar_optimized_kernel`. Arguments as `agb_gar_byzantine`, plus: `mailboxes`: R mailbox addresses (every rank's, its own at `rank`);
+// `partials`: [partial_ctas][561] floats of scratch (the grid never exceeds partial_ctas CTAs); `stats_out`: optional [562] floats,
+// gamma then the statistics summed over the ranks ([0, 496) honest pair distances, [496, 528) A_i, [528, 560) B_i, [560] C).
+// Cooperative launch; collective when R > 1.
+int agb_gar_byzantine_optimized(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                                unsigned byzantine, int mode, int deviation, int R, int rank, unsigned long long const* signals,
+                                unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long stats_out,
+                                unsigned epoch, unsigned long long epoch_ptr, void* stream) {
+    bool const bad_mode = (mode != kMinMax && mode != kMinSum) || deviation < kUnitVec || deviation > kStd;
+    ByzArgs a{};
+    long long work = 0;
+    int const status = craft_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, bad_mode ? 118 : 0,
+                                  __builtin_popcount(honest) < 2 ? 114 : 0, R, rank, signals, mailboxes, true, epoch, epoch_ptr, work);
+    if (status)
+        return status;
+    a.mode = mode;
+    a.deviation = deviation;
+    a.partials = reinterpret_cast<float*>(partials);
+    a.stats_out = reinterpret_cast<float*>(stats_out);
+    if (!a.partials || partial_ctas < 1)
+        return 108;
+    return launch_cooperative(a.H <= kBlockRows ? reinterpret_cast<void const*>(gar_optimized_kernel<kBlockRows>)
+                                                : reinterpret_cast<void const*>(gar_optimized_kernel<0>),
+                              a, work, partial_ctas, static_cast<cudaStream_t>(stream));
+}
+
+// Mimic over this rank's owned segments; see `gar_mimic_warmup_kernel`. Arguments as `agb_gar_byzantine_optimized`, plus: `warmup`: 1 runs
+// the warm-up update number t + 1 (`z`, `y`: local fp32 buffers of the owned coordinates, segments back to back: the direction estimate
+// and its scratch), 0 the copy pass alone;
+// `istar`: [1] local int32, the target slot, read and (warm-up) written; `stats_out`: optional [66] float64, s_i [0, 32), q_i [32, 64),
+// ||y||^2 [64], 1 / ||y|| [65]. The warm-up is a cooperative launch. Collective when R > 1.
+int agb_gar_byzantine_mimic(unsigned long long const* rows, int n, long long const* seg_lo, long long const* seg_hi, int nseg, unsigned honest,
+                            unsigned byzantine, int warmup, int t, int R, int rank, unsigned long long const* signals,
+                            unsigned long long const* mailboxes, unsigned long long partials, int partial_ctas, unsigned long long z,
+                            unsigned long long y, unsigned long long istar, unsigned long long stats_out, unsigned epoch,
+                            unsigned long long epoch_ptr, void* stream) {
+    bool const bad_args = __builtin_popcount(honest) < 2 || (warmup != 0 && warmup != 1) || t < 0 || t >= (1 << 24) || !istar ||
+                          (warmup && (!z || !y));
+    ByzArgs a{};
+    long long work = 0;
+    int const status = craft_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, 0, bad_args ? 124 : 0, R, rank, signals, mailboxes,
+                                  warmup != 0, epoch, epoch_ptr, work);
+    if (status)
+        return status;
+    a.t = t;
+    a.z = reinterpret_cast<float*>(z);
+    a.y = reinterpret_cast<float*>(y);
+    a.istar = reinterpret_cast<int*>(istar);
+    a.mimic_stats = reinterpret_cast<double*>(stats_out);
+    a.partials = reinterpret_cast<float*>(partials);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (!warmup) {
+        if (work == 0 && R == 1)
+            return 0;
+        gar_mimic_copy_kernel<<<plain_grid(work), kCraftThreads, 0, s>>>(a);
+        AGB_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+    if (!a.partials || partial_ctas < 1)
+        return 108;
+    return launch_cooperative(a.H <= kBlockRows ? reinterpret_cast<void const*>(gar_mimic_warmup_kernel<kBlockRows>)
+                                                : reinterpret_cast<void const*>(gar_mimic_warmup_kernel<0>),
+                              a, work, partial_ctas, s);
 }
 
 // fang-krum over this rank's owned segments; see `gar_fang_krum_kernel`. Arguments as `agb_gar_byzantine_optimized`, plus: `f`: the rule's
@@ -4461,7 +4297,8 @@ int agb_gar_byzantine_fang_krum(unsigned long long const* rows, int n, long long
                                 unsigned long long fang_out, unsigned epoch, unsigned long long epoch_ptr, void* stream) {
     ByzArgs a{};
     long long work = 0;
-    int const status = fang_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, R, rank, signals, epoch, epoch_ptr, work);
+    int const status = craft_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, 0, honest ? 0 : 114, R, rank, signals, mailboxes,
+                                  false, epoch, epoch_ptr, work);
     if (status)
         return status;
     unsigned const all = n == 32 ? 0xffffffffu : (1u << n) - 1u;
@@ -4471,34 +4308,17 @@ int agb_gar_byzantine_fang_krum(unsigned long long const* rows, int n, long long
     a.f = f;
     a.coef = threshold;
     a.search = search ? 1 : 0;
-    for (int q = 0; q < R; ++q) {
-        a.mailbox[q] = reinterpret_cast<float*>(mailboxes ? mailboxes[q] : 0ull);
+    for (int q = 0; q < R; ++q)
         if (!a.mailbox[q])
             return 108;
-    }
     a.partials = reinterpret_cast<float*>(partials);
     a.stats_out = reinterpret_cast<float*>(stats_out);
     a.fang_out = reinterpret_cast<double*>(fang_out);
     if (!a.partials || partial_ctas < 1)
         return 108;
-    // the grid depends only on the owned work (and the device), as for `gar_optimized_kernel`
-    int const threads = 256;
-    bool const in_registers = a.H <= kBlockRows;
-    int per_sm = 0;
-    AGB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, in_registers ? gar_fang_krum_kernel<kBlockRows> : gar_fang_krum_kernel<0>,
-                                                              threads, 0));
-    if (per_sm < 1)
-        return 2;
-    long long grid = (work + threads - 1) / threads;
-    long long cap = static_cast<long long>(agb::sm_count()) * per_sm;
-    cap = cap > partial_ctas ? partial_ctas : cap;
-    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still posts and signals
-    void* params[] = {&a};
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    AGB_CUDA_OK(cudaLaunchCooperativeKernel(in_registers ? reinterpret_cast<void*>(gar_fang_krum_kernel<kBlockRows>)
-                                                         : reinterpret_cast<void*>(gar_fang_krum_kernel<0>),
-                                            dim3(static_cast<unsigned>(grid)), dim3(threads), params, 0, s));
-    return 0;
+    return launch_cooperative(a.H <= kBlockRows ? reinterpret_cast<void const*>(gar_fang_krum_kernel<kBlockRows>)
+                                                : reinterpret_cast<void const*>(gar_fang_krum_kernel<0>),
+                              a, work, partial_ctas, static_cast<cudaStream_t>(stream));
 }
 
 // fang-trim over this rank's owned segments; see `gar_fang_trim_kernel`. Arguments as `agb_gar_byzantine`, plus: `scale`: beta, finite and
@@ -4508,7 +4328,8 @@ int agb_gar_byzantine_fang_trim(unsigned long long const* rows, int n, long long
                                 unsigned epoch, unsigned long long epoch_ptr, void* stream) {
     ByzArgs a{};
     long long work = 0;
-    int const status = fang_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, R, rank, signals, epoch, epoch_ptr, work);
+    int const status = craft_args(a, rows, n, seg_lo, seg_hi, nseg, honest, byzantine, 0, honest ? 0 : 114, R, rank, signals, nullptr,
+                                  false, epoch, epoch_ptr, work);
     if (status)
         return status;
     if (!(scale > 1.f) || !std::isfinite(scale))
@@ -4517,15 +4338,11 @@ int agb_gar_byzantine_fang_trim(unsigned long long const* rows, int n, long long
     a.key = key;
     if (work == 0 && R == 1)
         return 0;
-    int const threads = 256;
-    long long grid = (work + threads - 1) / threads;
-    long long const cap = static_cast<long long>(agb::sm_count()) * 8;
-    grid = grid < 1 ? 1 : grid > cap ? cap : grid;   // at least one CTA: a rank without owned coordinates still signals its peers
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (a.H <= kBlockRows)
-        gar_fang_trim_kernel<kBlockRows><<<static_cast<int>(grid), threads, 0, s>>>(a);
+        gar_fang_trim_kernel<kBlockRows><<<plain_grid(work), kCraftThreads, 0, s>>>(a);
     else
-        gar_fang_trim_kernel<0><<<static_cast<int>(grid), threads, 0, s>>>(a);
+        gar_fang_trim_kernel<0><<<plain_grid(work), kCraftThreads, 0, s>>>(a);
     AGB_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -7,8 +7,8 @@ the reference, which only ever had a CPU kernel: `native/op_krum/op.cpp:98-107`)
 """
 
 import ctypes
+import functools
 import os
-import struct
 
 import torch
 
@@ -21,34 +21,18 @@ MAX_RANKS = 16
 MAX_PAIRS = MAX_WORKERS * (MAX_WORKERS - 1) // 2
 MAX_SEGMENTS = 8
 MAX_ITERATIONS = 16   # geometric median, centered clipping: iterations
-# per segment: bucket entry; then exchange, exit, Byzantine crafting entry; one per iteration; NNM's exchange; Min-Max / Min-Sum's exchange
-# (mimic's first); DnC's exchange; ARC's exchange; mimic's second exchange; FLTrust's exchange; FoolsGold's exchange
-FLAG_SLOTS = MAX_SEGMENTS + 3 + MAX_ITERATIONS + 7
-SIGNAL_BYTES = FLAG_SLOTS * MAX_RANKS * 4
 # Min-Max / Min-Sum statistics of one rank: honest pair distances [0, 496), A_i [496, 528), B_i [528, 560), C [560]; mimic posts into the
 # same region: s_i [0, 32) in its first exchange, q_i [32, 64) and ||y||^2 [64] in its second
 CRAFT_STATS = MAX_PAIRS + 2 * MAX_WORKERS + 1
 # mimic's statistics of a warm-up step (float64): s_i [0, 32), q_i [32, 64), ||y||^2 [64], 1 / ||y|| [65]
 MIMIC_STATS = 2 * MAX_WORKERS + 2
 DNC_MAX_ITERATIONS = 8
-# DnC's post of one rank: the sampled distances of every iteration ([DNC_MAX_ITERATIONS][MAX_PAIRS]), then the loss
-DNC_STATS = DNC_MAX_ITERATIONS * MAX_PAIRS + 1
-# ARC's post of one rank: the partial squared norms of the rows ([MAX_WORKERS]), then the loss
-ARC_STATS = MAX_WORKERS + 1
-# FLTrust's post of one rank: P_i [0, 32), N_i [32, 64), N0 [64], then the loss
-FLTRUST_STATS = 2 * MAX_WORKERS + 2
-# FoolsGold's post of one rank: the sums P_ij, i <= j, row-major upper triangle [0, n (n + 1) / 2), the bad-row flags [528, 560), the loss
+# FoolsGold's sums P_ij, i <= j, row-major upper triangle [0, n (n + 1) / 2)
 FOOLSGOLD_SUMS = MAX_WORKERS * (MAX_WORKERS + 1) // 2
-FOOLSGOLD_STATS = FOOLSGOLD_SUMS + MAX_WORKERS + 1
-# seven regions: the rule's exchanges, NNM's exchange, Min-Max / Min-Sum's statistics, DnC's sampled distances, ARC's squared norms,
-# FLTrust's sums, FoolsGold's sums
-MAILBOX_BYTES = (2 * MAX_RANKS * (MAX_PAIRS + 1) + MAX_RANKS * CRAFT_STATS + MAX_RANKS * DNC_STATS + MAX_RANKS * ARC_STATS
-                 + MAX_RANKS * FLTRUST_STATS + MAX_RANKS * FOOLSGOLD_STATS) * 4
 # FLTrust's sums and coefficients of the last launch: P [0, 32), N [32, 64), N0 [64], a [65, 97)
 FLTRUST_OUT = 3 * MAX_WORKERS + 1
 # FoolsGold's of the last launch: the sums [0, n (n + 1) / 2), the bad-row flags [528, 560), c [560, 592)
 FOOLSGOLD_OUT = FOOLSGOLD_SUMS + 2 * MAX_WORKERS
-PTRS = 121
 # [0]: theta, [1, 1 + theta): selection masks; [32, 34): SMEA's winning score (float64 bits); [64, 64 + n): NNM masks;
 # [96, 96 + T): DnC's mask of every iteration; bucketing: [128, 128 + n_rows) the permutation, [160, 160 + n') the bucket masks
 INFO_INTS = 192
@@ -101,8 +85,42 @@ def max_ctas():
   return int(_lib().agb_gar_max_ctas())
 
 
+@functools.lru_cache(maxsize=None)
+def region_bytes():
+  """(signal pad, mailbox) bytes of one rank's communication regions, as the kernels lay them out."""
+  out = (ctypes.c_longlong * 2)()
+  _lib().agb_gar_region_bytes(out)
+  return int(out[0]), int(out[1])
+
+
+_ADDR = ctypes.c_ulonglong   # a pointer field of `GarArgs`: any integer address
+
+
+class GarArgs(ctypes.Structure):
+  """The arguments of the fused entry points: a field-for-field mirror of `struct GarArgs` in `native/op_gar/gar.cu` (see there for
+  what each field means). Every pointer is a device address (`_ADDR`), 0 when absent."""
+  _fields_ = [
+    ("n", ctypes.c_int), ("f", ctypes.c_int), ("m", ctypes.c_int), ("beta", ctypes.c_int), ("rule", ctypes.c_int),
+    ("n_rows", ctypes.c_int), ("bkt_size", ctypes.c_int), ("bkt_seed", ctypes.c_ulonglong), ("R", ctypes.c_int), ("rank", ctypes.c_int),
+    ("nseg", ctypes.c_int), ("first_seg", ctypes.c_int), ("seg_lo", ctypes.c_longlong * MAX_SEGMENTS),
+    ("seg_hi", ctypes.c_longlong * MAX_SEGMENTS), ("seg_ctas", ctypes.c_int * MAX_SEGMENTS), ("seg_max_ctas", ctypes.c_int),
+    ("grad", _ADDR * MAX_WORKERS), ("grad_mc", _ADDR), ("workers_per_rank", ctypes.c_int),
+    ("row_stride", ctypes.c_longlong), ("agg_out", _ADDR), ("opt", ctypes.c_int), ("lr", ctypes.c_float), ("h0", ctypes.c_float),
+    ("h1", ctypes.c_float), ("h2", ctypes.c_float), ("hyper_ptr", _ADDR), ("param", _ADDR), ("slot0", _ADDR),
+    ("slot1", _ADDR), ("param_dst", _ADDR * MAX_RANKS), ("param_mc", _ADDR),
+    ("param_bf16_dst", _ADDR * MAX_RANKS), ("signal", _ADDR * MAX_RANKS), ("mailbox", _ADDR * MAX_RANKS),
+    ("epoch", ctypes.c_uint32), ("epoch_ptr", _ADDR), ("cta_partials", _ADDR), ("seg_partials", _ADDR),
+    ("staging", _ADDR), ("dist_out", _ADDR), ("raw_dist_out", _ADDR), ("info", _ADDR),
+    ("loss_in", _ADDR), ("nloss", ctypes.c_int), ("loss_out", _ADDR), ("iterations", ctypes.c_int),
+    ("nu", ctypes.c_float), ("tau", ctypes.c_float), ("center", _ADDR), ("mix", ctypes.c_int), ("arc_out", _ADDR),
+    ("dnc_r", ctypes.c_int), ("dnc_b", ctypes.c_longlong), ("dnc_domain", ctypes.c_longlong), ("dnc_seed", ctypes.c_ulonglong),
+    ("dnc_step", ctypes.c_longlong), ("dnc_step_ptr", _ADDR), ("dnc_scratch", _ADDR), ("smea_scratch", _ADDR),
+    ("root", _ADDR), ("fltrust_out", _ADDR), ("history", _ADDR), ("foolsgold_out", _ADDR),
+    ("confidence", ctypes.c_double)]
+
+
 class FusedLauncher:
-  """Holds the scratch buffers and argument arrays of one rank's fused aggregation kernels (phase A kernels + finish kernel)."""
+  """Holds the scratch buffers of one rank's fused aggregation kernels (phase A kernels + finish kernel) and fills their `GarArgs`."""
 
   def __init__(self, device, n, phase_a_ctas=132, phase_a_threads=128):
     if n > MAX_WORKERS:
@@ -115,7 +133,7 @@ class FusedLauncher:
     self.phase_a_threads = int(os.environ.get("AGB_PHASE_A_THREADS", phase_a_threads))
     self.cta_partials = torch.zeros(ctas * MAX_PAIRS, dtype=torch.float32, device=self.device)
     self.seg_partials = torch.zeros(MAX_SEGMENTS * self.phase_a_ctas * MAX_PAIRS, dtype=torch.float32, device=self.device)
-    self.local_mailbox = torch.zeros(MAILBOX_BYTES // 4, dtype=torch.float32, device=self.device)
+    self.local_mailbox = torch.zeros(region_bytes()[1] // 4, dtype=torch.float32, device=self.device)
     self.dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)
     self.geo_dist_out = torch.zeros(MAX_ITERATIONS * n, dtype=torch.float32, device=self.device)   # iterative rules: D of every iteration, [T, n]
     self.raw_dist_out = torch.zeros(n * n, dtype=torch.float32, device=self.device)   # NNM: distances of the raw rows
@@ -135,13 +153,11 @@ class FusedLauncher:
     self.fltrust_out = torch.zeros(FLTRUST_OUT, dtype=torch.float32, device=self.device)   # FLTrust: P, N, N0, a
     self.foolsgold_out = torch.zeros(FOOLSGOLD_OUT, dtype=torch.float32, device=self.device)   # FoolsGold: P, bad, c
     self._mimic_y = None
-    self._ptrs = (ctypes.c_ulonglong * PTRS)()
-    self._ints = (ctypes.c_int * 32)()
-    self._longs = (ctypes.c_longlong * (1 + 2 * MAX_SEGMENTS + 7))()
-    self._floats = (ctypes.c_float * 6)()
     self._func = _lib().agb_gar_fused
+    self._func.argtypes = [ctypes.POINTER(GarArgs), ctypes.c_int, ctypes.c_longlong, ctypes.c_void_p]
     self._func.restype = ctypes.c_int
     self._phase_a = _lib().agb_gar_phase_a
+    self._phase_a.argtypes = [ctypes.POINTER(GarArgs), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     self._phase_a.restype = ctypes.c_int
     timeout = os.environ.get("AGB_FLAG_TIMEOUT_S")
     if timeout is not None:   # bound of the cross-GPU flag waits (default 120 s, 0 = wait forever)
@@ -149,12 +165,10 @@ class FusedLauncher:
         _check(_lib().agb_gar_set_flag_timeout(ctypes.c_double(float(timeout))), "gar_set_flag_timeout")
 
   def _fill(self, spec, rows, segments, *, agg_out=None, opt="none", lr=0.0, hyper=(0.0, 0.0, 0.0), param=None, slot0=None, slot1=None, param_dst=None, param_mc=0,
-            param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, max_ctas_limit=0, grad_mc=0, workers_per_rank=1, row_stride=0,
+            param_bf16_dst=None, rank=0, R=1, signals=None, mailboxes=None, epoch=1, staging=None, grad_mc=0, workers_per_rank=1, row_stride=0,
             first_seg=0, epoch_ptr=None, hyper_ptr=None, loss_in=None, loss_out=None, center=None, step=0, step_ptr=None, domain=None,
             bucketing_seed=0, root=None, history=None):
-    ptrs = self._ptrs
-    for i in range(PTRS):
-      ptrs[i] = 0
+    """A fresh `GarArgs` of one launch (every entry it does not set is 0), and the element count of the rule's scratch."""
     if not spec.gathered_rows(len(rows)):
       if spec.mix == FusedSpec.BUCKETING:
         raise tools.UserException("Bucketing with s = %d reduces %d gradient rows to %d, not the rule's %d" % (
@@ -162,47 +176,38 @@ class FusedLauncher:
       raise tools.UserException("Expected %d gradient rows, got %d" % (spec.n, len(rows)))
     if not 1 <= len(segments) <= MAX_SEGMENTS:
       raise tools.UserException("Between 1 and %d coordinate segments per rank (got %d)" % (MAX_SEGMENTS, len(segments)))
-    for i, row in enumerate(rows):
-      ptrs[i] = row
     addr = lambda t: 0 if t is None else (t if isinstance(t, int) else t.data_ptr())
-    ptrs[32], ptrs[33], ptrs[34], ptrs[35], ptrs[36] = addr(agg_out), addr(param), addr(slot0), addr(slot1), int(param_mc or 0)
-    dist_out = self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dnc_dist_out if spec.rule == "dnc" else self.dist_out
-    ptrs[37], ptrs[38], ptrs[39], ptrs[40], ptrs[41] = self.cta_partials.data_ptr(), addr(staging), dist_out.data_ptr(), self.info.data_ptr(), int(grad_mc or 0)
-    ptrs[42], ptrs[43], ptrs[44], ptrs[45], ptrs[46] = addr(epoch_ptr), addr(hyper_ptr), self.seg_partials.data_ptr(), addr(loss_in), addr(loss_out)
-    ptrs[47], ptrs[112] = addr(center), self.raw_dist_out.data_ptr()
-    if domain is None:
-      domain = max(hi for _, hi in segments)
-    scratch = self.dnc_scratch(spec, domain) if spec.rule == "dnc" else None
-    if spec.rule == "smea":
-      scratch = self.smea_scratch(spec)
-    ptrs[113], ptrs[114], ptrs[115] = addr(step_ptr), addr(scratch) if spec.rule == "dnc" else 0, self.arc_out.data_ptr()
-    ptrs[116] = addr(scratch) if spec.rule == "smea" else 0
-    ptrs[117], ptrs[118] = addr(root), self.fltrust_out.data_ptr()   # FLTrust: the root row (rank 0's, raw address or tensor)
-    ptrs[119], ptrs[120] = addr(history), self.foolsgold_out.data_ptr()   # FoolsGold: the [n, owned] histories (local)
+    a = GarArgs(n=spec.n, f=spec.f, m=spec.m, beta=spec.beta, rule=spec.rule_id, n_rows=len(rows), bkt_size=spec.bucket_size or 0,
+                bkt_seed=int(bucketing_seed), R=R, rank=rank, nseg=len(segments), first_seg=first_seg, seg_max_ctas=self.phase_a_ctas,
+                grad_mc=int(grad_mc or 0), workers_per_rank=workers_per_rank, row_stride=row_stride, agg_out=addr(agg_out),
+                opt=OPTIMIZERS[opt], lr=lr, h0=hyper[0], h1=hyper[1], h2=hyper[2], hyper_ptr=addr(hyper_ptr), param=addr(param),
+                slot0=addr(slot0), slot1=addr(slot1), param_mc=int(param_mc or 0), epoch=epoch & 0x7fffffff, epoch_ptr=addr(epoch_ptr),
+                cta_partials=self.cta_partials.data_ptr(), seg_partials=self.seg_partials.data_ptr(), staging=addr(staging),
+                raw_dist_out=self.raw_dist_out.data_ptr(), info=self.info.data_ptr(), loss_in=addr(loss_in),
+                nloss=loss_in.numel() if loss_in is not None else 0, loss_out=addr(loss_out), iterations=spec.iterations, nu=spec.nu,
+                tau=spec.tau, center=addr(center), mix=spec.mix_id, arc_out=self.arc_out.data_ptr(), dnc_b=spec.subsample, dnc_step=step,
+                dnc_seed=spec.seed, dnc_step_ptr=addr(step_ptr), root=addr(root), fltrust_out=self.fltrust_out.data_ptr(),
+                history=addr(history), foolsgold_out=self.foolsgold_out.data_ptr(), confidence=spec.confidence)
+    a.dist_out = (self.geo_dist_out if spec.rule in ITERATIVE_RULES else self.dnc_dist_out if spec.rule == "dnc" else self.dist_out).data_ptr()
+    for s, (lo, hi) in enumerate(segments):
+      a.seg_lo[s], a.seg_hi[s], a.seg_ctas[s] = lo, hi, self.phase_a_ctas if s < first_seg else 0
+    for i, row in enumerate(rows):
+      a.grad[i] = row
     for q in range(R):
-      ptrs[48 + q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
-      ptrs[64 + q] = addr(signals[q]) if signals is not None else 0
-      ptrs[80 + q] = addr(mailboxes[q]) if mailboxes is not None else (self.local_mailbox.data_ptr() if q == 0 else 0)
-      ptrs[96 + q] = addr(param_bf16_dst[q]) if param_bf16_dst is not None else 0
-    ints = self._ints
-    ints[0], ints[1], ints[2], ints[3], ints[4] = spec.n, spec.f, spec.m, spec.beta, spec.rule_id
-    ints[5], ints[6], ints[7], ints[8], ints[9] = R, rank, OPTIMIZERS[opt], epoch & 0x7fffffff, max_ctas_limit
-    ints[10], ints[11], ints[12], ints[13] = workers_per_rank, len(segments), first_seg, (loss_in.numel() if loss_in is not None else 0)
-    ints[14], ints[15], ints[24], ints[25], ints[26] = self.phase_a_ctas, self.phase_a_ctas, self.phase_a_threads, spec.iterations, spec.mix_id
-    self._longs[0] = row_stride
-    for s in range(MAX_SEGMENTS):
-      lo, hi = segments[s] if s < len(segments) else (0, 0)
-      self._longs[1 + s], self._longs[1 + MAX_SEGMENTS + s] = lo, hi
-      ints[16 + s] = self.phase_a_ctas if s < first_seg else 0
-    self._floats[0], self._floats[1], self._floats[2], self._floats[3], self._floats[4] = lr, hyper[0], hyper[1], hyper[2], spec.nu
-    self._floats[5] = spec.tau
-    ints[27] = spec.removed if spec.rule == "dnc" else 0
-    ints[28], ints[29] = spec.bucket_size or 0, len(rows)
-    longs = self._longs
-    signed = lambda seed: seed - (1 << 64) if seed >= 1 << 63 else seed
-    longs[17], longs[18], longs[19], longs[20] = spec.subsample, domain, signed(spec.seed), step
-    longs[21], longs[22] = scratch.numel() if scratch is not None else 0, signed(int(bucketing_seed))
-    longs[23] = struct.unpack("<q", struct.pack("<d", spec.confidence))[0]   # FoolsGold's kappa, float64 bits
+      a.param_dst[q] = addr(param_dst[q]) if param_dst is not None else (addr(param) if q == 0 else 0)
+      a.signal[q] = addr(signals[q]) if signals is not None else 0
+      a.mailbox[q] = addr(mailboxes[q]) if mailboxes is not None else (self.local_mailbox.data_ptr() if q == 0 else 0)
+      a.param_bf16_dst[q] = addr(param_bf16_dst[q]) if param_bf16_dst is not None else 0
+    a.dnc_domain = max(hi for _, hi in segments) if domain is None else domain
+    scratch = None
+    if spec.rule == "dnc":
+      a.dnc_r = spec.removed
+      scratch = self.dnc_scratch(spec, a.dnc_domain)
+      a.dnc_scratch = scratch.data_ptr()
+    elif spec.rule == "smea":
+      scratch = self.smea_scratch(spec)
+      a.smea_scratch = scratch.data_ptr()
+    return a, scratch.numel() if scratch is not None else 0
 
   def dnc_scratch(self, spec, domain):
     """DnC's scratch for rule `spec` over `domain` coordinates: the CTA partials of the sampled distances of the largest grid, then the
@@ -227,18 +232,19 @@ class FusedLauncher:
       self._mimic_y = torch.zeros(d, dtype=torch.float32, device=self.device)
     return self._mimic_y
 
-  def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, **kwargs):
+  def launch(self, spec, rows, lo=None, hi=None, *, segments=None, stream=None, max_ctas_limit=0, **kwargs):
     """The finish kernel (the whole aggregation unless `first_seg` segments were pre-accumulated by `phase_a`).
     `rows`: n device addresses of the workers' gradient rows (raw ints, local or peer-mapped); owned coordinates `[lo, hi)` or `segments`."""
-    self._fill(spec, rows, segments if segments is not None else [(lo, hi)], **kwargs)
+    args, scratch_elems = self._fill(spec, rows, segments if segments is not None else [(lo, hi)], **kwargs)
     with torch.cuda.device(self.device):
-      _check(self._func(self._ptrs, self._ints, self._longs, self._floats, _stream_ptr(stream)), "gar_fused")
+      _check(self._func(args, max_ctas_limit, scratch_elems, _stream_ptr(stream)), "gar_fused")
 
-  def phase_a(self, spec, rows, segments, seg, *, stream=None, **kwargs):
-    """Pre-accumulate the partial distances of owned segment `seg` (and stage its tile) on a few CTAs, e.g. under the backward pass."""
-    self._fill(spec, rows, segments, **kwargs)
+  def phase_a(self, spec, rows, segments, seg, *, stream=None, max_ctas_limit=0, **kwargs):
+    """Pre-accumulate the partial distances of owned segment `seg` (and stage its tile) on a few CTAs, e.g. under the backward pass.
+    Takes `launch`'s arguments; `max_ctas_limit` bounds the finish kernel alone."""
+    args, _ = self._fill(spec, rows, segments, **kwargs)
     with torch.cuda.device(self.device):
-      _check(self._phase_a(self._ptrs, self._ints, self._longs, self._floats, ctypes.c_int(seg), _stream_ptr(stream)), "gar_phase_a")
+      _check(self._phase_a(args, seg, self.phase_a_ctas, self.phase_a_threads, _stream_ptr(stream)), "gar_phase_a")
 
 
 _launchers = {}
@@ -317,16 +323,21 @@ def aggregate(spec, G, return_details=False, center=None, step=0, bucketing_seed
   return out
 
 
+def _padded(t, dp):
+  """The [d] vector or [n, d] matrix `t` itself when d = dp and it is contiguous on a 16-byte boundary, else a zero-padded [.., dp] copy.
+  A caller whose kernel writes the buffer copies [.., :d] back into `t` when it received a copy."""
+  d = t.shape[-1]
+  if d == dp and t.is_contiguous() and t.data_ptr() % 16 == 0:
+    return t
+  copy = torch.zeros(t.shape[:-1] + (dp,), dtype=t.dtype, device=t.device)
+  copy[..., :d] = t
+  return copy
+
+
 def _aligned_rows(G):
-  """Contiguous [n, dp] rows, dp the next multiple of 4, on a 16-byte boundary (zero padding) -> (rows, dp)."""
-  n, d = G.shape
-  G = G.contiguous()
-  pad = (-d) % 4
-  if pad or G.data_ptr() % 16:
-    Gp = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
-    Gp[:, :d] = G
-    G = Gp
-  return G, d + pad
+  """`_padded` rows of the [n, d] matrix G, dp the next multiple of 4 -> (rows, dp)."""
+  dp = G.shape[1] + (-G.shape[1]) % 4
+  return _padded(G, dp), dp
 
 
 def _staging(spec, dp, device):
@@ -381,11 +392,7 @@ def _aggregate_centered_clipping(spec, G, return_details, center, step=0, bucket
   if G.dtype != torch.float32 or center.dtype != torch.float32:
     raise tools.UserException("Centered clipping on the device needs fp32 rows and center (got %s, %s)" % (G.dtype, center.dtype))
   G, dp = _aligned_rows(G)
-  pad = dp - d
-  work = center
-  if pad or not center.is_contiguous() or center.data_ptr() % 16:
-    work = torch.zeros(dp, dtype=torch.float32, device=G.device)
-    work[:d] = center
+  work = _padded(center, dp)
   launcher = _launcher(G.device, n, m)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
@@ -415,15 +422,11 @@ def _aggregate_fltrust(spec, G, return_details, root):
     out = _aggregate_fltrust(spec, G.float(), return_details, root.float())
     return (out[0].to(G.dtype),) + out[1:] if return_details else out.to(G.dtype)
   G, dp = _aligned_rows(G)
-  work = root
-  if dp != d or not root.is_contiguous() or root.data_ptr() % 16:
-    work = torch.zeros(dp, dtype=torch.float32, device=G.device)
-    work[:d] = root
   launcher = _launcher(G.device, n)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
   staging = torch.empty((n, dp), dtype=torch.float32, device=G.device) if n > 8 else None   # beyond one 8-row block: the staged rows
-  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=staging, root=work)
+  launcher.launch(spec, rows, 0, dp, agg_out=out, staging=staging, root=_padded(root, dp))
   out = out[:d]
   if return_details:
     fo = launcher.fltrust_out.cpu()
@@ -446,10 +449,7 @@ def _aggregate_foolsgold(spec, G, return_details, history):
   if G.dtype != torch.float32:
     raise tools.UserException("FoolsGold on the device needs fp32 or float64 rows (got %s)" % (G.dtype,))
   G, dp = _aligned_rows(G)
-  work = history
-  if dp != d or not history.is_contiguous() or history.data_ptr() % 16:
-    work = torch.zeros((n, dp), dtype=torch.float32, device=G.device)
-    work[:, :d] = history
+  work = _padded(history, dp)
   launcher = _launcher(G.device, n)
   out = torch.empty(dp, dtype=torch.float32, device=G.device)
   rows = [G.data_ptr() + i * dp * 4 for i in range(n)]
@@ -523,14 +523,25 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
   lo = (ctypes.c_longlong * len(segments))(*[int(a) for a, _ in segments])
   hi = (ctypes.c_longlong * len(segments))(*[int(b) for _, b in segments])
   c_signals = (ctypes.c_ulonglong * R)(*[addr(signals[q]) for q in range(R)]) if signals is not None else None
-  if mode == "mimic":
-    if launcher is None or state is None or warmup is None:
-      raise tools.UserException("mimic needs the scratch of a FusedLauncher, its state and its warm-up length")
+  # the leading and trailing arguments of every crafting entry point
+  rows_args = (c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)))
+  epoch_args = (ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream))
+  if mode == "fang-krum":
+    threshold = _ops.check_fang_krum(n, len(set(byzantine)), f, threshold)
+  elif mode in ("min-max", "min-sum"):
+    if deviation is None:
+      deviation = "unit-vec"
+    if deviation not in DEVIATIONS:
+      raise tools.UserException("Unknown deviation %r for %s (expected one of %s)" % (deviation, mode, ", ".join(DEVIATIONS)))
+  if mode in ("mimic", "fang-krum", "min-max", "min-sum"):   # the launcher's scratch, and a cross-rank exchange through the mailboxes
+    if launcher is None or (mode == "mimic" and (state is None or warmup is None)):
+      raise tools.UserException(mode + " needs the scratch of a FusedLauncher" + (", its state and its warm-up length" if mode == "mimic" else ""))
     if mailboxes is None:
       if R != 1:
-        raise tools.UserException("mimic over %d ranks needs every rank's mailbox" % R)
+        raise tools.UserException("%s over %d ranks needs every rank's mailbox" % (mode, R))
       mailboxes = [launcher.local_mailbox]
     c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
+  if mode == "mimic":
     t = int(state["t"])
     warm = t < int(warmup)
     z = state["z"]
@@ -539,11 +550,10 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
     y = launcher.mimic_scratch(z.numel()) if warm else None
     func = _lib().agb_gar_byzantine_mimic
     func.restype = ctypes.c_int
-    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
-                ctypes.c_int(1 if warm else 0), ctypes.c_int(t), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+    _check(func(*rows_args, ctypes.c_int(1 if warm else 0), ctypes.c_int(t), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
                 ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(addr(z)),
                 ctypes.c_ulonglong(addr(y)), ctypes.c_ulonglong(addr(state["istar"])), ctypes.c_ulonglong(launcher.mimic_stats.data_ptr()),
-                ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_mimic")
+                *epoch_args), "gar_byzantine_mimic")
     if warm:
       state["t"] = t + 1
     return
@@ -552,51 +562,29 @@ def craft(rows, segments, honest, byzantine, mode, coef, *, deviation=None, laun
     key = _ops.fang_trim_key(0 if seed is None else seed, step)
     func = _lib().agb_gar_byzantine_fang_trim
     func.restype = ctypes.c_int
-    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
-                ctypes.c_float(scale), ctypes.c_ulonglong(key), ctypes.c_int(R), ctypes.c_int(rank), c_signals, ctypes.c_uint(epoch & 0x7fffffff),
-                ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_fang_trim")
+    _check(func(*rows_args, ctypes.c_float(scale), ctypes.c_ulonglong(key), ctypes.c_int(R), ctypes.c_int(rank), c_signals, *epoch_args),
+           "gar_byzantine_fang_trim")
     return
   if mode == "fang-krum":
-    threshold = _ops.check_fang_krum(n, len(set(byzantine)), f, threshold)
-    if launcher is None:
-      raise tools.UserException("fang-krum needs the scratch of a FusedLauncher")
-    if mailboxes is None:
-      if R != 1:
-        raise tools.UserException("fang-krum over %d ranks needs every rank's mailbox" % R)
-      mailboxes = [launcher.local_mailbox]
-    c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
     func = _lib().agb_gar_byzantine_fang_krum
     func.restype = ctypes.c_int
-    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
-                ctypes.c_int(f), ctypes.c_float(threshold), ctypes.c_int(1 if search else 0), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+    _check(func(*rows_args, ctypes.c_int(f), ctypes.c_float(threshold), ctypes.c_int(1 if search else 0), ctypes.c_int(R), ctypes.c_int(rank),
+                c_signals, c_mailboxes,
                 ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(launcher.craft_stats.data_ptr()),
-                ctypes.c_ulonglong(launcher.fang_out.data_ptr()), ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)),
-                _stream_ptr(stream)), "gar_byzantine_fang_krum")
+                ctypes.c_ulonglong(launcher.fang_out.data_ptr()), *epoch_args), "gar_byzantine_fang_krum")
     return
   if mode in ("min-max", "min-sum"):
-    if deviation is None:
-      deviation = "unit-vec"
-    if deviation not in DEVIATIONS:
-      raise tools.UserException("Unknown deviation %r for %s (expected one of %s)" % (deviation, mode, ", ".join(DEVIATIONS)))
-    if launcher is None:
-      raise tools.UserException("%s needs the scratch of a FusedLauncher" % mode)
-    if mailboxes is None:
-      if R != 1:
-        raise tools.UserException("%s over %d ranks needs every rank's mailbox" % (mode, R))
-      mailboxes = [launcher.local_mailbox]
-    c_mailboxes = (ctypes.c_ulonglong * R)(*[addr(mailboxes[q]) for q in range(R)])
     func = _lib().agb_gar_byzantine_optimized
     func.restype = ctypes.c_int
-    _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
-                ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_int(DEVIATIONS[deviation]), ctypes.c_int(R), ctypes.c_int(rank), c_signals, c_mailboxes,
+    _check(func(*rows_args, ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_int(DEVIATIONS[deviation]), ctypes.c_int(R), ctypes.c_int(rank),
+                c_signals, c_mailboxes,
                 ctypes.c_ulonglong(launcher.craft_partials.data_ptr()), ctypes.c_int(launcher.craft_ctas), ctypes.c_ulonglong(launcher.craft_stats.data_ptr()),
-                ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine_optimized")
+                *epoch_args), "gar_byzantine_optimized")
     return
   func = _lib().agb_gar_byzantine
   func.restype = ctypes.c_int
-  _check(func(c_rows, ctypes.c_int(n), lo, hi, ctypes.c_int(len(segments)), ctypes.c_uint(mask(honest)), ctypes.c_uint(mask(byzantine)),
-              ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_float(coef), ctypes.c_int(R), ctypes.c_int(rank), c_signals,
-              ctypes.c_uint(epoch & 0x7fffffff), ctypes.c_ulonglong(addr(epoch_ptr)), _stream_ptr(stream)), "gar_byzantine")
+  _check(func(*rows_args, ctypes.c_int(BYZANTINE_MODES[mode]), ctypes.c_float(coef), ctypes.c_int(R), ctypes.c_int(rank), c_signals,
+              *epoch_args), "gar_byzantine")
 
 
 def craft_details(launcher, mode, H):
@@ -639,10 +627,7 @@ def _craft_mimic_(G, byz_slots, state, warmup, return_details):
     raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
   work, dp = _aligned_rows(G)
   z = state["z"]
-  zwork = z
-  if dp != d or not z.is_contiguous() or z.data_ptr() % 16:
-    zwork = torch.zeros(dp, dtype=torch.float32, device=G.device)
-    zwork[:d] = z
+  zwork = _padded(z, dp)
   run = dict(state, z=zwork)
   warm = run["t"] < warmup
   launcher = _launcher(G.device, n)
@@ -692,12 +677,7 @@ def craft_byzantine_(G, byz_slots, mode, coef=None, deviation=None, return_detai
     return _ops.torch_craft_byzantine_(G, byz_slots, mode, coef, deviation=deviation, return_details=return_details, **fang)
   if G.dtype != torch.float32:
     raise tools.UserException("ops.gar.craft_byzantine_ expects fp32 rows (got %s)" % G.dtype)
-  pad = (-d) % 4
-  work = G
-  if pad or not G.is_contiguous() or G.data_ptr() % 16:
-    work = torch.zeros((n, d + pad), dtype=G.dtype, device=G.device)
-    work[:, :d] = G
-  dp = d + pad
+  work, dp = _aligned_rows(G)
   rows = [work.data_ptr() + i * dp * 4 for i in range(n)]
   launcher = _launcher(G.device, n) if optimized or mode == "fang-krum" else None
   with torch.cuda.device(G.device):

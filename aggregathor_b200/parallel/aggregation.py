@@ -392,7 +392,8 @@ class FusedAggregation(_AggregationBase):
     self.segments = self.segments_of[self.rank]
     self.lo, self.hi = self.segments[0][0], self.segments[-1][1]   # meaningful for a single bucket (contiguous slice)
     owned = sum(hi - lo for lo, hi in self.segments)
-    sizes = {"grads": w * d * 4, "params": d * 4, "signals": gar_ops.SIGNAL_BYTES, "mailbox": gar_ops.MAILBOX_BYTES}
+    signal_bytes, mailbox_bytes = gar_ops.region_bytes()
+    sizes = {"grads": w * d * 4, "params": d * 4, "signals": signal_bytes, "mailbox": mailbox_bytes}
     if bf16_copy:
       sizes["params_bf16"] = d * 2
     if self.needs_root:

@@ -2,6 +2,7 @@
 included), the kernel's permutation and masks against `_ops`, the status codes, fused (CUDA graph, device step key) vs baseline
 training with worker momentum under ALIE and flip, SMEA at (32, 4), and the multi-GPU engine."""
 
+import ctypes
 import json
 import math
 import os
@@ -142,7 +143,7 @@ def test_step_changes_the_permutation_and_fall_backs():
   _equal_bits(out, _ops.torch_median(_ops.torch_bucketing(G40.cuda(), 2, 0, 6)))
 
 
-def test_kernel_rejects_invalid_parameters():
+def test_kernel_rejects_invalid_bucketing_arguments():
   from aggregathor_b200.ops import gar as gar_ops
   G = torch.randn(8, 64, device="cuda")
   rows = [G.data_ptr() + i * 64 * 4 for i in range(8)]
@@ -156,11 +157,11 @@ def test_kernel_rejects_invalid_parameters():
     bad = FusedSpec("average", 1, mix="bucketing", bucket_size=2)
     launcher.launch(bad, rows[:1], 0, 64, agg_out=out, staging=staging)
   # argument blocks FusedSpec never produces, patched after `_fill`: bucketing with NNM or ARC, and n != ceil(n_rows / s)
-  for slot, value in ((26, FusedSpec.MIX_BUCKETING | FusedSpec.MIX_NNM), (26, FusedSpec.MIX_BUCKETING | FusedSpec.MIX_ARC), (0, 5)):
-    launcher._fill(spec, rows, [(0, 64)], agg_out=out, staging=staging)
-    launcher._ints[slot] = value
+  for field, value in (("mix", FusedSpec.MIX_BUCKETING | FusedSpec.MIX_NNM), ("mix", FusedSpec.MIX_BUCKETING | FusedSpec.MIX_ARC), ("n", 5)):
+    args, scratch_elems = launcher._fill(spec, rows, [(0, 64)], agg_out=out, staging=staging)
+    setattr(args, field, value)
     with pytest.raises(RuntimeError, match="status 123"):
-      gar_ops._check(launcher._func(launcher._ptrs, launcher._ints, launcher._longs, launcher._floats, gar_ops._stream_ptr()), "gar_fused")
+      gar_ops._check(gar_ops._lib().agb_gar_fused(ctypes.byref(args), 0, ctypes.c_longlong(scratch_elems), gar_ops._stream_ptr()), "gar_fused")
   with pytest.raises(tools.UserException, match="reduces 8 gradient rows to 4"):
     launcher.launch(FusedSpec("average", 3, mix="bucketing", bucket_size=2), rows, 0, 64, agg_out=out, staging=staging)
   krum = FusedSpec("krum", 4, f=0, m=1, mix="bucketing", bucket_size=2)
