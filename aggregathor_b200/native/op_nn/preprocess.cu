@@ -278,14 +278,22 @@ __global__ void __launch_bounds__(512) preprocess_kernel(PreprocParams const p) 
 
     float std_mean = 0.f, std_inv = 1.f;
     if (cifar) {   // per-image standardisation over all channels: second reduction (mean, mean of squares) of the adjusted image
+        // The sums run around a centre known before the sweep: contrast keeps each channel's mean at mean_c, so the mean of the
+        // mean_c is the image mean up to rounding. E[v^2] - E[v]^2 taken around 0 would lose the variance of bright, nearly uniform
+        // images (values near 300, variance near 0.02) to the rounding of E[v^2].
+        float centre = 0.f;
+        for (int c = 0; c < p.C; ++c)
+            centre += mean_c[c];
+        centre /= static_cast<float>(p.C);
         float a0 = 0.f, a1 = 0.f;
         for (int idx = threadIdx.x; idx < pixels; idx += blockDim.x) {
             float v[3];
             stage1(idx, v);
             stage2(v);
             for (int c = 0; c < p.C; ++c) {
-                a0 += v[c];
-                a1 += v[c] * v[c];
+                float const d = v[c] - centre;
+                a0 += d;
+                a1 += d * d;
             }
         }
         int const warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -303,9 +311,9 @@ __global__ void __launch_bounds__(512) preprocess_kernel(PreprocParams const p) 
                 t1 += red[w][4];
             }
             float const count = static_cast<float>(pixels) * p.C;
-            float const mean = t0 / count;
-            float const var = fmaxf(t1 / count - mean * mean, 0.f);
-            stats[3] = mean;
+            float const shift = t0 / count;   // mean - centre
+            float const var = fmaxf(t1 / count - shift * shift, 0.f);
+            stats[3] = centre + shift;
             stats[4] = 1.f / fmaxf(sqrtf(var), rsqrtf(count));   // tf.image.per_image_standardization: max(stddev, 1/sqrt(N))
         }
         __syncthreads();

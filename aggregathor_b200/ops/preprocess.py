@@ -200,9 +200,12 @@ class Preprocessor:
       v = v + per(p["brightness"])
       mean = v.mean(dim=(1, 2), keepdim=True)
       v = (v - mean) * per(p["contrast"]) + mean
-      m = v.mean(dim=(1, 2, 3), keepdim=True)
-      var = ((v * v).mean(dim=(1, 2, 3), keepdim=True) - m * m).clamp_min(0.0)
-      v = (v - m) / torch.maximum(var.sqrt(), torch.full_like(var, 1.0 / math.sqrt(oh * ow * c)))
+      # the variance around the mean of the channel means (what the contrast keeps), as the kernel takes it
+      centre = mean.mean(dim=3, keepdim=True)
+      d = v - centre
+      shift = d.mean(dim=(1, 2, 3), keepdim=True)
+      var = ((d * d).mean(dim=(1, 2, 3), keepdim=True) - shift * shift).clamp_min(0.0)
+      v = (v - (centre + shift)) / torch.maximum(var.sqrt(), torch.full_like(var, 1.0 / math.sqrt(oh * ow * c)))
     else:
       v = (v - torch.tensor(self.mean[:c], device=dev, dtype=torch.float32)) * self.scale
     return v.to(dtype).permute(0, 3, 1, 2)
